@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- Score() prompts/sec @4K tokens against a 10M-block / 256-pod index (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path (GetPodScores steps 2-4, pkg/kvcache/indexer.go:141-163) over one
 batch of synthetic 4096-token prompts.
@@ -13,6 +13,11 @@ batch of synthetic 4096-token prompts.
             the measured HBM copy bandwidth in MEASURED_PEAKS.json
   cpu_baseline  the C++ restatement of the reference's Go path (oracle/, kind "port") on this box's host cores,
             on a bounded sample of the same prompts against the same 10M-block index
+
+--dump-outputs DIR writes what the last timed step returned, for comparing two builds output for output (the inputs
+are seeded, so the same arguments give the same prompts): scores.npy, a fixed seeded sample of DUMP_ROWS dense score
+rows (f64, -1.0 = absent), has_keys.npy (f32, 1.0 = the prompt yields at least one block key) and rows.npy (f64, the
+sampled prompt indices).
 
 Multi-GPU (torchrun, one rank per GPU), "scaling": "weak" (every rank scores its own resident batch):
   value           hash-range SHARDED index (the north-star layout): tables partitioned over the ranks, probes and slot
@@ -43,6 +48,7 @@ N_BLOCKS = int(os.environ.get("KVIDX_BENCH_BLOCKS", "10000000"))
 N_PODS, BLOCK = 256, 16
 CONFIG_ID = 6
 WEIGHTS = (1.0, 0.8)
+DUMP_ROWS = 16384          # 16384 rows x 256 pods x 8 B = 32 MB
 
 
 def log(*a):
@@ -111,7 +117,7 @@ def algorithmic_bytes(wl, m):
 
 # ----------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -149,24 +155,19 @@ def measured_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
-def ncu_traffic():
-    """DRAM bytes (read+write) per prompt of one default Score() step from the committed ncu captures: the range profile of the
-    whole step (profiles/r2_step_range_profile.json, `ncu --replay-mode range --set full`, its kernels as one unit), else the sum
-    over the per-kernel launch list (profiles/score_step_traffic.json); None if neither is committed."""
-    try:
-        m = json.load(open(os.path.join(ROOT, "profiles", "r2_step_range_profile.json")))["metrics"]
-        unit = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}
-        tot = sum(float(m[k]["value"]) * unit[m[k]["unit"]] for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"))
-        return tot / 1048576.0
-    except Exception:
-        pass
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "score_step_traffic.json")))["dram_bytes_per_prompt"]
-    except Exception:
-        return None
+def dump_outputs(dirname, scores, has_keys):
+    """The timed path's result rows (see --dump-outputs), a seeded sample so that the files stay under 64 MB."""
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    n = scores.shape[0]
+    rows = np.sort(np.random.default_rng(0).choice(n, size=min(n, DUMP_ROWS), replace=False))
+    idx = torch.from_numpy(rows).to(scores.device)
+    np.save(os.path.join(dirname, "scores.npy"), scores.index_select(0, idx).cpu().numpy().astype(np.float64))
+    np.save(os.path.join(dirname, "has_keys.npy"), has_keys.index_select(0, idx).cpu().numpy().astype(np.float32))
+    np.save(os.path.join(dirname, "rows.npy"), rows.astype(np.float64))
 
 
 # ----------------------------------------------------------------------------------------------
@@ -430,6 +431,8 @@ def run_ours(args):
             b.record(stream)
         t_all1.record(stream)
         barrier()
+        if args.dump_outputs and mode == primary and rank == 0:
+            dump_outputs(args.dump_outputs, d_scores, d_has)
         launches = ixx.stats()["kernel_launches"] - launches0
         total_ms = max_ranks(t_all0.elapsed_time(t_all1))
         t_wait = time.time()
@@ -536,8 +539,8 @@ def run_ours(args):
                             "issued by the walk for the slots it actually visits). Both bit-exact vs the closed form."}
 
     # ---- SURVEY config #5: Score() with the write path running BESIDE it.  A writer thread applies BlockStored batches of new
-    # documents and BlockRemoved batches of the ones stored a moment ago through kvidx_apply_events (its own stream; slot
-    # updates are single-image publishes the readers never wait for) at >= 100 K events/s per GPU, while this thread runs
+    # documents and BlockRemoved batches of the ones stored a moment ago through kvidx_apply_events (its own stream; a reader
+    # waits only for a slot that a writer owns at that moment) at >= 100 K events/s per GPU, while this thread runs
     # Score() steps on the resident batch.  Scores of the resident batch must stay bit-exact.
     mixed = None
     if not os.environ.get("KVIDX_BENCH_SKIP_MIXED"):
@@ -604,17 +607,12 @@ def run_ours(args):
     peak, peak_src = measured_peak()
     kern_s = float(step_ms.mean()) / 1e3
     achieved = float(A.sum()) / kern_s / 1e9
-    default_cfg = (T_TOKENS, N_BLOCKS, Q) == (4096, 10_000_000, 1048576) and primary != "sharded"
-    traffic = ncu_traffic() if default_cfg else None          # the committed ncu capture is of the default single-GPU step only
     roof = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": None if traffic is None else traffic * Q,
             "peak_source": peak_src, "algorithmic_bytes_per_prompt_mean": float(A.mean()),
             "algorithmic_bytes_per_launch": float(A.sum()), "kernel_ms": float(step_ms.mean()),
             "kernel": "one step = prefix sort + rounds x parts x (group_round [cp.async token chunks], group_lists, hash_round, walk_round, finish_round), kernel G on low-priority streams; "
                       "achieved = step's algorithmic bytes / step GPU time (CUDA events around all of its launches), i.e. a lower bound for "
-                      "every kernel in it; per-kernel ncu summaries under profiles/",
-            "note": "traffic = DRAM bytes of one step from the committed ncu range profile of the whole step (profiles/r2_step_range_profile.json; "
-                    "per kernel: profiles/score_step_traffic.json), default single-GPU configuration only; null for any other configuration"}
+                      "every kernel in it"}
 
     # ---- e2e: host pinned buffers through the C ABI (H2D + kernels + D2H inside the timed region) ----
     #   headline e2e: kvidx_score_batch_sparse -- the reference's result shape (a map of <= 10 pods per prompt, indexer.go:134)
@@ -754,12 +752,12 @@ def run_ours(args):
                           "prompt_tokens": wl.T, "index_blocks": wl.n_blocks, "pods": wl.P, "block_size": BLOCK,
                           "batch_prompts_per_gpu": Q, "query_mix": "m uniform in [0,n] matched blocks + random tail",
                           "queries_per_document": Q / wl.D,
-                          "pipeline": "prefix-class rounds: each distinct prefix is hashed and probed once per batch (batches >= 393216 prompts; "
+                          "pipeline": "prefix-class rounds: each distinct prefix is hashed and probed once per batch (batches >= 131072 prompts; "
                                       "smaller ones, and batches with little repetition, take the per-prompt round kernels, <= 2048 prompts the "
                                       "warp-per-prompt cooperative kernel)"
                                       if launches / max(args.steps, 1) > 100 else "per-prompt rounds / cooperative kernel (batch below the class pipeline's size "
                                       "threshold, or too little repetition: fewer than ~6 prompts per distinct first block)",
-                          "l2_policy": "inputs (%.1f GB tokens + %.1f GB table) larger than the 126 MB L2; no flush" % (Q * wl.T * 4 / 1e9, fill["slots"] * 32 / 1e9),
+                          "l2_policy": "inputs (%.1f GB tokens + %.1f GB table) larger than the 50 MB L2; no flush" % (Q * wl.T * 4 / 1e9, fill["slots"] * 32 / 1e9),
                           "multi_gpu": {"single": "single GPU", "replicas": "replicas: full index per GPU, prompts sharded, no data-path collective",
                                         "sharded": "hash-range sharded tables (the north-star layout): probes and slot updates over NVLink peer memory "
                                                    "from the scoring / event kernels themselves (CUDA IPC), per-pod ingest ranks; value_replicas = "
@@ -819,6 +817,7 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

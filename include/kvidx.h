@@ -1,5 +1,5 @@
 /*
- * kvidx.h -- C ABI of libkvidx: the B200-resident KV-block locality index.
+ * kvidx.h -- C ABI of libkvidx: the GPU-resident KV-block locality index.
  *
  * This is the drop-in boundary for ONE hot path of llm-d/llm-d-kv-cache-manager:
  * kvcache.Indexer.GetPodScores() steps 2-4 (token blocks -> chain-hashed request

@@ -37,7 +37,7 @@ struct Fnv {
     // 33 instructions; the up-to-four extra bytes of wider tokens are committed under predicates
     // (hi by a predicated IMAD, lo by a select).  ncu on the branchy form showed the compiler's
     // jump chain re-executing the shared byte steps once per divergent group (7 steps / token
-    // instead of 5 for a warp that mixes 3- and 5-byte tokens); see profiles/r1a_*.
+    // instead of 5 for a warp that mixes 3- and 5-byte tokens).
 #define KVX_STEP_U(BYTE) BYTE "xor.b32 x, %0, b;\n\tmul.wide.u32 w, x, 0x1b3;\n\tmov.b64 {wl, wh}, w;\n\t" \
         "mad.lo.u32 u, %1, 0x1b3, wh;\n\tmad.lo.u32 %1, x, 256, u;\n\tmov.u32 %0, wl;\n\t"
 #define KVX_STEP_P(P, BYTE) BYTE "xor.b32 x, %0, b;\n\tmul.wide.u32 w, x, 0x1b3;\n\tmov.b64 {wl, wh}, w;\n\t" \

@@ -64,10 +64,10 @@ __device__ __forceinline__ uint32_t ballot_bit(uint32_t z, uint32_t bit) {
 // Bit plane k of the 8-bit recurrence L' = ((L ^ b) * 0xb3) & 0xff: every position contributes g = bit k of (b ^ Y), Y the
 // carry word (x mod 2^k) * 0xb3; L_k before a lane's first position is the XOR of all g of earlier lanes -- ONE ballot of
 // the lanes' parities and a popcount -- and inside the lane two more register XORs.  The planes are inherently sequential
-// (plane k+1's carries need plane k's x bits): a block is eight rounds of VOTE -> POPC -> (4 ALU) -> VOTE.  Measured
-// (scripts/ubench_coop2.cu, one warp): ~130 cycles per plane, of which the VOTE + POPC pair is the larger part -- preparing
-// the next plane's parity for both outcomes while the ballot is in flight (a single LOP3.P between POPC and the next VOTE)
-// changed nothing (1337 vs 1280 cycles per block), and a shuffle XOR scan instead of the ballot doubles it.
+// (plane k+1's carries need plane k's x bits): a block is eight rounds of VOTE -> POPC -> (4 ALU) -> VOTE.  The VOTE + POPC
+// pair is the larger part of a plane; scripts/ubench_coop2.cu times a block with one warp, and with alternatives such as
+// preparing the next plane's parity for both outcomes while the ballot is in flight, or a shuffle XOR scan instead of the
+// ballot.
 __device__ __forceinline__ uint64_t coop_hash_block(const CoopTables& tab, uint64_t parent, uint32_t tb, uint32_t b0, uint32_t b1, uint32_t b2,
                                                     uint32_t vmask, int lane, uint32_t lt) {
     if (lane < 4) {                                         // positions 2..9 carry the parent, most significant byte first

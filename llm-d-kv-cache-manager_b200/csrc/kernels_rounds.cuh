@@ -19,7 +19,7 @@
 //   R+D finish_round_kernel  followers copy their representative's fate; partial followers resume from its snapshot and
 //                            walk their own blocks; next round's live list
 //
-// The per-round cost is a fixed ~0.2 ms of short latency-bound kernels (hidden by running the batch as independent parts
+// Every round pays a fixed cost of short latency-bound kernels (hidden by running the batch as independent parts
 // on separate streams), so medium batches use kernels_rounds_plain.cuh instead (see kvidx.cu: launch_score).
 #pragma once
 #include <cuda_runtime.h>
@@ -33,8 +33,8 @@ constexpr int kRoundBlocks = 32;         // blocks hashed per prompt per round (
 #define KVIDX_HASH_THREADS 256
 #endif
 constexpr int kHashThreads = KVIDX_HASH_THREADS;
-constexpr int kHashStages = KVIDX_HASH_STAGES;   // token blocks staged per prompt.  (4 stages x 4 warps was measured: slower -- what a launch of this kernel
-                                         // waits for is room on an SM beside kernel G's CTAs, so the smaller footprint per warp wins: scripts/ab_step.py)
+constexpr int kHashStages = KVIDX_HASH_STAGES;   // token blocks staged per prompt.  (4 stages x 4 warps is the alternative: what a launch of this kernel
+                                         // waits for is room on an SM beside kernel G's CTAs, so the smaller footprint per warp is the choice; scripts/ab_step.py compares them)
 constexpr int kGroupThreads = 256;
 constexpr uint32_t kRoleSelf = 0xffffffffu;
 
@@ -97,8 +97,8 @@ struct RoundBufs {
 };
 constexpr uint8_t kFateMore = 1, kFateDone = 2;
 
-constexpr int kHashChunk = 1;            // blocks staged per copy step (2 = 128-byte accesses was measured: fewer, longer DRAM
-                                         // accesses but only 24 resident warps/SM -> 6 % slower; the kernel is pipe bound)
+constexpr int kHashChunk = 1;            // blocks staged per copy step (2 = 128-byte accesses: fewer, longer DRAM accesses
+                                         // but only 24 resident warps/SM, and the kernel is pipe bound)
 template <int BS> struct HashSmem {
     static constexpr int kRow = kHashChunk * BS * 4 + 16;   // 144 B: the four LDS.128 of a block stay conflict free
     unsigned char tok[kHashThreads / 32][kHashStages][32 * kRow];     // [warps of the CTA]: a launch with fewer warps passes that much less
@@ -131,7 +131,7 @@ constexpr int kGroupTile = KVIDX_GROUP_TILE;   // live prompts a warp of kernel 
 #ifndef KVIDX_GROUP_RING
 #define KVIDX_GROUP_RING 4
 #endif
-constexpr int kGroupRing = KVIDX_GROUP_RING;            // chunk slots per warp: one being examined, two in flight, the anchor (deeper rings measured: slower)
+constexpr int kGroupRing = KVIDX_GROUP_RING;            // chunk slots per warp: one being examined, two in flight, the anchor (deeper rings cost occupancy)
 struct GroupSmem {
     uint4 ring[kGroupThreads / 32][kGroupRing][4][32];                       // 64 KB
     unsigned long long bar[kGroupThreads / 32][kGroupRing];                  // TMA variant: one mbarrier per rotating slot
@@ -495,7 +495,7 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
             h = round == 0 ? t.init_hash : rb.hstate[p];
         }
         const int nb_max = __reduce_max_sync(0xffffffffu, nb);
-        // The chain below consumes one 64-byte block per prompt per ~0.6 us and stages only one block ahead: pull the whole
+        // The chain below consumes one 64-byte block per prompt per FNV block hash and stages only one block ahead: pull the whole
         // chunk (<= 2 KB per prompt) towards L2 now, so that the staging copies find it there instead of paying a loaded DRAM
         // round trip per block.
         if (prefetch && have) {
@@ -616,7 +616,7 @@ walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
             uint64_t slot = hm & t.req_mask & ~1ull;
             // A local probe fetches the aligned slot PAIR (one 64-byte DRAM access).  On a peer GPU's shard every byte crosses
             // NVLink, and at load <= 0.25 the home slot alone decides ~9 probes out of 10: fetch it first, its neighbour only
-            // if needed (halves the NVLink bytes of a sharded step, profiles/r2_sharded_nvlink.json).
+            // if needed (halves the NVLink bytes of a sharded step).
             const bool remote = base != t.req && !t.peer_pair;
             for (;;) {
                 uint4 A0, B0, A1, B1;

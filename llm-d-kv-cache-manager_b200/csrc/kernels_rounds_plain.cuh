@@ -13,7 +13,7 @@
 //
 // The batch is radix-sorted by a fingerprint of the first block so that prompts sharing a prefix sit in neighbouring
 // lanes and their probes coalesce.  kernels_rounds.cuh goes further for LARGE batches (it hashes and walks every
-// distinct prefix once); its per-round bookkeeping costs a fixed ~0.2 ms per round, which this path does not pay.
+// distinct prefix once); its per-round bookkeeping is a fixed cost per round, which this path does not pay.
 // Results are bit-identical on every path (tests run all of them against the oracle).
 #pragma once
 #include <cuda_runtime.h>
@@ -53,8 +53,8 @@ struct RoundBufs {
     int spec;
 };
 
-constexpr int kHashChunk = 1;            // blocks staged per copy step (2 = 128-byte accesses was measured: fewer, longer DRAM
-                                         // accesses but only 24 resident warps/SM -> 6 % slower; the kernel is pipe bound)
+constexpr int kHashChunk = 1;            // blocks staged per copy step (2 = 128-byte accesses: fewer, longer DRAM accesses
+                                         // but only 24 resident warps/SM, and the kernel is pipe bound)
 template <int BS> struct HashSmem {
     static constexpr int kRow = kHashChunk * BS * 4 + 16;   // 144 B: the four LDS.128 of a block stay conflict free
     unsigned char tok[kHashThreads / 32][2][32 * kRow];
@@ -64,7 +64,7 @@ template <int BS> struct HashSmem {
 // PM (prompt-major keys): key of block j of list slot i at keys[i * 32 + j] -- what the warp-per-prompt kernel P reads in one
 // coalesced 256-byte load; block-major (keys[j * n_prompts + i]) is what the lane-per-prompt kernel P wants.
 // NS: token blocks staged per prompt (NS - 1 copies in flight ahead of the chain).  With 2 a launch lasts 32 x max(FNV of a block,
-// one loaded DRAM round trip) -- fine when the list fills the machine, the floor of the round (~46 us) when it does not: the
+// one loaded DRAM round trip) -- fine when the list fills the machine, the floor of the round when it does not: the
 // warp-per-prompt configuration stages 3 and runs 128-thread CTAs (55 KB each, four per SM).
 template <int BS, bool PM, int NS>
 __global__ void __launch_bounds__(kHashThreads, 4)
@@ -157,8 +157,8 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
 
 // ---- kernel P ---------------------------------------------------------------------------------
 // Kernel P, lane-per-prompt.  (Two warp-per-prompt versions came first -- 32 lanes probing a prompt's 32 keys at
-// once, then the same software-pipelined.  Both cost ~700 issue slots per prompt-round because the walk itself
-// runs on <= 10 lanes while the other 22 idle, and stayed at ~25 % issue utilisation: profiles/r1d_*.)  Here a
+// once, then the same software-pipelined.  Both spent most issue slots idle because the walk itself
+// runs on <= 10 lanes while the other 22 wait.)  Here a
 // warp walks 32 prompts in lockstep, one block per iteration: every instruction serves 32 prompts, the 32 lanes'
 // probes are 32 independent 64-byte reads, and the slot pair for block j+1 is in flight while block j is scored.
 struct WalkSmem {
@@ -205,8 +205,8 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         const int nb_max = __reduce_max_sync(0xffffffffu, nb);
         bool done = !have || nb == 0;                          // walk ended (miss / no live pod); scores are final
         // slot pair of block 0
-        // (An L2 prefetch running 8 blocks ahead of the walk was tried and made this kernel 2x slower -- DRAM reads
-        //  grew 50 % and issue utilisation fell to 11 %; profiles/r1d_*.  The SM's outstanding-miss capacity, not the
+        // (An L2 prefetch running 8 blocks ahead of the walk is a poor fit: it adds DRAM reads and
+        //  lowers issue utilisation.  The SM's outstanding-miss capacity, not the
         //  DRAM latency of a single chain, is what bounds it; the batch is sorted by prefix instead so that lanes of
         //  a warp ask for the same slots.)
         uint64_t key = 0, slot = 0;
@@ -340,8 +340,8 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
 
 // ---- kernel P, warp per prompt -----------------------------------------------------------------
 // For batches of a few ten thousand prompts the lane-per-prompt kernel above is a latency chain: a warp walks its 32 prompts
-// through 32 dependent probe -> score iterations (~2 us each) while most of the machine idles (scripts/timeline.py: 64 us per
-// launch at 32 Ki prompts, DRAM and issue slots both under 15 % busy).  Here a warp takes ONE prompt: the 32 lanes probe the
+// through 32 dependent probe -> score iterations while most of the machine idles (scripts/timeline.py shows DRAM and issue
+// slots mostly idle in such launches).  Here a warp takes ONE prompt: the 32 lanes probe the
 // round's 32 keys at once (one memory round trip for the whole chunk), a ballot finds the first miss, and the blocks before it
 // are scored in order with lane q owning pod q (<= 10 pods); runs of blocks whose slot holds the same pods and tiers are runs of
 // in-order additions of the same addend.  ~700 issue slots per prompt-round instead of ~1/32 of a lockstep warp's: worth it

@@ -1,4 +1,4 @@
-// kernels_score.cuh -- the fused Score() kernel for sm_100a.
+// kernels_score.cuh -- the fused Score() kernel for sm_90a.
 //
 // Replaces steps 2-4 of kvcache.Indexer.GetPodScores (pkg/kvcache/indexer.go:141-163):
 //   TokensToKVBlockKeys  (kvblock/token_processor.go:141-162)   -> chain hash in registers
@@ -14,8 +14,8 @@
 //   * token staging global->shared is COOPERATIVE: the per-lane source pointers are exchanged with
 //     shuffles and each cp.async (LDGSTS, 16 B, L2-only) instruction moves 8 prompts x 64 B, so a
 //     16-token block per lane costs 4 copy instructions per warp; double buffered one block ahead.
-//     (The first version used one cp.async.bulk per lane; ncu showed it lowering to a serial
-//     ELECT/R2UR/UBLKCP waterfall, 9 instructions per lane -- profiles/r1a_*.)  Each lane's row is
+//     (The first version used one cp.async.bulk per lane; the profile showed it lowering to a serial
+//     ELECT/R2UR/UBLKCP waterfall, 9 instructions per lane.)  Each lane's row is
 //     padded to 80 B so the four LDS.128 of the hash loop are bank-conflict free;
 //   * the hash itself is branch-free (Fnv::token): 33 issue slots per token for every lane;
 //   * the probe for block b (home slot pair = one aligned 64-byte segment, 4 x LDG.128) is issued as
@@ -59,7 +59,7 @@ __device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src) {
 }
 // L2 eviction policy for data that is read or written exactly once per step (the token stream, the dense result rows):
 // evict_first keeps it from flushing what the latency-bound kernels of a round hand to each other (lists, walk states, keys)
-// and the index slots out of the 126 MB L2.
+// and the index slots out of the 50 MB L2.
 #ifndef KVIDX_L2_STREAM
 #define KVIDX_L2_STREAM 1
 #endif
@@ -92,7 +92,7 @@ __device__ __forceinline__ uint4 ld_nc_v4(const void* p) {
     return r;
 }
 
-// ---- TMA (1-D bulk copy) + mbarrier: the sm_90+/sm_100 way to move a contiguous run of bytes into shared memory ----
+// ---- TMA (1-D bulk copy) + mbarrier: the sm_90 way to move a contiguous run of bytes into shared memory ----
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(count) : "memory");
 }

@@ -1,4 +1,4 @@
-// kvidx.cu -- C ABI (include/kvidx.h) over the sm_100a kernels.  No torch types, no CPU fallback.
+// kvidx.cu -- C ABI (include/kvidx.h) over the sm_90a kernels.  No torch types, no CPU fallback.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -114,7 +114,7 @@ struct kvidx {
     kvidx_config_t cfg{};
     TableView tv{};
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     // Read path (Score / Lookup / hash) and write path (Add / Evict / events) run on their own streams and behind their own
     // mutexes: a Score() call and an event batch overlap on the device (table.cuh: readers never wait for writers).
     cudaStream_t own_stream = nullptr, stream = nullptr, copy_stream = nullptr, d2h_stream = nullptr, own_wstream = nullptr;
@@ -142,15 +142,17 @@ struct kvidx {
     int score_path = 0;            // 0 = by batch size, 1 = always the fused persistent kernel, 2 / 3 = always the plain / class round pipeline,
                                    // 4 = always the warp-per-prompt cooperative kernel
     int64_t coop_max = 2048;       // batches up to this many prompts use the warp-per-prompt cooperative kernel
-    int rounds_spec = 0;           // per-prompt rounds: run hash(t+1) beside walk(t) for small batches (measured at 65 536 prompts: 3 % slower, so off)
+    int rounds_spec = 0;           // per-prompt rounds: run hash(t+1) beside walk(t) for small batches (off by default)
     int64_t rounds_spec_max = 131072;
     cudaEvent_t ev_spec_h[2][2] = {}, ev_spec_p[2][2] = {};
     int64_t zerocopy_max = 32;     // host-buffer calls up to this many prompts skip the copy engine (tokens read from pinned host memory)
-    int group_tma = 0;             // class pipeline: token chunks by TMA bulk copy instead of cp.async (measured: 2 % slower per step)
+    int group_tma = 0;             // class pipeline: token chunks by TMA bulk copy instead of cp.async (off by default)
     struct SubmitQueue* queue = nullptr;   // coalesces concurrent host-buffer Score() callers (submit.cuh)
-    int64_t rounds_min = 4096;     // batches at least this large use the round pipeline (measured: warp-per-prompt rounds beat the fused
-                                   // kernel from 4096 prompts, profiles/r2_medium_batch_ab.txt)
-    int64_t classes_min = 393216;  // ... and at least this large, the prefix-class round pipeline
+    // Batch-size thresholds, from a sweep of the forced paths on an H100 SXM (10 M-block index, bench.py's query mix): the
+    // warp-per-prompt rounds beat the cooperative kernel from 4096 prompts (tie at 2048) and the fused kernel at every size
+    // from 2048 up; the class pipeline beats them from 131 072 prompts.
+    int64_t rounds_min = 2048;     // batches at least this large (and above coop_max) use the round pipeline
+    int64_t classes_min = 131072;  // ... and at least this large, the prefix-class round pipeline
     double classes_min_sharing = 0.85;   // ... if at least this fraction of the batch follows a representative in round 0
     DevBuf r_act0, r_act1, r_cnt, r_hstate, r_keys, r_pst, r_nbr, r_fp, r_sort, r_role, r_hl, r_map, r_src, r_fate, r_anch, r_snap, r_rec;
     int64_t host_chunk_tokens = 32ll << 20;   // tokens per H2D chunk of the host-buffer pipeline
@@ -167,8 +169,8 @@ struct kvidx {
     // G sharing the bandwidth, then all in the short kernels with DRAM idle -- scripts/timeline.py)
     int group_serial = 2, group_serial_grid = 2;
     int rounds_lane_stages = 2; int64_t rounds_lane_stages_max = 1 << 30;      // lane-per-prompt rounds: stages of kernel H (experiment knob)
-    int rounds_warp = 1, rounds_warp_stages = 3; int64_t rounds_warp_max = 57344;       // per-prompt rounds: kernel P warp per prompt up to this many prompts
-                                   // (measured crossover with the lane-per-prompt kernel P between 49152 and 65536)
+    int rounds_warp = 1, rounds_warp_stages = 3; int64_t rounds_warp_max = 131072;      // per-prompt rounds: kernel P warp per prompt up to this many prompts
+                                   // (faster than the lane-per-prompt kernel P at every size swept up to 131 072)
     int group_ctas = 0;            // > 0: CTAs of one part's kernel G (all parts' G CTAs resident at once: nothing queues behind them)
     int hash_prefetch = 0;         // kernel H pulls its chunks towards L2 before the chain starts (1; 2: evict_last)
     int small_cta = 256;           // threads per CTA of the short kernels (G2, H, P, R): small CTAs fit into what kernel G's CTAs leave of an SM
@@ -400,7 +402,7 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
         x->launches += 5;     // cub: histogram + 4 onesweep passes (the top 32 fingerprint bits order the groups well enough)
     }
     // Is the batch worth it?  The class pipeline pays a token pass and five kernels per round; with few prompts per distinct
-    // prefix (measured crossover: ~6 prompts per cached document) the per-prompt rounds are faster.  The sorted first-block
+    // prefix the per-prompt rounds are faster.  The sorted first-block
     // fingerprints tell before anything is spent: count the distinct ones, and hand the batch over if more than 15 % of the
     // prompts start differently from their neighbour.  (The device-resident entry point waits for the block count here anyway.)
     const bool adaptive = x->score_path == 0 && x->rounds_dedup && x->sort_prefix && x->classes_min_sharing > 0.0;
@@ -730,8 +732,8 @@ int score_host_locked(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int
     const uint32_t P = x->tv.max_pods, FW = x->tv.filter_words;
     const bool sparse = sp_cnt != nullptr;
     const size_t out_row = sparse ? (size_t)kMaxEnt * (sizeof(double) + sizeof(uint16_t)) + 2 : (size_t)P * sizeof(double) + 1;
-    // chunk = up to 32 Mi tokens (128 MiB): the H2D copy of a chunk (2.3 ms at 55 GB/s) must outlast its kernel
-    // (~1 ms for 8192 x 4K-token prompts) for the pipeline to be PCIe bound; 8 Mi-token chunks were kernel bound.
+    // chunk = up to 32 Mi tokens (128 MiB): the H2D copy of a chunk must outlast its kernel for the
+    // pipeline to be PCIe bound, and smaller chunks leave the fixed cost of a launch exposed.
     const int64_t kMaxTokChunk = x->host_chunk_tokens;
     const int64_t kMaxRowsChunk = std::max<int64_t>(1, (128ll << 20) / (int64_t)out_row);
     const bool tok_pinned = tok && is_device_accessible_host(tok);
@@ -1054,7 +1056,7 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     cudaDeviceProp prop{};
     CK(cudaGetDeviceProperties(&prop, c.device));
     x->sm_count = prop.multiProcessorCount;
-    if (prop.major < 10) return fail(KVIDX_ECUDA, "device sm_%d%d is not Blackwell; libkvidx is built for sm_100a only", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail(KVIDX_ECUDA, "device sm_%d%d is not Hopper; libkvidx is built for sm_90a only", prop.major, prop.minor);
     CK(cudaStreamCreateWithFlags(&x->own_stream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&x->own_wstream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&x->copy_stream, cudaStreamNonBlocking));

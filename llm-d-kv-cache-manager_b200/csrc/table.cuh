@@ -3,28 +3,33 @@
 //   request table : Key{model, chunk hash} -> pod-entry set   (lru.Cache[Key,*PodCache])
 //   engine  table : Key{model, engine hash} -> request hash    (lru.Cache[Key,Key])
 //
-// A slot of either table is exactly one naturally aligned 32-byte DRAM / L2 sector and is always read and
-// published as ONE 256-bit access (sm_100: LDG.E.256 / STG.E.256), so a probe that hits its home slot costs one
-// sector and a reader sees a slot image entirely before or entirely after any update:
+// A slot of either table is exactly one naturally aligned 32-byte DRAM / L2 sector, so a probe that hits its home
+// slot costs one sector.  Hopper's widest load / store is 16 bytes, so a slot moves as two halves
+// (a = bytes 0..15, b = bytes 16..31), each a single 128-bit access:
 //   request slot   bytes  0..7   tag      chunk hash
 //                  bytes  8..27  ent[10]  packed (pod<<4|tier), physically ordered oldest -> newest, which is
 //                                         the order golang-lru's Keys() returns (in_memory.go:128) and makes the
 //                                         per-key pod LRU (in_memory.go:199-203, cap = PodCacheSize) a shift.
-//                  bytes 28..31  meta     [1:0] state  [2] writer bit  [7:4] count  [31:16] model id
+//                  bytes 28..31  meta     [1:0] state  [2] writer bit  [7:4] count  [15:8] publish count  [31:16] model id
 //   engine slot    ehash, rhash, meta, pad, recency stamp
 // Linear probing, power-of-two slot count >= 4 x capacity (load factor <= 0.25).  Deletion leaves a tombstone; the
 // owner compacts when tombstones pile up (rebuild / kvidx_shard_compact in kvidx.cu).
 //
 // Concurrency (Index is called concurrently from gRPC goroutines and event workers, index.go:118):
-//   * READERS (Score / Lookup / GetRequestKey kernels) never wait and never write: one 256-bit load per slot, the
-//     writer bit is ignored (a slot with the bit set still holds its complete previous image), a BUSY slot (claimed
-//     by an insert that has not published yet) is stepped over like a slot of another key.  A reader therefore
-//     linearises before or after each individual Add / Evict of a key -- the guarantee the reference's per-key
-//     mutex gives (in_memory.go:199-203).
+//   * READERS (Score / Lookup / GetRequestKey kernels) never write.  The meta word is a sequence lock: a reader
+//     loads half b (acquire), then half a (acquire), then the meta word again, and keeps the image only if the
+//     meta word is unchanged and the writer bit clear; every publish bumps the publish count, so an unchanged meta
+//     word means no writer touched the slot in between (the 8-bit count would alias only after 256 publishes of
+//     one slot inside one three-load read, each a compare-and-swap round trip).  A reader waits only while a writer owns the very slot it
+//     reads.  A BUSY slot (claimed by an insert that has not published yet) is stepped over like a slot of another
+//     key.  A reader therefore linearises before or after each individual Add / Evict of a key -- the guarantee
+//     the reference's per-key mutex gives (in_memory.go:199-203).
 //   * WRITERS own a slot between a successful compare-and-swap on its meta word (FULL -> FULL|W, EMPTY -> BUSY) and
-//     ONE 256-bit store that publishes the complete new image with the bit cleared.  Ownership is per slot, never
-//     nested, held for a handful of instructions; there is no table-wide or per-pod lock and no host mutex between
-//     the read and the write path.  Slots may live in a peer GPU's shard: atomics and publishes are system scope.
+//     the publish of the complete new image: half a, then half b (which carries the meta word) with the bit cleared
+//     and the publish count bumped, both release stores.  A writer looking for its key's slot loads half b (acquire)
+//     before half a, so a FULL slot it sees always shows that key's tag.  Ownership is per slot, never nested, held for a handful of
+//     instructions; there is no table-wide or per-pod lock and no host mutex between the read and the write path.
+//     Slots may live in a peer GPU's shard: atomics and publishes are system scope.
 //   * Every probe loop is bounded by the slot count: a full shard makes an insert fail (Counters::nospc) instead of
 //     spinning.
 #pragma once
@@ -35,6 +40,7 @@ namespace kvx {
 
 constexpr uint32_t kStateEmpty = 0, kStateFull = 1, kStateTomb = 2, kStateBusy = 3;
 constexpr uint32_t kStateMask = 3u, kLockBit = 4u;
+constexpr uint32_t kPubShift = 8, kPubMask = 0xff00u;
 constexpr int kMaxEnt = 10;
 
 struct __align__(32) ReqSlot {
@@ -109,21 +115,68 @@ __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) { return 
 
 struct SlotWords { uint4 a, b; };   // a = {tag.lo, tag.hi, ent0|1, ent2|3}; b = {ent4|5, ent6|7, ent8|9, meta}
 
-// One 32-byte slot as a single 256-bit load (LDG.E.256).  Not the read-only (.nc) path: writers may publish while a
-// reader kernel runs, and a peer GPU's shard is NVLink-mapped memory.  `peer` is kept for call-site readability.
-__device__ __forceinline__ void ld_slot(const void* s, bool /*peer*/, uint4& a, uint4& b) {
-    asm volatile("ld.global.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(s) : "memory");
+__device__ __forceinline__ void spin_pause() { __nanosleep(40); }
+
+// 16-byte halves.  Not the read-only (.nc) path: writers may publish while a reader kernel runs, and a peer GPU's
+// shard is NVLink-mapped memory, so a sharded handle (`sys`) orders its accesses at system scope.
+__device__ __forceinline__ uint4 ld_half_acquire(const void* p, bool sys) {
+    uint4 r;
+    if (sys) asm volatile("ld.acquire.sys.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
+    else     asm volatile("ld.acquire.gpu.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
+    return r;
 }
-// ... the same with system-scope coherence (bypasses L1): what a writer reads under ownership and what a spin re-reads
+__device__ __forceinline__ uint32_t ld_word_relaxed(const void* p, bool sys) {
+    uint32_t r;
+    if (sys) asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(r) : "l"(p) : "memory");
+    else     asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(r) : "l"(p) : "memory");
+    return r;
+}
+__device__ __forceinline__ uint4 ld_half_fresh(const void* p) {
+    uint4 r;
+    asm volatile("ld.relaxed.sys.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
+    return r;
+}
+__device__ __forceinline__ void st_half_release(void* p, const uint4& v) {
+    asm volatile("st.release.sys.global.v4.u32 [%4], {%0,%1,%2,%3};" :: "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(p) : "memory");
+}
+
+// A consistent image of one published slot (the sequence-lock read described at the top).  kMeta is the index of the
+// meta word in half b: 3 for a request slot, 0 for an engine slot.  A slot that is not FULL needs no image beyond its
+// meta word; half a is then returned as zeros.
+template <int kMeta>
+__device__ __forceinline__ void ld_slot_t(const void* s, bool sys, uint4& a, uint4& b) {
+    const char* p = static_cast<const char*>(s);
+    for (;;) {
+        b = ld_half_acquire(p + 16, sys);
+        const uint32_t m = kMeta == 3 ? b.w : b.x;
+        if (meta_state(m) != kStateFull) { a = make_uint4(0u, 0u, 0u, 0u); return; }
+        if (m & kLockBit) { spin_pause(); continue; }
+        a = ld_half_acquire(p, sys);
+        if (ld_word_relaxed(p + 16 + 4 * kMeta, sys) == m) return;
+    }
+}
+__device__ __forceinline__ void ld_slot(const void* s, bool peer, uint4& a, uint4& b) { ld_slot_t<3>(s, peer, a, b); }
+// What a writer's acquire loop examines: half b (acquire), then half a.  A FULL meta word seen here was published
+// after its tag (release stores, half a first), so the tag read afterwards is that key's; tag, state and model of a
+// FULL slot then never change while it stays FULL.  Entries may still move: the owner re-reads them (ld_slot_fresh).
+__device__ __forceinline__ void ld_slot_probe(const void* s, uint4& a, uint4& b) {
+    b = ld_half_acquire(static_cast<const char*>(s) + 16, true);
+    a = ld_half_fresh(s);
+}
+// Both halves with system-scope coherence (bypasses L1), no consistency check: what a writer reads under ownership.
 __device__ __forceinline__ void ld_slot_fresh(const void* s, uint4& a, uint4& b) {
-    asm volatile("ld.relaxed.sys.global.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(s) : "memory");
+    a = ld_half_fresh(s);
+    b = ld_half_fresh(static_cast<const char*>(s) + 16);
 }
-// publish: the complete image, meta last word, in ONE 256-bit store
+// publish: half a, then half b carrying the meta word.  The first release also orders the owning compare-and-swap
+// before any byte of the new image.
 __device__ __forceinline__ void st_slot(void* s, const uint4& a, const uint4& b) {
-    asm volatile("st.relaxed.sys.global.v8.u32 [%8], {%0,%1,%2,%3,%4,%5,%6,%7};"
-                 :: "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w), "l"(s) : "memory");
+    st_half_release(s, a);
+    st_half_release(static_cast<char*>(s) + 16, b);
+}
+// meta word of a publish: the caller's state / count / model, writer bit clear, publish count of `old` plus one
+__device__ __forceinline__ uint32_t published_meta(uint32_t old, uint32_t new_meta) {
+    return (new_meta & ~(kLockBit | kPubMask)) | ((old + (1u << kPubShift)) & kPubMask);
 }
 __device__ __forceinline__ SlotWords load_slot(const ReqSlot* s, bool peer = false) {
     SlotWords w;
@@ -167,7 +220,7 @@ __device__ __forceinline__ bool eng_find(const TableView& t, uint32_t model, uin
     for (uint64_t step = 0; step <= t.eng_mask; ++step) {
         const EngSlot* s = base + i;
         uint4 a, b;
-        ld_slot(s, t.shard_bits != 0, a, b);
+        ld_slot_t<0>(s, t.shard_bits != 0, a, b);
         const uint32_t st = meta_state(b.x);
         if (st == kStateEmpty) return false;
         if (st == kStateFull && meta_model(b.x) == model && a.x == elo && a.y == ehi) {
@@ -227,8 +280,6 @@ struct EntList {
     }
 };
 
-__device__ __forceinline__ void spin_pause() { __nanosleep(40); }
-
 // Take ownership of the request slot of (model, tag); claim a fresh one if the key is absent (unless must_exist).
 // On success the slot's current image is in (a, b) (for a fresh slot: tag set, no entries) and *created tells which.
 // Returns nullptr if must_exist and the key is absent, or if the shard is full (*full set).
@@ -242,7 +293,7 @@ __device__ __forceinline__ ReqSlot* req_acquire(const TableView& t, uint32_t mod
     if (full) *full = false;
     for (uint64_t step = 0; step <= t.req_mask;) {
         ReqSlot* s = base + i;
-        ld_slot_fresh(s, a, b);
+        ld_slot_probe(s, a, b);
         const uint32_t m = b.w, st = meta_state(m);
         if (st == kStateBusy) { spin_pause(); continue; }              // another insert is publishing here: it may be this key
         if (st == kStateEmpty) {
@@ -267,9 +318,9 @@ __device__ __forceinline__ ReqSlot* req_acquire(const TableView& t, uint32_t mod
     if (full) *full = true;
     return nullptr;
 }
-// publish the image with the given meta (writer bit clear) and give the slot up
+// publish the image with the given meta (writer bit clear) and give the slot up; b.w still holds the owned meta word
 __device__ __forceinline__ void req_publish(ReqSlot* s, uint4& a, uint4& b, uint32_t new_meta) {
-    b.w = new_meta & ~kLockBit;
+    b.w = published_meta(b.w, new_meta);
     st_slot(s, a, b);
 }
 
@@ -284,7 +335,7 @@ __device__ __forceinline__ EngSlot* eng_acquire(const TableView& t, uint32_t mod
     if (full) *full = false;
     for (uint64_t step = 0; step <= t.eng_mask;) {
         EngSlot* s = base + i;
-        ld_slot_fresh(s, a, b);
+        ld_slot_probe(s, a, b);
         const uint32_t m = b.x, st = meta_state(m);
         if (st == kStateBusy) { spin_pause(); continue; }
         if (st == kStateEmpty) {
@@ -307,7 +358,7 @@ __device__ __forceinline__ EngSlot* eng_acquire(const TableView& t, uint32_t mod
     return nullptr;
 }
 __device__ __forceinline__ void eng_publish(EngSlot* s, uint4& a, uint4& b, uint32_t new_meta) {
-    b.x = new_meta & ~kLockBit;
+    b.x = published_meta(b.x, new_meta);
     st_slot(s, a, b);
 }
 

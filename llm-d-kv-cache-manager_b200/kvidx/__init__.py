@@ -1,4 +1,4 @@
-"""kvidx -- Python binding of libkvidx (the B200-resident KV-block locality index).
+"""kvidx -- Python binding of libkvidx (the GPU-resident KV-block locality index).
 
 The product is the CUDA library behind include/kvidx.h; this package only binds it
 (ctypes) and mirrors the reference's host-side interface for the same path.

@@ -1,6 +1,6 @@
 // ubench_coop.cu -- cycles per 16-token block of the warp-cooperative FNV (kernels_coop.cuh) vs the plain serial chain,
 // ONE warp, tokens already in shared memory; checks both against each other.  Build on the GPU box:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o scripts/ubench_coop scripts/ubench_coop.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o scripts/ubench_coop scripts/ubench_coop.cu
 #include <cstdio>
 #include <cstdint>
 #include <vector>

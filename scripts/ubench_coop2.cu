@@ -6,7 +6,7 @@
 //   5 bit planes only, ballot + popcount replaced by a 5-step shuffle XOR scan (what the ballot saves)
 //   6 full, TWO bit planes per ballot round: the upper plane's ballot for both outcomes of the lower plane's prefix parity
 //     (B0, BE) is issued together with the lower plane's ballot, the true upper ballot is B0 ^ (BE & prefix_xor(B_lower))
-// Build on the GPU box:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o scripts/ubench_coop2 scripts/ubench_coop2.cu
+// Build on the GPU box:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o scripts/ubench_coop2 scripts/ubench_coop2.cu
 #include <cstdio>
 #include <cstdint>
 #include <vector>

@@ -1,8 +1,8 @@
 // ubench_fnv.cu -- the lane-serial FNV-64a / CBOR block hash as a DEPENDENCY CHAIN: cycles per 16-token block for one warp per
-// SM sub-partition (what a launch with few chains waits for: the class pipeline's kernel H runs ~1.4 warps per SM and spends
-// 2900 cycles per block, profiles/r1h_hash_round_kernel.json) and at full occupancy (issue bound), for several ways of writing
+// SM sub-partition (what a launch with few chains waits for: the class pipeline's kernel H runs about one warp per SM
+// sub-partition) and at full occupancy (issue bound), for several ways of writing
 // the byte step.  All variants must give the same hash.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/ubench_fnv scripts/ubench_fnv.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/ubench_fnv scripts/ubench_fnv.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -115,7 +115,7 @@ int main() {
     uint32_t ht[1024]; uint64_t s = 1;
     for (int i = 0; i < 1024; ++i) { s = s * 6364136223846793005ull + 1442695040888963407ull; ht[i] = (uint32_t)((s >> 33) % 128256); if (i % 7 == 0) ht[i] %= 200; if (i % 11 == 0) ht[i] %= 20; }
     uint32_t* dt; uint64_t* dout; cudaMalloc(&dt, sizeof ht); cudaMemcpy(dt, ht, sizeof ht, cudaMemcpyHostToDevice);
-    cudaMalloc(&dout, 148 * 2048 * 8);
+    cudaMalloc(&dout, 132 * 2048 * 8);
     cudaDeviceProp p; cudaGetDeviceProperties(&p, 0);
     uint64_t first = 0;
     run<VA>("A  two IMADs on the hi chain, pred. move", dout, dt, p.multiProcessorCount, &first);

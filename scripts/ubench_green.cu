@@ -4,7 +4,7 @@
 // events and cross-stream waits work on streams created with cuGreenCtxStreamCreate, and that the kernels stay on their SMs;
 // (2) times a serial-chain kernel (an FNV-like dependent multiply chain + dependent loads, one warp per CTA, few CTAs) alone,
 // beside a DRAM-streaming kernel on ordinary streams with priorities, and beside it with the two kernels on disjoint partitions.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/ubench_green scripts/ubench_green.cu -lcuda
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/ubench_green scripts/ubench_green.cu -lcuda
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

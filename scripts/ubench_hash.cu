@@ -1,5 +1,5 @@
 // Micro-benchmark: issue rate of the branch-free FNV/CBOR block hash alone (no memory traffic),
-// as a function of resident warps per SM.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/ubench scripts/ubench_hash.cu
+// as a function of resident warps per SM.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/ubench scripts/ubench_hash.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -21,7 +21,7 @@ int main() {
     uint32_t ht[1024]; uint64_t s = 1;
     for (int i = 0; i < 1024; ++i) { s = s * 6364136223846793005ull + 1442695040888963407ull; ht[i] = (uint32_t)((s >> 33) % 128256); }
     uint32_t* dt; uint64_t* dout; cudaMalloc(&dt, sizeof ht); cudaMemcpy(dt, ht, sizeof ht, cudaMemcpyHostToDevice);
-    cudaMalloc(&dout, 148 * 2048 * 8);
+    cudaMalloc(&dout, 132 * 2048 * 8);
     cudaDeviceProp p; cudaGetDeviceProperties(&p, 0);
     const int iters = 2000;
     for (int wps = 4; wps <= 64; wps *= 2) {          // warps per SM
@@ -31,8 +31,9 @@ int main() {
         cudaEventRecord(a); k<<<grid, block>>>(dout, dt, iters); cudaEventRecord(b); cudaEventSynchronize(b);
         float ms; cudaEventElapsedTime(&ms, a, b);
         double blocks = (double)grid.x * block.x * iters;
-        printf("warps/SM %2d: %.3f ms  %.3e block-hashes/s  cycles/block/warp @1.965GHz = %.0f\n", wps, ms, blocks / (ms * 1e-3),
-               ms * 1e-3 * 1.965e9 / iters);
+        int khz = 0; cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);   // max SM clock
+        printf("warps/SM %2d: %.3f ms  %.3e block-hashes/s  cycles/block/warp @%.3fGHz = %.0f\n", wps, ms, blocks / (ms * 1e-3),
+               khz / 1e6, ms * 1e-3 * khz * 1e3 / iters);
     }
     return 0;
 }

@@ -1,9 +1,8 @@
 // ubench_lcp.cu -- how fast can "is this prompt's next chunk (32 blocks = 2 KB) equal to its list neighbour's, and if not, in which
 // block do they part" be answered lane-parallel?  Lane i of a warp owns prompt i of the (sorted) list: it reads its own chunk and
 // its predecessor's 16 bytes at a time (lane i's second load is lane i-1's first: the load unit merges them, nothing is read twice),
-// no shared memory, no shuffles.  Compare with kernel G's warp-serial streaming (one chunk at a time through a shared-memory ring:
-// ~380 warp instructions and ~2900 cycles per chunk, profiles/r2_group_round_cpasync_kernel.json).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/ubench_lcp scripts/ubench_lcp.cu
+// no shared memory, no shuffles.  Compare with kernel G's warp-serial streaming (one chunk at a time through a shared-memory ring).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/ubench_lcp scripts/ubench_lcp.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -45,7 +44,7 @@ int main() {
     const int n = 1 << 18, T = 4096, docs = n / 27;
     uint32_t *tok, *list; uint8_t* fb;
     cudaMalloc(&tok, (size_t)n * T * 4); cudaMalloc(&list, n * 4); cudaMalloc(&fb, n);
-    fill<<<148 * 8, 256>>>(tok, n, T, docs);
+    fill<<<132 * 8, 256>>>(tok, n, T, docs);
     // list: prompts sorted by document (what the prefix sort produces)
     uint32_t* h = new uint32_t[n];
     { uint32_t* key = new uint32_t[n]; for (int p = 0; p < n; ++p) { key[p] = (uint32_t)(p * 2654435761u) % docs; h[p] = p; }

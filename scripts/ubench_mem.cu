@@ -1,4 +1,4 @@
-// Micro-benchmark: random-access read throughput of B200 HBM3e as a function of the contiguous chunk size.
+// Micro-benchmark: random-access read throughput of H100 HBM3 as a function of the contiguous chunk size.
 // Each group of (S/16) lanes reads one S-byte chunk (16 B per lane) at a pseudo-random S-aligned offset of an
 // 8 GB buffer; 8 independent chunks in flight per lane group per iteration.
 #include <cstdio>
@@ -24,7 +24,7 @@ __global__ void k(const uint4* buf, uint64_t nchunks, int iters, uint32_t* out) 
 }
 template <int LPG> void run(const uint4* buf, uint64_t bytes, uint32_t* out) {
     const uint64_t nchunks = bytes / (LPG * 16);
-    const int iters = 64; dim3 grid(148 * 16), block(256);
+    const int iters = 64; dim3 grid(132 * 16), block(256);
     k<LPG><<<grid, block>>>(buf, nchunks, 2, out); cudaDeviceSynchronize();
     cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
     cudaEventRecord(a); k<LPG><<<grid, block>>>(buf, nchunks, iters, out); cudaEventRecord(b); cudaEventSynchronize(b);

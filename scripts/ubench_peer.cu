@@ -1,7 +1,7 @@
-// ubench_peer.cu -- how fast can one B200 read random 32-byte slots out of ANOTHER B200's HBM over NVLink (the access the
+// ubench_peer.cu -- how fast can one H100 read random 32-byte slots out of ANOTHER H100's HBM over NVLink (the access the
 // sharded index's walk makes), next to the same reads from its own HBM?  Independent reads, every lane its own address,
-// 256-bit loads (LDG.E.256) -- no dependence between a thread's loads except through the final checksum.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/ubench_peer scripts/ubench_peer.cu ; scripts/ubench_peer
+// a slot as two 16-byte loads (LDG.E.128, Hopper's widest) -- no dependence between a thread's loads except through the final checksum.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/ubench_peer scripts/ubench_peer.cu ; scripts/ubench_peer
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -18,8 +18,10 @@ __global__ void rd(const uint4* __restrict__ tab, uint64_t mask_slots, int iters
         for (int u = 0; u < PER; ++u) {
             s = mix(s + u);
             const uint4* p = tab + 2 * (s & mask_slots);
-            asm volatile("ld.global.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                         : "=r"(a[u].x), "=r"(a[u].y), "=r"(a[u].z), "=r"(a[u].w), "=r"(b[u].x), "=r"(b[u].y), "=r"(b[u].z), "=r"(b[u].w) : "l"(p) : "memory");
+            asm volatile("ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+                         : "=r"(a[u].x), "=r"(a[u].y), "=r"(a[u].z), "=r"(a[u].w) : "l"(p) : "memory");
+            asm volatile("ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+                         : "=r"(b[u].x), "=r"(b[u].y), "=r"(b[u].z), "=r"(b[u].w) : "l"(p + 1) : "memory");
         }
 #pragma unroll
         for (int u = 0; u < PER; ++u) acc += a[u].x ^ b[u].w;
@@ -43,7 +45,8 @@ int main() {
     for (int which = 0; which < 2; ++which) {
         const uint4* tab = which ? peer : local;
         if (!tab) continue;
-        for (int ctas : {148, 148 * 4, 148 * 16}) {
+        int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+        for (int ctas : {sms, sms * 4, sms * 16}) {
             const int T = 256, iters = 64;
             for (int per : {1, 4}) {
                 for (int rep = 0; rep < 2; ++rep) {
