@@ -190,6 +190,17 @@ int kvidx_apply_events(kvidx_t* idx, const kvidx_event_t* ev, int64_t n_events,
                        const uint64_t* hashes, int64_t n_hashes,
                        const uint32_t* tokens, int64_t n_tokens, int64_t* n_dropped_out);
 
+/* Drop every entry whose pod is in pod_mask (ceil(max_pods/64) words) and whose tier bit is set in tier_mask
+ * (bit t = tier t; 0xFFFF = all tiers); request keys left without entries are removed together with the engine
+ * mappings that point at them.  No reference counterpart: it removes the blocks of a pod that has gone away without
+ * sending BlockRemoved events.  Survivors keep their order, no key's recency changes, and an engine mapping whose
+ * request key was already absent before the call stays (Evict cleans those up, in_memory.go:225-230).  A concurrent
+ * reader sees each key before or after its update, as with a sequence of Evict calls.  Synchronous like every write
+ * call; works in both LRU modes; the tombstones it leaves are compacted by the usual rebuild policy.
+ * All-zero pod_mask or tier_mask == 0 -> KVIDX_EINVAL; sharded handle -> KVIDX_EINVAL.
+ * removed_out (may be NULL): {entries, request keys, engine keys} removed. */
+int kvidx_remove_pods(kvidx_t* idx, const uint64_t* pod_mask, uint32_t tier_mask, uint64_t removed_out[3]);
+
 /* ---- device-resident variants (inputs already in HBM; used by bench `value`, by the
  *      multi-GPU router and by callers that keep token buffers on the device) ------- */
 

@@ -12,6 +12,7 @@
  *   kvhost_pool_add_task     <-> kvevents.Pool.AddTask                pkg/kvcache/kvevents/pool.go:132-144
  *   kvhost_pool_process      <-> worker loop: processEvent + digestEvents       pkg/kvcache/kvevents/pool.go:149-338
  *   kvhost_decode_event_batch<-> processEvent's msgpack decoding      pkg/kvcache/kvevents/pool.go:177-244, events.go:38-96
+ *   kvhost_remove_pod        <-> (no counterpart) drop a departed pod's entries and free its id (kvidx_remove_pods)
  *   kvhost_prefix_store_*    <-> prefixstore.LRUTokenStore            pkg/tokenization/prefixstore/lru_store.go:54-190
  *   kvhost_get_metrics / _text <-> InstrumentedIndex + collectors      pkg/kvcache/kvblock/instrumented_index.go:30-92, metrics/collector.go:28-59
  */
@@ -33,6 +34,10 @@ typedef struct kvhost_config {
     double tier_weights[KVIDX_MAX_TIERS];
     int32_t no_device;               /* 1: host-only instance (interners, queues, decoder) without a kvidx handle       */
     int32_t enable_metrics;          /* IndexConfig.EnableMetrics (index.go:41-43): wrap the index in the instrumented one */
+    int32_t clear_on_all_blocks_cleared; /* 1: an AllBlocksCleared from pod P removes P's entries on the tier of a
+                                            Medium-less event ("gpu", pool.go:258-261) at its position in P's event order
+                                            (vLLM sends it when the GPU prefix cache is reset; offloaded blocks survive).
+                                            0 (default): a no-op, as in the reference (pool.go:332-333). */
 } kvhost_config_t;
 
 void kvhost_config_default(kvhost_config_t* cfg);       /* block 16, seed "", gpu 1.0 / cpu 0.8, concurrency 4 */
@@ -58,7 +63,10 @@ int kvhost_index_lookup(kvhost_t* h, const char* model, const uint64_t* keys, si
 
 /* kvevents.Pool.  add_task copies the payload into queue FNV-32a(pod) % concurrency; process drains every queue in
  * FIFO order, decodes the msgpack EventBatch of each message and applies all resulting events with ONE
- * kvidx_apply_events call.  Returns the number of events applied (or a negative code). */
+ * kvidx_apply_events call.  Returns the number of events applied (or a negative code).
+ * With clear_on_all_blocks_cleared, the drained batch is cut at the AllBlocksCleared markers: segment k holds each pod's
+ * events between its (k-1)-th and k-th marker and is one kvidx_apply_events call, followed by one kvidx_remove_pods for
+ * the pods that cleared at that boundary.  Per-pod order is kept; the order between pods stays unspecified. */
 int kvhost_pool_add_task(kvhost_t* h, const char* pod, const char* model, const void* payload, size_t len);
 int kvhost_pool_queue_index(kvhost_t* h, const char* pod);
 int64_t kvhost_pool_process(kvhost_t* h, int64_t* n_dropped_out);
@@ -67,7 +75,10 @@ int64_t kvhost_pool_process(kvhost_t* h, int64_t* n_dropped_out);
  * the given capacities and returns the number of events, or -KVIDX_ENOSPC-style negatives.  Malformed batches decode
  * to 0 events (poison pill dropped, pool.go:182-187); malformed events are skipped (pool.go:190-239).
  * Hashes rejected by getHashAsUint64 (pool.go:343-367) are left out of a BlockStored's list (pool.go:272-275); a rejected
- * parent hash skips the event (pool.go:283-287).  AllBlocksCleared decodes to nothing (pool.go:332-333). */
+ * parent hash skips the event (pool.go:283-287).  AllBlocksCleared decodes to nothing (pool.go:332-333), or, with
+ * clear_on_all_blocks_cleared, to a KVHOST_EV_ALL_BLOCKS_CLEARED marker record at its position (pod and model set, no
+ * hashes).  Markers are a host-level record: kvidx_apply_events rejects them. */
+#define KVHOST_EV_ALL_BLOCKS_CLEARED 2
 int64_t kvhost_decode_event_batch(kvhost_t* h, const char* pod, const char* model, const void* payload, size_t len,
                                   kvidx_event_t* ev_out, size_t ev_cap, uint64_t* hash_out, size_t hash_cap, size_t* n_hash_out,
                                   uint32_t* tok_out, size_t tok_cap, size_t* n_tok_out);
@@ -112,7 +123,17 @@ int64_t kvhost_prefix_store_find(kvhost_prefix_store_t* s, const char* prompt, s
 int64_t kvhost_prefix_store_len(kvhost_prefix_store_t* s);           /* blocks resident */
 uint64_t kvhost_xxhash64(const void* data, size_t len, uint64_t seed);
 
-/* interning introspection (ids are append-only and never reused) */
+/* Remove a pod that has gone away (no counterpart in the reference, where a dead pod's blocks only age out of the LRU):
+ * 1. drops the pod's messages still waiting in its queue; 2. removes its entries from the device index on the given tiers
+ * (kvidx_remove_pods; n_tiers == 0: all tiers); 3. with all tiers, frees the pod's id once the removal has completed and
+ * every read call that was already running has returned, so the next new pod name takes it (lowest freed id first) and
+ * kvhost_pod_id of the old name gives a new interning.  Serialised with kvhost_pool_process.  On a no_device instance
+ * steps 1 and 3 only.  An unknown pod name is a no-op.  Not counted in kvcache_index_evictions_total, which counts the
+ * reference's Evict calls.  Returns the number of queued messages dropped, or a negative KVIDX_E* code. */
+int kvhost_remove_pod(kvhost_t* h, const char* pod, const char* const* tiers, size_t n_tiers);
+
+/* interning introspection.  Model and tier ids are never reused; a pod id is freed by kvhost_remove_pod (all tiers) and
+ * reused lowest first.  Name pointers returned by the calls above stay valid for the life of the handle. */
 int kvhost_pod_id(kvhost_t* h, const char* pod);
 int kvhost_tier_id(kvhost_t* h, const char* tier);
 int kvhost_model_id(kvhost_t* h, const char* model);

@@ -19,6 +19,7 @@
 #include "../../include/kvidx.h"
 #include "kernels_v1.cuh"
 #include "kernels_write.cuh"
+#include "kernels_remove.cuh"
 #include "kernels_score.cuh"
 #include "kernels_rounds.cuh"
 #include "kernels_rounds_plain.cuh"
@@ -1632,6 +1633,43 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
     if (n_dropped_out) *n_dropped_out = (int64_t)(x->h_cnt->dropped_events - dropped_before);
     if (x->h_cnt->nospc != nospc_before) return fail(KVIDX_ENOSPC, "%llu inserts refused: the owning shard is full", x->h_cnt->nospc - nospc_before);
     return enforce_caps(x);
+}
+
+int kvidx_remove_pods(kvidx_t* x, const uint64_t* pod_mask, uint32_t tier_mask, uint64_t removed_out[3]) {
+    if (removed_out) removed_out[0] = removed_out[1] = removed_out[2] = 0;
+    if (!x || !pod_mask) return fail(KVIDX_EINVAL, "bad arguments");
+    // an engine mapping lives with its engine hash's owner and its request key with another rank: cleaning it up on a
+    // sharded index would need the removal bitmaps of every rank
+    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_remove_pods is not supported on a sharded index");
+    if ((tier_mask & 0xffffu) == 0) return fail(KVIDX_EINVAL, "empty tier mask");
+    const uint32_t FW = x->tv.filter_words;
+    uint64_t any = 0;
+    for (uint32_t w = 0; w < FW; ++w) any |= pod_mask[w];
+    if (!any) return fail(KVIDX_EINVAL, "empty pod mask");
+    std::lock_guard<std::mutex> g(x->mu_w);
+    CK(cudaSetDevice(x->device));
+    std::shared_lock<std::shared_mutex> tl(x->tables);
+    cudaStream_t st = wstream(x);
+    const uint64_t rs = x->tv.req_mask + 1;
+    // scratch: out[4] | pod mask | removed_slot (rs bits) | removed_home (rs / 2 bits)
+    const size_t mask_off = 32, slot_off = mask_off + (size_t)FW * 8, home_off = slot_off + rs / 8, total = home_off + rs / 16;
+    CK(x->d_misc.need(total));
+    CK(x->h_misc.need(32));
+    uint8_t* d = x->d_misc.as<uint8_t>();
+    CK(cudaMemsetAsync(d, 0, total, st));
+    CK(cudaMemcpyAsync(d + mask_off, pod_mask, (size_t)FW * 8, cudaMemcpyHostToDevice, st));
+    RemoveArgs ra{reinterpret_cast<const uint64_t*>(d + mask_off), tier_mask & 0xffffu, reinterpret_cast<uint32_t*>(d + slot_off),
+                  reinterpret_cast<uint32_t*>(d + home_off), reinterpret_cast<unsigned long long*>(d)};
+    const unsigned ctas = (unsigned)std::min<uint64_t>(rs / kRemoveThreads, (uint64_t)x->sm_count * 8);
+    remove_req_kernel<<<ctas, kRemoveThreads, 0, st>>>(x->tv, ra);
+    remove_eng_kernel<<<ctas, kRemoveThreads, 0, st>>>(x->tv, ra);
+    x->launches += 2;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(x->h_misc.p, d, 24, cudaMemcpyDeviceToHost, st));
+    int rc = refresh_counters(x);                      // synchronises the write stream: the removal has taken effect
+    if (rc) return rc;
+    if (removed_out) memcpy(removed_out, x->h_misc.p, 24);
+    return 0;
 }
 
 int kvidx_shard_export(kvidx_t* x, void* out) {

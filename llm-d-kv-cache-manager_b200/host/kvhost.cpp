@@ -8,8 +8,11 @@
 #include <deque>
 #include <list>
 #include <mutex>
+#include <set>
+#include <shared_mutex>
 #include <string>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/kvidx_host.h"
@@ -19,18 +22,28 @@ namespace {
 thread_local std::string g_herr;
 int hfail(int code, const std::string& m) { g_herr = m; return code; }
 
+// name <-> id.  A released id is handed to the next new name, lowest first.  Names are kept for the life of the handle
+// (node-based set: element addresses are stable), so a name pointer returned to a caller never dangles, even after its id
+// has been reused.
 struct Interner {
     std::unordered_map<std::string, uint32_t> ids;
-    std::deque<std::string> names;                   // deque: element addresses are stable
+    std::unordered_set<std::string> store;
+    std::vector<const std::string*> names;           // id -> name; nullptr: released
+    std::set<uint32_t> free_ids;
     int id(const std::string& s, uint32_t limit) {
         auto it = ids.find(s);
         if (it != ids.end()) return (int)it->second;
-        if (names.size() >= limit) return -1;
-        names.push_back(s);
-        ids.emplace(s, (uint32_t)names.size() - 1);
-        return (int)names.size() - 1;
+        uint32_t i;
+        if (!free_ids.empty() && *free_ids.begin() < limit) { i = *free_ids.begin(); free_ids.erase(free_ids.begin()); }
+        else if (names.size() < limit) { i = (uint32_t)names.size(); names.push_back(nullptr); }
+        else return -1;
+        names[i] = &*store.insert(s).first;
+        ids.emplace(s, i);
+        return (int)i;
     }
     int find(const std::string& s) const { auto it = ids.find(s); return it == ids.end() ? -1 : (int)it->second; }
+    const char* name(uint32_t i) const { return names[i]->c_str(); }
+    void release(uint32_t i) { ids.erase(*names[i]); names[i] = nullptr; free_ids.insert(i); }
 };
 
 // ---- minimal msgpack reader (vmihailenco/msgpack v5 type rules are applied by the callers) -------------------
@@ -127,6 +140,12 @@ struct kvhost {
     kvhost_config_t cfg{};
     Interner models, pods, tiers;
     std::mutex mu;
+    // Pod-id lifetime (kvhost_remove_pod frees ids).  read_mu: held shared by the read calls from their device call through
+    // the id -> name mapping, exclusively while an id is freed, so that a reused id never puts a new pod's name on an old
+    // pod's entries.  write_mu: held shared by the calls that intern a pod and then write its entries (pool_process from
+    // the drain through the apply, index_add / index_evict), exclusively by remove_pod, so that no entry of a pod can be
+    // written after its removal with the id it had.  Order: write_mu, read_mu, mu.
+    std::shared_mutex read_mu, write_mu;
     std::vector<std::deque<Msg>> queues;
     uint32_t filter_words = 4;
     uint32_t pod_cap = 256;                          // == index.max_pods: ids of pods that own entries
@@ -218,7 +237,13 @@ void decode_event(kvhost* h, uint32_t pod, uint32_t model, const uint8_t* p, con
         ev.n_hashes = (uint32_t)(hashes.size() - h0);
         evs.push_back(ev);
     }
-    // "AllBlocksCleared": no-op (pool.go:332-333); unknown tags: skipped (pool.go:229-231)
+    else if (t == "AllBlocksCleared" && h->cfg.clear_on_all_blocks_cleared) {     // host-level marker, never applied as is
+        kvidx_event_t ev{};
+        ev.op = KVHOST_EV_ALL_BLOCKS_CLEARED; ev.model = model; ev.podtier = KVIDX_PODTIER(pod, 0);
+        ev.hash_off = hashes.size(); ev.tok_off = toks.size();
+        evs.push_back(ev);
+    }
+    // "AllBlocksCleared" otherwise: no-op (pool.go:332-333); unknown tags: skipped (pool.go:229-231)
 }
 
 // EventBatch = [ts, events[], data_parallel_rank?] (events.go:38-43).  Any decode error drops the whole message.
@@ -358,6 +383,7 @@ static bool build_filter(kvhost* h, const char* const* pods, size_t n_pods, std:
 int kvhost_get_pod_scores(kvhost_t* h, const uint32_t* tokens, size_t n_tokens, const char* model, const char* const* pods, size_t n_pods,
                           const char** pod_out, double* score_out) {
     if (int rc = need_dev(h)) return rc;
+    std::shared_lock<std::shared_mutex> rl(h->read_mu);
     std::vector<uint64_t> mask;
     bool filtered; int mid;
     { std::lock_guard<std::mutex> g(h->mu); filtered = build_filter(h, pods, n_pods, mask); mid = h->models.id(model, 65536); }
@@ -385,7 +411,7 @@ int kvhost_get_pod_scores(kvhost_t* h, const uint32_t* tokens, size_t n_tokens, 
         observe_lookup(h, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), r2 == 0, pt.data(), kc.data(), nk);
     }
     std::lock_guard<std::mutex> g(h->mu);
-    for (int i = 0; i < cnt; ++i) { pod_out[i] = h->pods.names[ids[i]].c_str(); score_out[i] = sc[i]; }
+    for (int i = 0; i < cnt; ++i) { pod_out[i] = h->pods.name(ids[i]); score_out[i] = sc[i]; }
     return cnt;
 }
 
@@ -405,6 +431,7 @@ int kvhost_index_add(kvhost_t* h, const char* model, const uint64_t* engine, siz
     if (h->cfg.enable_metrics) { std::lock_guard<std::mutex> g(h->mu); h->met.admissions_total += n_request; }   // whatever Add returns
     if (n_engine == 0 || n_request == 0 || n_entries == 0) return hfail(KVIDX_EINVAL, "no keys or entries provided for adding to index");
     if (n_engine != n_request) return hfail(KVIDX_EINVAL, "mismatch between engine keys and request keys length");
+    std::shared_lock<std::shared_mutex> wl(h->write_mu);
     std::vector<kvidx_podtier_t> pt; int mid;
     { std::lock_guard<std::mutex> g(h->mu); if (int rc = entries_of(h, pods, tiers, n_entries, pt)) return rc; mid = h->models.id(model, 65536); }
     const int rc = kvidx_add(h->ix, (uint32_t)mid, engine, request, (int64_t)n_engine, pt.data(), (int32_t)pt.size());
@@ -416,6 +443,7 @@ int kvhost_index_evict(kvhost_t* h, const char* model, uint64_t engine, const ch
     if (int rc = need_dev(h)) return rc;
     if (h->cfg.enable_metrics) { std::lock_guard<std::mutex> g(h->mu); h->met.evictions_total += n_entries; }
     if (n_entries == 0) return hfail(KVIDX_EINVAL, "no entries provided for eviction from index");
+    std::shared_lock<std::shared_mutex> wl(h->write_mu);
     std::vector<kvidx_podtier_t> pt; int mid;
     { std::lock_guard<std::mutex> g(h->mu); if (int rc = entries_of(h, pods, tiers, n_entries, pt)) return rc; mid = h->models.id(model, 65536); }
     const int rc = kvidx_evict(h->ix, (uint32_t)mid, engine, pt.data(), (int32_t)pt.size());
@@ -437,6 +465,7 @@ int kvhost_index_lookup(kvhost_t* h, const char* model, const uint64_t* keys, si
     const auto t0 = std::chrono::steady_clock::now();
     auto secs = [&] { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); };
     if (n == 0) { observe_lookup(h, secs(), false, nullptr, nullptr, 0); return hfail(KVIDX_EINVAL, "no requestKeys provided for lookup"); }
+    std::shared_lock<std::shared_mutex> rl(h->read_mu);
     std::vector<uint64_t> mask; bool filtered; int mid;
     { std::lock_guard<std::mutex> g(h->mu); filtered = build_filter(h, pods, n_pods, mask); mid = h->models.id(model, 65536); }
     std::vector<kvidx_podtier_t> pt(n * KVIDX_MAX_PODS_PER_KEY);
@@ -448,8 +477,8 @@ int kvhost_index_lookup(kvhost_t* h, const char* model, const uint64_t* keys, si
     for (size_t i = 0; i < n; ++i)
         for (int j = 0; j < cnt_out[i]; ++j) {
             const kvidx_podtier_t e = pt[i * KVIDX_MAX_PODS_PER_KEY + j];
-            pod_out[i * KVIDX_MAX_PODS_PER_KEY + j] = h->pods.names[KVIDX_PT_POD(e)].c_str();
-            tier_out[i * KVIDX_MAX_PODS_PER_KEY + j] = h->tiers.names[KVIDX_PT_TIER(e)].c_str();
+            pod_out[i * KVIDX_MAX_PODS_PER_KEY + j] = h->pods.name(KVIDX_PT_POD(e));
+            tier_out[i * KVIDX_MAX_PODS_PER_KEY + j] = h->tiers.name(KVIDX_PT_TIER(e));
         }
     return 0;
 }
@@ -465,8 +494,53 @@ int kvhost_pool_add_task(kvhost_t* h, const char* pod, const char* model, const 
     return 0;
 }
 
+// clear_on_all_blocks_cleared: the drained batch cut at the AllBlocksCleared markers.  Segment k takes each pod's events
+// after its k-th marker (and before its (k+1)-th); the pods whose k-th marker closes segment k are removed right after it.
+static int64_t process_segments(kvhost* h, const std::vector<kvidx_event_t>& evs, const std::vector<uint64_t>& hashes,
+                                const std::vector<uint32_t>& toks, int64_t* n_dropped_out) {
+    std::vector<uint32_t> seg(evs.size()), cleared(KVIDX_MAX_PODS, 0);
+    uint32_t n_seg = 1;
+    for (size_t i = 0; i < evs.size(); ++i) {
+        const uint32_t p = KVIDX_PT_POD(evs[i].podtier);
+        seg[i] = cleared[p];
+        if (evs[i].op == KVHOST_EV_ALL_BLOCKS_CLEARED) n_seg = std::max(n_seg, ++cleared[p] + 1);
+    }
+    int gpu;
+    { std::lock_guard<std::mutex> g(h->mu); gpu = h->tiers.id("gpu", KVIDX_MAX_TIERS); }     // the tier of a Medium-less event
+    if (gpu < 0) return hfail(KVIDX_ERANGE, "tier id space exhausted");
+    int64_t applied = 0, dropped = 0;
+    std::vector<kvidx_event_t> part;
+    std::vector<uint64_t> mask(h->filter_words);
+    for (uint32_t k = 0; k < n_seg; ++k) {
+        part.clear();
+        std::fill(mask.begin(), mask.end(), 0ull);
+        bool any = false;
+        for (size_t i = 0; i < evs.size(); ++i) {
+            if (seg[i] != k) continue;
+            if (evs[i].op != KVHOST_EV_ALL_BLOCKS_CLEARED) { part.push_back(evs[i]); continue; }
+            const uint32_t p = KVIDX_PT_POD(evs[i].podtier);
+            mask[p >> 6] |= 1ull << (p & 63);
+            any = true;
+        }
+        if (!part.empty()) {
+            int64_t d = 0;
+            const int rc = kvidx_apply_events(h->ix, part.data(), (int64_t)part.size(), hashes.data(), (int64_t)hashes.size(), toks.data(),
+                                              (int64_t)toks.size(), &d);
+            if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+            applied += (int64_t)part.size(); dropped += d;
+        }
+        if (any) {
+            const int rc = kvidx_remove_pods(h->ix, mask.data(), 1u << gpu, nullptr);
+            if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+        }
+    }
+    if (n_dropped_out) *n_dropped_out = dropped;
+    return applied;
+}
+
 int64_t kvhost_pool_process(kvhost_t* h, int64_t* n_dropped_out) {
     if (int rc = need_dev(h)) return rc;
+    std::shared_lock<std::shared_mutex> wl(h->write_mu);
     std::vector<kvidx_event_t> evs; std::vector<uint64_t> hashes; std::vector<uint32_t> toks;
     {
         std::lock_guard<std::mutex> g(h->mu);
@@ -487,9 +561,49 @@ int64_t kvhost_pool_process(kvhost_t* h, int64_t* n_dropped_out) {
         h->met.admissions_total += adm; h->met.evictions_total += evi;
     }
     if (evs.empty()) return 0;
+    if (h->cfg.clear_on_all_blocks_cleared) return process_segments(h, evs, hashes, toks, n_dropped_out);
     const int rc = kvidx_apply_events(h->ix, evs.data(), (int64_t)evs.size(), hashes.data(), (int64_t)hashes.size(), toks.data(), (int64_t)toks.size(), n_dropped_out);
     if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
     return (int64_t)evs.size();
+}
+
+// Removes the pod's messages still waiting in its queue.  Caller holds mu.
+static int drop_queued(kvhost* h, const char* pod, uint32_t id) {
+    auto& q = h->queues[kvidx_queue_index(pod, strlen(pod), h->cfg.concurrency)];
+    const size_t before = q.size();
+    q.erase(std::remove_if(q.begin(), q.end(), [&](const Msg& m) { return m.pod == id; }), q.end());
+    return (int)(before - q.size());
+}
+
+int kvhost_remove_pod(kvhost_t* h, const char* pod, const char* const* tiers, size_t n_tiers) {
+    if (!h || !pod || (n_tiers && !tiers)) return hfail(KVIDX_EINVAL, "bad arguments");
+    std::unique_lock<std::shared_mutex> wl(h->write_mu);     // no pool_process / index_add of any pod meanwhile
+    int id, dropped;
+    uint32_t tier_mask = n_tiers ? 0u : 0xFFFFu;
+    {
+        std::lock_guard<std::mutex> g(h->mu);
+        for (size_t i = 0; i < n_tiers; ++i) {
+            const int t = h->tiers.id(lower(tiers[i] ? tiers[i] : ""), KVIDX_MAX_TIERS);
+            if (t < 0) return hfail(KVIDX_ERANGE, "tier id space exhausted");
+            tier_mask |= 1u << t;
+        }
+        id = h->pods.find(pod);
+        if (id < 0) return 0;                                    // never seen (or already removed): nothing to do
+        dropped = drop_queued(h, pod, (uint32_t)id);
+    }
+    if (h->ix && (uint32_t)id < h->pod_cap) {                  // ids from pod_cap up (filter-only names) own no entries
+        std::vector<uint64_t> mask(h->filter_words, 0);
+        mask[id >> 6] |= 1ull << (id & 63);
+        const int rc = kvidx_remove_pods(h->ix, mask.data(), tier_mask, nullptr);
+        if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+    }
+    if (n_tiers == 0) {
+        std::unique_lock<std::shared_mutex> rl(h->read_mu);   // waits for the read calls that may still map this id
+        std::lock_guard<std::mutex> g(h->mu);
+        dropped += drop_queued(h, pod, (uint32_t)id);            // queued while the removal ran: they carry the old id
+        h->pods.release((uint32_t)id);
+    }
+    return dropped;
 }
 
 int64_t kvhost_decode_event_batch(kvhost_t* h, const char* pod, const char* model, const void* payload, size_t len, kvidx_event_t* ev_out,

@@ -66,6 +66,7 @@ SYMBOLS = {
     "kvidx_evict": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, _u16p, C.c_int32]),
     "kvidx_get_request_key": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, _u64p]),
     "kvidx_apply_events": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, _u64p, C.c_int64, _u32p, C.c_int64, _i64p]),
+    "kvidx_remove_pods": (C.c_int, [C.c_void_p, _u64p, C.c_uint32, _u64p]),
     "kvidx_set_stream": (C.c_int, [C.c_void_p, C.c_void_p]),
     "kvidx_synchronize": (C.c_int, [C.c_void_p]),
     "kvidx_score_batch_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -305,6 +306,20 @@ class Index:
         rc = self.L.kvidx_apply_events(self.h, events.ctypes.data_as(C.c_void_p), len(events), _p(hashes, _u64p), len(hashes),
                                        _p(tokens, _u32p), len(tokens), C.byref(nd))
         return rc, nd.value
+
+    def remove_pods(self, pod_ids, tier_ids=None) -> dict:
+        """kvidx_remove_pods: drop every entry of these pods (on these tiers; None = all).  No reference counterpart.
+        -> {"entries", "request_keys", "engine_keys"} removed; raises KvidxError on failure."""
+        mask = np.zeros(self.filter_words, np.uint64)
+        for p in pod_ids:
+            p = int(p)
+            if not 0 <= p < self.max_pods:
+                raise KvidxError(ERANGE, "pod id %d outside 0..max_pods-1" % p)
+            mask[p >> 6] |= np.uint64(1) << np.uint64(p & 63)
+        tier_mask = 0xFFFF if tier_ids is None else sum(1 << (int(t) & 15) for t in set(tier_ids))
+        out = np.zeros(3, np.uint64)
+        self._ck(self.L.kvidx_remove_pods(self.h, _p(mask, _u64p), tier_mask, _p(out, _u64p)))
+        return {"entries": int(out[0]), "request_keys": int(out[1]), "engine_keys": int(out[2])}
 
 
 class _Raw:

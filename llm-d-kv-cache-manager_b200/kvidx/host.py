@@ -14,10 +14,12 @@ NO_KEYS = -1000
 
 class HostConfig(C.Structure):
     _fields_ = [("index", Config), ("concurrency", C.c_uint32), ("n_tiers", C.c_uint32), ("tier_names", C.c_char_p * MAX_TIERS),
-                ("tier_weights", C.c_double * MAX_TIERS), ("no_device", C.c_int32), ("enable_metrics", C.c_int32)]
+                ("tier_weights", C.c_double * MAX_TIERS), ("no_device", C.c_int32), ("enable_metrics", C.c_int32),
+                ("clear_on_all_blocks_cleared", C.c_int32)]
 
 
 LATENCY_BUCKETS = 11
+EV_ALL_BLOCKS_CLEARED = 2          # KVHOST_EV_ALL_BLOCKS_CLEARED: decoder marker record (clear_on_all_blocks_cleared)
 
 
 class HostMetrics(C.Structure):
@@ -50,6 +52,7 @@ SYMBOLS = {
     "kvhost_pool_add_task": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t]),
     "kvhost_pool_queue_index": (C.c_int, [C.c_void_p, C.c_char_p]),
     "kvhost_pool_process": (C.c_int64, [C.c_void_p, C.POINTER(C.c_int64)]),
+    "kvhost_remove_pod": (C.c_int, [C.c_void_p, C.c_char_p, _cpp, C.c_size_t]),
     "kvhost_decode_event_batch": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_size_t,
                                               C.POINTER(C.c_size_t), _u32p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "kvhost_pod_id": (C.c_int, [C.c_void_p, C.c_char_p]),
@@ -81,7 +84,7 @@ class HostIndexer:
     """kvcache.Indexer + kvblock.Index + kvevents.Pool with strings (pods, tiers, models are names)."""
 
     def __init__(self, block_size=16, hash_seed="", capacity=1 << 20, pods_per_key=10, tiers=(("gpu", 1.0), ("cpu", 0.8)), max_pods=256,
-                 concurrency=4, device=0, no_device=False, lru_exact=0, enable_metrics=False):
+                 concurrency=4, device=0, no_device=False, lru_exact=0, enable_metrics=False, clear_on_all_blocks_cleared=False):
         self.L = _lib()
         cfg = HostConfig()
         self.L.kvhost_config_default(C.byref(cfg))
@@ -89,6 +92,7 @@ class HostIndexer:
         cfg.index.max_pods, cfg.index.device, cfg.index.lru_exact = max_pods, device, lru_exact
         cfg.concurrency, cfg.n_tiers, cfg.no_device = concurrency, len(tiers), 1 if no_device else 0
         cfg.enable_metrics = 1 if enable_metrics else 0
+        cfg.clear_on_all_blocks_cleared = 1 if clear_on_all_blocks_cleared else 0
         self._tier_names = [t[0].encode() for t in tiers]
         for i, (n, w) in enumerate(tiers):
             cfg.tier_names[i] = self._tier_names[i]
@@ -172,6 +176,14 @@ class HostIndexer:
         nd = C.c_int64(0)
         n = self.L.kvhost_pool_process(self.h, C.byref(nd))
         return n, nd.value
+
+    def remove_pod(self, name, tiers=()):
+        """kvhost_remove_pod: drop the pod's queued messages and its entries on `tiers` (empty: all tiers, which also frees
+        its id for reuse).  No reference counterpart.  -> number of queued messages dropped."""
+        n = self.L.kvhost_remove_pod(self.h, name.encode(), _strs(list(tiers)), len(tiers))
+        if n < 0:
+            raise _native.KvidxError(n, self.err())
+        return n
 
     def decode(self, pod, model, payload: bytes, cap=4096):
         ev = np.zeros(cap, EVENT_DTYPE); hs = np.zeros(cap * 64, np.uint64); tk = np.zeros(cap * 1024, np.uint32)
