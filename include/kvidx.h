@@ -201,6 +201,50 @@ int kvidx_apply_events(kvidx_t* idx, const kvidx_event_t* ev, int64_t n_events,
  * removed_out (may be NULL): {entries, request keys, engine keys} removed. */
 int kvidx_remove_pods(kvidx_t* idx, const uint64_t* pod_mask, uint32_t tier_mask, uint64_t removed_out[3]);
 
+/* ---- snapshot / restore (no reference counterpart) ------------------------------------------------------------------
+ * The index's contents as a canonical image, and a bulk load of such an image into a fresh handle: an indexer that
+ * restarts, is upgraded, moves to another GPU or is replicated keeps the blocks the fleet has already cached (vLLM
+ * announces a block once, when it is first stored).  Restoring into a handle created with a larger capacity / table_slots
+ * is also how an index outgrows its configuration.  Events sent while no indexer ran are not in any image: a block stored
+ * or removed in that window is missed until Evict, kvidx_remove_pods or a later event of the same block corrects it.
+ *
+ * Image format v1, all values little-endian:
+ *   header, 64 bytes
+ *     0  char[8] "KVIDXSNP"      8  u32 version = 1     12  u32 flags (bit 0: recency section present; others 0)
+ *    16  u32 block_size         20  u32 pods_per_key   24  u64 init_hash
+ *    32  u64 n_request          40  u64 n_engine
+ *    48  u32 pod_span (1 + highest pod id in any entry; 0 if none)   52  u32 model_span (1 + highest model id; 0 if none)
+ *    56  u64 0
+ *   n_request request records, 32 bytes each: u64 hash, u16 model, u8 count, u8 0, u16 ent[10] -- packed (pod<<4|tier),
+ *     oldest -> newest (the slot's physical order, lru Keys()); positions >= count are 0
+ *   n_engine engine records, 24 bytes each: u64 engine_hash, u64 request_hash, u16 model, 6 zero bytes
+ *   recency section, only with flag bit 0 (exact-LRU handles): one u64 per request record, then one per engine record;
+ *     larger = more recent, only the order carries meaning; every value is below 2^63 and no value repeats within a section
+ * Request records are strictly ascending by (model, hash), engine records by (model, engine_hash): the image depends
+ * only on the contents, not on the table size, insertion history, tombstones or rebuilds.  It holds every resident
+ * request key and every engine mapping, including stale mappings whose request key is absent (GetRequestKey returns
+ * them, a BlockStored parent resolves through them, Evict cleans them up, in_memory.go:225-230).  Tombstones, counters
+ * and tier weights are not part of it: weights are configuration of the restoring process.
+ * Size: 64 + 32 R + 24 E (+ 8 (R + E) with recency), R / E = kvidx_get_stats' request_keys / engine_keys.
+ *
+ * kvidx_snapshot writes the image to buf.  It holds the write side for the whole call (readers keep running; in exact-LRU
+ * mode, where readers write recency, they wait) and refreshes no key's recency; a device-resident event batch issued
+ * before it is included.  A pageable buffer is filled through pinned staging chunks, a pinned one (kvidx_host_alloc) directly.  buf == NULL or cap below the size -> KVIDX_ENOSPC with *size_out set and nothing written;
+ * otherwise *size_out = bytes written.
+ * kvidx_restore loads an image into a handle holding no live key (tombstones are dropped first; live keys ->
+ * KVIDX_EINVAL).  block_size, init_hash and pods_per_key must equal the handle's (else KVIDX_EINVAL); pod_span > max_pods ->
+ * KVIDX_ERANGE; a bad magic or version, a length that does not match the header, or any record failing validation (order,
+ * 1 <= count <= pods_per_key, distinct entries with pod < max_pods, zero padding and entries past count, spans equal to
+ * the header's) -> KVIDX_EINVAL, and the handle is left as it was.  Every record is validated before any is inserted.
+ * table_slots / capacity may differ from the source's; more keys than the write path admits (90 % of a table's slots) ->
+ * KVIDX_ENOSPC.  An exact-LRU handle needs an image with recency (else KVIDX_EINVAL) and keeps the most recent `capacity`
+ * keys of each map, as after any write call (found from the sorted recency values: the cut costs one sort, not one table
+ * sweep per excess key); a default handle ignores recency, but a repeated value is still malformed.  A concurrent reader sees each key absent
+ * or whole.  restored_out (may be NULL): {request keys, engine keys} resident after the call.
+ * Both: synchronous like every write call; a sharded handle -> KVIDX_EINVAL. */
+int kvidx_snapshot(kvidx_t* idx, void* buf, uint64_t cap, uint64_t* size_out);
+int kvidx_restore(kvidx_t* idx, const void* buf, uint64_t len, uint64_t restored_out[2]);
+
 /* ---- device-resident variants (inputs already in HBM; used by bench `value`, by the
  *      multi-GPU router and by callers that keep token buffers on the device) ------- */
 

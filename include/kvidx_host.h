@@ -13,6 +13,7 @@
  *   kvhost_pool_process      <-> worker loop: processEvent + digestEvents       pkg/kvcache/kvevents/pool.go:149-338
  *   kvhost_decode_event_batch<-> processEvent's msgpack decoding      pkg/kvcache/kvevents/pool.go:177-244, events.go:38-96
  *   kvhost_remove_pod        <-> (no counterpart) drop a departed pod's entries and free its id (kvidx_remove_pods)
+ *   kvhost_snapshot / _restore <-> (no counterpart) names + index image, warm start of a fresh mirror (kvidx_snapshot)
  *   kvhost_prefix_store_*    <-> prefixstore.LRUTokenStore            pkg/tokenization/prefixstore/lru_store.go:54-190
  *   kvhost_get_metrics / _text <-> InstrumentedIndex + collectors      pkg/kvcache/kvblock/instrumented_index.go:30-92, metrics/collector.go:28-59
  */
@@ -131,6 +132,22 @@ uint64_t kvhost_xxhash64(const void* data, size_t len, uint64_t seed);
  * steps 1 and 3 only.  An unknown pod name is a no-op.  Not counted in kvcache_index_evictions_total, which counts the
  * reference's Evict calls.  Returns the number of queued messages dropped, or a negative KVIDX_E* code. */
 int kvhost_remove_pod(kvhost_t* h, const char* pod, const char* const* tiers, size_t n_tiers);
+
+/* Snapshot / restore of the whole mirror (no counterpart; kvidx_snapshot / kvidx_restore).  Host image, little-endian:
+ *   char[8] "KVHOSTSN", u32 version = 1, u32 0;
+ *   three name tables -- models, tiers, pods -- each a u32 id count, then per id a u32 byte length and the bytes;
+ *     0xFFFFFFFF (no bytes) marks a pod id freed by kvhost_remove_pod, so the lowest-first reuse order survives;
+ *   u64 length, then the kvidx image as opaque bytes (length 0 for a no_device instance).
+ * kvhost_snapshot holds the write side exclusively, as kvhost_remove_pod does, so names and entries agree; read calls keep
+ * running.  Messages still queued (kvhost_pool_add_task without kvhost_pool_process) are not part of the image.
+ * buf == NULL or cap too small -> KVIDX_ENOSPC with *size_out set.
+ * kvhost_restore needs a fresh target: no pod or model interned, only the configured tiers, empty queues (else
+ * KVIDX_EINVAL).  The image's tiers at the configured ids must carry the target's configured names (else KVIDX_EINVAL);
+ * tier weights stay the target's.  Every pod id owning an entry in the index section must have a name in the pod table
+ * (else KVIDX_EINVAL).  A no_device target accepts only an image without an index section.  The index section
+ * goes through kvidx_restore and its error codes; on any error the target is left as it was. */
+int kvhost_snapshot(kvhost_t* h, void* buf, uint64_t cap, uint64_t* size_out);
+int kvhost_restore(kvhost_t* h, const void* buf, uint64_t len);
 
 /* interning introspection.  Model and tier ids are never reused; a pod id is freed by kvhost_remove_pod (all tiers) and
  * reused lowest first.  Name pointers returned by the calls above stay valid for the life of the handle. */

@@ -20,6 +20,7 @@
 #include "kernels_v1.cuh"
 #include "kernels_write.cuh"
 #include "kernels_remove.cuh"
+#include "kernels_snapshot.cuh"
 #include "kernels_score.cuh"
 #include "kernels_rounds.cuh"
 #include "kernels_rounds_plain.cuh"
@@ -137,6 +138,11 @@ struct kvidx {
     // write-side scratch (guarded by mu_w)
     DevBuf d_misc, d_ev, d_hash, d_evtok, d_qoff, d_wkeys, d_wpred, d_wready, d_wmap;
     PinBuf h_misc;
+    // snapshot / restore (guarded by mu_w): two pinned chunks between the device and a caller's buffer, which may be
+    // pageable; the device scratch (records, sort buffers) is released when the call returns
+    DevBuf d_snap;
+    PinBuf h_snap[2];
+    cudaEvent_t ev_snap[2] = {nullptr, nullptr};
     int write_phase1 = -1;          // -1: by batch size, 0: never, 1: always (phase 1 = hash_events_kernel)
     int64_t write_phase1_min = 1024; // engine hashes in a batch from which phase 1 pays
     int score_kernel = 2;          // 1 = v1 (thread per prompt, global tokens), 2 = tuned
@@ -1078,6 +1084,7 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     }
     for (int q = 0; q < kMaxParts; ++q) { CK(cudaEventCreateWithFlags(&x->ev_g[q], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&x->ev_r[q], cudaEventDisableTiming)); }
     CK(cudaEventCreateWithFlags(&x->ev_write, cudaEventDisableTiming));
+    for (auto& e : x->ev_snap) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     for (int a_ = 0; a_ < 2; ++a_) for (int b_ = 0; b_ < 2; ++b_) {
         CK(cudaEventCreateWithFlags(&x->ev_spec_h[a_][b_], cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&x->ev_spec_p[a_][b_], cudaEventDisableTiming));
@@ -1207,6 +1214,8 @@ void kvidx_destroy(kvidx_t* x) {
     x->r_act0.release(); x->r_act1.release(); x->r_cnt.release(); x->r_hstate.release(); x->r_keys.release(); x->r_pst.release(); x->r_nbr.release(); x->r_fp.release(); x->r_sort.release(); x->r_role.release(); x->r_hl.release(); x->r_map.release(); x->r_src.release(); x->r_fate.release(); x->r_anch.release(); x->r_snap.release(); x->r_rec.release();
     x->d_misc.release(); x->d_rmisc.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
+    x->d_snap.release(); x->h_snap[0].release(); x->h_snap[1].release();
+    for (auto& e : x->ev_snap) if (e) cudaEventDestroy(e);
     if (x->tv.req) cudaFree(x->tv.req);
     if (x->tv.eng) cudaFree(x->tv.eng);
     if (x->tv.req_stamp) cudaFree(x->tv.req_stamp);
@@ -1670,6 +1679,329 @@ int kvidx_remove_pods(kvidx_t* x, const uint64_t* pod_mask, uint32_t tier_mask, 
     if (rc) return rc;
     if (removed_out) memcpy(removed_out, x->h_misc.p, 24);
     return 0;
+}
+
+}  // extern "C"
+
+namespace {
+// ---- snapshot / restore (format v1, include/kvidx.h; kernels_snapshot.cuh) ----------------------------------------------
+constexpr uint64_t kSnapHeaderBytes = 64;
+constexpr uint32_t kSnapVersion = 1, kSnapFlagRecency = 1;
+constexpr size_t kSnapChunk = 16u << 20;          // bytes per pinned staging chunk
+const char kSnapMagic[8] = {'K', 'V', 'I', 'D', 'X', 'S', 'N', 'P'};
+
+struct SnapHeader {                               // the 64 header bytes (little-endian hosts: x86-64, aarch64)
+    char magic[8];
+    uint32_t version, flags, block_size, pods_per_key;
+    uint64_t init_hash, n_request, n_engine;
+    uint32_t pod_span, model_span;
+    uint64_t zero;
+};
+static_assert(sizeof(SnapHeader) == kSnapHeaderBytes, "snapshot header is 64 bytes");
+
+void release_snap(kvidx* x) { x->d_snap.release(); }
+
+// device -> caller's buffer: directly if it is pinned, else through the two pinned chunks (the copy engine fills one while
+// the host empties the other)
+int stage_d2h(kvidx* x, void* dst, const void* src, size_t n, cudaStream_t st) {
+    if (n == 0) return 0;
+    if (is_device_accessible_host(dst)) {             // a pinned caller buffer: one copy, no staging
+        CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    }
+    CK(x->h_snap[0].need(kSnapChunk));
+    CK(x->h_snap[1].need(kSnapChunk));
+    const size_t nc = (n + kSnapChunk - 1) / kSnapChunk;
+    for (size_t k = 0; k <= nc; ++k) {
+        if (k < nc) {
+            const size_t off = k * kSnapChunk, len = std::min(kSnapChunk, n - off);
+            CK(cudaMemcpyAsync(x->h_snap[k & 1].p, static_cast<const char*>(src) + off, len, cudaMemcpyDeviceToHost, st));
+            CK(cudaEventRecord(x->ev_snap[k & 1], st));
+        }
+        if (k > 0) {
+            const size_t j = k - 1, off = j * kSnapChunk, len = std::min(kSnapChunk, n - off);
+            CK(cudaEventSynchronize(x->ev_snap[j & 1]));
+            memcpy(static_cast<char*>(dst) + off, x->h_snap[j & 1].p, len);
+        }
+    }
+    return 0;
+}
+// caller's buffer -> device, the same way round
+int stage_h2d(kvidx* x, void* dst, const void* src, size_t n, cudaStream_t st) {
+    if (n == 0) return 0;
+    if (is_device_accessible_host(src)) { CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, st)); return 0; }
+    CK(x->h_snap[0].need(kSnapChunk));
+    CK(x->h_snap[1].need(kSnapChunk));
+    const size_t nc = (n + kSnapChunk - 1) / kSnapChunk;
+    for (size_t k = 0; k < nc; ++k) {
+        const size_t off = k * kSnapChunk, len = std::min(kSnapChunk, n - off);
+        if (k >= 2) CK(cudaEventSynchronize(x->ev_snap[k & 1]));          // the copy out of this chunk two steps ago is done
+        memcpy(x->h_snap[k & 1].p, static_cast<const char*>(src) + off, len);
+        CK(cudaMemcpyAsync(static_cast<char*>(dst) + off, x->h_snap[k & 1].p, len, cudaMemcpyHostToDevice, st));
+        CK(cudaEventRecord(x->ev_snap[k & 1], st));
+    }
+    return 0;
+}
+
+unsigned snap_ctas(kvidx* x, uint64_t n) {
+    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((n + kSnapThreads - 1) / kSnapThreads, (uint64_t)x->sm_count * 8));
+}
+
+// sort buffers of N records: keys (2 x 8 B), slot indices (2 x 4 B), models (2 x 2 B); the cub scratch follows
+size_t snap_sort_bytes(uint64_t N) { return ((size_t)N * 28 + 255) & ~(size_t)255; }
+
+// One table's FULL slots, sorted by (model, hash): slot indices in *sorted (inside `sc`).  `sc` holds snap_sort_bytes()
+// plus the cub scratch; `misc` is zeroed by the caller.  Slot indices are 32-bit: a table of 2^32 slots would be 128 GB.
+template <int kMeta>
+int snap_sort_table(kvidx* x, const void* tab, uint64_t slots, uint64_t expect, uint8_t* sc, size_t sort_tmp, SnapMisc* d_misc,
+                    const uint32_t** sorted, const char* what, cudaStream_t st) {
+    const uint64_t N = std::max<uint64_t>(expect, 1);
+    uint64_t* k0 = reinterpret_cast<uint64_t*>(sc);
+    uint64_t* k1 = k0 + N;
+    uint32_t* i0 = reinterpret_cast<uint32_t*>(k1 + N);
+    uint32_t* i1 = i0 + N;
+    uint16_t* m0 = reinterpret_cast<uint16_t*>(i1 + N);
+    uint16_t* m1 = m0 + N;
+    void* tmp = sc + snap_sort_bytes(N);
+    const unsigned ctas = (unsigned)std::min<uint64_t>(slots / kSnapThreads, (uint64_t)x->sm_count * 8);
+    snap_compact_kernel<kMeta><<<ctas, kSnapThreads, 0, st>>>(static_cast<const uint4*>(tab), slots, expect, k0, i0, d_misc);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    SnapMisc* h = x->h_misc.as<SnapMisc>();
+    CK(cudaMemcpyAsync(h, d_misc, sizeof(SnapMisc), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (h->n != expect)
+        return fail(KVIDX_ECUDA, "snapshot: %llu FULL %s slots, but the handle counts %llu", (unsigned long long)h->n, what, (unsigned long long)expect);
+    *sorted = i0;
+    if (expect == 0) return 0;
+    size_t tb = sort_tmp;
+    CK(cub::DeviceRadixSort::SortPairs(tmp, tb, k0, k1, i0, i1, (int)expect, 0, 64, st));
+    *sorted = i1;
+    x->launches += 5;
+    if (h->model_span > 1) {                          // more than one model: a stable pass over the model bits
+        int bits = 0;
+        while ((1u << bits) < h->model_span) ++bits;
+        snap_models_kernel<kMeta><<<(unsigned)((expect + 255) / 256), 256, 0, st>>>(static_cast<const uint4*>(tab), i1, expect, m0);
+        tb = sort_tmp;
+        CK(cub::DeviceRadixSort::SortPairs(tmp, tb, m0, m1, i1, i0, (int)expect, 0, bits, st));
+        *sorted = i0;
+        x->launches += 4;
+    }
+    CK(cudaGetLastError());
+    return 0;
+}
+
+int snapshot_impl(kvidx* x, void* buf, uint64_t R, uint64_t E, bool rec) {
+    cudaStream_t st = wstream(x);
+    const uint64_t N = std::max<uint64_t>(std::max(R, E), 1);
+    size_t sort_tmp = 0, t2 = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)N, 0, 64, st));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, t2, (uint16_t*)nullptr, (uint16_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)N, 0, 16, st));
+    sort_tmp = std::max(sort_tmp, t2);
+    // device scratch: misc (2 x SnapMisc) | image body | sort buffers + cub scratch
+    const size_t body = (size_t)(32 * R + 24 * E + (rec ? 8 * (R + E) : 0));
+    const size_t body_off = 256, sc_off = body_off + ((body + 255) & ~(size_t)255);
+    CK(x->d_snap.need(sc_off + snap_sort_bytes(N) + sort_tmp));
+    CK(x->h_misc.need(64));
+    uint8_t* d = x->d_snap.as<uint8_t>();
+    SnapMisc* d_req = reinterpret_cast<SnapMisc*>(d);
+    SnapMisc* d_eng = d_req + 1;
+    uint8_t* out = d + body_off;
+    CK(cudaMemsetAsync(d, 0, 2 * sizeof(SnapMisc), st));
+    uint4* req_rec = reinterpret_cast<uint4*>(out);
+    unsigned long long* eng_rec = reinterpret_cast<unsigned long long*>(out + 32 * R);
+    unsigned long long* req_st = rec ? reinterpret_cast<unsigned long long*>(out + 32 * R + 24 * E) : nullptr;
+    unsigned long long* eng_st = rec ? req_st + R : nullptr;
+    const uint32_t* idx = nullptr;
+    int rc = snap_sort_table<3>(x, x->tv.req, x->tv.req_mask + 1, R, d + sc_off, sort_tmp, d_req, &idx, "request", st);
+    if (rc) return rc;
+    const uint32_t model_span_req = x->h_misc.as<SnapMisc>()->model_span;
+    if (R) {
+        snap_req_records_kernel<<<snap_ctas(x, R), kSnapThreads, 0, st>>>(x->tv.req, idx, R, req_rec, x->tv.req_stamp, req_st, d_req);
+        x->launches += 1;
+        CK(cudaGetLastError());
+    }
+    rc = snap_sort_table<0>(x, x->tv.eng, x->tv.eng_mask + 1, E, d + sc_off, sort_tmp, d_eng, &idx, "engine", st);
+    if (rc) return rc;
+    const uint32_t model_span_eng = x->h_misc.as<SnapMisc>()->model_span;
+    if (E) {
+        snap_eng_records_kernel<<<(unsigned)((E + 255) / 256), 256, 0, st>>>(x->tv.eng, idx, E, eng_rec, eng_st);
+        x->launches += 1;
+        CK(cudaGetLastError());
+    }
+    CK(cudaMemcpyAsync(x->h_misc.p, d_req, sizeof(SnapMisc), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    SnapHeader hd{};
+    memcpy(hd.magic, kSnapMagic, 8);
+    hd.version = kSnapVersion; hd.flags = rec ? kSnapFlagRecency : 0;
+    hd.block_size = x->tv.block_size; hd.pods_per_key = x->tv.pods_per_key; hd.init_hash = x->tv.init_hash;
+    hd.n_request = R; hd.n_engine = E;
+    hd.pod_span = x->h_misc.as<SnapMisc>()->pod_span;
+    hd.model_span = std::max(model_span_req, model_span_eng);
+    memcpy(buf, &hd, sizeof hd);
+    return stage_d2h(x, static_cast<char*>(buf) + kSnapHeaderBytes, out, body, st);
+}
+
+int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t restored_out[2]) {
+    cudaStream_t st = wstream(x);
+    const uint64_t R = hd.n_request, E = hd.n_engine;
+    const bool rec = hd.flags & kSnapFlagRecency;
+    const size_t nbody = (size_t)(32 * R + 24 * E + (rec ? 8 * (R + E) : 0));
+    const size_t body_off = 256, st_off = body_off + ((nbody + 255) & ~(size_t)255);
+    // recency images: each section's stamps sorted (8 B per record) + the cub scratch
+    size_t sort_tmp = 0;
+    if (rec) CK(cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                               (int)std::max<uint64_t>(std::max(R, E), 1), 0, 64, st));
+    const size_t tmp_off = st_off + (rec ? ((size_t)(R + E) * 8 + 255) & ~(size_t)255 : 0);
+    CK(x->d_snap.need(tmp_off + sort_tmp));
+    CK(x->h_misc.need(2 * sizeof(SnapCheck) + 16));
+    uint8_t* d = x->d_snap.as<uint8_t>();
+    SnapCheck* d_chk = reinterpret_cast<SnapCheck*>(d);
+    CK(cudaMemsetAsync(d, 0, 2 * sizeof(SnapCheck), st));
+    CK(cudaMemsetAsync(&d_chk[0].first_bad, 0xff, 8, st));
+    CK(cudaMemsetAsync(&d_chk[1].first_bad, 0xff, 8, st));
+    uint8_t* dbody = d + body_off;
+    int rc = stage_h2d(x, dbody, body, nbody, st);
+    if (rc) return rc;
+    const uint4* req_rec = reinterpret_cast<const uint4*>(dbody);
+    const unsigned long long* eng_rec = reinterpret_cast<const unsigned long long*>(dbody + 32 * R);
+    const unsigned long long* req_st = rec ? reinterpret_cast<const unsigned long long*>(dbody + 32 * R + 24 * E) : nullptr;
+    const unsigned long long* eng_st = rec ? req_st + R : nullptr;
+    // 1. validate every record before anything is inserted
+    if (R) snap_check_req_kernel<<<snap_ctas(x, R), kSnapThreads, 0, st>>>(req_rec, R, req_st, x->tv.pods_per_key, x->tv.max_pods, d_chk);
+    if (E) snap_check_eng_kernel<<<snap_ctas(x, E), kSnapThreads, 0, st>>>(eng_rec, E, eng_st, d_chk + 1);
+    x->launches += (R ? 1 : 0) + (E ? 1 : 0);
+    CK(cudaGetLastError());
+    // recency: no value repeats within a section; in exact-LRU mode the `capacity` most recent keys of each table are kept,
+    // which is what enforce_caps would leave, found here as the stamp of rank n - capacity instead of n - capacity sweeps
+    const bool keep = x->tv.req_stamp != nullptr;
+    SnapCheck* h = x->h_misc.as<SnapCheck>();
+    unsigned long long* h_from = reinterpret_cast<unsigned long long*>(h + 2);
+    h_from[0] = h_from[1] = 0;
+    if (rec) {
+        unsigned long long* sorted = reinterpret_cast<unsigned long long*>(d + st_off);
+        const unsigned long long* sect[2] = {req_st, eng_st};
+        const uint64_t cnt[2] = {R, E};
+        for (int tb = 0; tb < 2; ++tb) {
+            if (!cnt[tb]) continue;
+            size_t tb_bytes = sort_tmp;
+            CK(cub::DeviceRadixSort::SortKeys(d + tmp_off, tb_bytes, sect[tb], sorted, (int)cnt[tb], 0, 64, st));
+            snap_check_ties_kernel<<<snap_ctas(x, cnt[tb]), kSnapThreads, 0, st>>>(sorted, cnt[tb], d_chk + tb);
+            x->launches += 5;
+            if (keep && cnt[tb] > x->tv.capacity)
+                CK(cudaMemcpyAsync(&h_from[tb], sorted + (cnt[tb] - x->tv.capacity), 8, cudaMemcpyDeviceToHost, st));
+            sorted += cnt[tb];
+        }
+        CK(cudaGetLastError());
+    }
+    CK(cudaMemcpyAsync(h, d_chk, 2 * sizeof(SnapCheck), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int tb = 0; tb < 2; ++tb) {
+        const unsigned b = h[tb].bad;
+        if (b)
+            return fail(KVIDX_EINVAL, "malformed snapshot image: %s record %llu:%s%s%s%s%s%s", tb ? "engine" : "request", h[tb].first_bad,
+                        b & kSnapBadOrder ? " not in strictly ascending (model, hash) order;" : "",
+                        b & kSnapBadCount ? " entry count outside 1..pods_per_key;" : "",
+                        b & kSnapBadEntry ? " repeated entry or pod id >= max_pods;" : "",
+                        b & kSnapBadPad ? " non-zero padding or entry past the count;" : "",
+                        b & kSnapBadStamp ? " recency value >= 2^63;" : "",
+                        b & kSnapBadTie ? " a recency value repeats (index given in sorted order);" : "");
+    }
+    const uint32_t model_span = std::max(h[0].model_span, h[1].model_span);
+    if (h[0].pod_span != hd.pod_span || model_span != hd.model_span)
+        return fail(KVIDX_EINVAL, "malformed snapshot image: header pod_span %u / model_span %u, records %u / %u", hd.pod_span,
+                    hd.model_span, h[0].pod_span, model_span);
+    const unsigned long long stamp_max = std::max(h[0].stamp_max, h[1].stamp_max);
+    // 2. the target's tombstones go (it holds no live key, so this is clearing both tables)
+    const Counters& c = *x->h_cnt;
+    if (c.req_tomb || c.eng_tomb) {
+        CK(cudaMemsetAsync(x->tv.req, 0, (x->tv.req_mask + 1) * sizeof(ReqSlot), st));
+        CK(cudaMemsetAsync(x->tv.eng, 0, (x->tv.eng_mask + 1) * sizeof(EngSlot), st));
+        if (x->tv.req_stamp) CK(cudaMemsetAsync(x->tv.req_stamp, 0, (x->tv.req_mask + 1) * 8, st));
+        CK(cudaMemsetAsync(&x->d_cnt->req_tomb, 0, sizeof(unsigned long long), st));
+        CK(cudaMemsetAsync(&x->d_cnt->eng_tomb, 0, sizeof(unsigned long long), st));
+    }
+    // 3. insert; recency is kept only by an exact-LRU handle
+    const unsigned long long nospc_before = x->h_cnt->nospc, from_req = h_from[0], from_eng = h_from[1];
+    if (R) restore_req_kernel<<<snap_ctas(x, R), kSnapThreads, 0, st>>>(x->tv, req_rec, R, keep ? req_st : nullptr, from_req);
+    if (E) restore_eng_kernel<<<snap_ctas(x, E), kSnapThreads, 0, st>>>(x->tv, eng_rec, E, keep ? eng_st : nullptr, from_eng);
+    x->launches += (R ? 1 : 0) + (E ? 1 : 0);
+    CK(cudaGetLastError());
+    if ((rc = refresh_counters(x))) return rc;
+    if (x->h_cnt->nospc != nospc_before) return fail(KVIDX_ENOSPC, "%llu restored keys found no slot", x->h_cnt->nospc - nospc_before);
+    if (keep) {                                       // later stamps must be newer than every restored one
+        unsigned long long cur = x->clock.load();
+        while (cur <= stamp_max && !x->clock.compare_exchange_weak(cur, stamp_max + 1)) {}
+    }
+    release_snap(x);
+    if ((rc = enforce_caps(x))) return rc;            // a no-op after the cut above; kept as the invariant of every write call
+    if (restored_out) { restored_out[0] = x->h_cnt->req_full; restored_out[1] = x->h_cnt->eng_full; }
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int kvidx_snapshot(kvidx_t* x, void* buf, uint64_t cap, uint64_t* size_out) {
+    if (size_out) *size_out = 0;
+    if (!x || !size_out) return fail(KVIDX_EINVAL, "bad arguments");
+    // a sharded handle's keys live in several processes' tables: one image would need a collective export
+    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_snapshot is not supported on a sharded index");
+    std::lock_guard<std::mutex> g(x->mu_w);
+    CK(cudaSetDevice(x->device));
+    std::shared_lock<std::shared_mutex> tl(x->tables);
+    int rc = refresh_counters(x);                     // synchronises the write stream: earlier asynchronous batches are in
+    if (rc) return rc;
+    const uint64_t R = x->h_cnt->req_full, E = x->h_cnt->eng_full;
+    const bool rec = x->tv.req_stamp != nullptr;
+    const uint64_t size = kSnapHeaderBytes + 32 * R + 24 * E + (rec ? 8 * (R + E) : 0);
+    *size_out = size;
+    if (!buf || cap < size) return fail(KVIDX_ENOSPC, "the snapshot needs %llu bytes, the buffer has %llu", (unsigned long long)size,
+                                        (unsigned long long)(buf ? cap : 0));
+    rc = snapshot_impl(x, buf, R, E, rec);
+    release_snap(x);
+    return rc;
+}
+
+int kvidx_restore(kvidx_t* x, const void* buf, uint64_t len, uint64_t restored_out[2]) {
+    if (restored_out) restored_out[0] = restored_out[1] = 0;
+    if (!x || !buf) return fail(KVIDX_EINVAL, "bad arguments");
+    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_restore is not supported on a sharded index");
+    if (len < kSnapHeaderBytes) return fail(KVIDX_EINVAL, "malformed snapshot image: %llu bytes, shorter than the header", (unsigned long long)len);
+    SnapHeader hd;
+    memcpy(&hd, buf, sizeof hd);
+    if (memcmp(hd.magic, kSnapMagic, 8) != 0) return fail(KVIDX_EINVAL, "malformed snapshot image: bad magic");
+    if (hd.version != kSnapVersion) return fail(KVIDX_EINVAL, "unsupported snapshot version %u (this library reads %u)", hd.version, kSnapVersion);
+    if ((hd.flags & ~kSnapFlagRecency) || hd.zero) return fail(KVIDX_EINVAL, "malformed snapshot image: unknown flags or non-zero header padding");
+    const bool rec = hd.flags & kSnapFlagRecency;
+    const uint64_t R = hd.n_request, E = hd.n_engine;
+    if (R > (len >> 5) || E > len / 24 ||
+        len != kSnapHeaderBytes + 32 * R + 24 * E + (rec ? 8 * (R + E) : 0))
+        return fail(KVIDX_EINVAL, "malformed snapshot image: %llu bytes do not hold %llu request and %llu engine records%s",
+                    (unsigned long long)len, (unsigned long long)R, (unsigned long long)E, rec ? " with recency" : "");
+    if (hd.block_size != x->tv.block_size || hd.init_hash != x->tv.init_hash || hd.pods_per_key != x->tv.pods_per_key)
+        return fail(KVIDX_EINVAL, "snapshot of another configuration: block_size %u, init_hash %#llx, pods_per_key %u (this index: %u, %#llx, %u)",
+                    hd.block_size, (unsigned long long)hd.init_hash, hd.pods_per_key, x->tv.block_size, (unsigned long long)x->tv.init_hash,
+                    x->tv.pods_per_key);
+    if (hd.pod_span > x->tv.max_pods) return fail(KVIDX_ERANGE, "snapshot holds pod ids up to %u, max_pods is %u", hd.pod_span - 1, x->tv.max_pods);
+    if (hd.model_span > 65536) return fail(KVIDX_EINVAL, "malformed snapshot image: model_span %u", hd.model_span);
+    if (x->tv.req_stamp && !rec) return fail(KVIDX_EINVAL, "an exact-LRU index needs an image with recency (taken from an exact-LRU index)");
+    std::lock_guard<std::mutex> g(x->mu_w);
+    CK(cudaSetDevice(x->device));
+    std::shared_lock<std::shared_mutex> tl(x->tables);
+    int rc = refresh_counters(x);
+    if (rc) return rc;
+    if (x->h_cnt->req_full || x->h_cnt->eng_full)
+        return fail(KVIDX_EINVAL, "restore needs an empty index: this one holds %llu request and %llu engine keys",
+                    x->h_cnt->req_full, x->h_cnt->eng_full);
+    const uint64_t rs = x->tv.req_mask + 1, es = x->tv.eng_mask + 1;
+    if (R * 10 > rs * 9 || E * 10 > es * 9)          // the write path's limit: at most 90 % of a table's slots live
+        return fail(KVIDX_ENOSPC, "table full: %llu request / %llu engine keys in %llu / %llu slots", (unsigned long long)R,
+                    (unsigned long long)E, (unsigned long long)rs, (unsigned long long)es);
+    rc = restore_impl(x, static_cast<const uint8_t*>(buf) + kSnapHeaderBytes, hd, restored_out);
+    release_snap(x);
+    return rc;
 }
 
 int kvidx_shard_export(kvidx_t* x, void* out) {

@@ -149,6 +149,7 @@ struct kvhost {
     std::vector<std::deque<Msg>> queues;
     uint32_t filter_words = 4;
     uint32_t pod_cap = 256;                          // == index.max_pods: ids of pods that own entries
+    uint32_t cfg_tiers = 0;                          // tier ids interned from the configuration at create
     kvhost_metrics_t met{};              // guarded by mu
 };
 
@@ -297,6 +298,7 @@ int kvhost_create(const kvhost_config_t* cfg_in, const char* hash_seed, kvhost_t
     h->cfg = c;
     h->queues.resize(c.concurrency);
     for (uint32_t i = 0; i < c.n_tiers; ++i) h->tiers.id(lower(c.tier_names[i] ? c.tier_names[i] : ""), KVIDX_MAX_TIERS);
+    h->cfg_tiers = (uint32_t)h->tiers.names.size();
     const char* seed = hash_seed ? hash_seed : "";
     c.index.init_hash = kvidx_fnv64a(seed, strlen(seed));           // getInitHash, token_processor.go:81-90
     c.index.n_tier_weights = c.n_tiers;
@@ -604,6 +606,142 @@ int kvhost_remove_pod(kvhost_t* h, const char* pod, const char* const* tiers, si
         h->pods.release((uint32_t)id);
     }
     return dropped;
+}
+
+}  // extern "C"
+
+namespace {
+const char kHostSnapMagic[8] = {'K', 'V', 'H', 'O', 'S', 'T', 'S', 'N'};
+constexpr uint32_t kHostSnapVersion = 1, kReleased = 0xFFFFFFFFu;
+
+void put32(std::string& s, uint32_t v) { s.append(reinterpret_cast<const char*>(&v), 4); }   // little-endian hosts
+void put64(std::string& s, uint64_t v) { s.append(reinterpret_cast<const char*>(&v), 8); }
+void put_names(std::string& s, const Interner& in) {
+    put32(s, (uint32_t)in.names.size());
+    for (const std::string* n : in.names) {
+        if (!n) { put32(s, kReleased); continue; }
+        put32(s, (uint32_t)n->size());
+        s += *n;
+    }
+}
+// one entry of a name table read back: the name of the id, or a released pod id
+struct NameRec { std::string name; bool released; };
+bool get_names(const uint8_t*& p, const uint8_t* e, std::vector<NameRec>& out) {
+    uint32_t n;
+    if (e - p < 4) return false;
+    memcpy(&n, p, 4); p += 4;
+    for (uint32_t i = 0; i < n; ++i) {
+        uint32_t l;
+        if (e - p < 4) return false;
+        memcpy(&l, p, 4); p += 4;
+        if (l == kReleased) { out.push_back({std::string(), true}); continue; }
+        if ((uint64_t)(e - p) < l) return false;
+        out.push_back({std::string(reinterpret_cast<const char*>(p), l), false});
+        p += l;
+    }
+    return true;
+}
+bool distinct(const std::vector<NameRec>& v) {
+    std::unordered_set<std::string> seen;
+    for (const auto& r : v) if (!r.released && !seen.insert(r.name).second) return false;
+    return true;
+}
+void install(Interner& in, const std::vector<NameRec>& v, size_t from) {      // the interner holds ids [0, from) already
+    for (size_t i = from; i < v.size(); ++i) {
+        if (v[i].released) { in.names.push_back(nullptr); in.free_ids.insert((uint32_t)i); continue; }
+        in.names.push_back(&*in.store.insert(v[i].name).first);
+        in.ids.emplace(v[i].name, (uint32_t)i);
+    }
+}
+}  // namespace
+
+extern "C" {
+
+int kvhost_snapshot(kvhost_t* h, void* buf, uint64_t cap, uint64_t* size_out) {
+    if (size_out) *size_out = 0;
+    if (!h || !size_out) return hfail(KVIDX_EINVAL, "bad arguments");
+    std::unique_lock<std::shared_mutex> wl(h->write_mu);     // no entry of any pod is written meanwhile
+    std::string s(kHostSnapMagic, 8);
+    put32(s, kHostSnapVersion); put32(s, 0);
+    {
+        std::lock_guard<std::mutex> g(h->mu);
+        put_names(s, h->models); put_names(s, h->tiers); put_names(s, h->pods);
+    }
+    uint64_t isz = 0;
+    if (h->ix) {
+        const int rc = kvidx_snapshot(h->ix, nullptr, 0, &isz);             // size query
+        if (rc != KVIDX_ENOSPC) { g_herr = kvidx_last_error(h->ix); return rc ? rc : KVIDX_ECUDA; }
+    }
+    const uint64_t total = s.size() + 8 + isz;
+    *size_out = total;
+    if (!buf || cap < total) return hfail(KVIDX_ENOSPC, "the snapshot needs " + std::to_string(total) + " bytes");
+    put64(s, isz);
+    memcpy(buf, s.data(), s.size());
+    if (h->ix) {
+        uint64_t got = 0;
+        const int rc = kvidx_snapshot(h->ix, static_cast<char*>(buf) + s.size(), isz, &got);
+        if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+    }
+    return 0;
+}
+
+int kvhost_restore(kvhost_t* h, const void* buf, uint64_t len) {
+    if (!h || (!buf && len)) return hfail(KVIDX_EINVAL, "bad arguments");
+    const uint8_t* p = static_cast<const uint8_t*>(buf);
+    const uint8_t* e = p + len;
+    uint32_t ver = 0, zero = 1;
+    if (len < 16 || memcmp(p, kHostSnapMagic, 8) != 0) return hfail(KVIDX_EINVAL, "malformed host snapshot: bad magic");
+    memcpy(&ver, p + 8, 4); memcpy(&zero, p + 12, 4);
+    if (ver != kHostSnapVersion || zero) return hfail(KVIDX_EINVAL, "unsupported host snapshot version " + std::to_string(ver));
+    p += 16;
+    std::vector<NameRec> models, tiers, pods;
+    if (!get_names(p, e, models) || !get_names(p, e, tiers) || !get_names(p, e, pods))
+        return hfail(KVIDX_EINVAL, "malformed host snapshot: truncated name table");
+    uint64_t ilen = 0;
+    if (e - p < 8) return hfail(KVIDX_EINVAL, "malformed host snapshot: truncated");
+    memcpy(&ilen, p, 8); p += 8;
+    if ((uint64_t)(e - p) != ilen) return hfail(KVIDX_EINVAL, "malformed host snapshot: index section length mismatch");
+    for (const auto& r : models) if (r.released) return hfail(KVIDX_EINVAL, "malformed host snapshot: released model id");
+    for (const auto& r : tiers) if (r.released) return hfail(KVIDX_EINVAL, "malformed host snapshot: released tier id");
+    if (!distinct(models) || !distinct(tiers) || !distinct(pods)) return hfail(KVIDX_EINVAL, "malformed host snapshot: repeated name");
+    if (models.size() > 65536 || tiers.size() > KVIDX_MAX_TIERS || pods.size() > KVIDX_MAX_PODS)
+        return hfail(KVIDX_EINVAL, "malformed host snapshot: more ids than the id space holds");
+    std::unique_lock<std::shared_mutex> wl(h->write_mu);
+    std::lock_guard<std::mutex> g(h->mu);                    // held through the device restore: nothing interns meanwhile
+    bool queued = false;
+    for (const auto& q : h->queues) queued |= !q.empty();
+    if (!h->pods.names.empty() || !h->models.names.empty() || h->tiers.names.size() != h->cfg_tiers || queued)
+        return hfail(KVIDX_EINVAL, "restore needs a fresh host indexer (no pod or model seen, only the configured tiers, nothing queued)");
+    if (tiers.size() < h->cfg_tiers) return hfail(KVIDX_EINVAL, "snapshot has fewer tiers than this indexer's configuration");
+    for (uint32_t i = 0; i < h->cfg_tiers; ++i)
+        if (tiers[i].name != *h->tiers.names[i])
+            return hfail(KVIDX_EINVAL, "tier " + std::to_string(i) + " is \"" + tiers[i].name + "\" in the snapshot, \"" + *h->tiers.names[i] + "\" here");
+    if (!h->ix && ilen) return hfail(KVIDX_EINVAL, "a host-only instance cannot restore an index section");
+    if (ilen >= 64) {                                          // every pod owning an entry has a name (the rest is kvidx_restore's)
+        uint64_t nreq = 0;
+        memcpy(&nreq, p + 32, 8);
+        if (nreq <= (ilen - 64) / 32) {
+            for (uint64_t r = 0; r < nreq; ++r) {
+                const uint8_t* rec = p + 64 + 32 * r;
+                const uint32_t cnt = std::min<uint32_t>(rec[10], KVIDX_MAX_PODS_PER_KEY);
+                for (uint32_t j = 0; j < cnt; ++j) {
+                    uint16_t e;
+                    memcpy(&e, rec + 12 + 2 * j, 2);
+                    const uint32_t pod = KVIDX_PT_POD(e);
+                    if (pod >= pods.size() || pods[pod].released)
+                        return hfail(KVIDX_EINVAL, "malformed host snapshot: pod id " + std::to_string(pod) + " owns entries but has no name");
+                }
+            }
+        }
+    }
+    if (ilen) {
+        const int rc = kvidx_restore(h->ix, p, ilen, nullptr);
+        if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+    }
+    install(h->models, models, 0);
+    install(h->tiers, tiers, h->cfg_tiers);
+    install(h->pods, pods, 0);
+    return 0;
 }
 
 int64_t kvhost_decode_event_batch(kvhost_t* h, const char* pod, const char* model, const void* payload, size_t len, kvidx_event_t* ev_out,

@@ -67,6 +67,8 @@ SYMBOLS = {
     "kvidx_get_request_key": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, _u64p]),
     "kvidx_apply_events": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, _u64p, C.c_int64, _u32p, C.c_int64, _i64p]),
     "kvidx_remove_pods": (C.c_int, [C.c_void_p, _u64p, C.c_uint32, _u64p]),
+    "kvidx_snapshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "kvidx_restore": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, _u64p]),
     "kvidx_set_stream": (C.c_int, [C.c_void_p, C.c_void_p]),
     "kvidx_synchronize": (C.c_int, [C.c_void_p]),
     "kvidx_score_batch_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -146,6 +148,7 @@ class Index:
         self.h = h
         self.block_size, self.max_pods = block_size, max_pods
         self.filter_words = (max_pods + 63) // 64
+        self.lru_exact = bool(lru_exact)
 
     # -- plumbing --
     def close(self):
@@ -320,6 +323,29 @@ class Index:
         out = np.zeros(3, np.uint64)
         self._ck(self.L.kvidx_remove_pods(self.h, _p(mask, _u64p), tier_mask, _p(out, _u64p)))
         return {"entries": int(out[0]), "request_keys": int(out[1]), "engine_keys": int(out[2])}
+
+    # -- snapshot / restore (no reference counterpart; format v1 in include/kvidx.h) --
+    def snapshot(self) -> bytes:
+        """kvidx_snapshot: the index's contents as a canonical image.  Raises KvidxError on failure."""
+        st = self.stats()
+        R, E = st["request_keys"], st["engine_keys"]
+        size = 64 + 32 * R + 24 * E + (8 * (R + E) if self.lru_exact else 0)
+        while True:
+            buf = bytearray(size)
+            got = C.c_uint64(0)
+            rc = self.L.kvidx_snapshot(self.h, (C.c_char * size).from_buffer(buf), size, C.byref(got))
+            if rc == ENOSPC and got.value > size:          # keys were added since stats(): size again
+                size = got.value
+                continue
+            self._ck(rc)
+            return bytes(memoryview(buf)[:got.value])
+
+    def restore(self, image) -> dict:
+        """kvidx_restore: load an image into this (empty) handle.  -> {"request_keys", "engine_keys"} resident afterwards."""
+        image = image if isinstance(image, bytes) else bytes(image)
+        out = np.zeros(2, np.uint64)
+        self._ck(self.L.kvidx_restore(self.h, image, len(image), _p(out, _u64p)))
+        return {"request_keys": int(out[0]), "engine_keys": int(out[1])}
 
 
 class _Raw:

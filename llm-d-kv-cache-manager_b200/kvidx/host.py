@@ -53,6 +53,8 @@ SYMBOLS = {
     "kvhost_pool_queue_index": (C.c_int, [C.c_void_p, C.c_char_p]),
     "kvhost_pool_process": (C.c_int64, [C.c_void_p, C.POINTER(C.c_int64)]),
     "kvhost_remove_pod": (C.c_int, [C.c_void_p, C.c_char_p, _cpp, C.c_size_t]),
+    "kvhost_snapshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "kvhost_restore": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64]),
     "kvhost_decode_event_batch": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_size_t,
                                               C.POINTER(C.c_size_t), _u32p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "kvhost_pod_id": (C.c_int, [C.c_void_p, C.c_char_p]),
@@ -184,6 +186,26 @@ class HostIndexer:
         if n < 0:
             raise _native.KvidxError(n, self.err())
         return n
+
+    def snapshot(self) -> bytes:
+        """kvhost_snapshot: names (models, tiers, pods with freed ids) + the index image.  Queued messages are not included."""
+        size = C.c_uint64(0)
+        rc = self.L.kvhost_snapshot(self.h, None, 0, C.byref(size))
+        while True:
+            if rc != _native.ENOSPC:
+                raise _native.KvidxError(rc, self.err())
+            cap = size.value
+            buf = bytearray(cap)
+            rc = self.L.kvhost_snapshot(self.h, (C.c_char * cap).from_buffer(buf), cap, C.byref(size))
+            if rc == 0:
+                return bytes(memoryview(buf)[:size.value])
+
+    def restore(self, image):
+        """kvhost_restore: load a kvhost_snapshot image into this fresh indexer."""
+        image = image if isinstance(image, bytes) else bytes(image)
+        rc = self.L.kvhost_restore(self.h, image, len(image))
+        if rc:
+            raise _native.KvidxError(rc, self.err())
 
     def decode(self, pod, model, payload: bytes, cap=4096):
         ev = np.zeros(cap, EVENT_DTYPE); hs = np.zeros(cap * 64, np.uint64); tk = np.zeros(cap * 1024, np.uint32)
