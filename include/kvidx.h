@@ -197,7 +197,8 @@ int kvidx_apply_events(kvidx_t* idx, const kvidx_event_t* ev, int64_t n_events,
  * request key was already absent before the call stays (Evict cleans those up, in_memory.go:225-230).  A concurrent
  * reader sees each key before or after its update, as with a sequence of Evict calls.  Synchronous like every write
  * call; works in both LRU modes; the tombstones it leaves are compacted by the usual rebuild policy.
- * All-zero pod_mask or tier_mask == 0 -> KVIDX_EINVAL; sharded handle -> KVIDX_EINVAL.
+ * All-zero pod_mask or tier_mask == 0 -> KVIDX_EINVAL; sharded handle -> KVIDX_EINVAL (kvidx_shard_remove_pods is the
+ * collective form for those).
  * removed_out (may be NULL): {entries, request keys, engine keys} removed. */
 int kvidx_remove_pods(kvidx_t* idx, const uint64_t* pod_mask, uint32_t tier_mask, uint64_t removed_out[3]);
 
@@ -241,7 +242,8 @@ int kvidx_remove_pods(kvidx_t* idx, const uint64_t* pod_mask, uint32_t tier_mask
  * keys of each map, as after any write call (found from the sorted recency values: the cut costs one sort, not one table
  * sweep per excess key); a default handle ignores recency, but a repeated value is still malformed.  A concurrent reader sees each key absent
  * or whole.  restored_out (may be NULL): {request keys, engine keys} resident after the call.
- * Both: synchronous like every write call; a sharded handle -> KVIDX_EINVAL. */
+ * Both: synchronous like every write call; a sharded handle -> KVIDX_EINVAL (kvidx_shard_snapshot, kvidx_snapshot_merge
+ * and kvidx_shard_restore are the collective forms for those). */
 int kvidx_snapshot(kvidx_t* idx, void* buf, uint64_t cap, uint64_t* size_out);
 int kvidx_restore(kvidx_t* idx, const void* buf, uint64_t len, uint64_t restored_out[2]);
 
@@ -293,6 +295,40 @@ int kvidx_shard_attach(kvidx_t* idx, uint32_t rank, kvidx_t* other);
  * of the embedding program, no rank touches the index meanwhile (kvidx.dist.compact_shards does exactly that).  On an
  * unsharded handle it is the compaction the write path runs by itself when needed. */
 int kvidx_shard_compact(kvidx_t* idx);
+
+/* Maintenance of a sharded index: pod removal, snapshot and restore.  Collective by contract, like kvidx_shard_compact:
+ * every rank calls them between barriers of the embedding program and no rank writes to the index in the meantime (readers
+ * keep running and see each key before or after its update).  kvidx.dist.remove_pods_shards / snapshot_shards /
+ * restore_shards provide the barriers.  On an unsharded handle each does what its single-process counterpart does.
+ *
+ * kvidx_shard_remove_pods: kvidx_remove_pods over the whole sharded index, in two phases.  Phase 0 removes the entries
+ *   of this rank's request shard and marks the keys it removes in two bitmaps (slots/8 + slots/16 bytes, kept behind the
+ *   request slots, so that peers read them through the mapping they already hold); removed_out = {entries, request
+ *   keys, 0}.  Phase 1, after every rank's phase 0, drops this rank's engine mappings whose request key phase 0 removed,
+ *   on whichever rank owns it; removed_out = {0, 0, engine keys}.  Summed over ranks and phases the counters and the
+ *   resulting contents equal kvidx_remove_pods on an unsharded index with the same contents (a stale mapping, whose key
+ *   was absent before the call, stays).  KVIDX_EINVAL: phase 1 without a phase 0 on this handle, with other masks than
+ *   phase 0, or after a write call (add, evict, apply_events, restore, compaction) on this handle since phase 0; an
+ *   unconnected shard; an empty mask; phase > 1.
+ * kvidx_shard_snapshot: the v1 image of the request keys and engine mappings THIS rank owns (stale mappings included),
+ *   with kvidx_snapshot's buffer conventions.  Each part is a valid image on its own.
+ * kvidx_snapshot_merge: host only (no device, no handle).  Merges the parts of disjoint shards into the one canonical
+ *   image an unsharded index with the same contents would give: records in (model, hash) order, counts summed,
+ *   pod_span / model_span the maxima.  KVIDX_EINVAL: n_parts == 0, a header or length kvidx_restore would refuse, parts
+ *   of different block_size / init_hash / pods_per_key, a part with recency (sharded handles never track it, and stamps
+ *   of different ranks do not compare), records out of order inside a part, a (model, hash) in two parts.  Every
+ *   record is checked before anything is written.  out == NULL or cap below the size -> KVIDX_ENOSPC with *size_out set.
+ *   The message is kvidx_last_error(NULL)'s.
+ * kvidx_shard_restore: accepts any v1 image -- unsharded, merged, or a single part -- and inserts the records this rank
+ *   owns, so the same call restarts a layout and reshards it (1 -> N, N -> M, N -> 1).  The handle must hold no live
+ *   key (as kvidx_restore).  Every rank counts the records of every owner over the whole image and checks each owner's
+ *   share against 90 % of a shard's slots (the geometry is equal on all shards), so a malformed image or one too
+ *   large for any owner (KVIDX_ENOSPC) is refused by every rank before any rank inserts.  Recency is ignored, as on a
+ *   default handle (a repeated value is still malformed).  restored_out: {request keys, engine keys} of this shard. */
+int kvidx_shard_remove_pods(kvidx_t* idx, const uint64_t* pod_mask, uint32_t tier_mask, uint32_t phase, uint64_t removed_out[3]);
+int kvidx_shard_snapshot(kvidx_t* idx, void* buf, uint64_t cap, uint64_t* size_out);
+int kvidx_snapshot_merge(const void* const* parts, const uint64_t* lens, uint32_t n_parts, void* out, uint64_t cap, uint64_t* size_out);
+int kvidx_shard_restore(kvidx_t* idx, const void* buf, uint64_t len, uint64_t restored_out[2]);
 
 /* The ROUTED form of a sharded Score() (SURVEY 8(e): all-to-all of keys to their owners, slot images back), as three
  * device steps around an exchange the embedding program performs (kvidx.dist.score_alltoall does it with NCCL

@@ -19,6 +19,12 @@
 //           table from that home: the mapping goes if the probe reaches a tombstone of the key with its removed_slot bit
 //           set; a FULL slot of the key or an EMPTY slot keeps it.  (The key has at most one slot tombstoned by this call:
 //           a re-added key never reuses its old tombstone, and older tombstones of the key have no bit.)
+//
+// Sharded index (kvidx_shard_remove_pods): an engine mapping lives with its engine hash's owner, its request key with
+// the owner of the request hash.  Every rank runs pass 1 over its own request shard (phase 0), then, once all ranks have,
+// pass 2 over its own engine shard (phase 1).  Pass 2 therefore reads the request table AND the two bitmaps of the key's
+// owner: the bitmaps of a sharded handle sit right behind its request slots, in the same allocation, so the mapping every
+// peer already holds (CUDA IPC / kvidx_shard_attach) covers them.  Unsharded, owner 0 is the handle itself.
 #pragma once
 #include "table.cuh"
 #include "../../include/kvidx.h"
@@ -33,9 +39,12 @@ struct RemoveArgs {
     uint32_t* removed_slot;             // bit per request slot: tombstoned by this call
     uint32_t* removed_home;             // bit per home pair (home slot / 2) of a key tombstoned by this call
     unsigned long long* out;            // {entries, request keys, engine keys} removed
+    const uint32_t* owner_slot[8];      // pass 2: removed_slot / removed_home of request shard r (t.req_peer[r]); entry 0
+    const uint32_t* owner_home[8];      //         only on an unsharded handle
 };
 
-__device__ __forceinline__ bool test_bit(const uint32_t* bits, uint64_t i) { return (bits[i >> 5] >> (i & 31)) & 1u; }
+// system scope: a peer's bitmaps were written by a kernel of another process (or device) before the embedding program's barrier
+__device__ __forceinline__ bool test_bit(const uint32_t* bits, uint64_t i) { return (ld_word_relaxed(bits + (i >> 5), true) >> (i & 31)) & 1u; }
 
 // sum over the warp, one atomic per warp (the grid-stride loops below give every lane of a warp the same trip count)
 __device__ __forceinline__ void warp_add(unsigned long long* dst, unsigned long long v) {
@@ -105,17 +114,20 @@ __global__ void __launch_bounds__(kRemoveThreads) remove_eng_kernel(TableView t,
             if (meta_state(m) != kStateFull) break;
             const uint32_t model = meta_model(m);
             const uint64_t rhash = ((uint64_t)a.w << 32) | a.z;
-            const uint64_t home = slot_home(rhash, model, t.req_mask);
-            if (!test_bit(r.removed_home, home >> 1)) break;
+            const uint64_t mixed = home_of(rhash, model);
+            const uint32_t owner = shard_of(mixed, t.shard_bits);
+            const uint64_t home = mixed & t.req_mask & ~1ull;          // slot_home
+            if (!test_bit(r.owner_home[owner], home >> 1)) break;
+            const ReqSlot* req = t.req_peer[owner];
             bool drop = false;
             for (uint64_t j = home, step = 0; step <= t.req_mask; ++step, j = (j + 1) & t.req_mask) {
                 uint4 ra, rb;
-                ld_slot_fresh(t.req + j, ra, rb);
+                ld_slot_fresh(req + j, ra, rb);
                 const uint32_t st = meta_state(rb.w);
                 if (st == kStateEmpty) break;
                 if (ra.x == (uint32_t)rhash && ra.y == (uint32_t)(rhash >> 32) && meta_model(rb.w) == model) {
                     if (st == kStateFull) break;
-                    if (st == kStateTomb && test_bit(r.removed_slot, j)) { drop = true; break; }
+                    if (st == kStateTomb && test_bit(r.owner_slot[owner], j)) { drop = true; break; }
                 }
             }
             if (!drop) break;

@@ -21,6 +21,11 @@
 //   restore_*_kernel      thread per record at or above its table's threshold: claims a slot from the key's home with the compare-and-swap EMPTY -> BUSY and
 //                         publishes the image with the two-half protocol of table.cuh, as rebuild_*_kernel does, so a
 //                         concurrent reader sees each key either absent or whole.
+// Sharded import (kvidx_shard_restore): every rank reads the WHOLE image and inserts only the records it owns.
+//   snap_owner_hist_kernel records per owning shard in each section, so that every rank can hold every owner's share
+//                         against the room of a shard before any rank inserts (the verdict depends only on the image
+//                         and the common geometry, so all ranks reach the same one).
+//   restore_*_kernel      skip a record whose key another shard owns (unsharded: shard 0 owns every key).
 #pragma once
 #include "table.cuh"
 #include "../../include/kvidx.h"
@@ -246,6 +251,29 @@ __device__ __forceinline__ void warp_sum_add(unsigned long long* dst, unsigned l
     if ((threadIdx.x & 31) == 0 && v) atomicAdd(dst, v);
 }
 
+// counts[o]: request records owned by shard o, counts[8 + o]: engine records (shard = top shard_bits of the mixed key)
+__global__ void __launch_bounds__(kSnapThreads) snap_owner_hist_kernel(const uint4* __restrict__ req_rec, uint64_t R,
+                                                                       const unsigned long long* __restrict__ eng_rec, uint64_t E,
+                                                                       uint32_t shard_bits, unsigned long long* counts) {
+    __shared__ unsigned long long h[16];
+    if (threadIdx.x < 16) h[threadIdx.x] = 0;
+    __syncthreads();
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < R + E; i += stride) {
+        uint64_t hash; uint32_t model, sect;
+        if (i < R) {
+            const uint4 a = req_rec[2 * i];
+            hash = ((uint64_t)a.y << 32) | a.x; model = a.z & 0xffffu; sect = 0;
+        } else {
+            const uint64_t k = i - R;
+            hash = eng_rec[3 * k]; model = (uint32_t)(eng_rec[3 * k + 2] & 0xffffu); sect = 8;
+        }
+        atomicAdd(&h[sect + shard_of(home_of(hash, model), shard_bits)], 1ull);
+    }
+    __syncthreads();
+    if (threadIdx.x < 16 && h[threadIdx.x]) atomicAdd(&counts[threadIdx.x], h[threadIdx.x]);
+}
+
 // stamp: the record's recency stamp, or nullptr (default mode, or an image without recency)
 // keep_from: records whose stamp is below it are not inserted (the exact-LRU cut to `capacity`, done before inserting)
 __global__ void __launch_bounds__(kSnapThreads) restore_req_kernel(TableView t, const uint4* __restrict__ rec, uint64_t n,
@@ -259,6 +287,7 @@ __global__ void __launch_bounds__(kSnapThreads) restore_req_kernel(TableView t, 
         const uint4 r0 = rec[2 * i], r1 = rec[2 * i + 1];
         const uint64_t hash = ((uint64_t)r0.y << 32) | r0.x;
         const uint32_t model = r0.z & 0xffffu, cnt = (r0.z >> 16) & 0xffu;
+        if (shard_of(home_of(hash, model), t.shard_bits) != t.shard_rank) continue;      // another shard's key
         const uint4 a = make_uint4(r0.x, r0.y, r0.w, r1.x);
         const uint32_t busy = make_meta(kStateBusy, 0, model);
         uint4 b = make_uint4(r1.y, r1.z, r1.w, published_meta(busy, make_meta(kStateFull, cnt, model)));
@@ -286,6 +315,7 @@ __global__ void __launch_bounds__(kSnapThreads) restore_eng_kernel(TableView t, 
         if (i >= n) continue;
         const unsigned long long eh = rec[3 * i], rh = rec[3 * i + 1];
         const uint32_t model = (uint32_t)(rec[3 * i + 2] & 0xffffu);
+        if (shard_of(home_of(eh, model), t.shard_bits) != t.shard_rank) continue;
         const unsigned long long s = stamp ? stamp[i] : 0ull;
         if (s < keep_from) continue;
         const uint4 a = make_uint4((uint32_t)eh, (uint32_t)(eh >> 32), (uint32_t)rh, (uint32_t)(rh >> 32));

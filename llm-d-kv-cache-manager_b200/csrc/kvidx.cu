@@ -143,6 +143,11 @@ struct kvidx {
     DevBuf d_snap;
     PinBuf h_snap[2];
     cudaEvent_t ev_snap[2] = {nullptr, nullptr};
+    // collective pod removal (kvidx_shard_remove_pods, guarded by mu_w): phase 0 ran on this handle with these masks and
+    // neither phase 1 nor any write call has run since, so the removal bitmaps describe exactly that removal
+    bool rm_armed = false;
+    uint32_t rm_tiers = 0;
+    uint64_t rm_pods[KVIDX_MAX_PODS / 64] = {};
     int write_phase1 = -1;          // -1: by batch size, 0: never, 1: always (phase 1 = hash_events_kernel)
     int64_t write_phase1_min = 1024; // engine hashes in a batch from which phase 1 pays
     int score_kernel = 2;          // 1 = v1 (thread per prompt, global tokens), 2 = tuned
@@ -195,6 +200,9 @@ int check_shards(kvidx* x) {
 
 unsigned long long reserve_stamps(kvidx* x, unsigned long long n) { return x->clock.fetch_add(n + 1); }
 
+// removal bitmaps of a request table of `slots` slots: removed_slot (a bit per slot), then removed_home (a bit per home pair)
+size_t remove_bitmap_bytes(uint64_t slots) { return slots / 8 + slots / 16; }
+
 // The stream write kernels go to.  Exact-LRU mode keeps reads and writes on ONE stream (reads write recency stamps, so the
 // two sides are not independent there); otherwise the write path has its own.
 cudaStream_t wstream(kvidx* x) { return x->tv.req_stamp ? x->stream : x->own_wstream; }
@@ -217,12 +225,13 @@ int refresh_counters(kvidx* x) {
     return 0;
 }
 
-int alloc_tables(kvidx* x, uint64_t req_slots, uint64_t eng_slots, ReqSlot** req, EngSlot** eng, cudaStream_t st) {
+// req_tail: bytes allocated (and zeroed) behind the request slots -- a sharded handle keeps its removal bitmaps there
+int alloc_tables(kvidx* x, uint64_t req_slots, uint64_t eng_slots, ReqSlot** req, EngSlot** eng, cudaStream_t st, size_t req_tail = 0) {
     *req = nullptr; *eng = nullptr;
-    CK(cudaMalloc((void**)req, req_slots * sizeof(ReqSlot)));
+    CK(cudaMalloc((void**)req, req_slots * sizeof(ReqSlot) + req_tail));
     cudaError_t e = cudaMalloc((void**)eng, eng_slots * sizeof(EngSlot));
     if (e != cudaSuccess) { cudaFree(*req); *req = nullptr; return fail(KVIDX_ENOMEM, "cudaMalloc of %llu engine slots: %s", (unsigned long long)eng_slots, cudaGetErrorString(e)); }
-    CK(cudaMemsetAsync(*req, 0, req_slots * sizeof(ReqSlot), st));
+    CK(cudaMemsetAsync(*req, 0, req_slots * sizeof(ReqSlot) + req_tail, st));
     CK(cudaMemsetAsync(*eng, 0, eng_slots * sizeof(EngSlot), st));
     return 0;
 }
@@ -1109,7 +1118,9 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     t.max_pods = c.max_pods; t.filter_words = (c.max_pods + 63) / 64;
     for (int i = 0; i < 16; ++i) t.weight[i] = (uint32_t)i < c.n_tier_weights ? c.tier_weight[i] : 1.0;
     t.req_stamp = nullptr;
-    int rc = alloc_tables(x, slots, slots, &t.req, &t.eng, x->stream);
+    // a sharded handle's removal bitmaps (kvidx_shard_remove_pods) follow its request slots: its peers read them through
+    // the mapping they already hold, and the in-place compaction rewrites only the slots
+    int rc = alloc_tables(x, slots, slots, &t.req, &t.eng, x->stream, shard_bits ? remove_bitmap_bytes(slots) : 0);
     if (rc) return rc;
     if (c.lru_exact) {
         if (c.shard_count > 1) return fail(KVIDX_EINVAL, "lru_exact is not supported on a sharded index");
@@ -1448,6 +1459,7 @@ int kvidx_add(kvidx_t* x, uint32_t model, const uint64_t* engine, const uint64_t
     if (model > 0xffffu) return fail(KVIDX_ERANGE, "model id %u > 65535", model);
     if (int rc0 = check_podtiers(x, pts, m)) return rc0;
     std::lock_guard<std::mutex> g(x->mu_w);
+    x->rm_armed = false;
     CK(cudaSetDevice(x->device));
     if (int rc0 = check_shards(x)) return rc0;
     int rc = ensure_room(x, (uint64_t)n);
@@ -1490,6 +1502,7 @@ int kvidx_evict(kvidx_t* x, uint32_t model, uint64_t engine, const kvidx_podtier
     if (model > 0xffffu) return fail(KVIDX_ERANGE, "model id %u > 65535", model);
     if (int rc0 = check_podtiers(x, pts, m)) return rc0;
     std::lock_guard<std::mutex> g(x->mu_w);
+    x->rm_armed = false;
     CK(cudaSetDevice(x->device));
     if (int rc0 = check_shards(x)) return rc0;
     std::shared_lock<std::shared_mutex> tl(x->tables);
@@ -1569,6 +1582,7 @@ int kvidx_apply_events_dev(kvidx_t* x, const kvidx_event_t* d_ev_sorted, const i
     if (!x || n_queues < 0 || n_events < 0 || n_hashes < 0) return fail(KVIDX_EINVAL, "bad arguments");
     if (n_queues == 0 || n_events == 0) return 0;
     std::lock_guard<std::mutex> g(x->mu_w);
+    x->rm_armed = false;
     CK(cudaSetDevice(x->device));
     if (int rc0 = check_shards(x)) return rc0;
     int rc = ensure_room(x, (uint64_t)n_hashes);       // every hash of the batch may be a new key
@@ -1605,6 +1619,7 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
         qcount[KVIDX_PT_POD(e.podtier) + 1]++;
     }
     std::lock_guard<std::mutex> g(x->mu_w);
+    x->rm_armed = false;
     CK(cudaSetDevice(x->device));
     if (int rc0 = check_shards(x)) return rc0;
     int rc = ensure_room(x, new_keys);
@@ -1644,40 +1659,95 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
     return enforce_caps(x);
 }
 
-int kvidx_remove_pods(kvidx_t* x, const uint64_t* pod_mask, uint32_t tier_mask, uint64_t removed_out[3]) {
-    if (removed_out) removed_out[0] = removed_out[1] = removed_out[2] = 0;
+}  // extern "C"
+
+namespace {
+// Arguments shared by kvidx_remove_pods and kvidx_shard_remove_pods; 0 if they are usable.
+int check_removal(kvidx* x, const uint64_t* pod_mask, uint32_t tier_mask) {
     if (!x || !pod_mask) return fail(KVIDX_EINVAL, "bad arguments");
-    // an engine mapping lives with its engine hash's owner and its request key with another rank: cleaning it up on a
-    // sharded index would need the removal bitmaps of every rank
-    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_remove_pods is not supported on a sharded index");
     if ((tier_mask & 0xffffu) == 0) return fail(KVIDX_EINVAL, "empty tier mask");
-    const uint32_t FW = x->tv.filter_words;
     uint64_t any = 0;
-    for (uint32_t w = 0; w < FW; ++w) any |= pod_mask[w];
+    for (uint32_t w = 0; w < x->tv.filter_words; ++w) any |= pod_mask[w];
     if (!any) return fail(KVIDX_EINVAL, "empty pod mask");
-    std::lock_guard<std::mutex> g(x->mu_w);
-    CK(cudaSetDevice(x->device));
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    return 0;
+}
+
+// The two sweeps of a removal (kernels_remove.cuh).  Caller holds mu_w and `tables` shared.
+//   d_misc: out[4] | pod mask | unsharded only: removed_slot (rs bits) | removed_home (rs / 2 bits)
+//   sharded: this rank's bitmaps are the tail of its request-table allocation (alloc_tables), a peer's the tail of its own
+// pass 1 (remove_req_kernel) clears and fills this handle's bitmaps; pass 2 (remove_eng_kernel) reads those of every
+// request shard's owner.  removed_out: {entries, request keys, engine keys} removed by the passes that ran.
+int run_removal(kvidx* x, const uint64_t* pod_mask, uint32_t tier_mask, bool pass1, bool pass2, uint64_t removed_out[3]) {
     cudaStream_t st = wstream(x);
     const uint64_t rs = x->tv.req_mask + 1;
-    // scratch: out[4] | pod mask | removed_slot (rs bits) | removed_home (rs / 2 bits)
-    const size_t mask_off = 32, slot_off = mask_off + (size_t)FW * 8, home_off = slot_off + rs / 8, total = home_off + rs / 16;
-    CK(x->d_misc.need(total));
+    const uint32_t FW = x->tv.filter_words;
+    const bool sharded = x->tv.shard_bits != 0;
+    const size_t mask_off = 32, slot_off = mask_off + (size_t)FW * 8, total = slot_off + (sharded ? 0 : remove_bitmap_bytes(rs));
+    CK(x->d_misc.need(total));                        // a no-op in phase 1: phase 0 sized it and no write call came between
     CK(x->h_misc.need(32));
     uint8_t* d = x->d_misc.as<uint8_t>();
-    CK(cudaMemsetAsync(d, 0, total, st));
-    CK(cudaMemcpyAsync(d + mask_off, pod_mask, (size_t)FW * 8, cudaMemcpyHostToDevice, st));
-    RemoveArgs ra{reinterpret_cast<const uint64_t*>(d + mask_off), tier_mask & 0xffffu, reinterpret_cast<uint32_t*>(d + slot_off),
-                  reinterpret_cast<uint32_t*>(d + home_off), reinterpret_cast<unsigned long long*>(d)};
+    auto bits_of = [&](uint32_t r) {
+        return sharded ? reinterpret_cast<uint32_t*>(x->tv.req_peer[r] + rs) : reinterpret_cast<uint32_t*>(d + slot_off);
+    };
+    uint32_t* mine = bits_of(x->tv.shard_rank);
+    RemoveArgs ra{reinterpret_cast<const uint64_t*>(d + mask_off), tier_mask & 0xffffu, mine, mine + rs / 32,
+                  reinterpret_cast<unsigned long long*>(d), {}, {}};
+    for (uint32_t r = 0; r < (1u << x->tv.shard_bits); ++r) { ra.owner_slot[r] = bits_of(r); ra.owner_home[r] = bits_of(r) + rs / 32; }
+    CK(cudaMemsetAsync(d, 0, 32, st));
+    if (pass1) {
+        CK(cudaMemsetAsync(mine, 0, remove_bitmap_bytes(rs), st));
+        CK(cudaMemcpyAsync(d + mask_off, pod_mask, (size_t)FW * 8, cudaMemcpyHostToDevice, st));
+    }
     const unsigned ctas = (unsigned)std::min<uint64_t>(rs / kRemoveThreads, (uint64_t)x->sm_count * 8);
-    remove_req_kernel<<<ctas, kRemoveThreads, 0, st>>>(x->tv, ra);
-    remove_eng_kernel<<<ctas, kRemoveThreads, 0, st>>>(x->tv, ra);
-    x->launches += 2;
+    if (pass1) remove_req_kernel<<<ctas, kRemoveThreads, 0, st>>>(x->tv, ra);
+    if (pass2) remove_eng_kernel<<<ctas, kRemoveThreads, 0, st>>>(x->tv, ra);
+    x->launches += (pass1 ? 1 : 0) + (pass2 ? 1 : 0);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(x->h_misc.p, d, 24, cudaMemcpyDeviceToHost, st));
     int rc = refresh_counters(x);                      // synchronises the write stream: the removal has taken effect
     if (rc) return rc;
     if (removed_out) memcpy(removed_out, x->h_misc.p, 24);
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int kvidx_remove_pods(kvidx_t* x, const uint64_t* pod_mask, uint32_t tier_mask, uint64_t removed_out[3]) {
+    if (removed_out) removed_out[0] = removed_out[1] = removed_out[2] = 0;
+    if (!x || !pod_mask) return fail(KVIDX_EINVAL, "bad arguments");
+    // an engine mapping lives with its engine hash's owner and its request key with another rank: cleaning it up on a
+    // sharded index needs the removal bitmaps of every rank, which the collective kvidx_shard_remove_pods provides
+    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_remove_pods is not supported on a sharded index (kvidx_shard_remove_pods is its collective form)");
+    if (int rc = check_removal(x, pod_mask, tier_mask)) return rc;
+    std::lock_guard<std::mutex> g(x->mu_w);
+    x->rm_armed = false;
+    CK(cudaSetDevice(x->device));
+    std::shared_lock<std::shared_mutex> tl(x->tables);
+    return run_removal(x, pod_mask, tier_mask, true, true, removed_out);
+}
+
+int kvidx_shard_remove_pods(kvidx_t* x, const uint64_t* pod_mask, uint32_t tier_mask, uint32_t phase, uint64_t removed_out[3]) {
+    if (removed_out) removed_out[0] = removed_out[1] = removed_out[2] = 0;
+    if (phase > 1) return fail(KVIDX_EINVAL, "phase %u: a removal has phases 0 and 1", phase);
+    if (int rc = check_removal(x, pod_mask, tier_mask)) return rc;
+    const uint32_t FW = x->tv.filter_words;
+    std::lock_guard<std::mutex> g(x->mu_w);
+    CK(cudaSetDevice(x->device));
+    if (int rc = check_shards(x)) return rc;
+    if (phase == 1) {
+        if (!x->rm_armed)
+            return fail(KVIDX_EINVAL, "phase 1 without a preceding phase 0 on this handle, or a write call came between the phases");
+        if (x->rm_tiers != (tier_mask & 0xffffu) || memcmp(x->rm_pods, pod_mask, (size_t)FW * 8) != 0)
+            return fail(KVIDX_EINVAL, "phase 1 with other pod / tier masks than phase 0");
+    }
+    x->rm_armed = false;
+    std::shared_lock<std::shared_mutex> tl(x->tables);
+    int rc = run_removal(x, pod_mask, tier_mask, phase == 0, phase == 1, removed_out);
+    if (rc || phase == 1) return rc;
+    x->rm_armed = true;
+    x->rm_tiers = tier_mask & 0xffffu;
+    memcpy(x->rm_pods, pod_mask, (size_t)FW * 8);
     return 0;
 }
 
@@ -1855,10 +1925,11 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
                                                (int)std::max<uint64_t>(std::max(R, E), 1), 0, 64, st));
     const size_t tmp_off = st_off + (rec ? ((size_t)(R + E) * 8 + 255) & ~(size_t)255 : 0);
     CK(x->d_snap.need(tmp_off + sort_tmp));
-    CK(x->h_misc.need(2 * sizeof(SnapCheck) + 16));
+    CK(x->h_misc.need(2 * sizeof(SnapCheck) + 16 + 16 * 8));
     uint8_t* d = x->d_snap.as<uint8_t>();
     SnapCheck* d_chk = reinterpret_cast<SnapCheck*>(d);
-    CK(cudaMemsetAsync(d, 0, 2 * sizeof(SnapCheck), st));
+    unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(d_chk + 2);     // sharded: records per owner (16 x 8 B)
+    CK(cudaMemsetAsync(d, 0, 2 * sizeof(SnapCheck) + 16 * 8, st));
     CK(cudaMemsetAsync(&d_chk[0].first_bad, 0xff, 8, st));
     CK(cudaMemsetAsync(&d_chk[1].first_bad, 0xff, 8, st));
     uint8_t* dbody = d + body_off;
@@ -1872,12 +1943,18 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
     if (R) snap_check_req_kernel<<<snap_ctas(x, R), kSnapThreads, 0, st>>>(req_rec, R, req_st, x->tv.pods_per_key, x->tv.max_pods, d_chk);
     if (E) snap_check_eng_kernel<<<snap_ctas(x, E), kSnapThreads, 0, st>>>(eng_rec, E, eng_st, d_chk + 1);
     x->launches += (R ? 1 : 0) + (E ? 1 : 0);
+    const bool sharded = x->tv.shard_bits != 0;
+    if (sharded) {                                    // the whole image's records per owner, for the room check below
+        snap_owner_hist_kernel<<<snap_ctas(x, R + E), kSnapThreads, 0, st>>>(req_rec, R, eng_rec, E, x->tv.shard_bits, d_hist);
+        x->launches += 1;
+    }
     CK(cudaGetLastError());
     // recency: no value repeats within a section; in exact-LRU mode the `capacity` most recent keys of each table are kept,
     // which is what enforce_caps would leave, found here as the stamp of rank n - capacity instead of n - capacity sweeps
     const bool keep = x->tv.req_stamp != nullptr;
     SnapCheck* h = x->h_misc.as<SnapCheck>();
     unsigned long long* h_from = reinterpret_cast<unsigned long long*>(h + 2);
+    unsigned long long* h_hist = h_from + 2;
     h_from[0] = h_from[1] = 0;
     if (rec) {
         unsigned long long* sorted = reinterpret_cast<unsigned long long*>(d + st_off);
@@ -1896,6 +1973,7 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
         CK(cudaGetLastError());
     }
     CK(cudaMemcpyAsync(h, d_chk, 2 * sizeof(SnapCheck), cudaMemcpyDeviceToHost, st));
+    if (sharded) CK(cudaMemcpyAsync(h_hist, d_hist, 16 * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     for (int tb = 0; tb < 2; ++tb) {
         const unsigned b = h[tb].bad;
@@ -1913,6 +1991,15 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
         return fail(KVIDX_EINVAL, "malformed snapshot image: header pod_span %u / model_span %u, records %u / %u", hd.pod_span,
                     hd.model_span, h[0].pod_span, model_span);
     const unsigned long long stamp_max = std::max(h[0].stamp_max, h[1].stamp_max);
+    // sharded: every owner's share against the write path's limit (90 % of a shard's slots; kvidx_shard_attach enforces
+    // equal geometry on all shards), so that every rank refuses an image that does not fit before any rank inserts
+    if (sharded) {
+        const uint64_t rs = x->tv.req_mask + 1, es = x->tv.eng_mask + 1;
+        for (uint32_t o = 0; o < (1u << x->tv.shard_bits); ++o)
+            if (h_hist[o] * 10 > rs * 9 || h_hist[8 + o] * 10 > es * 9)
+                return fail(KVIDX_ENOSPC, "shard %u full: it owns %llu request / %llu engine keys of the image, %llu / %llu slots", o,
+                            h_hist[o], h_hist[8 + o], (unsigned long long)rs, (unsigned long long)es);
+    }
     // 2. the target's tombstones go (it holds no live key, so this is clearing both tables)
     const Counters& c = *x->h_cnt;
     if (c.req_tomb || c.eng_tomb) {
@@ -1939,15 +2026,78 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
     if (restored_out) { restored_out[0] = x->h_cnt->req_full; restored_out[1] = x->h_cnt->eng_full; }
     return 0;
 }
-}  // namespace
 
-extern "C" {
+// Header and length of an image as kvidx_restore checks them before looking at the handle.
+int check_image_header(const void* buf, uint64_t len, SnapHeader* out) {
+    if (len < kSnapHeaderBytes) return fail(KVIDX_EINVAL, "malformed snapshot image: %llu bytes, shorter than the header", (unsigned long long)len);
+    SnapHeader& hd = *out;
+    memcpy(&hd, buf, sizeof hd);
+    if (memcmp(hd.magic, kSnapMagic, 8) != 0) return fail(KVIDX_EINVAL, "malformed snapshot image: bad magic");
+    if (hd.version != kSnapVersion) return fail(KVIDX_EINVAL, "unsupported snapshot version %u (this library reads %u)", hd.version, kSnapVersion);
+    if ((hd.flags & ~kSnapFlagRecency) || hd.zero) return fail(KVIDX_EINVAL, "malformed snapshot image: unknown flags or non-zero header padding");
+    const bool rec = hd.flags & kSnapFlagRecency;
+    const uint64_t R = hd.n_request, E = hd.n_engine;
+    if (R > (len >> 5) || E > len / 24 ||
+        len != kSnapHeaderBytes + 32 * R + 24 * E + (rec ? 8 * (R + E) : 0))
+        return fail(KVIDX_EINVAL, "malformed snapshot image: %llu bytes do not hold %llu request and %llu engine records%s",
+                    (unsigned long long)len, (unsigned long long)R, (unsigned long long)E, rec ? " with recency" : "");
+    return 0;
+}
 
-int kvidx_snapshot(kvidx_t* x, void* buf, uint64_t cap, uint64_t* size_out) {
-    if (size_out) *size_out = 0;
-    if (!x || !size_out) return fail(KVIDX_EINVAL, "bad arguments");
-    // a sharded handle's keys live in several processes' tables: one image would need a collective export
-    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_snapshot is not supported on a sharded index");
+// The (model, hash) sort key of a record: model in the top bits of `hi`, so that pairs compare as one 80-bit number.
+struct RecKey {
+    uint64_t hi, lo;
+    bool operator<(const RecKey& o) const { return hi < o.hi || (hi == o.hi && lo < o.lo); }
+    bool operator==(const RecKey& o) const { return hi == o.hi && lo == o.lo; }
+};
+RecKey rec_key(const uint8_t* r, size_t model_off) {
+    uint64_t h; uint16_t m;
+    memcpy(&h, r, 8); memcpy(&m, r + model_off, 2);
+    return RecKey{m, h};
+}
+
+// k-way merge of the parts' request sections, then of their engine sections, into dst (nullptr: check only).  Records of
+// one part must be strictly ascending; a key in two parts is refused.  A linear scan over the part heads picks the next
+// record: the parts are shards, at most 8 of them in a sharded index.
+int merge_images(const void* const* parts, const std::vector<SnapHeader>& hd, uint8_t* dst) {
+    const size_t np = hd.size();
+    for (int sect = 0; sect < 2; ++sect) {
+        const size_t rb = sect ? 24 : 32, moff = sect ? 16 : 8;
+        const char* what = sect ? "engine" : "request";
+        std::vector<const uint8_t*> cur(np);
+        std::vector<uint64_t> left(np);
+        for (size_t p = 0; p < np; ++p) {
+            cur[p] = static_cast<const uint8_t*>(parts[p]) + kSnapHeaderBytes + (sect ? 32 * hd[p].n_request : 0);
+            left[p] = sect ? hd[p].n_engine : hd[p].n_request;
+        }
+        std::vector<RecKey> head(np);
+        for (size_t p = 0; p < np; ++p) if (left[p]) head[p] = rec_key(cur[p], moff);
+        bool have_prev = false;
+        RecKey prev{};
+        size_t prev_part = 0;
+        for (;;) {
+            size_t best = np;
+            for (size_t p = 0; p < np; ++p)
+                if (left[p] && (best == np || head[p] < head[best])) best = p;
+            if (best == np) break;
+            if (have_prev && head[best] == prev)
+                return fail(KVIDX_EINVAL, "%s key (model %llu, hash %#llx) is in parts %zu and %zu: parts must come from disjoint shards", what,
+                            (unsigned long long)prev.hi, (unsigned long long)prev.lo, prev_part, best);
+            if (dst) { memcpy(dst, cur[best], rb); dst += rb; }
+            prev = head[best]; prev_part = best; have_prev = true;
+            cur[best] += rb;
+            if (--left[best]) {
+                head[best] = rec_key(cur[best], moff);
+                if (!(prev < head[best]))
+                    return fail(KVIDX_EINVAL, "malformed snapshot image: part %zu %s record %llu: not in strictly ascending (model, hash) order", best,
+                                what, (unsigned long long)((sect ? hd[best].n_engine : hd[best].n_request) - left[best]));
+            }
+        }
+    }
+    return 0;
+}
+
+int snapshot_call(kvidx* x, void* buf, uint64_t cap, uint64_t* size_out) {
     std::lock_guard<std::mutex> g(x->mu_w);
     CK(cudaSetDevice(x->device));
     std::shared_lock<std::shared_mutex> tl(x->tables);
@@ -1964,22 +2114,13 @@ int kvidx_snapshot(kvidx_t* x, void* buf, uint64_t cap, uint64_t* size_out) {
     return rc;
 }
 
-int kvidx_restore(kvidx_t* x, const void* buf, uint64_t len, uint64_t restored_out[2]) {
-    if (restored_out) restored_out[0] = restored_out[1] = 0;
-    if (!x || !buf) return fail(KVIDX_EINVAL, "bad arguments");
-    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_restore is not supported on a sharded index");
-    if (len < kSnapHeaderBytes) return fail(KVIDX_EINVAL, "malformed snapshot image: %llu bytes, shorter than the header", (unsigned long long)len);
+// kvidx_restore after its argument checks; on a sharded handle only the records this shard owns are inserted, and the room
+// check is every owner's (restore_impl)
+int restore_call(kvidx* x, const void* buf, uint64_t len, uint64_t restored_out[2]) {
     SnapHeader hd;
-    memcpy(&hd, buf, sizeof hd);
-    if (memcmp(hd.magic, kSnapMagic, 8) != 0) return fail(KVIDX_EINVAL, "malformed snapshot image: bad magic");
-    if (hd.version != kSnapVersion) return fail(KVIDX_EINVAL, "unsupported snapshot version %u (this library reads %u)", hd.version, kSnapVersion);
-    if ((hd.flags & ~kSnapFlagRecency) || hd.zero) return fail(KVIDX_EINVAL, "malformed snapshot image: unknown flags or non-zero header padding");
+    if (int rc = check_image_header(buf, len, &hd)) return rc;
     const bool rec = hd.flags & kSnapFlagRecency;
     const uint64_t R = hd.n_request, E = hd.n_engine;
-    if (R > (len >> 5) || E > len / 24 ||
-        len != kSnapHeaderBytes + 32 * R + 24 * E + (rec ? 8 * (R + E) : 0))
-        return fail(KVIDX_EINVAL, "malformed snapshot image: %llu bytes do not hold %llu request and %llu engine records%s",
-                    (unsigned long long)len, (unsigned long long)R, (unsigned long long)E, rec ? " with recency" : "");
     if (hd.block_size != x->tv.block_size || hd.init_hash != x->tv.init_hash || hd.pods_per_key != x->tv.pods_per_key)
         return fail(KVIDX_EINVAL, "snapshot of another configuration: block_size %u, init_hash %#llx, pods_per_key %u (this index: %u, %#llx, %u)",
                     hd.block_size, (unsigned long long)hd.init_hash, hd.pods_per_key, x->tv.block_size, (unsigned long long)x->tv.init_hash,
@@ -1988,6 +2129,7 @@ int kvidx_restore(kvidx_t* x, const void* buf, uint64_t len, uint64_t restored_o
     if (hd.model_span > 65536) return fail(KVIDX_EINVAL, "malformed snapshot image: model_span %u", hd.model_span);
     if (x->tv.req_stamp && !rec) return fail(KVIDX_EINVAL, "an exact-LRU index needs an image with recency (taken from an exact-LRU index)");
     std::lock_guard<std::mutex> g(x->mu_w);
+    x->rm_armed = false;
     CK(cudaSetDevice(x->device));
     std::shared_lock<std::shared_mutex> tl(x->tables);
     int rc = refresh_counters(x);
@@ -1996,12 +2138,76 @@ int kvidx_restore(kvidx_t* x, const void* buf, uint64_t len, uint64_t restored_o
         return fail(KVIDX_EINVAL, "restore needs an empty index: this one holds %llu request and %llu engine keys",
                     x->h_cnt->req_full, x->h_cnt->eng_full);
     const uint64_t rs = x->tv.req_mask + 1, es = x->tv.eng_mask + 1;
-    if (R * 10 > rs * 9 || E * 10 > es * 9)          // the write path's limit: at most 90 % of a table's slots live
+    if (!x->tv.shard_bits && (R * 10 > rs * 9 || E * 10 > es * 9))          // the write path's limit: at most 90 % of a table's slots live
         return fail(KVIDX_ENOSPC, "table full: %llu request / %llu engine keys in %llu / %llu slots", (unsigned long long)R,
                     (unsigned long long)E, (unsigned long long)rs, (unsigned long long)es);
     rc = restore_impl(x, static_cast<const uint8_t*>(buf) + kSnapHeaderBytes, hd, restored_out);
     release_snap(x);
     return rc;
+}
+}  // namespace
+
+extern "C" {
+
+int kvidx_snapshot(kvidx_t* x, void* buf, uint64_t cap, uint64_t* size_out) {
+    if (size_out) *size_out = 0;
+    if (!x || !size_out) return fail(KVIDX_EINVAL, "bad arguments");
+    // a sharded handle's keys live in several processes' tables: kvidx_shard_snapshot + kvidx_snapshot_merge is the collective export
+    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_snapshot is not supported on a sharded index (kvidx_shard_snapshot is its collective form)");
+    return snapshot_call(x, buf, cap, size_out);
+}
+
+int kvidx_restore(kvidx_t* x, const void* buf, uint64_t len, uint64_t restored_out[2]) {
+    if (restored_out) restored_out[0] = restored_out[1] = 0;
+    if (!x || !buf) return fail(KVIDX_EINVAL, "bad arguments");
+    if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_restore is not supported on a sharded index (kvidx_shard_restore is its collective form)");
+    return restore_call(x, buf, len, restored_out);
+}
+
+int kvidx_shard_snapshot(kvidx_t* x, void* buf, uint64_t cap, uint64_t* size_out) {
+    if (size_out) *size_out = 0;
+    if (!x || !size_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return snapshot_call(x, buf, cap, size_out);
+}
+
+int kvidx_shard_restore(kvidx_t* x, const void* buf, uint64_t len, uint64_t restored_out[2]) {
+    if (restored_out) restored_out[0] = restored_out[1] = 0;
+    if (!x || !buf) return fail(KVIDX_EINVAL, "bad arguments");
+    return restore_call(x, buf, len, restored_out);
+}
+
+int kvidx_snapshot_merge(const void* const* parts, const uint64_t* lens, uint32_t n_parts, void* out, uint64_t cap, uint64_t* size_out) {
+    if (size_out) *size_out = 0;
+    if (!size_out || (n_parts && (!parts || !lens))) return fail(KVIDX_EINVAL, "bad arguments");
+    if (n_parts == 0) return fail(KVIDX_EINVAL, "no parts to merge");
+    std::vector<SnapHeader> hd(n_parts);
+    SnapHeader m{};
+    for (uint32_t p = 0; p < n_parts; ++p) {
+        if (!parts[p]) return fail(KVIDX_EINVAL, "part %u: NULL", p);
+        if (int rc = check_image_header(parts[p], lens[p], &hd[p])) {
+            const std::string why = g_err;
+            return fail(rc, "part %u: %s", p, why.c_str());
+        }
+        const SnapHeader& h = hd[p];
+        if (h.model_span > 65536) return fail(KVIDX_EINVAL, "part %u: malformed snapshot image: model_span %u", p, h.model_span);
+        if (h.flags & kSnapFlagRecency)
+            return fail(KVIDX_EINVAL, "part %u carries recency: parts come from sharded handles, which never track it", p);
+        if (p && (h.block_size != m.block_size || h.init_hash != m.init_hash || h.pods_per_key != m.pods_per_key))
+            return fail(KVIDX_EINVAL, "part %u is of another configuration: block_size %u, init_hash %#llx, pods_per_key %u (part 0: %u, %#llx, %u)",
+                        p, h.block_size, (unsigned long long)h.init_hash, h.pods_per_key, m.block_size, (unsigned long long)m.init_hash, m.pods_per_key);
+        if (!p) m = h;
+        else { m.n_request += h.n_request; m.n_engine += h.n_engine; }
+        m.pod_span = std::max(m.pod_span, h.pod_span);
+        m.model_span = std::max(m.model_span, h.model_span);
+    }
+    // every record is checked before anything is written: order inside each part, no key in two parts
+    if (int rc = merge_images(parts, hd, nullptr)) return rc;
+    const uint64_t size = kSnapHeaderBytes + 32 * m.n_request + 24 * m.n_engine;
+    *size_out = size;
+    if (!out || cap < size) return fail(KVIDX_ENOSPC, "the merged image needs %llu bytes, the buffer has %llu", (unsigned long long)size,
+                                        (unsigned long long)(out ? cap : 0));
+    memcpy(out, &m, sizeof m);
+    return merge_images(parts, hd, static_cast<uint8_t*>(out) + kSnapHeaderBytes);
 }
 
 int kvidx_shard_export(kvidx_t* x, void* out) {
@@ -2057,6 +2263,7 @@ int kvidx_shard_attach(kvidx_t* x, uint32_t rank, kvidx_t* other) {
 int kvidx_shard_compact(kvidx_t* x) {
     if (!x) return fail(KVIDX_EINVAL, "NULL handle");
     std::lock_guard<std::mutex> g(x->mu_w);
+    x->rm_armed = false;
     std::unique_lock<std::shared_mutex> tl(x->tables);
     CK(cudaSetDevice(x->device));
     return rebuild(x, x->tv.shard_bits != 0);

@@ -83,6 +83,10 @@ SYMBOLS = {
     "kvidx_shard_export": (C.c_int, [C.c_void_p, C.c_char_p]),
     "kvidx_shard_import": (C.c_int, [C.c_void_p, C.c_uint32, C.c_char_p]),
     "kvidx_shard_attach": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "kvidx_shard_remove_pods": (C.c_int, [C.c_void_p, _u64p, C.c_uint32, C.c_uint32, _u64p]),
+    "kvidx_shard_snapshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "kvidx_snapshot_merge": (C.c_int, [C.POINTER(C.c_char_p), _u64p, C.c_uint32, C.c_void_p, C.c_uint64, _u64p]),
+    "kvidx_shard_restore": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, _u64p]),
 }
 
 _lib = None
@@ -310,9 +314,8 @@ class Index:
                                        _p(tokens, _u32p), len(tokens), C.byref(nd))
         return rc, nd.value
 
-    def remove_pods(self, pod_ids, tier_ids=None) -> dict:
-        """kvidx_remove_pods: drop every entry of these pods (on these tiers; None = all).  No reference counterpart.
-        -> {"entries", "request_keys", "engine_keys"} removed; raises KvidxError on failure."""
+    def removal_masks(self, pod_ids, tier_ids=None):
+        """(pod mask words, tier mask) of a removal: tier_ids None = all tiers."""
         mask = np.zeros(self.filter_words, np.uint64)
         for p in pod_ids:
             p = int(p)
@@ -320,8 +323,22 @@ class Index:
                 raise KvidxError(ERANGE, "pod id %d outside 0..max_pods-1" % p)
             mask[p >> 6] |= np.uint64(1) << np.uint64(p & 63)
         tier_mask = 0xFFFF if tier_ids is None else sum(1 << (int(t) & 15) for t in set(tier_ids))
+        return mask, tier_mask
+
+    def remove_pods(self, pod_ids, tier_ids=None) -> dict:
+        """kvidx_remove_pods: drop every entry of these pods (on these tiers; None = all).  No reference counterpart.
+        -> {"entries", "request_keys", "engine_keys"} removed; raises KvidxError on failure."""
+        mask, tier_mask = self.removal_masks(pod_ids, tier_ids)
         out = np.zeros(3, np.uint64)
         self._ck(self.L.kvidx_remove_pods(self.h, _p(mask, _u64p), tier_mask, _p(out, _u64p)))
+        return {"entries": int(out[0]), "request_keys": int(out[1]), "engine_keys": int(out[2])}
+
+    def shard_remove_pods(self, pod_ids, tier_ids=None, *, phase: int) -> dict:
+        """kvidx_shard_remove_pods: one phase (0, then 1 once every rank has run 0) of the collective removal on a sharded
+        index (kvidx.dist.remove_pods_shards runs both with the barriers).  -> this rank's counters of the phase."""
+        mask, tier_mask = self.removal_masks(pod_ids, tier_ids)
+        out = np.zeros(3, np.uint64)
+        self._ck(self.L.kvidx_shard_remove_pods(self.h, _p(mask, _u64p), tier_mask, phase, _p(out, _u64p)))
         return {"entries": int(out[0]), "request_keys": int(out[1]), "engine_keys": int(out[2])}
 
     # -- snapshot / restore (no reference counterpart; format v1 in include/kvidx.h) --
@@ -346,6 +363,44 @@ class Index:
         out = np.zeros(2, np.uint64)
         self._ck(self.L.kvidx_restore(self.h, image, len(image), _p(out, _u64p)))
         return {"request_keys": int(out[0]), "engine_keys": int(out[1])}
+
+    def shard_snapshot(self) -> bytes:
+        """kvidx_shard_snapshot: the image of the keys and mappings this shard owns (a part for snapshot_merge)."""
+        while True:
+            st = self.stats()
+            size = 64 + 32 * st["request_keys"] + 24 * st["engine_keys"]
+            buf = bytearray(size)
+            got = C.c_uint64(0)
+            rc = self.L.kvidx_shard_snapshot(self.h, (C.c_char * size).from_buffer(buf), size, C.byref(got))
+            if rc == ENOSPC and got.value > size:          # a peer added keys to this shard since stats(): size again
+                continue
+            self._ck(rc)
+            return bytes(memoryview(buf)[:got.value])
+
+    def shard_restore(self, image) -> dict:
+        """kvidx_shard_restore: insert the records of any v1 image that this shard owns (the handle must hold no live key).
+        -> {"request_keys", "engine_keys"} resident in this shard afterwards."""
+        image = image if isinstance(image, bytes) else bytes(image)
+        out = np.zeros(2, np.uint64)
+        self._ck(self.L.kvidx_shard_restore(self.h, image, len(image), _p(out, _u64p)))
+        return {"request_keys": int(out[0]), "engine_keys": int(out[1])}
+
+
+def snapshot_merge(parts) -> bytes:
+    """kvidx_snapshot_merge: the canonical image of the union of shard images (disjoint shards).  Host only."""
+    L = load()
+    parts = [p if isinstance(p, bytes) else bytes(p) for p in parts]
+    ptrs = (C.c_char_p * max(len(parts), 1))(*parts)
+    lens = np.array([len(p) for p in parts] or [0], np.uint64)
+    size = C.c_uint64(0)
+    rc = L.kvidx_snapshot_merge(ptrs, _p(lens, _u64p), len(parts), None, 0, C.byref(size))
+    if rc != ENOSPC:
+        raise KvidxError(rc, L.kvidx_last_error(None).decode())
+    buf = bytearray(size.value)
+    rc = L.kvidx_snapshot_merge(ptrs, _p(lens, _u64p), len(parts), (C.c_char * len(buf)).from_buffer(buf), len(buf), C.byref(size))
+    if rc:
+        raise KvidxError(rc, L.kvidx_last_error(None).decode())
+    return bytes(buf)
 
 
 class _Raw:

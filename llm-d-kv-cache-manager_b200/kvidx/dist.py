@@ -4,6 +4,8 @@ The Score() path shards by prompt: every rank holds a full replica of the index 
 scores its own contiguous slice of the batch, and no data-path collective is needed.  What has to be replicated is
 the write path: every rank must apply the same KV events, in the same per-pod order.  `broadcast_event_batch` does
 that from the ingesting rank; `shard_range` splits a batch; `max_over_ranks` is the timing reduction bench.py uses.
+The hash-range sharded mode has its own helpers: `connect_shards`, and the collective maintenance calls
+`compact_shards`, `remove_pods_shards`, `snapshot_shards` and `restore_shards`, which put the barriers around them.
 """
 from __future__ import annotations
 
@@ -155,3 +157,105 @@ def score_alltoall(ix, d_tok, d_off, n, d_scores, block_size=16, model0=0, d_has
     slots_pm[order] = back
     ix.score_slots_dev(slots_pm.data_ptr(), koff.data_ptr(), n, d_scores.data_ptr(), d_has_keys=(d_has.data_ptr() if d_has is not None else 0))
     return {"keys": nk, "bytes_out": 8 * (nk - in_split[dist.get_rank()]), "bytes_back": 32 * (nk - in_split[dist.get_rank()])}
+
+
+# ---- maintenance of a sharded index: pod removal, snapshot, restore (collective; every rank calls them) ---------------
+
+def _all_ok(ok: bool, device=None) -> bool:
+    """True on every rank iff `ok` on every rank.  The all-reduce also keeps every rank here until all have arrived."""
+    t = torch.tensor([1 if ok else 0], dtype=torch.int64, device=device)
+    dist.all_reduce(t, op=dist.ReduceOp.MIN)
+    return bool(t.item())
+
+
+def _sum_over_ranks(values, device=None):
+    t = torch.tensor([int(v) for v in values], dtype=torch.int64, device=device)
+    dist.all_reduce(t)
+    return [int(v) for v in t.tolist()]
+
+
+def _collective_step(fn, what: str, device=None):
+    """Run this rank's part of a collective call; raise on every rank if it failed on any (this rank's own error first)."""
+    res, err = None, None
+    try:
+        res = fn()
+    except Exception as e:      # noqa: BLE001  (re-raised below, after the other ranks have heard of it)
+        err = e
+    if not _all_ok(err is None, device):
+        if err is not None:
+            raise err
+        raise RuntimeError("%s failed on another rank" % what)
+    return res
+
+
+def remove_pods_shards(ix, pod_ids, tier_ids=None, device=None) -> dict:
+    """kvidx_remove_pods over a hash-range sharded index: every rank removes the entries of its request shard (phase 0),
+    then, once all have, the engine mappings of its engine shard whose request key phase 0 removed on any rank (phase 1).
+    Every rank must pass the same pods and tiers; that is checked first (an all-gather of the masks).  No rank may write
+    to the index during the call; readers may run.  -> the summed {"entries", "request_keys", "engine_keys"}."""
+    mask, tier_mask = ix.removal_masks(pod_ids, tier_ids)
+    mine = torch.from_numpy(np.append(mask, np.uint64(tier_mask)).view(np.int64).copy())
+    if device is not None:
+        mine = mine.to(device)
+    parts = [torch.empty_like(mine) for _ in range(dist.get_world_size())]
+    dist.all_gather(parts, mine)
+    if any(not torch.equal(p, parts[0]) for p in parts):
+        raise ValueError("remove_pods_shards: the ranks were given different pod / tier sets")
+    dist.barrier()
+    r0 = _collective_step(lambda: ix.shard_remove_pods(pod_ids, tier_ids, phase=0), "phase 0 of the removal", device)
+    r1 = _collective_step(lambda: ix.shard_remove_pods(pod_ids, tier_ids, phase=1), "phase 1 of the removal", device)
+    tot = _sum_over_ranks([r0["entries"], r0["request_keys"], r1["engine_keys"]], device)
+    return {"entries": tot[0], "request_keys": tot[1], "engine_keys": tot[2]}
+
+
+def snapshot_shards(ix, dst: int = 0, device=None):
+    """The canonical image of the whole sharded index (what kvidx_snapshot gives on an unsharded index with the same
+    contents): every rank exports the keys it owns, the parts are gathered to `dst` and merged there.  No rank may write
+    to the index during the call.  -> the image on `dst`, None elsewhere."""
+    dist.barrier()
+    part = _collective_step(ix.shard_snapshot, "the shard snapshot", device)
+    world = dist.get_world_size()
+    sizes = [torch.zeros(1, dtype=torch.int64, device=device) for _ in range(world)]
+    dist.all_gather(sizes, torch.tensor([len(part)], dtype=torch.int64, device=device))
+    sizes = [int(s.item()) for s in sizes]
+    buf = torch.zeros(max(sizes), dtype=torch.uint8)
+    buf[: len(part)] = torch.frombuffer(bytearray(part), dtype=torch.uint8)
+    if device is not None:
+        buf = buf.to(device)
+    gathered = [torch.empty_like(buf) for _ in range(world)] if dist.get_rank() == dst else None
+    dist.gather(buf, gathered, dst=dst)
+    if dist.get_rank() != dst:
+        return None
+    from . import _native
+    return _native.snapshot_merge([g.cpu().numpy().tobytes()[:n] for g, n in zip(gathered, sizes)])
+
+
+def restore_shards(ix, image=None, src: int = 0, device=None) -> dict:
+    """Load a v1 image (unsharded, merged or a single part) into an empty sharded index: each rank inserts the records it
+    owns, so this also reshards (1 -> N, N -> M).  The image is broadcast from `src` unless every rank has it.  Raises on
+    every rank unless every shard is empty, and on every rank if any rank's restore fails (a malformed image or one too
+    large for an owner is refused by all before any inserts).  -> the summed {"request_keys", "engine_keys"} restored."""
+    have = _all_ok(image is not None, device)
+    if not have:
+        if dist.get_rank() == src:
+            if image is None:
+                raise ValueError("restore_shards: rank %d holds no image" % src)
+            payload = torch.frombuffer(bytearray(image), dtype=torch.uint8)
+            n = torch.tensor([len(image)], dtype=torch.int64, device=device)
+        else:
+            n = torch.zeros(1, dtype=torch.int64, device=device)
+        dist.broadcast(n, src)
+        if dist.get_rank() != src:
+            payload = torch.empty(int(n.item()), dtype=torch.uint8)
+        if device is not None:
+            payload = payload.to(device)
+        dist.broadcast(payload, src)
+        image = payload.cpu().numpy().tobytes()
+    st = ix.stats()
+    live = _sum_over_ranks([st["request_keys"], st["engine_keys"]], device)
+    if any(live):
+        raise RuntimeError("restore_shards needs an empty index: the shards hold %d request and %d engine keys" % tuple(live))
+    dist.barrier()
+    got = _collective_step(lambda: ix.shard_restore(image), "the shard restore", device)
+    tot = _sum_over_ranks([got["request_keys"], got["engine_keys"]], device)
+    return {"request_keys": tot[0], "engine_keys": tot[1]}
