@@ -28,13 +28,9 @@
 namespace kvx {
 
 constexpr int kRoundBlocks = 32;         // blocks hashed per prompt per round (== lanes per warp in kernel P)
-#ifndef KVIDX_HASH_STAGES
-#define KVIDX_HASH_STAGES 2
-#define KVIDX_HASH_THREADS 256
-#endif
-constexpr int kHashThreads = KVIDX_HASH_THREADS;
-constexpr int kHashStages = KVIDX_HASH_STAGES;   // token blocks staged per prompt.  (4 stages x 4 warps is the alternative: what a launch of this kernel
-                                         // waits for is room on an SM beside kernel G's CTAs, so the smaller footprint per warp is the choice; scripts/ab_step.py compares them)
+constexpr int kHashThreads = 256;
+constexpr int kHashStages = 2;           // token blocks staged per prompt.  (4 stages x 4 warps is the alternative: what a launch of this kernel
+                                         // waits for is room on an SM beside kernel G's CTAs, so the smaller footprint per warp is the choice)
 constexpr int kGroupThreads = 256;
 constexpr uint32_t kRoleSelf = 0xffffffffu;
 
@@ -124,38 +120,20 @@ __device__ __forceinline__ void chunk_load(const uint32_t* sp, int nw, int lane,
     }
 }
 
-#ifndef KVIDX_GROUP_TILE
-#define KVIDX_GROUP_TILE 32
-#endif
-constexpr int kGroupTile = KVIDX_GROUP_TILE;   // live prompts a warp of kernel G takes at a time (their chunks stream through the warp one after the other)
-#ifndef KVIDX_GROUP_RING
-#define KVIDX_GROUP_RING 4
-#endif
-constexpr int kGroupRing = KVIDX_GROUP_RING;            // chunk slots per warp: one being examined, two in flight, the anchor (deeper rings cost occupancy)
+constexpr int kGroupTile = 32;           // live prompts a warp of kernel G takes at a time (their chunks stream through the warp one after the other)
+constexpr int kGroupRing = 4;            // chunk slots per warp: one being examined, two in flight, the anchor (deeper rings cost occupancy)
 struct GroupSmem {
     uint4 ring[kGroupThreads / 32][kGroupRing][4][32];                       // 64 KB
-    unsigned long long bar[kGroupThreads / 32][kGroupRing];                  // TMA variant: one mbarrier per rotating slot
 };
 
-// TMA = true: a chunk (<= 2 KB, contiguous, 16-byte aligned) is ONE cp.async.bulk issued by an elected lane onto the slot's
-// mbarrier (UBLKCP in SASS) instead of four 16-byte cp.async per lane (LDGSTS); chunks that do not start on a 16-byte
-// boundary are copied with plain loads in both variants.
-template <int BS, bool TMA>
-__global__ void __launch_bounds__(kGroupThreads, kGroupRing <= 4 ? 3 : 2)
+template <int BS>
+__global__ void __launch_bounds__(kGroupThreads, 3)
 group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round, const int dedup) {
     static_assert(BS == 16 && kRoundBlocks == 32, "a chunk is 4 x 32 lanes x 16 bytes");
     extern __shared__ __align__(128) unsigned char smem_raw_g[];
     uint4 (*ring)[4][32] = reinterpret_cast<GroupSmem*>(smem_raw_g)->ring[threadIdx.x >> 5];
-    unsigned long long* bar = reinterpret_cast<GroupSmem*>(smem_raw_g)->bar[threadIdx.x >> 5];
     const int lane = threadIdx.x & 31;
-    uint32_t tma_pending = 0, tma_phase = 0;          // per rotating slot: a bulk copy is in flight / parity of its next wait
     const uint64_t l2pol = l2_policy_stream();
-    if (TMA) {
-        if (lane == 0) for (int s = 0; s < kGroupRing - 1; ++s) mbar_init(&bar[s], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        fence_proxy_async();
-        __syncwarp();
-    }
     const unsigned int n_act = rb.n_act[cur];
     if (blockIdx.x == 0 && threadIdx.x == 0) { rb.n_act[cur ^ 1] = 0; rb.n_hl[0] = 0; rb.n_hl[1] = 0; rb.n_hl[2] = 0; rb.n_hl[3] = 0; }   // lists built below / by G2
     const unsigned int total_warps = gridDim.x * (kGroupThreads / 32);
@@ -200,23 +178,17 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
                 const uint32_t* sp = reinterpret_cast<const uint32_t*>(__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)tp, qi));
                 const int nw = __shfl_sync(0xffffffffu, nb, qi) * BS;
                 const bool al = (reinterpret_cast<uintptr_t>(sp) & 15u) == 0;
-                if (TMA && al) {
-                    __syncwarp();                              // every lane has taken the slot's previous chunk into registers
-                    if (lane == 0) { fence_proxy_async(); mbar_expect_tx(&bar[slot], (uint32_t)nw * 4u); tma_load_1d(&ring[slot][0][0], sp, (uint32_t)nw * 4u, &bar[slot]); }
-                    tma_pending |= 1u << slot;
-                }
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
                     const int w0 = (c * 32 + lane) * 4;
                     uint4* dst = &ring[slot][c][lane];
                     if (w0 < nw) {
-                        if (TMA && al) {}
-                        else if (al) cp_async_16_stream(smem_addr(dst), sp + w0, l2pol);
+                        if (al) cp_async_16_stream(smem_addr(dst), sp + w0, l2pol);
                         else *dst = make_uint4(__ldg(sp + w0), __ldg(sp + w0 + 1), __ldg(sp + w0 + 2), __ldg(sp + w0 + 3));
                     } else *dst = make_uint4(0, 0, 0, 0);
                 }
             }
-            if (!TMA) cp_async_commit();
+            cp_async_commit();
         };
         constexpr int RS = kGroupRing - 1;            // rotating slots; slot RS holds the anchor
         constexpr int PD = RS - 1;                    // chunks in flight
@@ -237,11 +209,7 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
                 pend &= pend - 1;
                 issue(issued % RS, qi); ++issued;
             }
-            if (TMA) {
-                const int s_ = ord % RS;
-                if ((tma_pending >> s_) & 1u) { mbar_wait(&bar[s_], (tma_phase >> s_) & 1u); tma_phase ^= 1u << s_; tma_pending &= ~(1u << s_); }
-                __syncwarp();                                  // plain-store chunks (unaligned starts, zero tails) are visible too
-            } else cp_async_wait<PD>();
+            cp_async_wait<PD>();
             uint4 v[4];
 #pragma unroll
             for (int c = 0; c < 4; ++c) v[c] = ring[ord % RS][c][lane];
@@ -299,7 +267,7 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
             }
             ++ord;
         }
-        if (!TMA) cp_async_wait<0>();
+        cp_async_wait<0>();
         // election among the prompts that are not members of an anchor's class
         uint32_t cand = kRoleSelf;
         if (cls && !eqanch) {
@@ -461,7 +429,7 @@ group_lists_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
 // ---- kernel H ---------------------------------------------------------------------------------
 template <int BS>
 __global__ void __launch_bounds__(kHashThreads, 3)
-hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round, const int prefetch) {
+hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round) {
     static_assert(BS == 16, "staging pattern is written for 16-token blocks");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     using SM = HashSmem<BS>;
@@ -495,16 +463,6 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
             h = round == 0 ? t.init_hash : rb.hstate[p];
         }
         const int nb_max = __reduce_max_sync(0xffffffffu, nb);
-        // The chain below consumes one 64-byte block per prompt per FNV block hash and stages only one block ahead: pull the whole
-        // chunk (<= 2 KB per prompt) towards L2 now, so that the staging copies find it there instead of paying a loaded DRAM
-        // round trip per block.
-        if (prefetch && have) {
-            const char* pb = reinterpret_cast<const char*>(src);
-            for (int o = 128; o < nb * BS * 4; o += 128) {
-                if (prefetch == 2) asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(pb + o));
-                else asm volatile("prefetch.global.L2 [%0];" ::"l"(pb + o));
-            }
-        }
         // stage chunk c (kHashChunk blocks) of every lane's prompt: 4*kHashChunk lanes move one prompt's contiguous bytes.
         auto stage = [&](int s, int c) {
             const int b0 = c * kHashChunk;
@@ -845,10 +803,7 @@ __device__ __forceinline__ uint64_t hash_block16(uint64_t parent, const uint32_t
     }
     return f.end_block();
 }
-#ifndef KVIDX_DETACH_BLOCKS
-#define KVIDX_DETACH_BLOCKS 3
-#endif
-constexpr int kDetachBlocks = KVIDX_DETACH_BLOCKS;          // blocks a partial follower walks alone inside the round before it is re-queued
+constexpr int kDetachBlocks = 3;         // blocks a partial follower walks alone inside the round before it is re-queued
 struct DetachWarp { double sc[kMaxEnt][32]; uint16_t pod[kMaxEnt][32]; };     // per warp (dynamic shared memory: warps of the CTA x this)
 template <int BS>
 __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs& a, const RoundBufs& rb, const int cur, const int round, const int trace, DetachWarp* smw,
@@ -1038,8 +993,7 @@ __global__ void count_distinct_prefixes_kernel(const uint64_t* __restrict__ fp_s
 
 inline int rounds_init() {
     if (cudaFuncSetAttribute(hash_round_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(group_round_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(group_round_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(group_round_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GroupSmem)) != cudaSuccess) return -1;
     return 0;
 }
 

@@ -18,25 +18,12 @@
 #pragma once
 #include <cuda_runtime.h>
 #include "kernels_score.cuh"
-#include "kernels_rounds.cuh"      // ld_slot_pair, ent_of
+#include "kernels_rounds.cuh"      // PromptState, HashSmem, rounds_init_kernel, ld_slot_pair, ent_of
 
 namespace kvx {
 namespace plain {
 
-constexpr int kRoundBlocks = 32;         // blocks hashed per prompt per round (== lanes per warp in kernel P)
-constexpr int kHashThreads = 256;
 constexpr int kProbeThreads = 256;
-
-struct __align__(8) PromptState {        // walk state carried between rounds (only for prompts that continue)
-    double sc[kMaxEnt];
-    uint16_t pod[kMaxEnt];
-    uint32_t pat[6];                     // entry words + count of the last scored block's slot
-    uint16_t alive;                      // bitmask over [0,k)
-    uint8_t k;
-    uint8_t pad;
-    uint8_t bt[kMaxEnt];                 // tier giving pod q its max weight in that slot (0xff: 0.0)
-    uint8_t pad2[2];
-};
 
 struct RoundBufs {
     uint32_t* act[2];                    // active prompt lists (ping-pong)
@@ -46,18 +33,6 @@ struct RoundBufs {
                                          // block j of list slot i at keys[j * n_prompts + i] (coalesced both ways)
     uint32_t* nbr;                       // [n_act] per list slot: blocks hashed this round | (more blocks follow) << 8
     PromptState* pst;                    // per prompt
-    // Speculative schedule (small batches, latency bound): kernel H of round t+1 runs BESIDE kernel P of round t.  It cannot
-    // know yet which prompts survive round t, so it hashes the next 32 blocks of every prompt of round t's list; P of round
-    // t+1 then finds its prompts' keys through prev[] (slot in the list H ran over).  keys / nbr alternate between two buffers.
-    uint32_t* prev[2];                   // [n_act] per slot of act[x]: the prompt's slot in the previous round's list
-    int spec;
-};
-
-constexpr int kHashChunk = 1;            // blocks staged per copy step (2 = 128-byte accesses: fewer, longer DRAM accesses
-                                         // but only 24 resident warps/SM, and the kernel is pipe bound)
-template <int BS> struct HashSmem {
-    static constexpr int kRow = kHashChunk * BS * 4 + 16;   // 144 B: the four LDS.128 of a block stay conflict free
-    unsigned char tok[kHashThreads / 32][2][32 * kRow];
 };
 
 // ---- kernel H ---------------------------------------------------------------------------------
@@ -66,10 +41,11 @@ template <int BS> struct HashSmem {
 // NS: token blocks staged per prompt (NS - 1 copies in flight ahead of the chain).  With 2 a launch lasts 32 x max(FNV of a block,
 // one loaded DRAM round trip) -- fine when the list fills the machine, the floor of the round when it does not: the
 // warp-per-prompt configuration stages 3 and runs 128-thread CTAs (55 KB each, four per SM).
-template <int BS, bool PM, int NS>
+template <int BS, bool PM>
 __global__ void __launch_bounds__(kHashThreads, 4)
 hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round) {
     static_assert(BS == 16, "staging pattern is written for 16-token blocks");
+    constexpr int NS = PM ? 3 : 2;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     using SM = HashSmem<BS>;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -77,15 +53,13 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
     const uint32_t wbase = smem_addr(wtok);         // 32-bit shared-window address of the warp's stages
     const uint64_t l2pol = l2_policy_stream();      // created once, in uniform control flow (a policy built inside the divergent
                                                     // staging branch made ptxas 12.9 emit an LDGSTS with an unset descriptor: illegal instruction)
-    // the list this kernel works on: the round's own list, or (speculative schedule) the list of the round before
-    const int src = rb.spec ? (round == 0 ? 0 : ((round - 1) & 1)) : cur;
-    const unsigned int n_act = rb.n_act[src];
-    if (!rb.spec && blockIdx.x == 0 && threadIdx.x == 0) rb.n_act[cur ^ 1] = 0;      // next round's list starts empty
+    const unsigned int n_act = rb.n_act[cur];
+    if (blockIdx.x == 0 && threadIdx.x == 0) rb.n_act[cur ^ 1] = 0;      // next round's list starts empty
     const unsigned int total_warps = gridDim.x * (blockDim.x / 32);
     for (unsigned int w = blockIdx.x * (blockDim.x / 32) + wid; w * 32u < n_act; w += total_warps) {
         const unsigned int i = w * 32u + lane;                            // slot in the active list
         const bool have = i < n_act;
-        const uint32_t p = have ? rb.act[src][i] : 0u;
+        const uint32_t p = have ? rb.act[cur][i] : 0u;
         int nb = 0;                                                      // blocks of this prompt in this round
         const uint32_t* src = nullptr;
         bool aligned = true;
@@ -188,8 +162,7 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         const unsigned int i = w * 32u + lane;
         const bool have = i < n_act;
         const uint32_t p = have ? rb.act[cur][i] : 0u;
-        const unsigned int ks = (have && rb.spec && round > 0) ? rb.prev[cur][i] : i;      // slot the keys of this prompt were written at
-        const uint32_t meta = have ? rb.nbr[ks] : 0u;
+        const uint32_t meta = have ? rb.nbr[i] : 0u;
         const int nb = (int)(meta & 63u);
         const bool has_more = (meta >> 8) & 1u;
         const uint32_t mdl = (have && a.model) ? a.model[p] : a.model0;
@@ -213,12 +186,12 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         const ReqSlot* base = t.req;                           // table (shard) of the current block's key
         uint4 A0 = {0, 0, 0, 0}, B0 = {0, 0, 0, 0}, A1 = {0, 0, 0, 0}, B1 = {0, 0, 0, 0};
         if (!done) {
-            key = rb.keys[ks];
+            key = rb.keys[i];
             const uint64_t hm = home_of(key, mdl);
             base = t.req_peer[shard_of(hm, t.shard_bits)]; slot = hm & t.req_mask & ~1ull;
             ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
         }
-        uint64_t key1 = (!done && nb > 1) ? rb.keys[kstride + ks] : 0ull;                        // key of block j+1
+        uint64_t key1 = (!done && nb > 1) ? rb.keys[kstride + i] : 0ull;                        // key of block j+1
         for (int j = 0; j < nb_max; ++j) {
             // next block's pair is requested before this block is scored; keys are read one iteration ahead of their use
             uint64_t nkey = key1, nslot = 0;
@@ -230,7 +203,7 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
                 nbase = t.req_peer[shard_of(hm, t.shard_bits)]; nslot = hm & t.req_mask & ~1ull;
                 ld_slot_pair(nbase + nslot, peer, nA0, nB0, nA1, nB1);
             }
-            key1 = (!done && j + 2 < nb) ? rb.keys[(size_t)(j + 2) * kstride + ks] : 0ull;
+            key1 = (!done && j + 2 < nb) ? rb.keys[(size_t)(j + 2) * kstride + i] : 0ull;
             if (!done && j < nb) {
                 uint4 A = A0, B = B0;
                 bool hit = slot_matches(A, B, key, mdl);
@@ -303,7 +276,6 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
             if (more) {
                 const unsigned int ns = base + __popc(mm & ((1u << lane) - 1u));
                 rb.act[cur ^ 1][ns] = p;
-                if (rb.spec) rb.prev[cur ^ 1][ns] = i;
                 PromptState& ps = rb.pst[p];
                 ps.k = (uint8_t)k; ps.alive = (uint16_t)alive;
                 ps.pat[0] = pv0; ps.pat[1] = pv1; ps.pat[2] = pv2; ps.pat[3] = pv3; ps.pat[4] = pv4; ps.pat[5] = pvc;
@@ -503,41 +475,9 @@ probe_round_warp_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb
     }
 }
 
-// List setup + a 64-bit fingerprint of every prompt's first block.  The batch is then radix-sorted by fingerprint so
-// that prompts sharing a prefix sit in neighbouring lanes: their probes are the same 64-byte segments, which the
-// load unit merges within a warp and L2 serves across warps.  (Any order gives the same results; this one lets the
-// prefix sharing the system exists for -- system prompts, shared documents -- show up as memory locality.)
-__global__ void rounds_init_kernel(const ScoreArgs a, uint32_t block_size, unsigned long long* max_blocks, uint64_t* fp, uint32_t* idx,
-                                   unsigned int* n_act, unsigned int n_first) {
-    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    unsigned long long nb = 0;
-    if (i < a.n_prompts) {
-        const int64_t b = a.tok_off[i] - a.tok_base, e = a.tok_off[i + 1] - a.tok_base;
-        nb = (unsigned long long)((e - b) / block_size);
-        uint64_t f = ~0ull;                                   // prompts without a full block sort last
-        if (nb > 0) {
-            f = 0x9E3779B97F4A7C15ull;
-            const uint32_t* tk = a.tok + b;
-            // (independent mixes of token pairs, not a chain: this kernel is one thread per prompt and latency bound)
-            const uint32_t nt = block_size < 16u ? block_size : 16u;
-            uint64_t g = 0;
-            for (uint32_t j = 0; j + 1 < nt; j += 2) g ^= mix64(((uint64_t)__ldg(tk + j + 1) << 32 | __ldg(tk + j)) + 0xC2B2AE3D27D4EB4Full * (j + 1));
-            if (nt & 1u) g ^= mix64(__ldg(tk + nt - 1) + 0x165667B19E3779F9ull);
-            f = mix64(f ^ g);
-            f &= ~(1ull << 63);
-        }
-        fp[i] = f; idx[i] = (uint32_t)i;
-    }
-    nb = __reduce_max_sync(0xffffffffu, (unsigned)min(nb, 0xffffffffull));
-    if ((threadIdx.x & 31) == 0 && nb) atomicMax(max_blocks, nb);
-    if (i == 0) { n_act[0] = n_first; n_act[1] = 0; n_act[2] = (unsigned int)a.n_prompts - n_first; n_act[3] = 0; }
-}
-
 inline int rounds_init() {
-    if (cudaFuncSetAttribute(hash_round_kernel<16, false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(hash_round_kernel<16, true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(hash_round_kernel<16, true, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(hash_round_kernel<16, false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(hash_round_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(hash_round_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
     if (cudaFuncSetAttribute(probe_round_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem)) != cudaSuccess) return -1;
     return 0;
 }

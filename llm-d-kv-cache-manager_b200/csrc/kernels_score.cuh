@@ -26,7 +26,6 @@
 //     reused and scoring is one DADD per live pod; at retirement the whole warp writes the dense row.
 #pragma once
 #include <cuda_runtime.h>
-#include <cstdlib>
 #include "kernels_v1.cuh"
 
 #ifndef KVX_ABLATE
@@ -371,27 +370,15 @@ inline int score_tuned_init() {
     return 0;
 }
 
-inline int score_ctas_per_sm() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("KVIDX_SCORE_CTAS_PER_SM"); v = e ? atoi(e) : kScoreCtasPerSm; if (v < 1 || v > kScoreCtasPerSm) v = kScoreCtasPerSm; }
-    return v;
-}
-
 inline int launch_score_tuned(const TableView& t, int sm_count, const uint32_t* d_tok, const int64_t* d_off, int64_t tok_base, int64_t n,
                               const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, double* dense, uint16_t* sp_pods,
                               double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys, unsigned long long* d_next, cudaStream_t st,
                               uint64_t* launches) {
-    if (t.block_size != 16) {
-        const int T = 128;
-        score_kernel_v1<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(t, d_tok, d_off, tok_base, n, d_model, model0, d_filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
-        *launches += 1;
-        return cudaGetLastError() == cudaSuccess ? 0 : -1;
-    }
     if (cudaMemsetAsync(d_next, 0, sizeof(unsigned long long), st) != cudaSuccess) return -1;
     ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, dense, sp_pods, sp_scores, sp_cnt, has_keys, d_next};
     const int64_t lanes_per_cta = kScoreThreads;
     int64_t ctas = (n + lanes_per_cta - 1) / lanes_per_cta;
-    const int64_t max_ctas = (int64_t)sm_count * score_ctas_per_sm();
+    const int64_t max_ctas = (int64_t)sm_count * kScoreCtasPerSm;
     if (ctas > max_ctas) ctas = max_ctas;
     score_kernel_tuned<16><<<(unsigned)ctas, kScoreThreads, sizeof(ScoreSmem<16>), st>>>(t, a);
     *launches += 1;

@@ -154,11 +154,7 @@ struct kvidx {
     int score_path = 0;            // 0 = by batch size, 1 = always the fused persistent kernel, 2 / 3 = always the plain / class round pipeline,
                                    // 4 = always the warp-per-prompt cooperative kernel
     int64_t coop_max = 2048;       // batches up to this many prompts use the warp-per-prompt cooperative kernel
-    int rounds_spec = 0;           // per-prompt rounds: run hash(t+1) beside walk(t) for small batches (off by default)
-    int64_t rounds_spec_max = 131072;
-    cudaEvent_t ev_spec_h[2][2] = {}, ev_spec_p[2][2] = {};
     int64_t zerocopy_max = 32;     // host-buffer calls up to this many prompts skip the copy engine (tokens read from pinned host memory)
-    int group_tma = 0;             // class pipeline: token chunks by TMA bulk copy instead of cp.async (off by default)
     struct SubmitQueue* queue = nullptr;   // coalesces concurrent host-buffer Score() callers (submit.cuh)
     // Batch-size thresholds, from a sweep of the forced paths on an H100 SXM (10 M-block index, bench.py's query mix): the
     // warp-per-prompt rounds beat the cooperative kernel from 4096 prompts (tie at 2048) and the fused kernel at every size
@@ -176,17 +172,10 @@ struct kvidx {
     int rounds_overlap = 1;        // run the two halves of a large batch on two streams
     int64_t rounds_overlap_min = 65536;
     cudaStream_t aux_stream[kMaxParts - 1] = {}; cudaEvent_t ev_fork = nullptr, ev_join[kMaxParts - 1] = {};
-    // group_serial: every part's kernel G runs on ONE stream, one after the other at full bandwidth, while the other parts'
-    // latency-bound kernels (G2, H, P, R) run beside it on their own streams (otherwise the parts drift into lock step: all in
-    // G sharing the bandwidth, then all in the short kernels with DRAM idle -- scripts/timeline.py)
-    int group_serial = 2, group_serial_grid = 2;
-    int rounds_lane_stages = 2; int64_t rounds_lane_stages_max = 1 << 30;      // lane-per-prompt rounds: stages of kernel H (experiment knob)
-    int rounds_warp = 1, rounds_warp_stages = 3; int64_t rounds_warp_max = 131072;      // per-prompt rounds: kernel P warp per prompt up to this many prompts
+    int rounds_warp = 1; int64_t rounds_warp_max = 131072;      // per-prompt rounds: kernel P warp per prompt up to this many prompts
                                    // (faster than the lane-per-prompt kernel P at every size swept up to 131 072)
-    int group_ctas = 0;            // > 0: CTAs of one part's kernel G (all parts' G CTAs resident at once: nothing queues behind them)
-    int hash_prefetch = 0;         // kernel H pulls its chunks towards L2 before the chain starts (1; 2: evict_last)
-    int small_cta = 256;           // threads per CTA of the short kernels (G2, H, P, R): small CTAs fit into what kernel G's CTAs leave of an SM
-    cudaStream_t g_stream = nullptr, hp_stream[kMaxParts] = {}, lp_stream[kMaxParts] = {}; cudaEvent_t ev_g[kMaxParts] = {}, ev_r[kMaxParts] = {};
+    // multi-part class pipeline: a part's kernel G on a low-priority stream, its short kernels (G2, H, P, R) on a high-priority one
+    cudaStream_t hp_stream[kMaxParts] = {}, lp_stream[kMaxParts] = {}; cudaEvent_t ev_g[kMaxParts] = {}, ev_r[kMaxParts] = {};
 };
 
 namespace {
@@ -347,6 +336,33 @@ int launch_score_rounds_plain(kvidx* x, const uint32_t* d_tok, const int64_t* d_
                               const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, const ScoreOut& o, cudaStream_t st,
                               int64_t max_blocks);
 
+// Batch setup of both round pipelines: clear the counters in r_cnt (part q's list lengths at word 8 * q, the batch's largest
+// block count and the distinct-prefix count as two 64-bit words at word 8 * kMaxParts), fingerprint every prompt's first
+// block and set the parts' first list lengths (rounds_init_kernel), and with sort_prefix order the batch by fingerprint into
+// r_act0.  *fp_sorted (if not null): the sorted fingerprints.
+int rounds_setup(kvidx* x, const ScoreArgs& a, const PartSizes& ps, cudaStream_t st, const uint64_t** fp_sorted) {
+    const int64_t n = a.n_prompts;
+    unsigned int* cnt = x->r_cnt.as<unsigned int>();
+    CK(cudaMemsetAsync(cnt, 0, 1024, st));
+    CK(x->r_fp.need((size_t)n * 8 * 2 + (size_t)n * 4));
+    uint64_t* fp_in = x->r_fp.as<uint64_t>(); uint64_t* fp_out = fp_in + n;
+    uint32_t* idx_in = reinterpret_cast<uint32_t*>(fp_out + n);
+    uint32_t* act0 = x->r_act0.as<uint32_t>();
+    rounds_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, x->tv.block_size, reinterpret_cast<unsigned long long*>(cnt + 8 * kMaxParts), fp_in,
+                                                                    x->sort_prefix ? idx_in : act0, cnt, ps);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    if (x->sort_prefix) {
+        size_t tmp = 0;
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, fp_in, fp_out, idx_in, act0, (int)n, 32, 64, st));
+        CK(x->r_sort.need(tmp));
+        CK(cub::DeviceRadixSort::SortPairs(x->r_sort.p, tmp, fp_in, fp_out, idx_in, act0, (int)n, 32, 64, st));
+        x->launches += 5;     // cub: histogram + 4 onesweep passes (the top 32 fingerprint bits order the groups well enough)
+    }
+    if (fp_sorted) *fp_sorted = fp_out;
+    return 0;
+}
+
 // Large batches: rounds of group / hash / walk / resolve kernels (kernels_rounds.cuh).  max_blocks < 0: computed on the
 // device.  The sorted batch is split into parts that run their rounds on separate streams, so that one part's
 // latency-bound kernels (the serial FNV chain of few representatives, the dependent probes) share the SMs with
@@ -401,29 +417,17 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
         rb[q].grp = rb[q].map + map_slots;
     }
     ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
-    CK(cudaMemsetAsync(x->r_cnt.p, 0, 1024, st));
-    CK(x->r_fp.need((size_t)n * 8 * 2 + (size_t)n * 4));
-    uint64_t* fp_in = x->r_fp.as<uint64_t>(); uint64_t* fp_out = fp_in + n;
-    uint32_t* idx_in = reinterpret_cast<uint32_t*>(fp_out + n);
     PartSizes ps{};
     for (int q = 0; q < kMaxParts; ++q) ps.n[q] = (unsigned int)psz[q];
-    rounds_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, x->tv.block_size, d_maxb, fp_in, x->sort_prefix ? idx_in : rb[0].act[0], cnt, ps);
-    x->launches += 1;
-    CK(cudaGetLastError());
-    if (x->sort_prefix) {
-        size_t tmp = 0;
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, fp_in, fp_out, idx_in, rb[0].act[0], (int)n, 32, 64, st));
-        CK(x->r_sort.need(tmp));
-        CK(cub::DeviceRadixSort::SortPairs(x->r_sort.p, tmp, fp_in, fp_out, idx_in, rb[0].act[0], (int)n, 32, 64, st));
-        x->launches += 5;     // cub: histogram + 4 onesweep passes (the top 32 fingerprint bits order the groups well enough)
-    }
+    const uint64_t* fp_sorted = nullptr;
+    if (int rc = rounds_setup(x, a, ps, st, &fp_sorted)) return rc;
     // Is the batch worth it?  The class pipeline pays a token pass and five kernels per round; with few prompts per distinct
     // prefix the per-prompt rounds are faster.  The sorted first-block
     // fingerprints tell before anything is spent: count the distinct ones, and hand the batch over if more than 15 % of the
     // prompts start differently from their neighbour.  (The device-resident entry point waits for the block count here anyway.)
     const bool adaptive = x->score_path == 0 && x->rounds_dedup && x->sort_prefix && x->classes_min_sharing > 0.0;
     if (adaptive) {
-        count_distinct_prefixes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(fp_out, n, d_maxb + 1);
+        count_distinct_prefixes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(fp_sorted, n, d_maxb + 1);
         x->launches += 1;
     }
     if (max_blocks < 0 || adaptive) {
@@ -449,39 +453,36 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
         for (int q = 1; q < np; ++q) CK(cudaStreamWaitEvent(strm[q], x->ev_fork, 0));
     }
     const auto t_enq = std::chrono::steady_clock::now();
-    // Where kernel G runs: 0 the part's stream; 1 ONE stream for every part's G; 2 a low-priority stream per part, with the part's
-    // short kernels on a high-priority one (a CTA slot that frees up goes to a waiting latency-bound kernel before the next G CTA).
-    const int gmode = np > 1 ? x->group_serial : 0;
+    // With several parts, kernel G of a part runs on a low-priority stream and the part's short kernels on a high-priority one:
+    // a CTA slot that frees up goes to a waiting latency-bound kernel before the next G CTA (otherwise the parts drift into lock
+    // step: all in G sharing the bandwidth, then all in the short kernels with DRAM idle -- scripts/timeline.py).
+    const bool prio = np > 1;
     cudaStream_t sS[kMaxParts], sG[kMaxParts];
-    for (int q = 0; q < kMaxParts; ++q) { sS[q] = gmode == 2 ? x->hp_stream[q] : strm[q]; sG[q] = gmode == 2 ? x->lp_stream[q] : gmode == 1 ? x->g_stream : strm[q]; }
-    if (gmode == 1) CK(cudaStreamWaitEvent(x->g_stream, x->ev_fork, 0));
-    if (gmode == 2) for (int q = 0; q < np; ++q) { CK(cudaStreamWaitEvent(sS[q], x->ev_fork, 0)); CK(cudaStreamWaitEvent(sG[q], x->ev_fork, 0)); }
-    const int T = x->small_cta, W = T / 32, kf = 256 / T;        // threads / warps of the short kernels' CTAs; CTAs per 256 threads
+    for (int q = 0; q < kMaxParts; ++q) { sS[q] = prio ? x->hp_stream[q] : strm[q]; sG[q] = prio ? x->lp_stream[q] : strm[q]; }
+    if (prio) for (int q = 0; q < np; ++q) { CK(cudaStreamWaitEvent(sS[q], x->ev_fork, 0)); CK(cudaStreamWaitEvent(sG[q], x->ev_fork, 0)); }
+    constexpr int T = 256, W = T / 32;                // threads / warps of the short kernels' CTAs
     for (int64_t r = 0; r < rounds; ++r) {
         const int cur = (int)(r & 1);
         for (int q = 0; q < np; ++q) {
             const int64_t m = psz[q];
             if (m <= 0) continue;
-            unsigned ggrid = (unsigned)std::min<int64_t>((m + kGroupThreads / 32 * kGroupTile - 1) / (kGroupThreads / 32 * kGroupTile), (int64_t)x->sm_count * (np == 1 ? 3 : gmode == 1 ? x->group_serial_grid : x->rounds_grid[0]));
-            if (x->group_ctas > 0 && np > 1) ggrid = std::min<unsigned>(ggrid, (unsigned)x->group_ctas);
-            if (gmode && r > 0) CK(cudaStreamWaitEvent(sG[q], x->ev_r[q], 0));       // this part's previous round has built the live list
-            if (x->group_tma) group_round_kernel<16, true><<<ggrid, kGroupThreads, sizeof(GroupSmem), sG[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup);
-            else group_round_kernel<16, false><<<ggrid, kGroupThreads, sizeof(GroupSmem), sG[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup);
-            if (gmode) { CK(cudaEventRecord(x->ev_g[q], sG[q])); CK(cudaStreamWaitEvent(sS[q], x->ev_g[q], 0)); }
-            const unsigned lgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * kf * (np <= 2 ? 8 : x->rounds_grid[1]));
+            const unsigned ggrid = (unsigned)std::min<int64_t>((m + kGroupThreads / 32 * kGroupTile - 1) / (kGroupThreads / 32 * kGroupTile), (int64_t)x->sm_count * (np == 1 ? 3 : x->rounds_grid[0]));
+            if (prio && r > 0) CK(cudaStreamWaitEvent(sG[q], x->ev_r[q], 0));       // this part's previous round has built the live list
+            group_round_kernel<16><<<ggrid, kGroupThreads, sizeof(GroupSmem), sG[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup);
+            if (prio) { CK(cudaEventRecord(x->ev_g[q], sG[q])); CK(cudaStreamWaitEvent(sS[q], x->ev_g[q], 0)); }
+            const unsigned lgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : x->rounds_grid[1]));
             group_lists_kernel<16><<<lgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup >= 2);
         }
         for (int q = 0; q < np; ++q) {
             const int64_t m = psz[q];
             if (m <= 0) continue;
-            const int TH = std::min(T, kHashThreads);
-            const unsigned hgrid = (unsigned)std::min<int64_t>((m + TH - 1) / TH, (int64_t)x->sm_count * (256 / TH) * (np == 1 ? 4 : x->rounds_grid[2]));
-            hash_round_kernel<16><<<hgrid, TH, sizeof(HashSmem<16>) / (kHashThreads / 32) * (TH / 32), sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->hash_prefetch);
-            const unsigned wgrid = (unsigned)std::min<int64_t>((m + W - 1) / W, (int64_t)x->sm_count * kf * (np == 1 ? 8 : x->rounds_grid[3]));
+            const unsigned hgrid = (unsigned)std::min<int64_t>((m + kHashThreads - 1) / kHashThreads, (int64_t)x->sm_count * (np == 1 ? 4 : x->rounds_grid[2]));
+            hash_round_kernel<16><<<hgrid, kHashThreads, sizeof(HashSmem<16>), sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
+            const unsigned wgrid = (unsigned)std::min<int64_t>((m + W - 1) / W, (int64_t)x->sm_count * (np == 1 ? 8 : x->rounds_grid[3]));
             walk_round_kernel<<<wgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
-            const unsigned rgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * kf * (np <= 2 ? 8 : x->rounds_grid[4]));
+            const unsigned rgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : x->rounds_grid[4]));
             finish_round_kernel<16><<<rgrid, T, sizeof(DetachWarp) * W, sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup >= 2, x->rounds_trace);
-            if (gmode && r + 1 < rounds) CK(cudaEventRecord(x->ev_r[q], sS[q]));
+            if (prio && r + 1 < rounds) CK(cudaEventRecord(x->ev_r[q], sS[q]));
             x->launches += 5;
             if (x->rounds_trace == 1) {      // debugging aid: list sizes of this round (synchronises)
                 unsigned int c[8];
@@ -496,121 +497,69 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
                                       std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enq).count());
     CK(cudaGetLastError());
     for (int q = 1; q < np; ++q) { CK(cudaEventRecord(x->ev_join[q - 1], sS[q])); CK(cudaStreamWaitEvent(st, x->ev_join[q - 1], 0)); }
-    if (gmode == 2) { CK(cudaEventRecord(x->ev_g[0], sS[0])); CK(cudaStreamWaitEvent(st, x->ev_g[0], 0)); }
+    if (prio) { CK(cudaEventRecord(x->ev_g[0], sS[0])); CK(cudaStreamWaitEvent(st, x->ev_g[0], 0)); }
     return 0;
 }
 
 // Medium batches: hash / walk rounds, every prompt on its own (kernels_rounds_plain.cuh); two halves on two streams.
-// Below rounds_spec_max prompts the rounds are latency bound (a few warps per SM walking dependent chains), so kernel H of
-// round t+1 is launched BESIDE kernel P of round t on a second stream per half: it hashes the next 32 blocks of every prompt
-// of round t's list without waiting to learn which of them survive (at most one round of hashing per prompt is wasted).
 int launch_score_rounds_plain(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int64_t tok_base, int64_t n,
                         const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, const ScoreOut& o, cudaStream_t st,
                         int64_t max_blocks) {
-    const bool spec = x->rounds_spec && n <= x->rounds_spec_max;
-    const bool warp_walk = !spec && x->rounds_warp && n <= x->rounds_warp_max;      // kernel P: warp per prompt (batch too small to fill the machine lane per prompt)
-    CK(x->r_act0.need((size_t)n * 4)); CK(x->r_act1.need((size_t)n * 4)); CK(x->r_cnt.need(64));
-    CK(x->r_hstate.need((size_t)n * 8)); CK(x->r_keys.need((size_t)n * plain::kRoundBlocks * 8 * (spec ? 2 : 1))); CK(x->r_pst.need((size_t)n * sizeof(plain::PromptState)));
-    CK(x->r_nbr.need((size_t)n * 4 * (spec ? 2 : 1)));
-    if (spec) CK(x->r_hl.need((size_t)n * 4 * 2));
+    const bool warp_walk = x->rounds_warp && n <= x->rounds_warp_max;      // kernel P: warp per prompt (batch too small to fill the machine lane per prompt)
+    CK(x->r_act0.need((size_t)n * 4)); CK(x->r_act1.need((size_t)n * 4)); CK(x->r_cnt.need(1024));
+    CK(x->r_hstate.need((size_t)n * 8)); CK(x->r_keys.need((size_t)n * kRoundBlocks * 8)); CK(x->r_pst.need((size_t)n * sizeof(PromptState)));
+    CK(x->r_nbr.need((size_t)n * 4));
     const bool overlap = x->rounds_overlap && n >= x->rounds_overlap_min;
     const int64_t nA = overlap ? ((n / 2 + 31) & ~31ll) : n, nB = n - nA;
     unsigned int* cnt = x->r_cnt.as<unsigned int>();
-    unsigned long long* d_maxb = reinterpret_cast<unsigned long long*>(x->r_cnt.as<unsigned char>() + 16);
     plain::RoundBufs rb[2]{};
     for (int hlf = 0; hlf < 2; ++hlf) {
         const int64_t off = hlf ? nA : 0;
         rb[hlf].act[0] = x->r_act0.as<uint32_t>() + off; rb[hlf].act[1] = x->r_act1.as<uint32_t>() + off;
-        rb[hlf].n_act = cnt + 2 * hlf;
-        rb[hlf].hstate = x->r_hstate.as<uint64_t>(); rb[hlf].pst = x->r_pst.as<plain::PromptState>();
-        rb[hlf].keys = x->r_keys.as<uint64_t>() + (warp_walk ? off * plain::kRoundBlocks : off); rb[hlf].nbr = x->r_nbr.as<uint32_t>() + off;      // prompt-major keys: a half's rows are contiguous
-        rb[hlf].spec = spec ? 1 : 0;
-        if (spec) { rb[hlf].prev[0] = x->r_hl.as<uint32_t>() + off; rb[hlf].prev[1] = x->r_hl.as<uint32_t>() + n + off; }
+        rb[hlf].n_act = cnt + 8 * hlf;                // the halves are parts 0 and 1 of rounds_setup's counters
+        rb[hlf].hstate = x->r_hstate.as<uint64_t>(); rb[hlf].pst = x->r_pst.as<PromptState>();
+        rb[hlf].keys = x->r_keys.as<uint64_t>() + (warp_walk ? off * kRoundBlocks : off); rb[hlf].nbr = x->r_nbr.as<uint32_t>() + off;      // prompt-major keys: a half's rows are contiguous
     }
     ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
-    CK(cudaMemsetAsync(x->r_cnt.p, 0, 64, st));
-    CK(x->r_fp.need((size_t)n * 8 * 2 + (size_t)n * 4));
-    uint64_t* fp_in = x->r_fp.as<uint64_t>(); uint64_t* fp_out = fp_in + n;
-    uint32_t* idx_in = reinterpret_cast<uint32_t*>(fp_out + n);
-    plain::rounds_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, x->tv.block_size, d_maxb, fp_in, x->sort_prefix ? idx_in : rb[0].act[0], cnt,
-                                                                    (unsigned int)nA);
-    x->launches += 1;
-    CK(cudaGetLastError());
-    if (x->sort_prefix) {
-        size_t tmp = 0;
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, fp_in, fp_out, idx_in, rb[0].act[0], (int)n, 32, 64, st));
-        CK(x->r_sort.need(tmp));
-        CK(cub::DeviceRadixSort::SortPairs(x->r_sort.p, tmp, fp_in, fp_out, idx_in, rb[0].act[0], (int)n, 32, 64, st));
-        x->launches += 5;     // cub: histogram + 4 onesweep passes (the top 32 fingerprint bits order the groups well enough)
-    }
+    if (int rc = rounds_setup(x, a, PartSizes{{(unsigned int)nA, (unsigned int)nB}}, st, nullptr)) return rc;
     if (max_blocks < 0) {
         unsigned long long mb = 0;
-        CK(cudaMemcpyAsync(&mb, d_maxb, sizeof mb, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(&mb, cnt + 8 * kMaxParts, sizeof mb, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         max_blocks = (int64_t)mb;
     }
-    int64_t rounds = (max_blocks + plain::kRoundBlocks - 1) / plain::kRoundBlocks;
+    int64_t rounds = (max_blocks + kRoundBlocks - 1) / kRoundBlocks;
     if (rounds < 1) rounds = 1;                       // round 0 also retires the prompts that have no full block
     const int nh = nB > 0 ? 2 : 1;
-    const int per_sm_h = nh == 2 ? 2 : 4, per_sm_p = nh == 2 ? 2 : 4;
-    if (!spec) {
-        cudaStream_t strm[2] = {st, x->aux_stream[0]};
-        if (nh == 2) { CK(cudaEventRecord(x->ev_fork, st)); CK(cudaStreamWaitEvent(x->aux_stream[0], x->ev_fork, 0)); }
-        for (int64_t r = 0; r < rounds; ++r) {
-            const int cur = (int)(r & 1);
-            for (int hlf = 0; hlf < nh; ++hlf) {
-                const int64_t m = hlf ? nB : nA;
-                const unsigned hgrid = (unsigned)std::min<int64_t>((m + plain::kHashThreads - 1) / plain::kHashThreads, (int64_t)x->sm_count * per_sm_h);
-                if (warp_walk && x->rounds_warp_stages == 3) {      // 128-thread CTAs, three stages: 55 KB, four CTAs per SM
-                    const unsigned hg = (unsigned)std::min<int64_t>((m + 127) / 128, (int64_t)x->sm_count * 4);
-                    plain::hash_round_kernel<16, true, 3><<<hg, 128, sizeof(plain::HashSmem<16>) / 8 / 2 * 3 * 4, strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
-                } else if (warp_walk) plain::hash_round_kernel<16, true, 2><<<hgrid, plain::kHashThreads, sizeof(plain::HashSmem<16>), strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
-                else if (x->rounds_lane_stages == 3 && n <= x->rounds_lane_stages_max) {
-                    const unsigned hg = (unsigned)std::min<int64_t>((m + 127) / 128, (int64_t)x->sm_count * 4);
-                    plain::hash_round_kernel<16, false, 3><<<hg, 128, sizeof(plain::HashSmem<16>) / 8 / 2 * 3 * 4, strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
-                } else plain::hash_round_kernel<16, false, 2><<<hgrid, plain::kHashThreads, sizeof(plain::HashSmem<16>), strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
-            }
-            for (int hlf = 0; hlf < nh; ++hlf) {
-                const int64_t m = hlf ? nB : nA;
-                if (warp_walk) {      // warp per prompt: 8 prompts per CTA iteration
-                    const unsigned pgrid = (unsigned)std::min<int64_t>((m + 7) / 8, (int64_t)x->sm_count * 8);
-                    plain::probe_round_warp_kernel<<<pgrid, plain::kProbeThreads, 0, strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
-                    continue;
-                }
-                const unsigned pgrid = (unsigned)std::min<int64_t>((m + plain::kProbeThreads - 1) / plain::kProbeThreads, (int64_t)x->sm_count * per_sm_p);
-                plain::probe_round_kernel<<<pgrid, plain::kProbeThreads, sizeof(plain::WalkSmem), strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
-            }
-            x->launches += 2 * nh;
-        }
-        CK(cudaGetLastError());
-        if (nh == 2) { CK(cudaEventRecord(x->ev_join[0], x->aux_stream[0])); CK(cudaStreamWaitEvent(st, x->ev_join[0], 0)); }
-        return 0;
-    }
-    // speculative schedule: per half one H stream and one P stream; H(t+1) waits for P(t-1) (its list), P(t) for H(t) (its keys)
-    cudaStream_t sH[2] = {st, x->aux_stream[0]}, sP[2] = {x->aux_stream[1], x->aux_stream[2]};
-    CK(cudaEventRecord(x->ev_fork, st));
-    for (int q = 0; q < 3; ++q) CK(cudaStreamWaitEvent(x->aux_stream[q], x->ev_fork, 0));
+    const int per_sm = nh == 2 ? 2 : 4;               // CTAs per SM of a half's lane-per-prompt kernels H and P
+    cudaStream_t strm[2] = {st, x->aux_stream[0]};
+    if (nh == 2) { CK(cudaEventRecord(x->ev_fork, st)); CK(cudaStreamWaitEvent(x->aux_stream[0], x->ev_fork, 0)); }
     for (int64_t r = 0; r < rounds; ++r) {
         const int cur = (int)(r & 1);
         for (int hlf = 0; hlf < nh; ++hlf) {
             const int64_t m = hlf ? nB : nA;
-            plain::RoundBufs rr = rb[hlf];
-            rr.keys += (size_t)cur * (size_t)n * plain::kRoundBlocks; rr.nbr += (size_t)cur * (size_t)n;
-            if (r >= 2) CK(cudaStreamWaitEvent(sH[hlf], x->ev_spec_p[hlf][cur], 0));                 // P(r-2) built the list H(r) runs over ... (r-1)&1 == cur^1; see below
-            const unsigned hgrid = (unsigned)std::min<int64_t>((m + plain::kHashThreads - 1) / plain::kHashThreads, (int64_t)x->sm_count * per_sm_h);
-            plain::hash_round_kernel<16, false, 2><<<hgrid, plain::kHashThreads, sizeof(plain::HashSmem<16>), sH[hlf]>>>(x->tv, a, rr, cur, (int)r);
-            CK(cudaEventRecord(x->ev_spec_h[hlf][cur], sH[hlf]));
-            CK(cudaStreamWaitEvent(sP[hlf], x->ev_spec_h[hlf][cur], 0));
-            CK(cudaMemsetAsync(rb[hlf].n_act + (cur ^ 1), 0, sizeof(unsigned int), sP[hlf]));      // the list P(r) appends to starts empty
-            const unsigned pgrid = (unsigned)std::min<int64_t>((m + plain::kProbeThreads - 1) / plain::kProbeThreads, (int64_t)x->sm_count * per_sm_p);
-            plain::probe_round_kernel<<<pgrid, plain::kProbeThreads, sizeof(plain::WalkSmem), sP[hlf]>>>(x->tv, a, rr, cur, (int)r);
-            CK(cudaEventRecord(x->ev_spec_p[hlf][cur], sP[hlf]));
+            if (warp_walk) {      // 128-thread CTAs, three stages: 55 KB, four CTAs per SM
+                const unsigned hg = (unsigned)std::min<int64_t>((m + 127) / 128, (int64_t)x->sm_count * 4);
+                plain::hash_round_kernel<16, true><<<hg, 128, 4 * 3 * 32 * HashSmem<16>::kRow, strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
+            } else {
+                const unsigned hgrid = (unsigned)std::min<int64_t>((m + kHashThreads - 1) / kHashThreads, (int64_t)x->sm_count * per_sm);
+                plain::hash_round_kernel<16, false><<<hgrid, kHashThreads, sizeof(HashSmem<16>), strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
+            }
+        }
+        for (int hlf = 0; hlf < nh; ++hlf) {
+            const int64_t m = hlf ? nB : nA;
+            if (warp_walk) {      // warp per prompt: 8 prompts per CTA iteration
+                const unsigned pgrid = (unsigned)std::min<int64_t>((m + 7) / 8, (int64_t)x->sm_count * 8);
+                plain::probe_round_warp_kernel<<<pgrid, plain::kProbeThreads, 0, strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
+                continue;
+            }
+            const unsigned pgrid = (unsigned)std::min<int64_t>((m + plain::kProbeThreads - 1) / plain::kProbeThreads, (int64_t)x->sm_count * per_sm);
+            plain::probe_round_kernel<<<pgrid, plain::kProbeThreads, sizeof(plain::WalkSmem), strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
         }
         x->launches += 2 * nh;
     }
     CK(cudaGetLastError());
-    if (nh == 2) { CK(cudaEventRecord(x->ev_join[0], sH[1])); CK(cudaStreamWaitEvent(st, x->ev_join[0], 0)); }
-    for (int hlf = 0; hlf < nh; ++hlf) { CK(cudaEventRecord(x->ev_join[1 + hlf], sP[hlf])); CK(cudaStreamWaitEvent(st, x->ev_join[1 + hlf], 0)); }
+    if (nh == 2) { CK(cudaEventRecord(x->ev_join[0], x->aux_stream[0])); CK(cudaStreamWaitEvent(st, x->ev_join[0], 0)); }
     return 0;
 }
 
@@ -620,21 +569,22 @@ int launch_score(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int64_t 
                  int64_t max_blocks = -1) {
     if (n <= 0) return 0;
     if (int rc = check_shards(x)) return rc;
-    if (x->score_kernel == 1 || x->tv.req_stamp) {
-        // exact-LRU mode always takes this kernel: Lookup must touch every present key of a prompt (no early exit)
+    if (x->score_kernel == 1 || x->tv.req_stamp || x->tv.block_size != 16) {
+        // exact-LRU mode always takes this kernel: Lookup must touch every present key of a prompt (no early exit); so does
+        // every block size but 16, which the other kernels' token staging is written for
         const int T = 128;
         const unsigned long long stride = 1ull << 20;
         const unsigned long long sb = x->tv.req_stamp ? reserve_stamps(x, (unsigned long long)n * stride) : 0;
         score_kernel_v1<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, d_tok, d_off, tok_base, n, d_model, model0, d_filter,
                                                                   o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, sb, stride);
         x->launches += 1;
-    } else if (x->tv.block_size == 16 && (x->score_path == 4 || (x->score_path == 0 && n <= x->coop_max))) {
+    } else if (x->score_path == 4 || (x->score_path == 0 && n <= x->coop_max)) {
         // small batches: a warp per prompt, warp-cooperative hashing, TMA-staged tokens (kernels_coop.cuh)
         ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
         const int64_t ctas = std::min<int64_t>((n + kCoopWarps - 1) / kCoopWarps, (int64_t)x->sm_count * 4);
         coop_score_kernel<16><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem), st>>>(x->tv, a);
         x->launches += 1;
-    } else if (x->tv.block_size == 16 && n < (1ll << 31) && ((x->score_path >= 2 && x->score_path <= 3) || (x->score_path == 0 && n >= x->rounds_min))) {
+    } else if (n < (1ll << 31) && ((x->score_path >= 2 && x->score_path <= 3) || (x->score_path == 0 && n >= x->rounds_min))) {
         // path 2: plain rounds, 3: prefix classes; automatic: by batch size (the class pipeline has a fixed cost per round)
         const bool classes = x->score_path == 3 || (x->score_path == 0 && n >= x->classes_min);
         return classes ? launch_score_rounds(x, d_tok, d_off, tok_base, n, d_model, model0, d_filter, o, st, max_blocks)
@@ -1082,7 +1032,6 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
         CK(cudaEventCreateWithFlags(&x->ev_join[q], cudaEventDisableTiming));
     }
     CK(cudaEventCreateWithFlags(&x->ev_fork, cudaEventDisableTiming));
-    CK(cudaStreamCreateWithFlags(&x->g_stream, cudaStreamNonBlocking));
     {
         int lo = 0, hi = 0;
         CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
@@ -1094,10 +1043,6 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     for (int q = 0; q < kMaxParts; ++q) { CK(cudaEventCreateWithFlags(&x->ev_g[q], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&x->ev_r[q], cudaEventDisableTiming)); }
     CK(cudaEventCreateWithFlags(&x->ev_write, cudaEventDisableTiming));
     for (auto& e : x->ev_snap) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    for (int a_ = 0; a_ < 2; ++a_) for (int b_ = 0; b_ < 2; ++b_) {
-        CK(cudaEventCreateWithFlags(&x->ev_spec_h[a_][b_], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&x->ev_spec_p[a_][b_], cudaEventDisableTiming));
-    }
     x->stream = x->own_stream;
     for (int i = 0; i < 2; ++i) {
         CK(cudaEventCreateWithFlags(&x->ev_h2d[i], cudaEventDisableTiming));
@@ -1142,8 +1087,6 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     if (const char* k = getenv("KVIDX_SCORE_PATH")) x->score_path = !strcmp(k, "fused") ? 1 : !strcmp(k, "rounds") ? 2 : !strcmp(k, "classes") ? 3 : !strcmp(k, "coop") ? 4 : 0;
     if (const char* k = getenv("KVIDX_COOP_MAX")) x->coop_max = atoll(k);
     if (const char* k = getenv("KVIDX_ZEROCOPY_MAX")) x->zerocopy_max = atoll(k);
-    if (const char* k = getenv("KVIDX_ROUNDS_SPEC")) x->rounds_spec = atoi(k) != 0;
-    if (const char* k = getenv("KVIDX_ROUNDS_SPEC_MAX")) x->rounds_spec_max = atoll(k);
     if (const char* k = getenv("KVIDX_ROUNDS_MIN")) x->rounds_min = atoll(k);
     if (const char* k = getenv("KVIDX_CLASSES_MIN")) x->classes_min = atoll(k);
     if (const char* k = getenv("KVIDX_CLASSES_SHARING")) x->classes_min_sharing = atof(k);
@@ -1153,20 +1096,12 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     if (const char* k = getenv("KVIDX_HOST_CHUNK_TOKENS")) x->host_chunk_tokens = std::max<int64_t>(1 << 16, atoll(k));
     if (const char* k = getenv("KVIDX_ROUNDS_TRACE")) x->rounds_trace = atoi(k);
     if (const char* k = getenv("KVIDX_ROUNDS_PARTS")) x->rounds_parts = atoi(k);
-    if (const char* k = getenv("KVIDX_GROUP_SERIAL")) x->group_serial = atoi(k);
-    if (const char* k = getenv("KVIDX_HASH_PREFETCH")) x->hash_prefetch = atoi(k);
     if (const char* k = getenv("KVIDX_PEER_PAIR")) x->tv.peer_pair = atoi(k) != 0;
-    if (const char* k = getenv("KVIDX_GROUP_CTAS")) x->group_ctas = atoi(k);
     if (const char* k = getenv("KVIDX_ROUNDS_WARP")) x->rounds_warp = atoi(k) != 0;
     if (const char* k = getenv("KVIDX_ROUNDS_WARP_MAX")) x->rounds_warp_max = atoll(k);
-    if (const char* k = getenv("KVIDX_ROUNDS_LANE_STAGES")) x->rounds_lane_stages = atoi(k) == 3 ? 3 : 2;
-    if (const char* k = getenv("KVIDX_ROUNDS_WARP_STAGES")) x->rounds_warp_stages = atoi(k) == 3 ? 3 : 2;
-    if (const char* k = getenv("KVIDX_SMALL_CTA")) { const int v = atoi(k); if (v == 32 || v == 64 || v == 128 || v == 256) x->small_cta = v; }
-    if (const char* k = getenv("KVIDX_GROUP_SERIAL_GRID")) x->group_serial_grid = std::max(1, atoi(k));
     if (const char* k = getenv("KVIDX_ROUNDS_DEDUP")) x->rounds_dedup = atoi(k);
     if (const char* k = getenv("KVIDX_ROUNDS_OVERLAP_MIN")) x->rounds_overlap_min = atoll(k);
     if (const char* k = getenv("KVIDX_WRITE_PHASE1")) x->write_phase1 = atoi(k);
-    if (const char* k = getenv("KVIDX_GROUP_TMA")) x->group_tma = atoi(k) != 0;
     x->queue = new_submit_queue();
     if (rounds_init() || plain::rounds_init() || coop_init()) return fail(KVIDX_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaGetLastError()));
     if (score_tuned_init()) return fail(KVIDX_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -1243,14 +1178,9 @@ void kvidx_destroy(kvidx_t* x) {
         if (x->ev_join[q]) cudaEventDestroy(x->ev_join[q]);
     }
     if (x->ev_fork) cudaEventDestroy(x->ev_fork);
-    if (x->g_stream) cudaStreamDestroy(x->g_stream);
     for (int q = 0; q < kMaxParts; ++q) { if (x->hp_stream[q]) cudaStreamDestroy(x->hp_stream[q]); if (x->lp_stream[q]) cudaStreamDestroy(x->lp_stream[q]); }
     for (int q = 0; q < kMaxParts; ++q) { if (x->ev_g[q]) cudaEventDestroy(x->ev_g[q]); if (x->ev_r[q]) cudaEventDestroy(x->ev_r[q]); }
     if (x->ev_write) cudaEventDestroy(x->ev_write);
-    for (int a_ = 0; a_ < 2; ++a_) for (int b_ = 0; b_ < 2; ++b_) {
-        if (x->ev_spec_h[a_][b_]) cudaEventDestroy(x->ev_spec_h[a_][b_]);
-        if (x->ev_spec_p[a_][b_]) cudaEventDestroy(x->ev_spec_p[a_][b_]);
-    }
     cudaGetLastError();
     delete x;
 }

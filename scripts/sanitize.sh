@@ -8,6 +8,6 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_concurrency.py -x -q -m gpu -k "coop_kernel_short"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_parity.py -x -q -m gpu -k "ragged and coop"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_parity.py -x -q -m gpu -k "test_random_event_stream and rounds"
-compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_parity.py -x -q -m gpu -k "prefix_tree and rounds2 and not lane and not spec and not nospec"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_parity.py -x -q -m gpu -k "prefix_tree and rounds2 and not lane"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_snapshot.py -x -q -m gpu -k "golden or error_paths or equal_contents or exact_lru"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_shard_ops.py -x -q -m gpu -k "same-gpu-2 or guards or all_or_nothing or unsharded_handle or (round_trips and coop and same)"

@@ -302,8 +302,8 @@ def test_batched_events_per_pod_order_vs_oracle():
 def _select_path(monkeypatch, path):
     """v1: thread-per-prompt kernel; fused: persistent lane-worker kernel; rounds*: hash / walk rounds, every prompt on
     its own (one stream / two halves on two streams / without the prefix sort); classes*: the round pipeline that hashes
-    and walks one representative per distinct prefix (one part / 2 / 8 parts / unsorted / sharing switched off / whole
-    chunks only, no partial followers)."""
+    and walks one representative per distinct prefix (one part / 2 / 8 / 16 parts / unsorted / sharing switched off /
+    whole chunks only, no partial followers; the variants also with the batch split into parts)."""
     if path == "v1":
         monkeypatch.setenv("KVIDX_SCORE_KERNEL", "v1")
         return
@@ -328,26 +328,13 @@ def _select_path(monkeypatch, path):
         monkeypatch.setenv("KVIDX_ROUNDS_DEDUP", "0")
     elif var == "whole":
         monkeypatch.setenv("KVIDX_ROUNDS_DEDUP", "1")
-    elif var == "tma":                       # token chunks of the class pipeline by TMA bulk copy instead of cp.async
-        monkeypatch.setenv("KVIDX_GROUP_TMA", "1")
-    elif var == "nospec":                    # per-prompt rounds without the speculative hash / walk overlap
-        monkeypatch.setenv("KVIDX_ROUNDS_SPEC", "0")
-    elif var == "serial0":                   # class pipeline: every kernel of a part on the part's stream
-        monkeypatch.setenv("KVIDX_GROUP_SERIAL", "0")
-    elif var == "serial1":                   # ... all parts' token-streaming kernels on ONE stream
-        monkeypatch.setenv("KVIDX_GROUP_SERIAL", "1")
-    elif var == "cta64":                     # ... short kernels with 64-thread CTAs, hash kernel pulling its chunks to L2 first
-        monkeypatch.setenv("KVIDX_SMALL_CTA", "64")
-        monkeypatch.setenv("KVIDX_HASH_PREFETCH", "1")
     elif var == "lane":                      # per-prompt rounds with the lane-per-prompt kernel P (what batches above 131 072 take)
         monkeypatch.setenv("KVIDX_ROUNDS_WARP", "0")
-    elif var == "spec":                      # ... with the speculative hash / walk overlap (off by default)
-        monkeypatch.setenv("KVIDX_ROUNDS_SPEC", "1")
 
 
-ROUND_PATHS = ["rounds", "rounds2", "rounds-nosort", "rounds-lane", "rounds2-lane", "rounds2-spec", "rounds-nospec", "rounds2-nospec", "classes", "classes2", "classes8", "classes-nosort",
-               "classes-nodedup", "classes-whole", "classes4-whole", "classes-tma", "classes8-tma", "classes8-serial0", "classes8-serial1",
-               "classes4-cta64", "auto"]
+ROUND_PATHS = ["rounds", "rounds2", "rounds-nosort", "rounds2-nosort", "rounds-lane", "rounds2-lane", "classes", "classes2", "classes8",
+               "classes16", "classes-nosort", "classes2-nosort", "classes8-nosort", "classes-nodedup", "classes2-nodedup",
+               "classes8-nodedup", "classes-whole", "classes2-whole", "classes4-whole", "classes8-whole", "auto"]
 PATHS = ["v1", "fused", "coop"] + ROUND_PATHS
 
 
