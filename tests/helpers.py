@@ -78,3 +78,54 @@ def dense_from_map(scores, pods: Interner, P):
         for p, s in scores.items():
             row[pods.ids[p]] = s
     return row
+
+
+# ---- GPU Score() paths: a handle reads these variables when it is created, so every path needs its own handle ----------
+def _index_pair(**kw):
+    import kvidx
+    from oracle.kvoracle_c import COracle
+    w = kw.pop("tier_weights", (1.0, 0.8))
+    ix = kvidx.Index(tier_weights=w, **kw)
+    co = COracle(block_size=kw.get("block_size", 16), init_hash=kvidx.fnv64a(kw.get("hash_seed", "").encode()),
+                 size=kw.get("capacity", 1 << 20), pod_cache_size=kw.get("pods_per_key", 10), tier_weights=w,
+                 max_pods=kw.get("max_pods", 256))
+    return ix, co
+
+
+def _select_path(monkeypatch, path):
+    """v1: thread-per-prompt kernel; fused: persistent lane-worker kernel; rounds*: hash / walk rounds, every prompt on
+    its own (one stream / two halves on two streams / without the prefix sort); classes*: the round pipeline that hashes
+    and walks one representative per distinct prefix (one part / 2 / 8 / 16 parts / unsorted / sharing switched off /
+    whole chunks only, no partial followers; the variants also with the batch split into parts)."""
+    if path == "v1":
+        monkeypatch.setenv("KVIDX_SCORE_KERNEL", "v1")
+        return
+    if path == "auto":                       # the library chooses: here every batch is "large", so it is the class pipeline
+        monkeypatch.setenv("KVIDX_ROUNDS_MIN", "1")        # or the per-prompt rounds, by how much the batch repeats itself
+        monkeypatch.setenv("KVIDX_COOP_MAX", "0")          # (small batches would otherwise take the warp-per-prompt kernel)
+        monkeypatch.setenv("KVIDX_CLASSES_MIN", "64")
+        monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP_MIN", "64")
+        return
+    base, _, var = path.partition("-")
+    parts = base.lstrip("abcdefghijklmnopqrstuvwxyz")
+    base = base[: len(base) - len(parts)]
+    monkeypatch.setenv("KVIDX_SCORE_PATH", base)
+    if parts:
+        monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP_MIN", "64")
+        monkeypatch.setenv("KVIDX_ROUNDS_PARTS", parts)
+    else:
+        monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP", "0")
+    if var == "nosort":
+        monkeypatch.setenv("KVIDX_SORT_PREFIX", "0")
+    elif var == "nodedup":
+        monkeypatch.setenv("KVIDX_ROUNDS_DEDUP", "0")
+    elif var == "whole":
+        monkeypatch.setenv("KVIDX_ROUNDS_DEDUP", "1")
+    elif var == "lane":                      # per-prompt rounds with the lane-per-prompt kernel P (what batches above 131 072 take)
+        monkeypatch.setenv("KVIDX_ROUNDS_WARP", "0")
+
+
+ROUND_PATHS = ["rounds", "rounds2", "rounds-nosort", "rounds2-nosort", "rounds-lane", "rounds2-lane", "classes", "classes2", "classes8",
+               "classes16", "classes-nosort", "classes2-nosort", "classes8-nosort", "classes-nodedup", "classes2-nodedup",
+               "classes8-nodedup", "classes-whole", "classes2-whole", "classes4-whole", "classes8-whole", "auto"]
+PATHS = ["v1", "fused", "coop"] + ROUND_PATHS

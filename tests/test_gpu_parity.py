@@ -2,7 +2,8 @@
 import numpy as np
 import pytest
 
-from helpers import EVENT_DTYPE, Interner, csr, dense_from_map, filter_mask, golden, scenario_events
+from helpers import (EVENT_DTYPE, PATHS, ROUND_PATHS, Interner, _index_pair, _select_path, csr, dense_from_map, filter_mask, golden,
+                     scenario_events)
 import kvidx
 from kvidx import synth
 from oracle import kvoracle as ko
@@ -36,15 +37,6 @@ def test_hash_keys_ragged_batch_vs_oracle():
         k1, o1 = ix.hash_keys(tok, off, par, val)
         k2, o2 = co.hash_keys(tok, off, par, val)
         assert np.array_equal(o1, o2) and np.array_equal(k1, k2)
-
-
-def _index_pair(**kw):
-    w = kw.pop("tier_weights", (1.0, 0.8))
-    ix = kvidx.Index(tier_weights=w, **kw)
-    co = COracle(block_size=kw.get("block_size", 16), init_hash=kvidx.fnv64a(kw.get("hash_seed", "").encode()),
-                 size=kw.get("capacity", 1 << 20), pod_cache_size=kw.get("pods_per_key", 10), tier_weights=w,
-                 max_pods=kw.get("max_pods", 256))
-    return ix, co
 
 
 def PT(p, t=0):
@@ -297,45 +289,6 @@ def test_batched_events_per_pod_order_vs_oracle():
     s1, _ = ix.score_batch(tok, off)
     s2, _, _, _ = co.score_batch(tok, off)
     assert np.array_equal(s1, s2)
-
-
-def _select_path(monkeypatch, path):
-    """v1: thread-per-prompt kernel; fused: persistent lane-worker kernel; rounds*: hash / walk rounds, every prompt on
-    its own (one stream / two halves on two streams / without the prefix sort); classes*: the round pipeline that hashes
-    and walks one representative per distinct prefix (one part / 2 / 8 / 16 parts / unsorted / sharing switched off /
-    whole chunks only, no partial followers; the variants also with the batch split into parts)."""
-    if path == "v1":
-        monkeypatch.setenv("KVIDX_SCORE_KERNEL", "v1")
-        return
-    if path == "auto":                       # the library chooses: here every batch is "large", so it is the class pipeline
-        monkeypatch.setenv("KVIDX_ROUNDS_MIN", "1")        # or the per-prompt rounds, by how much the batch repeats itself
-        monkeypatch.setenv("KVIDX_COOP_MAX", "0")          # (small batches would otherwise take the warp-per-prompt kernel)
-        monkeypatch.setenv("KVIDX_CLASSES_MIN", "64")
-        monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP_MIN", "64")
-        return
-    base, _, var = path.partition("-")
-    parts = base.lstrip("abcdefghijklmnopqrstuvwxyz")
-    base = base[: len(base) - len(parts)]
-    monkeypatch.setenv("KVIDX_SCORE_PATH", base)
-    if parts:
-        monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP_MIN", "64")
-        monkeypatch.setenv("KVIDX_ROUNDS_PARTS", parts)
-    else:
-        monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP", "0")
-    if var == "nosort":
-        monkeypatch.setenv("KVIDX_SORT_PREFIX", "0")
-    elif var == "nodedup":
-        monkeypatch.setenv("KVIDX_ROUNDS_DEDUP", "0")
-    elif var == "whole":
-        monkeypatch.setenv("KVIDX_ROUNDS_DEDUP", "1")
-    elif var == "lane":                      # per-prompt rounds with the lane-per-prompt kernel P (what batches above 131 072 take)
-        monkeypatch.setenv("KVIDX_ROUNDS_WARP", "0")
-
-
-ROUND_PATHS = ["rounds", "rounds2", "rounds-nosort", "rounds2-nosort", "rounds-lane", "rounds2-lane", "classes", "classes2", "classes8",
-               "classes16", "classes-nosort", "classes2-nosort", "classes8-nosort", "classes-nodedup", "classes2-nodedup",
-               "classes8-nodedup", "classes-whole", "classes2-whole", "classes4-whole", "classes8-whole", "auto"]
-PATHS = ["v1", "fused", "coop"] + ROUND_PATHS
 
 
 @pytest.mark.parametrize("kernel", PATHS)
