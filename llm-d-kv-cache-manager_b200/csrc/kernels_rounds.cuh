@@ -17,7 +17,8 @@
 //   H   hash_round_kernel    FNV-64a / CBOR chain keys of the representatives' chunks
 //   P   walk_round_kernel    warp per representative: 32 probes at once, ordered scoring of the hits, run snapshots
 //   R+D finish_round_kernel  followers copy their representative's fate; partial followers resume from its snapshot and
-//                            walk their own blocks; next round's live list
+//                            walk their own blocks
+//   C   compact_round_kernel next round's live list: the prompts that continue, in the order of this round's list
 //
 // Every round pays a fixed cost of short latency-bound kernels (hidden by running the batch as independent parts
 // on separate streams), so medium batches use kernels_rounds_plain.cuh instead (see kvidx.cu: launch_score).
@@ -62,11 +63,15 @@ struct RoundBufs {
     // tokens is identical get identical keys, probes, scores and fate this round.  One representative per class is
     // hashed and walked; the others wait in the follower list and take the representative's outcome.
     uint32_t* role;                      // [n_act] kRoleSelf: representative (or alone); else the live slot of its representative
-    uint8_t* fate;                       // [n_act] written for representatives by kernel P: kFateMore / kFateDone
+    uint8_t* fate;                       // [n_act] kFateMore (continues next round) / kFateDone, for every live slot: written by
+                                         // kernel P for representatives, R for followers, D for partial followers; read by C
     uint32_t* hl;                        // [n_act] representative list (live slots), compacted
     uint32_t* fl;                        // [n_act] follower list (live slots), compacted
     uint32_t* dl;                        // [n_act] partial-follower list (live slots), compacted
     unsigned int* n_hl;                  // [0] representatives, [1] followers, [2] partial followers (zeroed before every round)
+    unsigned int* stat;                  // with KVIDX_ROUNDS_TRACE=1, running totals of the batch: [0] chunks kernel G streams,
+                                         // [1] election losers that read two chunks again in G, [2] chunk compares in G2,
+                                         // [3] blocks kernel H hashes
     // partial followers: a prompt alone in its class whose chunk starts like a neighbouring class's chunk (it leaves a
     // popular prefix inside this chunk) shares the first dmin blocks with that class -- keys and walk -- and continues on
     // its own from there (detach_round_kernel)
@@ -76,6 +81,7 @@ struct RoundBufs {
     uint8_t* dmin;                       // [n_act] ... and the number of leading blocks it shares (0: none)
     uint32_t* apos;                      // [n_act] live slot -> position in the representative list
     uint32_t* lslot;                     // per prompt: its slot in the current live list (written when the list is built)
+    unsigned long long* scan;            // [tiles of kernel C] per tile: round + 1 << 32 | prefix done << 31 | live slots (zeroed per batch)
     uint4* rec;                          // [n_hl] per representative {prompt, live slot, nbr word, src}: one load instead of a chain
     uint4* drec;                         // [n_dl] per partial follower {prompt, representative's live slot, shared blocks << 16 | nbr word, representative's prompt}
     uint32_t* grp;                       // [n_act] by live slot of last round's representative R: a class of this round whose members
@@ -128,14 +134,14 @@ struct GroupSmem {
 
 template <int BS>
 __global__ void __launch_bounds__(kGroupThreads, 3)
-group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round, const int dedup) {
+group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round, const int dedup, const int trace) {
     static_assert(BS == 16 && kRoundBlocks == 32, "a chunk is 4 x 32 lanes x 16 bytes");
     extern __shared__ __align__(128) unsigned char smem_raw_g[];
     uint4 (*ring)[4][32] = reinterpret_cast<GroupSmem*>(smem_raw_g)->ring[threadIdx.x >> 5];
     const int lane = threadIdx.x & 31;
     const uint64_t l2pol = l2_policy_stream();
     const unsigned int n_act = rb.n_act[cur];
-    if (blockIdx.x == 0 && threadIdx.x == 0) { rb.n_act[cur ^ 1] = 0; rb.n_hl[0] = 0; rb.n_hl[1] = 0; rb.n_hl[2] = 0; rb.n_hl[3] = 0; }   // lists built below / by G2
+    if (blockIdx.x == 0 && threadIdx.x == 0) { rb.n_hl[0] = 0; rb.n_hl[1] = 0; rb.n_hl[2] = 0; rb.n_hl[3] = 0; }   // lists built by G2
     const unsigned int total_warps = gridDim.x * (kGroupThreads / 32);
     for (unsigned int w = blockIdx.x * (kGroupThreads / 32) + (threadIdx.x >> 5); w * (unsigned)kGroupTile < n_act; w += total_warps) {
         const unsigned int i = w * (unsigned)kGroupTile + lane;
@@ -173,6 +179,7 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         int dh = 0, hlane = -1;                       // hint: shares dh leading blocks with the chunk of lane hlane
         int anchor = -1, members = 0;                 // warp-uniform: the anchor's lane, prompts that matched it so far
         uint32_t todo = __ballot_sync(0xffffffffu, cls);
+        if (trace && lane == 0 && todo) atomicAdd(&rb.stat[0], (unsigned int)__popc(todo));
         auto issue = [&](int slot, int qi) {
             if (qi >= 0) {
                 const uint32_t* sp = reinterpret_cast<const uint32_t*>(__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)tp, qi));
@@ -294,6 +301,7 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         // ... and the tokens warp-wide
         bool shared = false;
         uint32_t vm = __ballot_sync(0xffffffffu, okm);
+        if (trace && lane == 0 && vm) atomicAdd(&rb.stat[1], (unsigned int)__popc(vm));
         while (vm) {
             const int l = __ffs(vm) - 1; vm &= vm - 1;
             const uint32_t* s1 = reinterpret_cast<const uint32_t*>(__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)tp, l));
@@ -341,7 +349,7 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
 // token by token against that class's chunk (warp-wide), so that the prompt detaches at the right block.
 template <int BS>
 __global__ void __launch_bounds__(256)
-group_lists_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round, const int partial) {
+group_lists_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round, const int partial, const int trace) {
     const int lane = threadIdx.x & 31;
     const unsigned int n_act = rb.n_act[cur];
     const unsigned int total_warps = gridDim.x * (blockDim.x / 32);
@@ -387,6 +395,7 @@ group_lists_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         }
         int dshare = dknown;
         uint32_t wm = __ballot_sync(0xffffffffu, nbc > 0);
+        if (trace && lane == 0 && wm) atomicAdd(&rb.stat[2], (unsigned int)__popc(wm));
         while (wm) {
             const int l = __ffs(wm) - 1; wm &= wm - 1;
             const uint32_t* s1 = reinterpret_cast<const uint32_t*>(__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)tp, l));
@@ -429,7 +438,7 @@ group_lists_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
 // ---- kernel H ---------------------------------------------------------------------------------
 template <int BS>
 __global__ void __launch_bounds__(kHashThreads, 3)
-hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round) {
+hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round, const int trace) {
     static_assert(BS == 16, "staging pattern is written for 16-token blocks");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     using SM = HashSmem<BS>;
@@ -463,6 +472,7 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
             h = round == 0 ? t.init_hash : rb.hstate[p];
         }
         const int nb_max = __reduce_max_sync(0xffffffffu, nb);
+        if (trace) { const unsigned int nbs = __reduce_add_sync(0xffffffffu, (unsigned int)nb); if (lane == 0 && nbs) atomicAdd(&rb.stat[3], nbs); }
         // stage chunk c (kHashChunk blocks) of every lane's prompt: 4*kHashChunk lanes move one prompt's contiguous bytes.
         auto stage = [&](int s, int c) {
             const int b0 = c * kHashChunk;
@@ -712,28 +722,14 @@ walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
 // ---- kernel R: followers take their representative's outcome --------------------------------------------------
 // Lane per follower.  Representative continues: so does the follower, with the representative's chain state, and its
 // walk state stays where the representative left it (src).  Representative finished: same pods, same scores -- the warp
-// writes the follower's result from the representative's final state.
+// writes the follower's result from the representative's final state.  Either way the follower's slot takes the
+// representative's fate, for kernel C.
 __device__ __forceinline__ void resolve_round(const TableView& t, const ScoreArgs& a, const RoundBufs& rb, const int cur, const int round,
                                               const unsigned int bid, const unsigned int nbl, const uint64_t l2pol) {
     const int lane = threadIdx.x & 31;
     {   // kernel P is done with need_snap: clear it for the next round
         uint32_t* f4 = reinterpret_cast<uint32_t*>(rb.need_snap);
         for (size_t x = bid * (size_t)blockDim.x + threadIdx.x; x < rb.part_size / 4; x += (size_t)nbl * blockDim.x) f4[x] = 0u;
-    }
-    {                                                          // representatives that continue (walk_round_kernel leaves the list to us)
-        const unsigned int n_a = rb.n_hl[0];
-        const unsigned int tw = nbl * (blockDim.x / 32);
-        for (unsigned int w = bid * (blockDim.x / 32) + (threadIdx.x >> 5); w * 32u < n_a; w += tw) {
-            const unsigned int i = w * 32u + lane;
-            const unsigned int li = i < n_a ? rb.hl[i] : 0u;
-            const bool more = i < n_a && rb.fate[li] == kFateMore;
-            const uint32_t mm = __ballot_sync(0xffffffffu, more);
-            if (!mm) continue;
-            unsigned int base = 0;
-            if (lane == 0) base = atomicAdd(&rb.n_act[cur ^ 1], (unsigned int)__popc(mm));
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (more) { const unsigned int ns = base + __popc(mm & ((1u << lane) - 1u)); const uint32_t pp = rb.act[cur][li]; rb.act[cur ^ 1][ns] = pp; rb.lslot[pp] = ns; }
-        }
     }
     const unsigned int n_fl = rb.n_hl[1];
     const PromptState* pst_cur = rb.pst[round & 1];
@@ -745,18 +741,12 @@ __device__ __forceinline__ void resolve_round(const TableView& t, const ScoreArg
         if (have) {
             const unsigned int li = rb.fl[f], lj = rb.role[li];
             p = rb.act[cur][li]; pl = rb.act[cur][lj]; ft = rb.fate[lj];
+            rb.fate[li] = ft;
         }
         const bool more = have && ft == kFateMore;
-        const uint32_t mm = __ballot_sync(0xffffffffu, more);
-        if (mm) {
-            unsigned int base = 0;
-            if (lane == 0) base = atomicAdd(&rb.n_act[cur ^ 1], (unsigned int)__popc(mm));
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (more) {
-                { const unsigned int ns = base + __popc(mm & ((1u << lane) - 1u)); rb.act[cur ^ 1][ns] = p; rb.lslot[p] = ns; }
-                rb.src[p] = pl;
-                rb.hstate[p] = rb.hstate[pl]; rb.pos[p] = rb.pos[pl];
-            }
+        if (more) {
+            rb.src[p] = pl;
+            rb.hstate[p] = rb.hstate[pl]; rb.pos[p] = rb.pos[pl];
         }
         uint32_t dm = __ballot_sync(0xffffffffu, have && !more);
         while (dm) {
@@ -894,19 +884,13 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
             }
         }
         // continue on its own next round, or write the result
-        const uint32_t mm = __ballot_sync(0xffffffffu, more);
-        if (mm) {
-            unsigned int base = 0;
-            if (lane == 0) base = atomicAdd(&rb.n_act[cur ^ 1], (unsigned int)__popc(mm));
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (more) {
-                { const unsigned int ns = base + __popc(mm & ((1u << lane) - 1u)); rb.act[cur ^ 1][ns] = p; rb.lslot[p] = ns; }
-                rb.hstate[p] = h; rb.src[p] = p; rb.pos[p] = pos0 + adv;
-                PromptState& ps = pst_cur[p];
-                ps.k = (uint8_t)s.k; ps.alive = (uint16_t)s.alive;
-                ps.pat[5] = 0xffffffffu;                        // no cached slot pattern: the next block is scored the long way
-                for (uint32_t q = 0; q < s.k; ++q) { ps.sc[q] = s.sc[q]; ps.pod[q] = s.pod[q]; ps.bt[q] = 0xffu; }
-            }
+        if (have) rb.fate[rb.dl[f]] = more ? kFateMore : kFateDone;
+        if (more) {
+            rb.hstate[p] = h; rb.src[p] = p; rb.pos[p] = pos0 + adv;
+            PromptState& ps = pst_cur[p];
+            ps.k = (uint8_t)s.k; ps.alive = (uint16_t)s.alive;
+            ps.pat[5] = 0xffffffffu;                        // no cached slot pattern: the next block is scored the long way
+            for (uint32_t q = 0; q < s.k; ++q) { ps.sc[q] = s.sc[q]; ps.pod[q] = s.pod[q]; ps.bt[q] = 0xffu; }
         }
         for (uint32_t q = 0; q < s.k; ++q) { sm.sc[q][lane] = s.sc[q]; sm.pod[q][lane] = s.pod[q]; }
         __syncwarp();
@@ -936,10 +920,9 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
     }
 }
 
-// Kernels R and D in one launch (they work on different lists and neither reads what the other writes, except the next
-// live list, which both append to).
+// Kernels R and D in one launch (they work on different lists and neither reads what the other writes).
 template <int BS>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, 4)       // (4: 64 registers, what it used anyway; left free, ptxas picks 48 and spills)
 finish_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round, const int detach, const int trace) {
     extern __shared__ __align__(16) unsigned char smem_raw_f[];
     DetachWarp* sm = reinterpret_cast<DetachWarp*>(smem_raw_f);
@@ -950,6 +933,84 @@ finish_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, co
     if (gridDim.x < 2) { resolve_round(t, a, rb, cur, round, 0, 1, l2pol); detach_round<BS>(t, a, rb, cur, round, trace, sm, 0, 1, l2pol); }
     else if (blockIdx.x & 1) { if (blockIdx.x / 2 < half) resolve_round(t, a, rb, cur, round, blockIdx.x / 2, half, l2pol); }
     else detach_round<BS>(t, a, rb, cur, round, trace, sm, blockIdx.x / 2, (gridDim.x + 1) / 2, l2pol);
+}
+
+// ---- kernel C: next round's live list --------------------------------------------------------------------------
+// The prompts whose fate is kFateMore, in the order of this round's list.  A prompt that leaves never comes back, so a
+// stable compaction keeps the round-0 order (sorted by prefix) in every round: class-mates stay list neighbours, and kernel
+// G's anchor takes them without the election and its second read of two chunks.  One pass: a CTA counts its tile, publishes
+// the count, adds up its predecessors' published counts (decoupled look-back) and writes its prompts from there.  A tile's
+// status word carries round + 1 in its upper half, so a word of an earlier round of the batch reads as not yet published.
+constexpr int kCompactThreads = 256;
+constexpr int kCompactItems = 8;                           // consecutive live slots per thread
+constexpr int kCompactTile = kCompactThreads * kCompactItems;
+constexpr unsigned long long kScanDone = 1ull << 31;       // the word holds the tile's inclusive prefix, not only its own count
+
+__global__ void __launch_bounds__(kCompactThreads)
+compact_round_kernel(const RoundBufs rb, const int cur, const int round) {
+    __shared__ unsigned int s_warp[kCompactThreads / 32];
+    __shared__ unsigned int s_base;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const unsigned int n_act = rb.n_act[cur];
+    const unsigned int tile = blockIdx.x;
+    const unsigned int i0 = tile * (unsigned)kCompactTile;
+    if (tile > 0 && i0 >= n_act) return;                   // nothing of the list here, and no later tile looks back this far
+    const unsigned int s0 = i0 + threadIdx.x * (unsigned)kCompactItems;
+    uint32_t m = 0;                                        // bit k: slot s0 + k continues
+    if (s0 + kCompactItems <= n_act) {
+        const uint2 f = *reinterpret_cast<const uint2*>(rb.fate + s0);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            if (((f.x >> (8 * k)) & 0xffu) == kFateMore) m |= 1u << k;
+            if (((f.y >> (8 * k)) & 0xffu) == kFateMore) m |= 16u << k;
+        }
+    } else {
+        for (int k = 0; k < kCompactItems && s0 + k < n_act; ++k)
+            if (rb.fate[s0 + k] == kFateMore) m |= 1u << k;
+    }
+    // offset of this thread's slots within the tile
+    const unsigned int c = __popc(m);
+    unsigned int incl = c;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const unsigned int v = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += v; }
+    if (lane == 31) s_warp[wid] = incl;
+    __syncthreads();
+    unsigned int wbase = 0, agg = 0;
+#pragma unroll
+    for (int w = 0; w < kCompactThreads / 32; ++w) { const unsigned int v = s_warp[w]; wbase += w < wid ? v : 0u; agg += v; }
+    // offset of the tile within the list
+    if (wid == 0) {
+        const unsigned long long tag = (unsigned long long)(round + 1) << 32;
+        volatile unsigned long long* st = rb.scan;
+        if (lane == 0) st[tile] = tag | (tile == 0 ? kScanDone : 0ull) | agg;
+        unsigned int excl = 0;
+        if (tile > 0) {
+            for (int j = (int)tile - 1 - lane;; j -= 32) {          // lane l reads the (l+1)-th nearest predecessor not yet added
+                unsigned long long s;
+                for (;;) {
+                    s = j >= 0 ? st[j] : (tag | kScanDone);         // before tile 0: a prefix of zero
+                    if (__all_sync(0xffffffffu, (s & ~0xffffffffull) == tag)) break;
+                    __nanosleep(64);
+                }
+                const uint32_t done = __ballot_sync(0xffffffffu, (s & kScanDone) != 0ull);
+                const int last = done ? __ffs(done) - 1 : 31;       // nearest predecessor whose word is a full prefix
+                excl += __reduce_add_sync(0xffffffffu, lane <= last ? (unsigned int)(s & (kScanDone - 1)) : 0u);
+                if (done) break;
+            }
+            if (lane == 0) st[tile] = tag | kScanDone | (excl + agg);
+        }
+        if (lane == 0) s_base = excl;
+    }
+    __syncthreads();
+    unsigned int at = s_base + wbase + incl - c;
+    const uint32_t* act = rb.act[cur];
+    uint32_t* nxt = rb.act[cur ^ 1];
+    while (m) {
+        const int k = __ffs(m) - 1; m &= m - 1;
+        const uint32_t p = act[s0 + k];
+        nxt[at] = p; rb.lslot[p] = at; ++at;
+    }
+    if (threadIdx.x == 0 && (n_act == 0 || (n_act - 1) / (unsigned)kCompactTile == tile)) rb.n_act[cur ^ 1] = s_base + agg;
 }
 
 // List setup + a 64-bit fingerprint of every prompt's first block.  The batch is then radix-sorted by fingerprint so

@@ -162,7 +162,7 @@ struct kvidx {
     int64_t rounds_min = 2048;     // batches at least this large (and above coop_max) use the round pipeline
     int64_t classes_min = 131072;  // ... and at least this large, the prefix-class round pipeline
     double classes_min_sharing = 0.85;   // ... if at least this fraction of the batch follows a representative in round 0
-    DevBuf r_act0, r_act1, r_cnt, r_hstate, r_keys, r_pst, r_nbr, r_fp, r_sort, r_role, r_hl, r_map, r_src, r_fate, r_anch, r_snap, r_rec;
+    DevBuf r_act0, r_act1, r_cnt, r_hstate, r_keys, r_pst, r_nbr, r_fp, r_sort, r_role, r_hl, r_map, r_src, r_fate, r_anch, r_snap, r_rec, r_scan;
     int64_t host_chunk_tokens = 32ll << 20;   // tokens per H2D chunk of the host-buffer pipeline
     int rounds_trace = 0;
     int rounds_grid[5] = {2, 4, 2, 4, 4};   // CTAs per SM a part's group / lists / hash / walk / finish kernel may occupy (multi-part runs)
@@ -337,7 +337,8 @@ int launch_score_rounds_plain(kvidx* x, const uint32_t* d_tok, const int64_t* d_
                               int64_t max_blocks);
 
 // Batch setup of both round pipelines: clear the counters in r_cnt (part q's list lengths at word 8 * q, the batch's largest
-// block count and the distinct-prefix count as two 64-bit words at word 8 * kMaxParts), fingerprint every prompt's first
+// block count and the distinct-prefix count as two 64-bit words at word 8 * kMaxParts, part q's four trace counters of the
+// class pipeline at word 8 * kMaxParts + 4 + 4 * q), fingerprint every prompt's first
 // block and set the parts' first list lengths (rounds_init_kernel), and with sort_prefix order the batch by fingerprint into
 // r_act0.  *fp_sorted (if not null): the sorted fingerprints.
 int rounds_setup(kvidx* x, const ScoreArgs& a, const PartSizes& ps, cudaStream_t st, const uint64_t** fp_sorted) {
@@ -363,7 +364,7 @@ int rounds_setup(kvidx* x, const ScoreArgs& a, const PartSizes& ps, cudaStream_t
     return 0;
 }
 
-// Large batches: rounds of group / hash / walk / resolve kernels (kernels_rounds.cuh).  max_blocks < 0: computed on the
+// Large batches: rounds of group / hash / walk / resolve / compact kernels (kernels_rounds.cuh).  max_blocks < 0: computed on the
 // device.  The sorted batch is split into parts that run their rounds on separate streams, so that one part's
 // latency-bound kernels (the serial FNV chain of few representatives, the dependent probes) share the SMs with
 // another part's bandwidth-bound ones.
@@ -386,6 +387,8 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
         int64_t at = 0;
         for (int q = 0; q < np; ++q) { poff[q] = at; psz[q] = std::max<int64_t>(0, std::min(per, n - at)); at += psz[q]; }
     }
+    const int64_t ctiles = (psz[0] + kCompactTile - 1) / kCompactTile;      // kernel C's tiles per part (part 0 is the largest)
+    CK(x->r_scan.need((size_t)std::max<int64_t>(ctiles, 1) * np * 8));
     const uint64_t map_slots = pow2ceil((uint64_t)std::max<int64_t>(4 * ((n + np - 1) / np), 1024));
     const size_t gstride = map_slots + (size_t)((((n + np - 1) / np) + 32 + 3) & ~3ll);      // election map + grp per part, cleared together
     CK(x->r_map.need(gstride * 4 * np));
@@ -397,6 +400,7 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
         rb[q].act[0] = x->r_act0.as<uint32_t>() + off; rb[q].act[1] = x->r_act1.as<uint32_t>() + off;
         rb[q].n_act = cnt + 8 * q;
         rb[q].n_hl = cnt + 8 * q + 2;
+        rb[q].stat = cnt + 8 * kMaxParts + 4 + 4 * q;
         rb[q].hstate = x->r_hstate.as<uint64_t>(); rb[q].src = x->r_src.as<uint32_t>();
         rb[q].pst[0] = x->r_pst.as<PromptState>(); rb[q].pst[1] = x->r_pst.as<PromptState>() + n;
         rb[q].keys = x->r_keys.as<uint64_t>() + off; rb[q].nbr = x->r_nbr.as<uint32_t>() + off; rb[q].pos = x->r_nbr.as<uint32_t>() + n;
@@ -415,6 +419,7 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
         rb[q].hl = x->r_hl.as<uint32_t>() + off; rb[q].fl = x->r_hl.as<uint32_t>() + n + off;
         rb[q].map = x->r_map.as<uint32_t>() + (size_t)q * gstride; rb[q].map_mask = (uint32_t)(map_slots - 1);
         rb[q].grp = rb[q].map + map_slots;
+        rb[q].scan = x->r_scan.as<unsigned long long>() + (size_t)q * ctiles;
     }
     ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
     PartSizes ps{};
@@ -448,6 +453,7 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
     for (int q = 1; q < kMaxParts; ++q) strm[q] = x->aux_stream[q - 1];
     CK(cudaMemsetAsync(x->r_map.p, 0xff, gstride * 4 * np, st));
     CK(cudaMemsetAsync(x->r_fate.as<uint8_t>() + 2 * n_al, 0, (size_t)n_al * 2 + 64 * kMaxParts, st));     // nfol, need_snap
+    CK(cudaMemsetAsync(x->r_scan.p, 0, (size_t)ctiles * np * 8, st));     // kernel C's tile words: nothing published
     if (np > 1) {
         CK(cudaEventRecord(x->ev_fork, st));
         for (int q = 1; q < np; ++q) CK(cudaStreamWaitEvent(strm[q], x->ev_fork, 0));
@@ -461,6 +467,8 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
     for (int q = 0; q < kMaxParts; ++q) { sS[q] = prio ? x->hp_stream[q] : strm[q]; sG[q] = prio ? x->lp_stream[q] : strm[q]; }
     if (prio) for (int q = 0; q < np; ++q) { CK(cudaStreamWaitEvent(sS[q], x->ev_fork, 0)); CK(cudaStreamWaitEvent(sG[q], x->ev_fork, 0)); }
     constexpr int T = 256, W = T / 32;                // threads / warps of the short kernels' CTAs
+    const int trace = x->rounds_trace == 1;           // count the token work of every round (kernels_rounds.cuh: RoundBufs::stat)
+    unsigned int stat0[kMaxParts][4] = {};            // ... the counts up to the last round, to print each round's own
     for (int64_t r = 0; r < rounds; ++r) {
         const int cur = (int)(r & 1);
         for (int q = 0; q < np; ++q) {
@@ -468,28 +476,33 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
             if (m <= 0) continue;
             const unsigned ggrid = (unsigned)std::min<int64_t>((m + kGroupThreads / 32 * kGroupTile - 1) / (kGroupThreads / 32 * kGroupTile), (int64_t)x->sm_count * (np == 1 ? 3 : x->rounds_grid[0]));
             if (prio && r > 0) CK(cudaStreamWaitEvent(sG[q], x->ev_r[q], 0));       // this part's previous round has built the live list
-            group_round_kernel<16><<<ggrid, kGroupThreads, sizeof(GroupSmem), sG[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup);
+            group_round_kernel<16><<<ggrid, kGroupThreads, sizeof(GroupSmem), sG[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup, trace);
             if (prio) { CK(cudaEventRecord(x->ev_g[q], sG[q])); CK(cudaStreamWaitEvent(sS[q], x->ev_g[q], 0)); }
             const unsigned lgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : x->rounds_grid[1]));
-            group_lists_kernel<16><<<lgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup >= 2);
+            group_lists_kernel<16><<<lgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup >= 2, trace);
         }
         for (int q = 0; q < np; ++q) {
             const int64_t m = psz[q];
             if (m <= 0) continue;
             const unsigned hgrid = (unsigned)std::min<int64_t>((m + kHashThreads - 1) / kHashThreads, (int64_t)x->sm_count * (np == 1 ? 4 : x->rounds_grid[2]));
-            hash_round_kernel<16><<<hgrid, kHashThreads, sizeof(HashSmem<16>), sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
+            hash_round_kernel<16><<<hgrid, kHashThreads, sizeof(HashSmem<16>), sS[q]>>>(x->tv, a, rb[q], cur, (int)r, trace);
             const unsigned wgrid = (unsigned)std::min<int64_t>((m + W - 1) / W, (int64_t)x->sm_count * (np == 1 ? 8 : x->rounds_grid[3]));
             walk_round_kernel<<<wgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
             const unsigned rgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : x->rounds_grid[4]));
             finish_round_kernel<16><<<rgrid, T, sizeof(DetachWarp) * W, sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup >= 2, x->rounds_trace);
+            compact_round_kernel<<<(unsigned)((m + kCompactTile - 1) / kCompactTile), kCompactThreads, 0, sS[q]>>>(rb[q], cur, (int)r);
             if (prio && r + 1 < rounds) CK(cudaEventRecord(x->ev_r[q], sS[q]));
-            x->launches += 5;
-            if (x->rounds_trace == 1) {      // debugging aid: list sizes of this round (synchronises)
-                unsigned int c[8];
-                CK(cudaMemcpyAsync(c, rb[q].n_act, sizeof c, cudaMemcpyDeviceToHost, sS[q]));
+            x->launches += 6;
+            if (trace) {      // debugging aid: list sizes and token work of this round (synchronises)
+                unsigned int c[256];
+                CK(cudaMemcpyAsync(c, cnt, sizeof c, cudaMemcpyDeviceToHost, sS[q]));
                 CK(cudaStreamSynchronize(sS[q]));
-                fprintf(stderr, "[kvidx rounds] round %lld part %d: live %u -> representatives %u, followers %u, partial %u (%u blocks walked alone) -> next %u\n",
-                        (long long)r, q, c[cur], c[2], c[3], c[4], c[5], c[cur ^ 1]);
+                const unsigned int* l = c + 8 * q;
+                const unsigned int* s = c + (rb[q].stat - cnt);
+                fprintf(stderr, "[kvidx rounds] round %lld part %d: live %u -> representatives %u, followers %u, partial %u (%u blocks walked alone) -> next %u;"
+                        " G streamed %u chunks, %u losers re-read, G2 compared %u, H hashed %u blocks\n",
+                        (long long)r, q, l[cur], l[2], l[3], l[4], l[5], l[cur ^ 1], s[0] - stat0[q][0], s[1] - stat0[q][1], s[2] - stat0[q][2], s[3] - stat0[q][3]);
+                for (int k = 0; k < 4; ++k) stat0[q][k] = s[k];
             }
         }
     }
@@ -1157,7 +1170,7 @@ void kvidx_destroy(kvidx_t* x) {
         if (x->ev_done[i]) cudaEventDestroy(x->ev_done[i]);
         if (x->ev_k[i]) cudaEventDestroy(x->ev_k[i]);
     }
-    x->r_act0.release(); x->r_act1.release(); x->r_cnt.release(); x->r_hstate.release(); x->r_keys.release(); x->r_pst.release(); x->r_nbr.release(); x->r_fp.release(); x->r_sort.release(); x->r_role.release(); x->r_hl.release(); x->r_map.release(); x->r_src.release(); x->r_fate.release(); x->r_anch.release(); x->r_snap.release(); x->r_rec.release();
+    x->r_act0.release(); x->r_act1.release(); x->r_cnt.release(); x->r_hstate.release(); x->r_keys.release(); x->r_pst.release(); x->r_nbr.release(); x->r_fp.release(); x->r_sort.release(); x->r_role.release(); x->r_hl.release(); x->r_map.release(); x->r_src.release(); x->r_fate.release(); x->r_anch.release(); x->r_snap.release(); x->r_rec.release(); x->r_scan.release();
     x->d_misc.release(); x->d_rmisc.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
     x->d_snap.release(); x->h_snap[0].release(); x->h_snap[1].release();
