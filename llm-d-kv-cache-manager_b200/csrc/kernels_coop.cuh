@@ -1,7 +1,8 @@
 // kernels_coop.cuh -- Score() for SMALL batches: one WARP per prompt, warp-cooperative FNV, TMA-staged tokens.
 //
-// Same reference path as kernels_score.cuh (GetPodScores steps 2-4, pkg/kvcache/indexer.go:141-163): chain keys
-// (kvblock/token_processor.go:94-162), Lookup (in_memory.go:105-146), LongestPrefixScorer.Score (kvblock_scorer.go:108-151).
+// Same reference path as every Score() kernel (GetPodScores steps 2-4, pkg/kvcache/indexer.go:141-163): chain keys
+// (kvblock/token_processor.go:94-162), Lookup (in_memory.go:105-146), LongestPrefixScorer.Score (kvblock_scorer.go:108-151);
+// the probe decision, the warp walk and the result row are the ones of score_common.cuh.
 //
 // The lane-per-prompt kernels need tens of thousands of prompts to fill the machine: one prompt is ONE serial FNV-1a
 // chain (~19 K dependent byte steps at 4 K tokens), so a single GetPodScores RPC runs at the latency of that chain.  Here
@@ -28,6 +29,7 @@
 // and the hits are scored in block order with lane q owning pod q -- the arithmetic of every other path, bit for bit.
 #pragma once
 #include <cuda_runtime.h>
+#include "score_common.cuh"
 #include "kernels_rounds.cuh"
 
 namespace kvx {
@@ -215,10 +217,7 @@ coop_score_kernel(const TableView t, const ScoreArgs a) {
         const uint32_t* tokp = a.tok + tb0;
         const bool aligned = (reinterpret_cast<uintptr_t>(tokp) & 15u) == 0;
         const uint32_t mdl = a.model ? a.model[pi] : a.model0;
-        // walk state: lane q < k owns pod q
-        uint32_t k = 0, alive = 0, mypod = 0xffffffffu, mybt = 0xffu;
-        double mysc = 0.0;
-        uint32_t pv0 = 0, pv1 = 0, pv2 = 0, pv3 = 0, pv4 = 0, pvc = 0xffffffffu;
+        WarpWalk ws;
         uint64_t h = t.init_hash;
         auto stage = [&](int c) {                                         // chunk c -> buffer c & 1
             const int nbc = min(kRoundBlocks, nblk - c * kRoundBlocks);
@@ -247,18 +246,14 @@ coop_score_kernel(const TableView t, const ScoreArgs a) {
             uint4 A0 = {0, 0, 0, 0}, B0 = {0, 0, 0, 0}, A1 = {0, 0, 0, 0}, B1 = {0, 0, 0, 0};
             const ReqSlot* base = t.req; uint64_t slot = 0;
             bool issued = false, hit = false, decided = false;
-            uint32_t e0 = 0, e1 = 0, e2 = 0, e3 = 0, e4 = 0, cnt = 0;
+            SlotPat mine = {};
             auto resolve = [&]() {                                        // the slot pair has (or will have) arrived: hit or miss
-                for (;;) {
-                    uint4 A = A0, B = B0;
-                    hit = slot_matches(A, B, key, mdl);
-                    bool stop = hit || meta_state(B.w) == kStateEmpty;
-                    if (!stop) { A = A1; B = B1; hit = slot_matches(A, B, key, mdl); stop = hit || meta_state(B.w) == kStateEmpty; }
-                    if (hit) { e0 = A.z; e1 = A.w; e2 = B.x; e3 = B.y; e4 = B.z; cnt = meta_count(B.w); }
-                    if (stop) break;
+                uint4 A, B;
+                while (!pair_decides(A0, B0, A1, B1, key, mdl, A, B, hit)) {
                     slot = (slot + 2) & t.req_mask;                       // rare: displaced past the home pair
                     ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
                 }
+                if (hit) mine = SlotPat::of(A, B);
                 decided = true;
             };
             const int nhashed = coop_hash_chunk(sm, W, W.tok[c & 1], h, nb, lane, lt, key, last, [&](int ndone) -> bool {
@@ -284,83 +279,12 @@ coop_score_kernel(const TableView t, const ScoreArgs a) {
             const uint32_t hm_ = __ballot_sync(0xffffffffu, hit && lane < nhashed);
             const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from the chunk's first block
             // ---- ordered scoring of the hits (kvblock_scorer.go:108-151), lane q owns pod q ----
-            uint32_t samemask;
-            {
-                const uint32_t u0 = __shfl_up_sync(0xffffffffu, e0, 1), u1 = __shfl_up_sync(0xffffffffu, e1, 1), u2 = __shfl_up_sync(0xffffffffu, e2, 1),
-                               u3 = __shfl_up_sync(0xffffffffu, e3, 1), u4 = __shfl_up_sync(0xffffffffu, e4, 1), uc = __shfl_up_sync(0xffffffffu, cnt, 1);
-                const bool sm_ = lane > 0 ? (((u0 ^ e0) | (u1 ^ e1) | (u2 ^ e2) | (u3 ^ e3) | (u4 ^ e4) | (uc ^ cnt)) == 0u)
-                                          : (c > 0 && ((pv0 ^ e0) | (pv1 ^ e1) | (pv2 ^ e2) | (pv3 ^ e3) | (pv4 ^ e4) | (pvc ^ cnt)) == 0u);
-                samemask = __ballot_sync(0xffffffffu, sm_ && lane < nhit);
-            }
-            int j = 0;
-            bool dead = false;
-            while (j < nhit && !dead) {
-                if ((samemask >> j) & 1u) {                               // same pods and tiers as the block before: the same addends again
-                    const uint32_t rest = ~(samemask >> j);
-                    const int run = min(rest ? __ffs(rest) - 1 : 32, nhit - j);
-                    if ((alive >> lane) & 1u) {
-                        const double add = mybt == 0xffu ? 0.0 : t.weight[mybt & 15u];
-                        for (int u = 0; u < run; ++u) mysc = __dadd_rn(mysc, add);
-                    }
-                    j += run;
-                    continue;
-                }
-                const uint32_t w0 = __shfl_sync(0xffffffffu, e0, j), w1 = __shfl_sync(0xffffffffu, e1, j), w2 = __shfl_sync(0xffffffffu, e2, j),
-                               w3 = __shfl_sync(0xffffffffu, e3, j), w4 = __shfl_sync(0xffffffffu, e4, j), cj = __shfl_sync(0xffffffffu, cnt, j);
-                if (c == 0 && j == 0) {
-                    // activePods := pods of block 0 (after the filter), in entry order; score = max weight   (kvblock_scorer.go:118-128)
-                    const uint64_t* frow = filter_row(a.filter, pi, t.filter_words);
-                    k = 0;
-                    for (uint32_t e = 0; e < cj; ++e) {
-                        const uint32_t pt = ent_of(w0, w1, w2, w3, w4, (int)e), pd = pt >> 4;
-                        if (frow && !filter_has(frow, pd)) continue;
-                        const double wt = t.weight[pt & 15u];
-                        const uint32_t own = __ballot_sync(0xffffffffu, (uint32_t)lane < k && mypod == pd);
-                        const int q = own ? __ffs(own) - 1 : (int)k;
-                        if (!own) { if (lane == q) { mypod = pd; mysc = 0.0; mybt = 0xffu; } ++k; }
-                        if (lane == q && wt > mysc) { mysc = wt; mybt = pt & 15u; }
-                    }
-                    alive = (1u << k) - 1u;
-                } else {
-                    // activePods &= pods(block); score[p] += max weight, in block order   (kvblock_scorer.go:130-147)
-                    bool present = false; double mx = 0.0; uint32_t bt = 0xffu;
-                    if ((alive >> lane) & 1u) {
-                        for (uint32_t e = 0; e < cj; ++e) {
-                            const uint32_t pt = ent_of(w0, w1, w2, w3, w4, (int)e);
-                            if ((pt >> 4) == mypod) { present = true; const double wt = t.weight[pt & 15u]; if (wt > mx) { mx = wt; bt = pt & 15u; } }
-                        }
-                        if (present) { mysc = __dadd_rn(mysc, mx); mybt = bt; }
-                    }
-                    alive = __ballot_sync(0xffffffffu, present);
-                }
-                if (!alive) dead = true;
-                ++j;
-            }
-            if (j > 0) {
-                const int lj = j - 1;
-                pv0 = __shfl_sync(0xffffffffu, e0, lj); pv1 = __shfl_sync(0xffffffffu, e1, lj); pv2 = __shfl_sync(0xffffffffu, e2, lj);
-                pv3 = __shfl_sync(0xffffffffu, e3, lj); pv4 = __shfl_sync(0xffffffffu, e4, lj); pvc = __shfl_sync(0xffffffffu, cnt, lj);
-            }
-            if (dead || nhit < nb || !has_more) done = true;
+            ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, c > 0, nhit), c == 0, a.filter, pi, [](int) {});
+            if (!ws.alive || nhit < nb || !has_more) done = true;
             h = last;
         }
         // ---- result ----
-        if (a.dense) {
-            double* row = a.dense + pi * (long long)t.max_pods;
-            const uint32_t P = t.max_pods;
-            if ((P & 1u) == 0 && ((reinterpret_cast<uintptr_t>(row) & 15u) == 0)) {
-                for (uint32_t c2 = lane * 2; c2 < P; c2 += 64) st_stream_f64x2(row + c2, -1.0, -1.0, l2pol);
-            } else {
-                for (uint32_t c2 = lane; c2 < P; c2 += 32) row[c2] = -1.0;
-            }
-            __syncwarp();
-            if ((uint32_t)lane < k && mypod < P) row[mypod] = mysc;
-        }
-        if (a.sp_cnt) {
-            if ((uint32_t)lane < k) { a.sp_pods[pi * kMaxEnt + lane] = (uint16_t)mypod; a.sp_scores[pi * kMaxEnt + lane] = mysc; }
-            if (lane == 0) a.sp_cnt[pi] = (uint8_t)k;
-        }
-        if (a.has_keys && lane == 0) a.has_keys[pi] = nblk > 0;
+        warp_write_row(t, a, pi, ws.k, ws.pod, ws.sc, nblk > 0, l2pol);
         // a chunk that was prefetched but never consumed (the walk ended before it) still lands in its buffer: let it, so that
         // the buffer and its barrier are free for the next prompt
         if (aligned && consumed < nchunks && consumed > 0) { mbar_wait(&W.bar[consumed & 1], (phases >> (consumed & 1)) & 1u); phases ^= 1u << (consumed & 1); }

@@ -1,7 +1,8 @@
 // kernels_rounds.cuh -- Score() for LARGE batches: rounds over PREFIX CLASSES.
 //
-// Same reference path as kernels_score.cuh (GetPodScores steps 2-4, pkg/kvcache/indexer.go:141-163): chain keys
-// (token_processor.go:94-162), Lookup (in_memory.go:105-146), LongestPrefixScorer.Score (kvblock_scorer.go:108-151).
+// Same reference path as every Score() kernel (GetPodScores steps 2-4, pkg/kvcache/indexer.go:141-163): chain keys
+// (token_processor.go:94-162), Lookup (in_memory.go:105-146), LongestPrefixScorer.Score (kvblock_scorer.go:108-151); the
+// probe, the fold and the result row are the ones of score_common.cuh.
 //
 // A large batch repeats itself: thousands of prompts share a system prompt or a document, and the per-prompt kernels
 // hash and probe that shared prefix once per prompt.  Here the batch is processed in rounds of kRoundBlocks blocks, and
@@ -24,7 +25,7 @@
 // on separate streams), so medium batches use kernels_rounds_plain.cuh instead (see kvidx.cu: launch_score).
 #pragma once
 #include <cuda_runtime.h>
-#include "kernels_score.cuh"
+#include "score_common.cuh"
 
 namespace kvx {
 
@@ -99,10 +100,8 @@ struct RoundBufs {
 };
 constexpr uint8_t kFateMore = 1, kFateDone = 2;
 
-constexpr int kHashChunk = 1;            // blocks staged per copy step (2 = 128-byte accesses: fewer, longer DRAM accesses
-                                         // but only 24 resident warps/SM, and the kernel is pipe bound)
 template <int BS> struct HashSmem {
-    static constexpr int kRow = kHashChunk * BS * 4 + 16;   // 144 B: the four LDS.128 of a block stay conflict free
+    static constexpr int kRow = BS * 4 + 16;                 // 80 B: the four LDS.128 of a block stay conflict free
     unsigned char tok[kHashThreads / 32][kHashStages][32 * kRow];     // [warps of the CTA]: a launch with fewer warps passes that much less
 };
 
@@ -473,69 +472,36 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
         }
         const int nb_max = __reduce_max_sync(0xffffffffu, nb);
         if (trace) { const unsigned int nbs = __reduce_add_sync(0xffffffffu, (unsigned int)nb); if (lane == 0 && nbs) atomicAdd(&rb.stat[3], nbs); }
-        // stage chunk c (kHashChunk blocks) of every lane's prompt: 4*kHashChunk lanes move one prompt's contiguous bytes.
+        // stage block c of every lane's prompt: 4 lanes move one prompt's 64 bytes, 8 prompts per copy instruction
         auto stage = [&](int s, int c) {
-            const int b0 = c * kHashChunk;
-            const bool issue = b0 < nb;
-            const int nbytes = issue ? min(kHashChunk, nb - b0) * BS * 4 : 0;
-            const unsigned long long srcv = (issue && aligned) ? (unsigned long long)(uintptr_t)(src + (size_t)b0 * BS) : 0ull;
+            const bool issue = c < nb;
+            const unsigned long long srcv = (issue && aligned) ? (unsigned long long)(uintptr_t)(src + (size_t)c * BS) : 0ull;
             __syncwarp();
-            constexpr int LPP = 4 * kHashChunk;             // lanes that move one prompt's chunk (16 B each)
-            constexpr int PPI = 32 / LPP;                   // prompts per copy instruction
 #pragma unroll
-            for (int r = 0; r < 32 / PPI; ++r) {
-                const int q = PPI * r + lane / LPP;
+            for (int r = 0; r < 4; ++r) {
+                const int q = 8 * r + lane / 4;
                 const unsigned long long sp = __shfl_sync(0xffffffffu, srcv, q);
-                const int nby = kHashChunk == 1 ? BS * 4 : __shfl_sync(0xffffffffu, nbytes, q);
-                if (sp && (lane % LPP) * 16 < nby)
-                    cp_async_16_stream(smem_addr(&sm.tok[wid][s][q * SM::kRow + (lane % LPP) * 16]), reinterpret_cast<const char*>(sp) + (lane % LPP) * 16, l2pol);
+                if (sp) cp_async_16_stream(smem_addr(&sm.tok[wid][s][q * SM::kRow + (lane % 4) * 16]), reinterpret_cast<const char*>(sp) + (lane % 4) * 16, l2pol);
             }
             cp_async_commit();
             if (issue && !aligned) {
                 uint32_t* dst = reinterpret_cast<uint32_t*>(&sm.tok[wid][s][lane * SM::kRow]);
-                const uint32_t* g = src + (size_t)b0 * BS;
-                for (int j = 0; j < nbytes / 4; ++j) dst[j] = __ldg(g + j);
+                const uint32_t* g = src + (size_t)c * BS;
+                for (int j = 0; j < BS; ++j) dst[j] = __ldg(g + j);
             }
         };
 #pragma unroll
         for (int c = 0; c < kHashStages - 1; ++c) stage(c, c);
-        const int nchunks = (nb_max + kHashChunk - 1) / kHashChunk;
-        for (int c = 0; c < nchunks; ++c) {
+        for (int c = 0; c < nb_max; ++c) {
             stage((c + kHashStages - 1) % kHashStages, c + kHashStages - 1);
             cp_async_wait<kHashStages - 1>();
             __syncwarp();
-#pragma unroll
-            for (int u = 0; u < kHashChunk; ++u) {
-                const int b = c * kHashChunk + u;
-                Fnv f;
-                f.begin_block(h, BS);
-                const uint4* tp = reinterpret_cast<const uint4*>(&sm.tok[wid][c % kHashStages][lane * SM::kRow + u * BS * 4]);
-                const uint4 v0 = tp[0], v1 = tp[1];
-                f.token(v0.x); f.token(v0.y); f.token(v0.z); f.token(v0.w);
-                const uint4 v2 = tp[2];
-                f.token(v1.x); f.token(v1.y); f.token(v1.z); f.token(v1.w);
-                const uint4 v3 = tp[3];
-                f.token(v2.x); f.token(v2.y); f.token(v2.z); f.token(v2.w);
-                f.token(v3.x); f.token(v3.y); f.token(v3.z); f.token(v3.w);
-                const uint64_t key = f.end_block();
-                if (b < nb) { h = key; rb.keys[(size_t)b * a.n_prompts + i] = key; }
-            }
+            const uint64_t key = hash_row16(h, &sm.tok[wid][c % kHashStages][lane * SM::kRow]);
+            if (c < nb) { h = key; rb.keys[(size_t)c * a.n_prompts + i] = key; }
         }
         cp_async_wait<0>();
         __syncwarp();
     }
-}
-
-// ---- helpers shared with kernels_rounds_plain.cuh ---------------------------------------------
-__device__ __forceinline__ void ld_slot_pair(const ReqSlot* s, bool peer, uint4& a0, uint4& b0, uint4& a1, uint4& b1) {
-    ld_slot(s, peer, a0, b0);
-    ld_slot(s + 1, peer, a1, b1);
-}
-
-// entry j (0..9) of a slot whose words live in this lane's registers
-__device__ __forceinline__ uint32_t ent_of(uint32_t e0, uint32_t e1, uint32_t e2, uint32_t e3, uint32_t e4, int j) {
-    const uint32_t word = j < 2 ? e0 : j < 4 ? e1 : j < 6 ? e2 : j < 8 ? e3 : e4;
-    return (j & 1) ? (word >> 16) : (word & 0xffffu);
 }
 
 // ---- kernel P: warp per representative ------------------------------------------------------------------------
@@ -557,7 +523,7 @@ walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
     const unsigned int total_warps = gridDim.x * (blockDim.x / 32);
     for (unsigned int i = blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5); i < n_a; i += total_warps) {
         const uint4 rc = __ldg(rb.rec + i);
-        uint64_t key = rb.keys[(size_t)lane * kstride + i];   // lanes >= nb read a stale key and ignore it
+        const uint64_t key = rb.keys[(size_t)lane * kstride + i];   // lanes >= nb read a stale key and ignore it
         const unsigned int li = rc.y;
         const uint32_t p = rc.x;
         const uint32_t meta = rc.z;
@@ -565,156 +531,43 @@ walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
         const bool has_more = (meta >> 8) & 1u;
         const uint32_t mdl = a.model ? a.model[p] : a.model0;
         const bool snapf = rb.need_snap[li];
-        // walk state: lane q < k owns pod q
-        uint32_t k = 0, alive = 0, mypod = 0xffffffffu, mybt = 0xffu;
-        double mysc = 0.0;
-        uint32_t pv0 = 0, pv1 = 0, pv2 = 0, pv3 = 0, pv4 = 0, pvc = 0xffffffffu;
-        if (round > 0) {
-            const PromptState& ps = pst_prev[rc.w];
-            k = ps.k; alive = ps.alive;
-            pv0 = ps.pat[0]; pv1 = ps.pat[1]; pv2 = ps.pat[2]; pv3 = ps.pat[3]; pv4 = ps.pat[4]; pvc = ps.pat[5];
-            if ((uint32_t)lane < k) { mysc = ps.sc[lane]; mypod = ps.pod[lane]; mybt = ps.bt[lane]; }
-        }
+        WarpWalk ws;
+        if (round > 0) ws.load(pst_prev[rc.w], lane);
         // probe: lane j looks up block j's key
-        uint32_t e0 = 0, e1 = 0, e2 = 0, e3 = 0, e4 = 0, cnt = 0;
+        SlotPat mine = {};
         bool hit = false;
         if (lane < nb) {
-            const uint64_t hm = home_of(key, mdl);
-            const ReqSlot* base = t.req_peer[shard_of(hm, t.shard_bits)];
-            uint64_t slot = hm & t.req_mask & ~1ull;
-            // A local probe fetches the aligned slot PAIR (one 64-byte DRAM access).  On a peer GPU's shard every byte crosses
-            // NVLink, and at load <= 0.25 the home slot alone decides ~9 probes out of 10: fetch it first, its neighbour only
-            // if needed (halves the NVLink bytes of a sharded step).
-            const bool remote = base != t.req && !t.peer_pair;
-            for (;;) {
-                uint4 A0, B0, A1, B1;
-                ld_slot(base + slot, peer, A0, B0);
-                if (!remote) ld_slot(base + slot + 1, peer, A1, B1);
-                uint4 A = A0, B = B0;
-                hit = slot_matches(A, B, key, mdl);
-                bool stop = hit || meta_state(B.w) == kStateEmpty;
-                if (!stop) {
-                    if (remote) ld_slot(base + slot + 1, peer, A1, B1);
-                    A = A1; B = B1; hit = slot_matches(A, B, key, mdl); stop = hit || meta_state(B.w) == kStateEmpty;
-                }
-                if (hit) { e0 = A.z; e1 = A.w; e2 = B.x; e3 = B.y; e4 = B.z; cnt = meta_count(B.w); }
-                if (stop) break;
-                slot = (slot + 2) & t.req_mask;                         // rare: displaced past the home pair
-            }
+            HomeProbe pr;
+            uint4 A, B;
+            hit = pr.find(t, key, mdl, peer, A, B);
+            if (hit) mine = SlotPat::of(A, B);
         }
         const uint32_t hm_ = __ballot_sync(0xffffffffu, hit);
         const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from block 0 (lanes >= nb never hit)
-        uint32_t nwalk = 0;
-        bool done = nb == 0;
-        // blocks whose slot holds the same pods and tiers as the block before: every live pod gets the same addend again,
-        // so a run of them is a run of in-order additions (most documents live on the same pods block after block)
-        uint32_t samemask;
-        {
-            const uint32_t u0 = __shfl_up_sync(0xffffffffu, e0, 1), u1 = __shfl_up_sync(0xffffffffu, e1, 1), u2 = __shfl_up_sync(0xffffffffu, e2, 1),
-                           u3 = __shfl_up_sync(0xffffffffu, e3, 1), u4 = __shfl_up_sync(0xffffffffu, e4, 1), uc = __shfl_up_sync(0xffffffffu, cnt, 1);
-            bool sm_ = lane > 0 ? (((u0 ^ e0) | (u1 ^ e1) | (u2 ^ e2) | (u3 ^ e3) | (u4 ^ e4) | (uc ^ cnt)) == 0u)
-                                : (round > 0 && ((pv0 ^ e0) | (pv1 ^ e1) | (pv2 ^ e2) | (pv3 ^ e3) | (pv4 ^ e4) | (pvc ^ cnt)) == 0u);
-            samemask = __ballot_sync(0xffffffffu, sm_ && lane < nhit);
-        }
-        int j = 0;
-        while (j < nhit && !done) {
-            if ((samemask >> j) & 1u) {
-                const uint32_t rest = ~(samemask >> j);
-                const int run = min(rest ? __ffs(rest) - 1 : 32, nhit - j);           // >= 1
-                const bool mine = (alive >> lane) & 1u;
-                const double add = mybt == 0xffu ? 0.0 : t.weight[mybt & 15u];
-                int u = 0;
-                if (j == 0) {                                  // the chunk opens inside a run: its first block is the snapshot
-                    if (mine) mysc = __dadd_rn(mysc, add);
-                    if (snapf) {
-                        if ((uint32_t)lane < k) { rb.snap_sc[(size_t)i * kRoundBlocks * kMaxEnt + lane] = mysc; rb.snap_bt[(size_t)i * kRoundBlocks * kMaxEnt + lane] = (uint8_t)mybt; }
-                        if (lane == 0) rb.snap_alive[(size_t)i * kRoundBlocks] = (uint16_t)alive;
-                    }
-                    u = 1;
-                }
-                if (mine) for (; u < run; ++u) mysc = __dadd_rn(mysc, add);
-                j += run;
-                nwalk = (uint32_t)j;
-                continue;
-            }
-            const uint32_t w0 = __shfl_sync(0xffffffffu, e0, j), w1 = __shfl_sync(0xffffffffu, e1, j), w2 = __shfl_sync(0xffffffffu, e2, j),
-                           w3 = __shfl_sync(0xffffffffu, e3, j), w4 = __shfl_sync(0xffffffffu, e4, j), c = __shfl_sync(0xffffffffu, cnt, j);
-            const bool first_block = round == 0 && j == 0;
-            if (first_block) {
-                // activePods := pods of block 0 (after the filter), in entry order; score = max weight   (kvblock_scorer.go:118-128)
-                const uint64_t* frow = filter_row(a.filter, p, t.filter_words);
-                k = 0;
-                for (uint32_t e = 0; e < c; ++e) {
-                    const uint32_t pt = ent_of(w0, w1, w2, w3, w4, (int)e), pd = pt >> 4;
-                    if (frow && !filter_has(frow, pd)) continue;
-                    const double wt = t.weight[pt & 15u];
-                    const uint32_t own = __ballot_sync(0xffffffffu, (uint32_t)lane < k && mypod == pd);
-                    const int q = own ? __ffs(own) - 1 : (int)k;
-                    if (!own) { if (lane == q) { mypod = pd; mysc = 0.0; mybt = 0xffu; } ++k; }
-                    if (lane == q && wt > mysc) { mysc = wt; mybt = pt & 15u; }
-                }
-                alive = (1u << k) - 1u;
-            } else {
-                // activePods &= pods(block); score[p] += max weight, in block order   (kvblock_scorer.go:130-147)
-                bool present = false; double mx = 0.0; uint32_t bt = 0xffu;
-                if ((alive >> lane) & 1u) {
-                    for (uint32_t e = 0; e < c; ++e) {
-                        const uint32_t pt = ent_of(w0, w1, w2, w3, w4, (int)e);
-                        if ((pt >> 4) == mypod) { present = true; const double wt = t.weight[pt & 15u]; if (wt > mx) { mx = wt; bt = pt & 15u; } }
-                    }
-                    if (present) { mysc = __dadd_rn(mysc, mx); mybt = bt; }
-                }
-                alive = __ballot_sync(0xffffffffu, present);
-            }
-            if (!alive) done = true;
-            else {
-                nwalk = (uint32_t)j + 1u;
-                if (snapf) {
-                    if ((uint32_t)lane < k) { rb.snap_sc[((size_t)i * kRoundBlocks + j) * kMaxEnt + lane] = mysc; rb.snap_bt[((size_t)i * kRoundBlocks + j) * kMaxEnt + lane] = (uint8_t)mybt; }
-                    if (lane == 0) rb.snap_alive[(size_t)i * kRoundBlocks + j] = (uint16_t)alive;
-                }
-            }
-            ++j;
-        }
+        const uint32_t samemask = ws.same_mask(lane, mine, round > 0, nhit);
+        // snapshot of the walk state at every run start
+        const int j = ws.walk<true>(t, lane, mine, nhit, samemask, round == 0, a.filter, p, [&](int b) {
+            if (!snapf) return;
+            const size_t sb = (size_t)i * kRoundBlocks + b;
+            if ((uint32_t)lane < ws.k) { rb.snap_sc[sb * kMaxEnt + lane] = ws.sc; rb.snap_bt[sb * kMaxEnt + lane] = (uint8_t)ws.bt; }
+            if (lane == 0) rb.snap_alive[sb] = (uint16_t)ws.alive;
+        });
+        const uint32_t nwalk = (uint32_t)(j > 0 && !ws.alive ? j - 1 : j);      // blocks after which the walk was still alive
         if (snapf) {                                           // block -> first block of its run
             const uint32_t starts = ~samemask & ((2u << lane) - 1u);
             rb.snap_run[(size_t)i * kRoundBlocks + lane] = (uint8_t)(starts ? 31 - __clz(starts) : 0);
         }
-        // pattern of the last scored block, for the next round's first comparison
-        if (j > 0) {
-            const int lj = j - 1;
-            pv0 = __shfl_sync(0xffffffffu, e0, lj); pv1 = __shfl_sync(0xffffffffu, e1, lj); pv2 = __shfl_sync(0xffffffffu, e2, lj);
-            pv3 = __shfl_sync(0xffffffffu, e3, lj); pv4 = __shfl_sync(0xffffffffu, e4, lj); pvc = __shfl_sync(0xffffffffu, cnt, lj);
-        }
-        if (nhit < nb) done = true;                            // a block of the round is not in the index
+        const bool done = nb == 0 || nhit < nb || !ws.alive;   // no block, a block of the round is not in the index, or no pod left
         const bool more = !done && has_more;
         PromptState& ps = pst_cur[p];
-        if ((uint32_t)lane < k) { ps.sc[lane] = mysc; ps.pod[lane] = (uint16_t)mypod; ps.bt[lane] = (uint8_t)mybt; }
+        ws.store_lane(ps, lane);
         if (lane == 0) {
-            ps.k = (uint8_t)k; ps.alive = (uint16_t)alive;
-            ps.pat[0] = pv0; ps.pat[1] = pv1; ps.pat[2] = pv2; ps.pat[3] = pv3; ps.pat[4] = pv4; ps.pat[5] = pvc;
+            ws.store_uniform(ps);
             rb.fate[li] = more ? kFateMore : kFateDone; rb.nwalk[i] = (uint8_t)nwalk;
             if (more) { rb.src[p] = p; rb.pos[p] = (round > 0 ? rb.pos[p] : 0u) + (uint32_t)nb; }
         }
         if (more) { if (lane == nb - 1) rb.hstate[p] = key; }   // chain state for the next round: key of the round's last block
-        else {
-            if (a.dense) {
-                double* row = a.dense + (long long)p * t.max_pods;
-                const uint32_t P = t.max_pods;
-                if ((P & 1u) == 0 && ((reinterpret_cast<uintptr_t>(row) & 15u) == 0)) {
-                    for (uint32_t c2 = lane * 2; c2 < P; c2 += 64) st_stream_f64x2(row + c2, -1.0, -1.0, l2pol);
-                } else {
-                    for (uint32_t c2 = lane; c2 < P; c2 += 32) row[c2] = -1.0;
-                }
-                __syncwarp();
-                if ((uint32_t)lane < k && mypod < P) row[mypod] = mysc;
-            }
-            if (a.sp_cnt) {
-                if ((uint32_t)lane < k) { a.sp_pods[(long long)p * kMaxEnt + lane] = (uint16_t)mypod; a.sp_scores[(long long)p * kMaxEnt + lane] = mysc; }
-                if (lane == 0) a.sp_cnt[p] = (uint8_t)k;
-            }
-            if (a.has_keys && lane == 0) a.has_keys[p] = (round > 0) || nb > 0;
-        }
+        else warp_write_row(t, a, p, ws.k, ws.pod, ws.sc, round > 0 || nb > 0, l2pol);
         __syncwarp();
     }
 }
@@ -754,22 +607,8 @@ __device__ __forceinline__ void resolve_round(const TableView& t, const ScoreArg
             const uint32_t pp = __shfl_sync(0xffffffffu, p, l);
             const PromptState& ps = pst_cur[__shfl_sync(0xffffffffu, pl, l)];
             const uint32_t pk = ps.k;
-            if (a.dense) {
-                double* row = a.dense + (long long)pp * t.max_pods;
-                const uint32_t P = t.max_pods;
-                if ((P & 1u) == 0 && ((reinterpret_cast<uintptr_t>(row) & 15u) == 0)) {
-                    for (uint32_t c = lane * 2; c < P; c += 64) st_stream_f64x2(row + c, -1.0, -1.0, l2pol);
-                } else {
-                    for (uint32_t c = lane; c < P; c += 32) row[c] = -1.0;
-                }
-                __syncwarp();
-                if ((uint32_t)lane < pk) { const uint32_t pd = ps.pod[lane]; if (pd < P) row[pd] = ps.sc[lane]; }
-            }
-            if (a.sp_cnt) {
-                if ((uint32_t)lane < pk) { a.sp_pods[(long long)pp * kMaxEnt + lane] = ps.pod[lane]; a.sp_scores[(long long)pp * kMaxEnt + lane] = ps.sc[lane]; }
-                if (lane == 0) a.sp_cnt[pp] = (uint8_t)pk;
-            }
-            if (a.has_keys && lane == 0) a.has_keys[pp] = 1;     // followers always have a block in the round
+            const bool in = (uint32_t)lane < pk;
+            warp_write_row(t, a, pp, pk, in ? ps.pod[lane] : 0u, in ? ps.sc[lane] : 0.0, true, l2pol);   // followers always have a block in the round
         }
         __syncwarp();
     }
@@ -835,8 +674,7 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
                     double v = rb.snap_sc[sj * kMaxEnt + q];
                     if (j0 < d - 1 && ((s.alive >> q) & 1u)) {          // later blocks of the run: the same addend again, in order
                         const uint32_t bt = rb.snap_bt[sj * kMaxEnt + q];
-                        const double add = bt == 0xffu ? 0.0 : t.weight[bt & 15u];
-                        for (int u = j0; u < d - 1; ++u) v = __dadd_rn(v, add);
+                        v = run_add(v, bt == 0xffu ? 0.0 : t.weight[bt & 15u], d - 1 - j0);
                     }
                     s.sc[q] = v;
                 }
@@ -850,31 +688,12 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
                 int b = d;
                 for (; b < bend; ++b) {
                     if (trace) atomicAdd(&rb.n_hl[3], 1u);
-                    const uint64_t hm = home_of(hk, mdl);
-                    const ReqSlot* base = t.req_peer[shard_of(hm, t.shard_bits)];
-                    uint64_t slot = hm & t.req_mask & ~1ull;
-                    const bool remote = base != t.req && !t.peer_pair;                  // a peer's shard: home slot first, its neighbour only if needed
-                    uint4 A0, B0, A1, B1;
-                    ld_slot(base + slot, peer, A0, B0);
-                    if (!remote) ld_slot(base + slot + 1, peer, A1, B1);
+                    HomeProbe pr;
+                    pr.issue(t, hk, mdl, peer);
                     // the next key does not depend on the probe: hash it while the probe is in flight
                     const uint64_t hn = b + 1 < nb ? hash_block16(hk, tk + (size_t)(b + 1) * BS) : 0ull;
                     SlotWords sw;
-                    bool hit;
-                    for (;;) {
-                        sw.a = A0; sw.b = B0;
-                        hit = slot_matches(sw.a, sw.b, hk, mdl);
-                        bool stop = hit || meta_state(sw.b.w) == kStateEmpty;
-                        if (!stop) {
-                            if (remote) ld_slot(base + slot + 1, peer, A1, B1);
-                            sw.a = A1; sw.b = B1; hit = slot_matches(sw.a, sw.b, hk, mdl); stop = hit || meta_state(sw.b.w) == kStateEmpty;
-                        }
-                        if (stop) break;
-                        slot = (slot + 2) & t.req_mask;                 // rare: displaced past the home pair
-                        ld_slot(base + slot, peer, A0, B0);
-                        if (!remote) ld_slot(base + slot + 1, peer, A1, B1);
-                    }
-                    if (!hit) { walking = false; break; }
+                    if (!pr.resolve(t, hk, mdl, peer, sw.a, sw.b)) { walking = false; break; }
                     s.next(t, sw);
                     if (!s.alive) { walking = false; break; }
                     h = hk; hk = hn;
@@ -899,22 +718,8 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
             const int l = __ffs(dm) - 1; dm &= dm - 1;
             const uint32_t pp = __shfl_sync(0xffffffffu, p, l);
             const uint32_t pk = __shfl_sync(0xffffffffu, s.k, l);
-            if (a.dense) {
-                double* row = a.dense + (long long)pp * t.max_pods;
-                const uint32_t P = t.max_pods;
-                if ((P & 1u) == 0 && ((reinterpret_cast<uintptr_t>(row) & 15u) == 0)) {
-                    for (uint32_t c = lane * 2; c < P; c += 64) st_stream_f64x2(row + c, -1.0, -1.0, l2pol);
-                } else {
-                    for (uint32_t c = lane; c < P; c += 32) row[c] = -1.0;
-                }
-                __syncwarp();
-                if ((uint32_t)lane < pk) { const uint32_t pd = sm.pod[lane][l]; if (pd < P) row[pd] = sm.sc[lane][l]; }
-            }
-            if (a.sp_cnt) {
-                if ((uint32_t)lane < pk) { a.sp_pods[(long long)pp * kMaxEnt + lane] = sm.pod[lane][l]; a.sp_scores[(long long)pp * kMaxEnt + lane] = sm.sc[lane][l]; }
-                if (lane == 0) a.sp_cnt[pp] = (uint8_t)pk;
-            }
-            if (a.has_keys && lane == 0) a.has_keys[pp] = 1;
+            const bool in = (uint32_t)lane < pk;
+            warp_write_row(t, a, pp, pk, in ? sm.pod[lane][l] : 0u, in ? sm.sc[lane][l] : 0.0, true, l2pol);
         }
         __syncwarp();
     }

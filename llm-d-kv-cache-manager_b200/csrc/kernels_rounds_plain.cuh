@@ -1,7 +1,7 @@
 // kernels_rounds_plain.cuh -- Score() for MEDIUM batches: alternating hash / walk rounds, every prompt on its own.
 //
-// Same reference path as kernels_score.cuh (GetPodScores steps 2-4, pkg/kvcache/indexer.go:141-163).  Two kernels per
-// round and nothing else:
+// Same reference path as every Score() kernel (GetPodScores steps 2-4, pkg/kvcache/indexer.go:141-163), with the probe,
+// the fold and the result row of score_common.cuh.  Two kernels per round and nothing else:
 //
 //   round r, kernel H (hash_round_kernel):  prompts that are still on the consecutive-prefix walk hash their next
 //       kRoundBlocks blocks.  Lockstep, thin lanes (no score / probe state), the branch-free FNV/CBOR code at the
@@ -17,11 +17,17 @@
 // Results are bit-identical on every path (tests run all of them against the oracle).
 #pragma once
 #include <cuda_runtime.h>
-#include "kernels_score.cuh"
-#include "kernels_rounds.cuh"      // PromptState, HashSmem, rounds_init_kernel, ld_slot_pair, ent_of
+#include "score_common.cuh"
+#include "kernels_rounds.cuh"      // PromptState, HashSmem, rounds_init_kernel
 
 namespace kvx {
 namespace plain {
+
+// Blocks staged per copy step (2 = 128-byte accesses: fewer, longer DRAM accesses but only 24 resident warps/SM, and the
+// kernel is pipe bound).  Always 1; kernel H's staging below keeps the general form because ptxas 12.9 compiles the
+// one-block spelling of it to different code (40 / 56 registers instead of 48 / 52) that made the lane-walk step at 262 144
+// prompts ~1.5 % slower (H100 80GB HBM3, 400 W power limit).
+constexpr int kHashChunk = 1;
 
 constexpr int kProbeThreads = 256;
 
@@ -109,17 +115,7 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
 #pragma unroll
             for (int u = 0; u < kHashChunk; ++u) {
                 const int b = c * kHashChunk + u;
-                Fnv f;
-                f.begin_block(h, BS);
-                const uint4* tp = reinterpret_cast<const uint4*>(wtok + (size_t)(c % NS) * 32 * SM::kRow + lane * SM::kRow + u * BS * 4);
-                const uint4 v0 = tp[0], v1 = tp[1];
-                f.token(v0.x); f.token(v0.y); f.token(v0.z); f.token(v0.w);
-                const uint4 v2 = tp[2];
-                f.token(v1.x); f.token(v1.y); f.token(v1.z); f.token(v1.w);
-                const uint4 v3 = tp[3];
-                f.token(v2.x); f.token(v2.y); f.token(v2.z); f.token(v2.w);
-                f.token(v3.x); f.token(v3.y); f.token(v3.z); f.token(v3.w);
-                const uint64_t key = f.end_block();
+                const uint64_t key = hash_row16(h, wtok + (size_t)(c % NS) * 32 * SM::kRow + lane * SM::kRow + u * BS * 4);
                 if (b < nb) { h = key; rb.keys[PM ? (size_t)i * kRoundBlocks + b : (size_t)b * a.n_prompts + i] = key; }
             }
         }
@@ -136,12 +132,7 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
 // warp walks 32 prompts in lockstep, one block per iteration: every instruction serves 32 prompts, the 32 lanes'
 // probes are 32 independent 64-byte reads, and the slot pair for block j+1 is in flight while block j is scored.
 struct WalkSmem {
-    struct Warp {
-        double sc[kMaxEnt][32];
-        uint16_t pod[kMaxEnt][32];
-        uint8_t bt[kMaxEnt][32];
-    };
-    Warp w[kProbeThreads / 32];
+    LaneCols w[kProbeThreads / 32];
     double weight[16];
 };
 
@@ -150,7 +141,7 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
     extern __shared__ __align__(16) unsigned char smem_raw_w[];
     WalkSmem& sm = *reinterpret_cast<WalkSmem*>(smem_raw_w);
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    WalkSmem::Warp& W = sm.w[wid];
+    LaneCols& W = sm.w[wid];
     if (threadIdx.x < 16) sm.weight[threadIdx.x] = t.weight[threadIdx.x];
     __syncthreads();
     const unsigned int n_act = rb.n_act[cur];
@@ -167,14 +158,14 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         const bool has_more = (meta >> 8) & 1u;
         const uint32_t mdl = (have && a.model) ? a.model[p] : a.model0;
         uint32_t k = 0, alive = 0;
-        uint32_t pv0 = 0, pv1 = 0, pv2 = 0, pv3 = 0, pv4 = 0, pvc = 0;      // last scored pattern
+        SlotPat pv = {};                                       // last scored pattern
         if (round > 0 && have) {
             const PromptState& ps = rb.pst[p];
             k = ps.k; alive = ps.alive;
-            pv0 = ps.pat[0]; pv1 = ps.pat[1]; pv2 = ps.pat[2]; pv3 = ps.pat[3]; pv4 = ps.pat[4]; pvc = ps.pat[5];
+#pragma unroll
+            for (int x = 0; x < 6; ++x) pv.w[x] = ps.pat[x];
             for (uint32_t q = 0; q < k; ++q) { W.sc[q][lane] = ps.sc[q]; W.pod[q][lane] = ps.pod[q]; W.bt[q][lane] = ps.bt[q]; }
         }
-        const uint64_t* frow = nullptr;
         const int nb_max = __reduce_max_sync(0xffffffffu, nb);
         bool done = !have || nb == 0;                          // walk ended (miss / no live pod); scores are final
         // slot pair of block 0
@@ -205,62 +196,23 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
             }
             key1 = (!done && j + 2 < nb) ? rb.keys[(size_t)(j + 2) * kstride + i] : 0ull;
             if (!done && j < nb) {
-                uint4 A = A0, B = B0;
-                bool hit = slot_matches(A, B, key, mdl);
-                if (!hit && meta_state(B.w) != kStateEmpty) {
-                    A = A1; B = B1;
-                    hit = slot_matches(A, B, key, mdl);
-                    while (!hit && meta_state(B.w) != kStateEmpty) {          // rare: displaced past the home pair
-                        slot = (slot + 2) & t.req_mask;
-                        ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
-                        A = A0; B = B0; hit = slot_matches(A, B, key, mdl);
-                        if (!hit && meta_state(B.w) != kStateEmpty) { A = A1; B = B1; hit = slot_matches(A, B, key, mdl); }
-                    }
+                uint4 A, B;
+                bool hit;
+                // (the loop `while (!pair_decides(..))`, spelled out: written that way, ptxas 12.9 spills 40 bytes more in this kernel)
+                pair_decides(A0, B0, A1, B1, key, mdl, A, B, hit);
+                while (!hit && meta_state(B.w) != kStateEmpty) {              // rare: displaced past the home pair
+                    slot = (slot + 2) & t.req_mask;
+                    ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
+                    pair_decides(A0, B0, A1, B1, key, mdl, A, B, hit);
                 }
                 if (!hit) { done = true; }
                 else {
-                    SlotWords sw; sw.a = A; sw.b = B;
-                    const uint32_t cnt = meta_count(B.w);
+                    const SlotPat w = SlotPat::of(A, B);
                     const bool first_block = (round == 0 && j == 0);
-                    const bool same = !first_block && (((pv0 ^ A.z) | (pv1 ^ A.w) | (pv2 ^ B.x) | (pv3 ^ B.y) | (pv4 ^ B.z) | (pvc ^ cnt)) == 0u);
-                    if (same) {
-                        uint32_t am = alive;
-                        while (am) {
-                            const int q = __ffs(am) - 1; am &= am - 1;
-                            const uint32_t bt = W.bt[q][lane];
-                            const double mx = bt == 0xffu ? 0.0 : sm.weight[bt];
-                            W.sc[q][lane] = __dadd_rn(W.sc[q][lane], mx);
-                        }
-                    } else if (first_block) {
-                        // activePods := pods of block 0 (after the filter); score = max weight   (kvblock_scorer.go:118-128)
-                        frow = filter_row(a.filter, p, t.filter_words);
-                        k = 0;
-                        for (uint32_t e = 0; e < cnt; ++e) {
-                            const uint32_t pt = slot_ent(sw, e), pd = pt >> 4;
-                            if (frow && !filter_has(frow, pd)) continue;
-                            const double wt = sm.weight[pt & 15u];
-                            uint32_t q = 0;
-                            for (; q < k; ++q) if (W.pod[q][lane] == pd) break;
-                            if (q == k) { W.pod[k][lane] = (uint16_t)pd; W.sc[k][lane] = 0.0; W.bt[k][lane] = 0xffu; ++k; }
-                            if (wt > W.sc[q][lane]) { W.sc[q][lane] = wt; W.bt[q][lane] = (uint8_t)(pt & 15u); }
-                        }
-                        alive = (1u << k) - 1u;
-                    } else {
-                        // activePods &= pods(block); score[p] += max weight, in block order   (kvblock_scorer.go:130-147)
-                        uint32_t am = alive;
-                        while (am) {
-                            const int q = __ffs(am) - 1; am &= am - 1;
-                            const uint32_t want = W.pod[q][lane];
-                            double mx = 0.0; bool present = false; uint32_t bt = 0xffu;
-                            for (uint32_t e = 0; e < cnt; ++e) {
-                                const uint32_t pt = slot_ent(sw, e);
-                                if ((pt >> 4) == want) { present = true; const double wt = sm.weight[pt & 15u]; if (wt > mx) { mx = wt; bt = pt & 15u; } }
-                            }
-                            if (present) { W.sc[q][lane] = __dadd_rn(W.sc[q][lane], mx); W.bt[q][lane] = (uint8_t)bt; }
-                            else alive &= ~(1u << q);
-                        }
-                    }
-                    pv0 = A.z; pv1 = A.w; pv2 = B.x; pv3 = B.y; pv4 = B.z; pvc = cnt;
+                    if (!first_block && w == pv) W.repeat(lane, sm.weight, alive);
+                    else if (first_block) W.first(lane, w, filter_row(a.filter, p, t.filter_words), sm.weight, k, alive);
+                    else W.next(lane, w, sm.weight, alive);
+                    pv = w;
                     if (!alive) done = true;
                 }
             }
@@ -278,7 +230,8 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
                 rb.act[cur ^ 1][ns] = p;
                 PromptState& ps = rb.pst[p];
                 ps.k = (uint8_t)k; ps.alive = (uint16_t)alive;
-                ps.pat[0] = pv0; ps.pat[1] = pv1; ps.pat[2] = pv2; ps.pat[3] = pv3; ps.pat[4] = pv4; ps.pat[5] = pvc;
+#pragma unroll
+                for (int x = 0; x < 6; ++x) ps.pat[x] = pv.w[x];
                 for (uint32_t q = 0; q < k; ++q) { ps.sc[q] = W.sc[q][lane]; ps.pod[q] = W.pod[q][lane]; ps.bt[q] = W.bt[q][lane]; }
             }
         }
@@ -289,22 +242,8 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
             const uint32_t pp = __shfl_sync(0xffffffffu, p, l);
             const uint32_t pk = __shfl_sync(0xffffffffu, k, l);
             const uint32_t pmeta = __shfl_sync(0xffffffffu, meta, l);
-            if (a.dense) {
-                double* row = a.dense + (long long)pp * t.max_pods;
-                const uint32_t P = t.max_pods;
-                if ((P & 1u) == 0 && ((reinterpret_cast<uintptr_t>(row) & 15u) == 0)) {
-                    for (uint32_t c = lane * 2; c < P; c += 64) st_stream_f64x2(row + c, -1.0, -1.0, l2pol);
-                } else {
-                    for (uint32_t c = lane; c < P; c += 32) row[c] = -1.0;
-                }
-                __syncwarp();
-                if ((uint32_t)lane < pk) { const uint32_t pd = W.pod[lane][l]; if (pd < P) row[pd] = W.sc[lane][l]; }
-            }
-            if (a.sp_cnt) {
-                if ((uint32_t)lane < pk) { a.sp_pods[(long long)pp * kMaxEnt + lane] = W.pod[lane][l]; a.sp_scores[(long long)pp * kMaxEnt + lane] = W.sc[lane][l]; }
-                if (lane == 0) a.sp_cnt[pp] = (uint8_t)pk;
-            }
-            if (a.has_keys && lane == 0) a.has_keys[pp] = (round > 0) || (pmeta & 63u) > 0;
+            const bool in = (uint32_t)lane < pk;
+            warp_write_row(t, a, pp, pk, in ? W.pod[lane][l] : 0u, in ? W.sc[lane][l] : 0.0, round > 0 || (pmeta & 63u) > 0, l2pol);
         }
         __syncwarp();
     }
@@ -339,100 +278,21 @@ probe_round_warp_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb
         const uint32_t mdl = (have && a.model) ? a.model[p] : a.model0;
         uint64_t key = 0;
         if (lane < nb) key = rb.keys[(size_t)i * kRoundBlocks + lane];
-        // walk state: lane q < k owns pod q
-        uint32_t k = 0, alive = 0, mypod = 0xffffffffu, mybt = 0xffu;
-        double mysc = 0.0;
-        uint32_t pv0 = 0, pv1 = 0, pv2 = 0, pv3 = 0, pv4 = 0, pvc = 0xffffffffu;
-        if (round > 0 && have) {
-            const PromptState& ps = rb.pst[p];
-            k = ps.k; alive = ps.alive;
-            pv0 = ps.pat[0]; pv1 = ps.pat[1]; pv2 = ps.pat[2]; pv3 = ps.pat[3]; pv4 = ps.pat[4]; pvc = ps.pat[5];
-            if ((uint32_t)lane < k) { mysc = ps.sc[lane]; mypod = ps.pod[lane]; mybt = ps.bt[lane]; }
-        }
+        WarpWalk ws;
+        if (round > 0 && have) ws.load(rb.pst[p], lane);
         // probe: lane j looks up block j's key
-        uint32_t e0 = 0, e1 = 0, e2 = 0, e3 = 0, e4 = 0, cnt = 0;
+        SlotPat mine = {};
         bool hit = false;
         if (lane < nb) {
-            const uint64_t hm = home_of(key, mdl);
-            const ReqSlot* base = t.req_peer[shard_of(hm, t.shard_bits)];
-            uint64_t slot = hm & t.req_mask & ~1ull;
-            const bool remote = base != t.req && !t.peer_pair;                  // a peer's shard: home slot first, its neighbour only if needed
-            for (;;) {
-                uint4 A0, B0, A1, B1;
-                ld_slot(base + slot, peer, A0, B0);
-                if (!remote) ld_slot(base + slot + 1, peer, A1, B1);
-                uint4 A = A0, B = B0;
-                hit = slot_matches(A, B, key, mdl);
-                bool stop = hit || meta_state(B.w) == kStateEmpty;
-                if (!stop) {
-                    if (remote) ld_slot(base + slot + 1, peer, A1, B1);
-                    A = A1; B = B1; hit = slot_matches(A, B, key, mdl); stop = hit || meta_state(B.w) == kStateEmpty;
-                }
-                if (hit) { e0 = A.z; e1 = A.w; e2 = B.x; e3 = B.y; e4 = B.z; cnt = meta_count(B.w); }
-                if (stop) break;
-                slot = (slot + 2) & t.req_mask;                 // rare: displaced past the home pair
-            }
+            HomeProbe pr;
+            uint4 A, B;
+            hit = pr.find(t, key, mdl, peer, A, B);
+            if (hit) mine = SlotPat::of(A, B);
         }
         const uint32_t hm_ = __ballot_sync(0xffffffffu, hit);
         const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from block 0 (lanes >= nb never hit)
-        bool done = nb == 0;
-        uint32_t samemask;                                      // block j's slot holds the same pods and tiers as block j-1's
-        {
-            const uint32_t u0 = __shfl_up_sync(0xffffffffu, e0, 1), u1 = __shfl_up_sync(0xffffffffu, e1, 1), u2 = __shfl_up_sync(0xffffffffu, e2, 1),
-                           u3 = __shfl_up_sync(0xffffffffu, e3, 1), u4 = __shfl_up_sync(0xffffffffu, e4, 1), uc = __shfl_up_sync(0xffffffffu, cnt, 1);
-            const bool sm_ = lane > 0 ? (((u0 ^ e0) | (u1 ^ e1) | (u2 ^ e2) | (u3 ^ e3) | (u4 ^ e4) | (uc ^ cnt)) == 0u)
-                                      : (round > 0 && ((pv0 ^ e0) | (pv1 ^ e1) | (pv2 ^ e2) | (pv3 ^ e3) | (pv4 ^ e4) | (pvc ^ cnt)) == 0u);
-            samemask = __ballot_sync(0xffffffffu, sm_ && lane < nhit);
-        }
-        int j = 0;
-        while (j < nhit && !done) {
-            if ((samemask >> j) & 1u) {
-                const uint32_t rest = ~(samemask >> j);
-                const int run = min(rest ? __ffs(rest) - 1 : 32, nhit - j);           // >= 1
-                if ((alive >> lane) & 1u) {
-                    const double add = mybt == 0xffu ? 0.0 : t.weight[mybt & 15u];
-                    for (int u = 0; u < run; ++u) mysc = __dadd_rn(mysc, add);
-                }
-                j += run;
-                continue;
-            }
-            const uint32_t w0 = __shfl_sync(0xffffffffu, e0, j), w1 = __shfl_sync(0xffffffffu, e1, j), w2 = __shfl_sync(0xffffffffu, e2, j),
-                           w3 = __shfl_sync(0xffffffffu, e3, j), w4 = __shfl_sync(0xffffffffu, e4, j), c = __shfl_sync(0xffffffffu, cnt, j);
-            if (round == 0 && j == 0) {
-                // activePods := pods of block 0 (after the filter), in entry order; score = max weight   (kvblock_scorer.go:118-128)
-                const uint64_t* frow = filter_row(a.filter, p, t.filter_words);
-                k = 0;
-                for (uint32_t e = 0; e < c; ++e) {
-                    const uint32_t pt = ent_of(w0, w1, w2, w3, w4, (int)e), pd = pt >> 4;
-                    if (frow && !filter_has(frow, pd)) continue;
-                    const double wt = t.weight[pt & 15u];
-                    const uint32_t own = __ballot_sync(0xffffffffu, (uint32_t)lane < k && mypod == pd);
-                    const int q = own ? __ffs(own) - 1 : (int)k;
-                    if (!own) { if (lane == q) { mypod = pd; mysc = 0.0; mybt = 0xffu; } ++k; }
-                    if (lane == q && wt > mysc) { mysc = wt; mybt = pt & 15u; }
-                }
-                alive = (1u << k) - 1u;
-            } else {
-                // activePods &= pods(block); score[p] += max weight, in block order   (kvblock_scorer.go:130-147)
-                bool present = false; double mx = 0.0; uint32_t bt = 0xffu;
-                if ((alive >> lane) & 1u) {
-                    for (uint32_t e = 0; e < c; ++e) {
-                        const uint32_t pt = ent_of(w0, w1, w2, w3, w4, (int)e);
-                        if ((pt >> 4) == mypod) { present = true; const double wt = t.weight[pt & 15u]; if (wt > mx) { mx = wt; bt = pt & 15u; } }
-                    }
-                    if (present) { mysc = __dadd_rn(mysc, mx); mybt = bt; }
-                }
-                alive = __ballot_sync(0xffffffffu, present);
-            }
-            if (!alive) done = true;
-            ++j;
-        }
-        if (j > 0) {                                            // pattern of the last scored block, for the next round's first comparison
-            const int lj = j - 1;
-            pv0 = __shfl_sync(0xffffffffu, e0, lj); pv1 = __shfl_sync(0xffffffffu, e1, lj); pv2 = __shfl_sync(0xffffffffu, e2, lj);
-            pv3 = __shfl_sync(0xffffffffu, e3, lj); pv4 = __shfl_sync(0xffffffffu, e4, lj); pvc = __shfl_sync(0xffffffffu, cnt, lj);
-        }
-        if (nhit < nb) done = true;                             // a block of the round is not in the index
+        ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, round > 0, nhit), round == 0, a.filter, p, [](int) {});
+        const bool done = nb == 0 || nhit < nb || !ws.alive;   // no block, a block of the round is not in the index, or no pod left
         const bool more = have && !done && has_more;
         // survivors of the CTA's 8 slots, in slot order
         if (lane == 0) sm.p[wid] = more ? p : 0xffffffffu;
@@ -447,30 +307,12 @@ probe_round_warp_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb
             unsigned int rank = 0;
             for (int w = 0; w < wid; ++w) rank += sm.p[w] != 0xffffffffu;
             PromptState& ps = rb.pst[p];
-            if ((uint32_t)lane < k) { ps.sc[lane] = mysc; ps.pod[lane] = (uint16_t)mypod; ps.bt[lane] = (uint8_t)mybt; }
+            ws.store_lane(ps, lane);
             if (lane == 0) {
                 rb.act[cur ^ 1][sm.base + rank] = p;
-                ps.k = (uint8_t)k; ps.alive = (uint16_t)alive;
-                ps.pat[0] = pv0; ps.pat[1] = pv1; ps.pat[2] = pv2; ps.pat[3] = pv3; ps.pat[4] = pv4; ps.pat[5] = pvc;
+                ws.store_uniform(ps);
             }
-        } else if (have) {
-            if (a.dense) {
-                double* row = a.dense + (long long)p * t.max_pods;
-                const uint32_t P = t.max_pods;
-                if ((P & 1u) == 0 && ((reinterpret_cast<uintptr_t>(row) & 15u) == 0)) {
-                    for (uint32_t c2 = lane * 2; c2 < P; c2 += 64) st_stream_f64x2(row + c2, -1.0, -1.0, l2pol);
-                } else {
-                    for (uint32_t c2 = lane; c2 < P; c2 += 32) row[c2] = -1.0;
-                }
-                __syncwarp();
-                if ((uint32_t)lane < k && mypod < P) row[mypod] = mysc;
-            }
-            if (a.sp_cnt) {
-                if ((uint32_t)lane < k) { a.sp_pods[(long long)p * kMaxEnt + lane] = (uint16_t)mypod; a.sp_scores[(long long)p * kMaxEnt + lane] = mysc; }
-                if (lane == 0) a.sp_cnt[p] = (uint8_t)k;
-            }
-            if (a.has_keys && lane == 0) a.has_keys[p] = (round > 0) || nb > 0;
-        }
+        } else if (have) warp_write_row(t, a, p, ws.k, ws.pod, ws.sc, round > 0 || nb > 0, l2pol);
         __syncthreads();                                        // sm.p / sm.base are rewritten by the next iteration
     }
 }

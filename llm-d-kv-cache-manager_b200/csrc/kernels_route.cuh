@@ -45,10 +45,7 @@ __global__ void score_slots_kernel(TableView t, const uint4* __restrict__ slots,
         if (k == k0) s.first(t, w, frow); else s.next(t, w);
         if (!s.alive) break;
     }
-    if (has_keys) has_keys[i] = k1 > k0;
-    double* row = dense_out + i * (int64_t)t.max_pods;
-    for (uint32_t p = 0; p < t.max_pods; ++p) row[p] = -1.0;
-    for (uint32_t q = 0; q < s.k; ++q) if (s.pod[q] < t.max_pods) row[s.pod[q]] = s.sc[q];
+    s.write_row(t, i, k1 > k0, dense_out, nullptr, nullptr, nullptr, has_keys);
 }
 
 }  // namespace kvx

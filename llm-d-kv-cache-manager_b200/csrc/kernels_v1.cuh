@@ -2,7 +2,7 @@
 // straight from global memory.  Kept as the in-library cross-check for the tuned kernels
 // (KVIDX_SCORE_KERNEL=v1) and used for the small, latency-insensitive entry points.
 #pragma once
-#include "table.cuh"
+#include "score_common.cuh"
 
 namespace kvx {
 
@@ -32,17 +32,6 @@ __global__ void hash_keys_kernel_v1(TableView t, const uint32_t* __restrict__ to
     }
 }
 
-__device__ __forceinline__ bool filter_has(const uint64_t* __restrict__ frow, uint32_t pod) {
-    return (frow[pod >> 6] >> (pod & 63)) & 1ull;
-}
-__device__ __forceinline__ const uint64_t* filter_row(const uint64_t* __restrict__ filter, int64_t i, uint32_t words) {
-    if (!filter) return nullptr;
-    const uint64_t* r = filter + i * words;
-    uint64_t any = 0;
-    for (uint32_t w = 0; w < words; ++w) any |= r[w];
-    return any ? r : nullptr;      // empty set == all pods (in_memory.go:126)
-}
-
 // Index.Lookup (in_memory.go:105-146): thread per key.  (A FULL slot always holds >= 1 entry --
 // Evict tombstones a slot the moment it empties -- so the present-but-empty cut of
 // in_memory.go:119-122 cannot trigger; it is still honoured via cut_out for completeness.)
@@ -67,44 +56,6 @@ __global__ void lookup_kernel_v1(TableView t, uint32_t model, const uint64_t* __
     }
     cnt_out[i] = (uint8_t)c;
 }
-
-// Per-prompt scoring state == LongestPrefixScorer.Score's podScores/activePods
-// (kvblock_scorer.go:108-151), restricted to the <= 10 pods block 0 can hold.
-struct ScoreState {
-    uint16_t pod[kMaxEnt];
-    double sc[kMaxEnt];
-    uint32_t k;        // pods present at block 0 (after the filter)
-    uint32_t alive;    // bitmask over [0,k): still on the consecutive prefix
-
-    __device__ __forceinline__ void first(const TableView& t, const SlotWords& w, const uint64_t* frow) {
-        k = 0; alive = 0;
-        const uint32_t cnt = meta_count(w.b.w);
-        for (uint32_t j = 0; j < cnt; ++j) {
-            const uint32_t pt = slot_ent(w, j);
-            const uint32_t p = pt >> 4;
-            if (frow && !filter_has(frow, p)) continue;
-            const double wt = t.weight[pt & 15u];
-            uint32_t q = 0;
-            for (; q < k; ++q) if (pod[q] == p) break;
-            if (q == k) { pod[k] = (uint16_t)p; sc[k] = 0.0; ++k; }
-            if (wt > sc[q]) sc[q] = wt;                      // getMaxWeight starts at 0.0 (kvblock_scorer.go:90)
-        }
-        alive = (1u << k) - 1u;
-    }
-    __device__ __forceinline__ void next(const TableView& t, const SlotWords& w) {
-        const uint32_t cnt = meta_count(w.b.w);
-        for (uint32_t q = 0; q < k; ++q) {
-            if (!((alive >> q) & 1u)) continue;
-            double mx = 0.0; bool present = false;
-            for (uint32_t j = 0; j < cnt; ++j) {
-                const uint32_t pt = slot_ent(w, j);
-                if ((pt >> 4) == pod[q]) { present = true; const double wt = t.weight[pt & 15u]; if (wt > mx) mx = wt; }
-            }
-            if (present) sc[q] = __dadd_rn(sc[q], mx);       // in-order f64 add (kvblock_scorer.go:143-146)
-            else alive &= ~(1u << q);
-        }
-    }
-};
 
 // Indexer.GetPodScores steps 2-4 (indexer.go:141-163): thread per prompt.
 __global__ void score_kernel_v1(TableView t, const uint32_t* __restrict__ tok, const int64_t* __restrict__ tok_off,
@@ -135,16 +86,7 @@ __global__ void score_kernel_v1(TableView t, const uint32_t* __restrict__ tok, c
         }
         if (!walking && !t.req_stamp) break;
     }
-    if (has_keys) has_keys[i] = nblk > 0;
-    if (dense_out) {
-        double* row = dense_out + i * (int64_t)t.max_pods;
-        for (uint32_t p = 0; p < t.max_pods; ++p) row[p] = -1.0;
-        for (uint32_t q = 0; q < s.k; ++q) if (s.pod[q] < t.max_pods) row[s.pod[q]] = s.sc[q];
-    }
-    if (sp_cnt) {
-        sp_cnt[i] = (uint8_t)s.k;
-        for (uint32_t q = 0; q < s.k; ++q) { sp_pods[i * kMaxEnt + q] = s.pod[q]; sp_scores[i * kMaxEnt + q] = s.sc[q]; }
-    }
+    s.write_row(t, i, nblk > 0, dense_out, sp_pods, sp_scores, sp_cnt, has_keys);
 }
 
 }  // namespace kvx
