@@ -95,8 +95,22 @@ typedef struct kvidx_config {
     uint32_t shard_rank;       /* hash-range sharding over the GPUs of one NVSwitch domain (SURVEY 8e): this handle */
     uint32_t shard_count;      /* owns shard `shard_rank` of `shard_count` (power of two <= 8; 0 or 1 = unsharded).   */
                                /* `capacity` stays the TOTAL key budget; each shard holds capacity/shard_count.        */
-    uint32_t reserved[5];
+    uint32_t evict_policy;     /* KVIDX_EVICT_CLOCK: hold each map to `capacity` keys on the fast paths.  One reference bit per
+                                  slot is set wherever golang-lru refreshes recency (Add, Evict, GetRequestKey, a BlockStored
+                                  parent, Lookup) and, for Score(), on the present keys among the blocks the walk probes: block 0
+                                  up to and including the block that empties the active pod set, or the last full block (the
+                                  early exit stays).  After every write call (add, evict, apply_events[_dev], restore) a CLOCK
+                                  sweep evicts keys until each map holds at most `capacity`: unreferenced keys go before referenced
+                                  ones, whose bits are cleared as the hand passes them.  Request keys and engine mappings are
+                                  evicted independently, as in the reference.  A read running at the same moment as a sweep sees
+                                  each key before or after its eviction, and may or may not protect the keys it touches.
+                                  KVIDX_EVICT_NONE (0, default): `capacity` only sizes the table.  Other values, CLOCK with
+                                  lru_exact, or CLOCK on a sharded handle -> KVIDX_EINVAL. */
+    uint32_t reserved[4];
 } kvidx_config_t;
+
+#define KVIDX_EVICT_NONE  0u
+#define KVIDX_EVICT_CLOCK 1u
 
 void        kvidx_config_default(kvidx_config_t* cfg);
 int         kvidx_create(const kvidx_config_t* cfg, kvidx_t** out);   /* NewInMemoryIndex + NewChunkedTokenDatabase + NewKVBlockScorer */
@@ -358,6 +372,15 @@ typedef struct kvidx_stats {
     uint64_t coalesced_calls;   /* host-buffer Score() calls that were served as part of another call's launch      */
 } kvidx_stats_t;
 int kvidx_get_stats(kvidx_t* idx, kvidx_stats_t* out);
+/* {request keys, engine mappings} dropped by the capacity bound since the handle was created: CLOCK sweeps and exact-LRU
+ * evictions.  Evict / BlockRemoved and kvidx_remove_pods are not counted.  On a CLOCK handle every write call reads the
+ * device's counters before it runs (waiting for the batches queued before it), so that the tombstones evictions leave
+ * are compacted by the usual rebuild also when only kvidx_apply_events_dev writes. */
+int kvidx_get_evictions(kvidx_t* idx, uint64_t out[2]);
+/* CLOCK mode: {sweeps that evicted, those of them whose hand went past a full turn} since the handle was created, over both
+ * maps (a sweep makes at most two turns).  Both kvidx_get_evictions and this read the device's counters without waiting
+ * for a write batch in flight: they report the batches completed so far. */
+int kvidx_get_sweeps(kvidx_t* idx, uint64_t out[2]);
 
 #ifdef __cplusplus
 }

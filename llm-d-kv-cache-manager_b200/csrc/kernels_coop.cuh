@@ -247,13 +247,14 @@ coop_score_kernel(const TableView t, const ScoreArgs a) {
             const ReqSlot* base = t.req; uint64_t slot = 0;
             bool issued = false, hit = false, decided = false;
             SlotPat mine = {};
+            uint64_t hslot = 0;                                           // CLOCK: slot of this lane's hit
             auto resolve = [&]() {                                        // the slot pair has (or will have) arrived: hit or miss
                 uint4 A, B;
                 while (!pair_decides(A0, B0, A1, B1, key, mdl, A, B, hit)) {
                     slot = (slot + 2) & t.req_mask;                       // rare: displaced past the home pair
                     ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
                 }
-                if (hit) mine = SlotPat::of(A, B);
+                if (hit) { mine = SlotPat::of(A, B); if (t.req_ref) hslot = pair_hit_slot(slot, A0, B0, key, mdl); }
                 decided = true;
             };
             const int nhashed = coop_hash_chunk(sm, W, W.tok[c & 1], h, nb, lane, lt, key, last, [&](int ndone) -> bool {
@@ -279,7 +280,8 @@ coop_score_kernel(const TableView t, const ScoreArgs a) {
             const uint32_t hm_ = __ballot_sync(0xffffffffu, hit && lane < nhashed);
             const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from the chunk's first block
             // ---- ordered scoring of the hits (kvblock_scorer.go:108-151), lane q owns pod q ----
-            ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, c > 0, nhit), c == 0, a.filter, pi, [](int) {});
+            const int nwalked = ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, c > 0, nhit), c == 0, a.filter, pi, [](int) {});
+            WarpWalk::mark_walked(t, lane, nwalked, hit, hslot);
             if (!ws.alive || nhit < nb || !has_more) done = true;
             h = last;
         }

@@ -511,6 +511,8 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
 // round's 32 keys at once (one DRAM latency for the whole chunk), a ballot finds the first miss, and the blocks before
 // it are scored in order with lane q owning pod q of the first block (<= 10 pods), the block's entries broadcast by
 // shuffle.  Same arithmetic in the same order as everywhere else: max weight per pod per block, added in block order.
+// kClock: CLOCK marking of the blocks walked (a template parameter: the default instance keeps its register allocation)
+template <bool kClock>
 __global__ void __launch_bounds__(256)
 walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round) {
     const int lane = threadIdx.x & 31;
@@ -536,11 +538,12 @@ walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
         // probe: lane j looks up block j's key
         SlotPat mine = {};
         bool hit = false;
+        uint64_t hslot = 0;                                  // CLOCK: slot of this lane's hit
         if (lane < nb) {
             HomeProbe pr;
             uint4 A, B;
             hit = pr.find(t, key, mdl, peer, A, B);
-            if (hit) mine = SlotPat::of(A, B);
+            if (hit) { mine = SlotPat::of(A, B); if (kClock) hslot = pr.hit_slot(key, mdl); }
         }
         const uint32_t hm_ = __ballot_sync(0xffffffffu, hit);
         const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from block 0 (lanes >= nb never hit)
@@ -552,6 +555,9 @@ walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
             if ((uint32_t)lane < ws.k) { rb.snap_sc[sb * kMaxEnt + lane] = ws.sc; rb.snap_bt[sb * kMaxEnt + lane] = (uint8_t)ws.bt; }
             if (lane == 0) rb.snap_alive[sb] = (uint16_t)ws.alive;
         });
+        // CLOCK: the representative's walk marks the blocks it looked at for its whole class (class-mates share model, filter,
+        // walk state and these keys; a partial follower marks the blocks it walks alone in kernel D)
+        if (kClock) WarpWalk::mark_walked(t, lane, j, hit, hslot);
         const uint32_t nwalk = (uint32_t)(j > 0 && !ws.alive ? j - 1 : j);      // blocks after which the walk was still alive
         if (snapf) {                                           // block -> first block of its run
             const uint32_t starts = ~samemask & ((2u << lane) - 1u);
@@ -694,6 +700,7 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
                     const uint64_t hn = b + 1 < nb ? hash_block16(hk, tk + (size_t)(b + 1) * BS) : 0ull;
                     SlotWords sw;
                     if (!pr.resolve(t, hk, mdl, peer, sw.a, sw.b)) { walking = false; break; }
+                    if (t.req_ref) ref_touch(t.req_ref, pr.hit_slot(hk, mdl));
                     s.next(t, sw);
                     if (!s.alive) { walking = false; break; }
                     h = hk; hk = hn;

@@ -136,6 +136,8 @@ struct WalkSmem {
     double weight[16];
 };
 
+// kClock: CLOCK marking of the blocks walked (a template parameter: the default instance keeps its register allocation)
+template <bool kClock>
 __global__ void __launch_bounds__(kProbeThreads, 4)
 probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, const int cur, const int round) {
     extern __shared__ __align__(16) unsigned char smem_raw_w[];
@@ -207,6 +209,7 @@ probe_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
                 }
                 if (!hit) { done = true; }
                 else {
+                    if (kClock) mark_hit(t, slot, A0, B0, key, mdl);
                     const SlotPat w = SlotPat::of(A, B);
                     const bool first_block = (round == 0 && j == 0);
                     if (!first_block && w == pv) W.repeat(lane, sm.weight, alive);
@@ -283,15 +286,17 @@ probe_round_warp_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb
         // probe: lane j looks up block j's key
         SlotPat mine = {};
         bool hit = false;
+        uint64_t hslot = 0;                                  // CLOCK: slot of this lane's hit
         if (lane < nb) {
             HomeProbe pr;
             uint4 A, B;
             hit = pr.find(t, key, mdl, peer, A, B);
-            if (hit) mine = SlotPat::of(A, B);
+            if (hit) { mine = SlotPat::of(A, B); if (t.req_ref) hslot = pr.hit_slot(key, mdl); }
         }
         const uint32_t hm_ = __ballot_sync(0xffffffffu, hit);
         const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from block 0 (lanes >= nb never hit)
-        ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, round > 0, nhit), round == 0, a.filter, p, [](int) {});
+        const int nwalked = ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, round > 0, nhit), round == 0, a.filter, p, [](int) {});
+        WarpWalk::mark_walked(t, lane, nwalked, hit, hslot);
         const bool done = nb == 0 || nhit < nb || !ws.alive;   // no block, a block of the round is not in the index, or no pod left
         const bool more = have && !done && has_more;
         // survivors of the CTA's 8 slots, in slot order
@@ -320,7 +325,8 @@ probe_round_warp_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb
 inline int rounds_init() {
     if (cudaFuncSetAttribute(hash_round_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
     if (cudaFuncSetAttribute(hash_round_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HashSmem<16>)) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(probe_round_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem)) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(probe_round_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem)) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(probe_round_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem)) != cudaSuccess) return -1;
     return 0;
 }
 

@@ -166,8 +166,9 @@ score_kernel_tuned(const TableView t, const ScoreArgs a) {
                     pslot = (pslot + 2) & t.req_mask;
                     ld_slot_pair(pbase + pslot, peer, pa0, pb0, pa1, pb1);
                 }
-                // leave the resolved slot in the registers: step 4 consumes it without a retry
-                if (hit) { pa0 = A; pb0 = B; } else { pb0.w = 0; }
+                // leave the resolved slot in the registers: step 4 consumes it without a retry (as slot 0 of the pair at
+                // pslot, so a hit in slot 1 moves pslot on by one for the CLOCK marking)
+                if (hit) { pslot += slot_matches(pa0, pb0, pkey, mdl) ? 0u : 1u; pa0 = A; pb0 = B; } else { pb0.w = 0; }
             }
             h = key;
             W.kq[hblk & (kKeyRing - 1)][lane] = key;
@@ -186,6 +187,7 @@ score_kernel_tuned(const TableView t, const ScoreArgs a) {
                 pend = false; finished = true;
             } else {
                 pend = false;
+                mark_hit(t, pslot, pa0, pb0, pkey, mdl);
                 const SlotPat w = SlotPat::of(A, B);
                 if (KVX_ABLATE & 1) { if (pblk == 0) { k = 0; alive = 1u; } }
                 else {

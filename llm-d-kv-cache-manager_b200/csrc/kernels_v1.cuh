@@ -46,6 +46,7 @@ __global__ void lookup_kernel_v1(TableView t, uint32_t model, const uint64_t* __
     uint64_t slot = 0;
     if (req_find(t, model, keys[i], w, &slot)) {
         if (t.req_stamp) t.req_stamp[slot] = stamp_base + (unsigned long long)i;      // data.Get refreshes recency (in_memory.go:118)
+        if (t.req_ref) ref_touch(t.req_ref, slot);
         const uint32_t cnt = meta_count(w.b.w);
         if (cnt == 0) atomicMin(cut_out, (int)min(i, (int64_t)0x7fffffff));
         for (uint32_t j = 0; j < cnt; ++j) {
@@ -82,7 +83,11 @@ __global__ void score_kernel_v1(TableView t, const uint32_t* __restrict__ tok, c
         if (hit && t.req_stamp) t.req_stamp[slot] = stamp_base + (unsigned long long)i * stamp_stride + (unsigned long long)k;
         if (walking) {
             if (!hit) walking = false;
-            else { if (k == 0) s.first(t, w, frow); else s.next(t, w); if (!s.alive) walking = false; }
+            else {
+                if (t.req_ref) ref_touch(t.req_ref, slot);                                // CLOCK: a block the walk looks at
+                if (k == 0) s.first(t, w, frow); else s.next(t, w);
+                if (!s.alive) walking = false;
+            }
         }
         if (!walking && !t.req_stamp) break;
     }

@@ -40,6 +40,7 @@ __device__ __forceinline__ void do_add(const TableView& t, uint32_t model, uint6
         else {
             a.z = (uint32_t)rhash; a.w = (uint32_t)(rhash >> 32);
             if (t.req_stamp) { b.z = (uint32_t)stamp; b.w = (uint32_t)(stamp >> 32); }       // lru Add: insert or refresh
+            if (t.eng_ref) ref_touch(t.eng_ref, es - t.eng);
             if (created) atomicAdd_system(&cnt_of(t, ehash, model)->eng_full, 1ull);
             eng_publish(es, a, b, make_meta(kStateFull, 0, model));
         }
@@ -52,6 +53,7 @@ __device__ __forceinline__ void do_add(const TableView& t, uint32_t model, uint6
         for (int j = 0; j < m; ++j) count = L.add(count, pts[j], t.pods_per_key);
         L.pack(a, b);
         if (t.req_stamp) t.req_stamp[rs - t.req] = stamp + 1;                             // data.Get refresh / ContainsOrAdd insert
+        if (t.req_ref) ref_touch(t.req_ref, rs - t.req);
         if (created) atomicAdd_system(&cnt_of(t, rhash, model)->req_full, 1ull);
         req_publish(rs, a, b, make_meta(kStateFull, count, model));
     }
@@ -61,7 +63,7 @@ __device__ __forceinline__ void do_add(const TableView& t, uint32_t model, uint6
 __device__ __forceinline__ void do_evict(const TableView& t, uint32_t model, uint64_t ehash,
                                          const uint16_t* __restrict__ pts, int m, unsigned long long stamp = 0) {
     uint64_t rhash;
-    if (!eng_find(t, model, ehash, &rhash, nullptr, stamp)) return;      // :219-223 silent no-op (a hit refreshes recency)
+    if (!eng_find(t, model, ehash, &rhash, nullptr, stamp, true)) return;   // :219-223 silent no-op (a hit refreshes recency)
     bool created;
     uint4 a, b;
     ReqSlot* rs = req_acquire(t, model, rhash, true, &created, a, b);
@@ -71,6 +73,7 @@ __device__ __forceinline__ void do_evict(const TableView& t, uint32_t model, uin
     } else {
         uint32_t count = meta_count(b.w);
         if (t.req_stamp) t.req_stamp[rs - t.req] = stamp + 1;                         // data.Get (:225)
+        if (t.req_ref) ref_touch(t.req_ref, rs - t.req);
         EntList L; L.unpack(a, b);
         for (int j = 0; j < m; ++j) count = L.remove(count, pts[j]);
         L.pack(a, b);
@@ -113,7 +116,7 @@ __global__ void evict_kernel(TableView t, uint32_t model, uint64_t engine, const
 __global__ void get_request_key_kernel(TableView t, uint32_t model, uint64_t engine, uint64_t* out, int* found, unsigned long long stamp) {
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         uint64_t r = 0;
-        const bool ok = eng_find(t, model, engine, &r, nullptr, stamp);
+        const bool ok = eng_find(t, model, engine, &r, nullptr, stamp, true);
         *out = r; *found = ok ? 1 : 0;
     }
 }
@@ -266,7 +269,7 @@ __global__ void apply_events_kernel(TableView t, const kvidx_event_t* __restrict
         if (evt.op == KVIDX_EV_BLOCK_STORED) {
             // parent request key: GetRequestKey(parent engine key); a miss restarts at the seed (pool.go:279-294)
             uint64_t h = t.init_hash;
-            if (evt.has_parent) { uint64_t r; if (eng_find(t, evt.model, evt.parent_hash, &r, nullptr, lane == 0 ? sb + 1 : 0)) h = r; }
+            if (evt.has_parent) { uint64_t r; if (eng_find(t, evt.model, evt.parent_hash, &r, nullptr, lane == 0 ? sb + 1 : 0, lane == 0)) h = r; }
             if (evt.n_hashes == 0) continue;                                 // pool.go:299 `if len(engineKeys) > 0`
             const uint32_t nblk = evt.n_tokens / B;
             if (nblk == 0 || nblk != evt.n_hashes) {                         // in_memory.go:150-155 -> event dropped
@@ -331,7 +334,7 @@ __global__ void lru_drop_req_kernel(ReqSlot* tab, const unsigned long long* __re
     if (i < slots && meta_state(tab[i].meta) == kStateFull && stamp[i] == *victim) {
         for (int j = 0; j < kMaxEnt; ++j) tab[i].ent[j] = 0;
         tab[i].meta = make_meta(kStateTomb, 0, meta_model(tab[i].meta));
-        atomicAdd(&cnt->req_full, ~0ull); atomicAdd(&cnt->req_tomb, 1ull);
+        atomicAdd(&cnt->req_full, ~0ull); atomicAdd(&cnt->req_tomb, 1ull); atomicAdd(&cnt->cap_evicted[0], 1ull);
     }
 }
 __global__ void lru_min_eng_kernel(const EngSlot* __restrict__ tab, uint64_t slots, unsigned long long* out_min) {
@@ -342,13 +345,15 @@ __global__ void lru_drop_eng_kernel(EngSlot* tab, uint64_t slots, const unsigned
     const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (i < slots && meta_state(tab[i].meta) == kStateFull && tab[i].stamp == *victim) {
         tab[i].meta = make_meta(kStateTomb, 0, meta_model(tab[i].meta));
-        atomicAdd(&cnt->eng_full, ~0ull); atomicAdd(&cnt->eng_tomb, 1ull);
+        atomicAdd(&cnt->eng_full, ~0ull); atomicAdd(&cnt->eng_tomb, 1ull); atomicAdd(&cnt->cap_evicted[1], 1ull);
     }
 }
 
-// Re-insert every FULL slot of an old table into a fresh one (drops tombstones).  Runs with the tables quiesced.
+// Re-insert every FULL slot of an old table into a fresh one (drops tombstones).  Runs with the tables quiesced.  A CLOCK
+// handle's reference bit moves with its key (old_ref / new_ref; nullptr otherwise).
 __global__ void rebuild_req_kernel(const ReqSlot* __restrict__ old_tab, uint64_t old_slots, ReqSlot* new_tab, uint64_t new_mask,
-                                   const unsigned long long* __restrict__ old_stamp, unsigned long long* new_stamp) {
+                                   const unsigned long long* __restrict__ old_stamp, unsigned long long* new_stamp,
+                                   const uint32_t* __restrict__ old_ref, uint32_t* new_ref) {
     const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (i >= old_slots) return;
     const uint4* src = reinterpret_cast<const uint4*>(old_tab + i);
@@ -362,12 +367,14 @@ __global__ void rebuild_req_kernel(const ReqSlot* __restrict__ old_tab, uint64_t
         if (atomicCAS(&new_tab[j].meta, 0u, make_meta(kStateBusy, 0, 0)) == 0u) {
             st_slot(new_tab + j, a, b);
             if (new_stamp) new_stamp[j] = old_stamp[i];
+            if (old_ref && ((old_ref[i >> 5] >> (i & 31)) & 1u)) atomicOr(&new_ref[j >> 5], 1u << (j & 31));
             return;
         }
         j = (j + 1) & new_mask;
     }
 }
-__global__ void rebuild_eng_kernel(const EngSlot* __restrict__ old_tab, uint64_t old_slots, EngSlot* new_tab, uint64_t new_mask) {
+__global__ void rebuild_eng_kernel(const EngSlot* __restrict__ old_tab, uint64_t old_slots, EngSlot* new_tab, uint64_t new_mask,
+                                   const uint32_t* __restrict__ old_ref, uint32_t* new_ref) {
     const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (i >= old_slots) return;
     const uint4* src = reinterpret_cast<const uint4*>(old_tab + i);
@@ -380,6 +387,7 @@ __global__ void rebuild_eng_kernel(const EngSlot* __restrict__ old_tab, uint64_t
     for (;;) {
         if (atomicCAS(&new_tab[j].meta, 0u, make_meta(kStateBusy, 0, 0)) == 0u) {
             st_slot(new_tab + j, a, b);
+            if (old_ref && ((old_ref[i >> 5] >> (i & 31)) & 1u)) atomicOr(&new_ref[j >> 5], 1u << (j & 31));
             return;
         }
         j = (j + 1) & new_mask;

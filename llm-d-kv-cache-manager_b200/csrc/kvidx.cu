@@ -19,6 +19,7 @@
 #include "../../include/kvidx.h"
 #include "kernels_v1.cuh"
 #include "kernels_write.cuh"
+#include "kernels_clock.cuh"
 #include "kernels_remove.cuh"
 #include "kernels_snapshot.cuh"
 #include "kernels_score.cuh"
@@ -137,6 +138,7 @@ struct kvidx {
     PinBuf h_stage[2], h_out[2];
     // write-side scratch (guarded by mu_w)
     DevBuf d_misc, d_ev, d_hash, d_evtok, d_qoff, d_wkeys, d_wpred, d_wready, d_wmap;
+    DevBuf d_sweep;                 // CLOCK sweep scratch: bitmap image, per-tile counts, control block
     PinBuf h_misc;
     // snapshot / restore (guarded by mu_w): two pinned chunks between the device and a caller's buffer, which may be
     // pageable; the device scratch (records, sort buffers) is released when the call returns
@@ -240,13 +242,19 @@ int rebuild(kvidx* x, bool in_place) {
     const int T = 256;
     unsigned long long* nstamp = nullptr;
     if (x->tv.req_stamp) { CK(cudaMalloc((void**)&nstamp, rs * 8)); CK(cudaMemsetAsync(nstamp, 0, rs * 8, st)); }
-    rebuild_req_kernel<<<(unsigned)((rs + T - 1) / T), T, 0, st>>>(x->tv.req, rs, nreq, rs - 1, x->tv.req_stamp, nstamp);
-    rebuild_eng_kernel<<<(unsigned)((es + T - 1) / T), T, 0, st>>>(x->tv.eng, es, neng, es - 1);
+    uint32_t *nrref = nullptr, *neref = nullptr;       // CLOCK: every key's reference bit moves with it
+    if (x->tv.req_ref) {
+        CK(cudaMalloc((void**)&nrref, rs / 8)); CK(cudaMemsetAsync(nrref, 0, rs / 8, st));
+        CK(cudaMalloc((void**)&neref, es / 8)); CK(cudaMemsetAsync(neref, 0, es / 8, st));
+    }
+    rebuild_req_kernel<<<(unsigned)((rs + T - 1) / T), T, 0, st>>>(x->tv.req, rs, nreq, rs - 1, x->tv.req_stamp, nstamp, x->tv.req_ref, nrref);
+    rebuild_eng_kernel<<<(unsigned)((es + T - 1) / T), T, 0, st>>>(x->tv.eng, es, neng, es - 1, x->tv.eng_ref, neref);
     x->launches += 2;
     CK(cudaGetLastError());
-    // zero the tombstone counters on the device
+    // zero the tombstone counters on the device, and the CLOCK hands (slot positions of the old layout)
     CK(cudaMemsetAsync(&x->d_cnt->req_tomb, 0, sizeof(unsigned long long), st));
     CK(cudaMemsetAsync(&x->d_cnt->eng_tomb, 0, sizeof(unsigned long long), st));
+    CK(cudaMemsetAsync(x->d_cnt->hand, 0, sizeof x->d_cnt->hand, st));
     if (in_place) {
         CK(cudaMemcpyAsync(x->tv.req, nreq, rs * sizeof(ReqSlot), cudaMemcpyDeviceToDevice, st));
         CK(cudaMemcpyAsync(x->tv.eng, neng, es * sizeof(EngSlot), cudaMemcpyDeviceToDevice, st));
@@ -256,6 +264,7 @@ int rebuild(kvidx* x, bool in_place) {
         CK(cudaStreamSynchronize(st));
         cudaFree(x->tv.req); cudaFree(x->tv.eng);
         if (x->tv.req_stamp) { cudaFree(x->tv.req_stamp); x->tv.req_stamp = nstamp; }
+        if (x->tv.req_ref) { cudaFree(x->tv.req_ref); cudaFree(x->tv.eng_ref); x->tv.req_ref = nrref; x->tv.eng_ref = neref; }
         x->tv.req = nreq; x->tv.eng = neng;
         x->tv.req_peer[0] = nreq; x->tv.eng_peer[0] = neng;
     }
@@ -269,6 +278,10 @@ int rebuild(kvidx* x, bool in_place) {
 //              each must have room for the whole batch; compaction is the collective kvidx_shard_compact.
 int ensure_room(kvidx* x, uint64_t incoming) {
     const uint64_t rs = x->tv.req_mask + 1, es = x->tv.eng_mask + 1;
+    // CLOCK: every eviction leaves a tombstone, so under churn tombstones are the steady state.  The host copy of the counters
+    // is stale after an asynchronous batch (kvidx_apply_events_dev never reads them back): read them here, after the batches
+    // queued before this call, so that the tombstones are compacted before they fill the table
+    if (x->tv.req_ref) { int rc = refresh_counters(x); if (rc) return rc; }
     auto over = [&](uint64_t full, uint64_t tomb, uint64_t slots) { return (full + tomb + incoming) * 10 > slots * 8; };
     if (x->tv.shard_bits) {
         const uint32_t ns = 1u << x->tv.shard_bits;
@@ -328,6 +341,44 @@ int enforce_caps(kvidx* x) {
         if ((rc = refresh_counters(x))) return rc;
     }
     return 0;
+}
+
+// CLOCK mode: queue the sweeps that bring both tables back to `capacity` keys (kernels_clock.cuh) on the write stream.
+// The excess is read from the counters on the device, so this never waits for the device.  Caller holds mu_w and
+// `tables` (shared or exclusive).
+int clock_sweep(kvidx* x) {
+    if (!x->tv.req_ref) return 0;
+    const uint64_t slots = x->tv.req_mask + 1;        // both tables have the same slot count
+    const uint64_t words = slots / 32, tiles = (slots + kSweepTile - 1) / kSweepTile;
+    const size_t tile_off = (words * 4 + 255) & ~(size_t)255, ctl_off = tile_off + ((tiles * 16 + 255) & ~(size_t)255);
+    CK(x->d_sweep.need(ctl_off + sizeof(SweepCtl)));
+    uint8_t* d = x->d_sweep.as<uint8_t>();
+    uint32_t* snap = reinterpret_cast<uint32_t*>(d);
+    unsigned long long* tile_cnt = reinterpret_cast<unsigned long long*>(d + tile_off);
+    SweepCtl* ctl = reinterpret_cast<SweepCtl*>(d + ctl_off);
+    cudaStream_t st = wstream(x);
+    const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)x->sm_count * 8);
+    const unsigned wgrid = (unsigned)std::min<uint64_t>((words + 255) / 256, (uint64_t)x->sm_count * 8);
+    Counters* c = x->d_cnt;
+    const uint64_t cap = x->tv.capacity;
+    sweep_snap_kernel<<<wgrid, 256, 0, st>>>(x->tv.req_ref, snap, words, &c->req_full, cap);
+    sweep_count_kernel<ReqSlot><<<grid, kSweepThreads, 0, st>>>(x->tv.req, x->tv.req_mask, snap, &c->req_full, cap, &c->hand[0], tile_cnt);
+    sweep_cut_kernel<ReqSlot><<<1, kCutThreads, 0, st>>>(x->tv.req, x->tv.req_mask, snap, &c->req_full, cap, &c->hand[0], tile_cnt, ctl, &c->sweeps, &c->turns2);
+    sweep_apply_kernel<ReqSlot><<<grid, kSweepThreads, 0, st>>>(x->tv.req, x->tv.req_mask, x->tv.req_ref, snap, ctl, &c->req_full, &c->req_tomb, &c->cap_evicted[0]);
+    sweep_snap_kernel<<<wgrid, 256, 0, st>>>(x->tv.eng_ref, snap, words, &c->eng_full, cap);
+    sweep_count_kernel<EngSlot><<<grid, kSweepThreads, 0, st>>>(x->tv.eng, x->tv.eng_mask, snap, &c->eng_full, cap, &c->hand[1], tile_cnt);
+    sweep_cut_kernel<EngSlot><<<1, kCutThreads, 0, st>>>(x->tv.eng, x->tv.eng_mask, snap, &c->eng_full, cap, &c->hand[1], tile_cnt, ctl, &c->sweeps, &c->turns2);
+    sweep_apply_kernel<EngSlot><<<grid, kSweepThreads, 0, st>>>(x->tv.eng, x->tv.eng_mask, x->tv.eng_ref, snap, ctl, &c->eng_full, &c->eng_tomb, &c->cap_evicted[1]);
+    x->launches += 8;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// The key cap of a synchronous write call: exact LRU or CLOCK, then the counters as the call leaves them.
+int cap_keys(kvidx* x) {
+    if (!x->tv.req_ref) return enforce_caps(x);
+    int rc = clock_sweep(x);
+    return rc ? rc : refresh_counters(x);
 }
 
 struct ScoreOut { double* dense; uint16_t* sp_pods; double* sp_scores; uint8_t* sp_cnt; uint8_t* has_keys; };
@@ -487,7 +538,8 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
             const unsigned hgrid = (unsigned)std::min<int64_t>((m + kHashThreads - 1) / kHashThreads, (int64_t)x->sm_count * (np == 1 ? 4 : x->rounds_grid[2]));
             hash_round_kernel<16><<<hgrid, kHashThreads, sizeof(HashSmem<16>), sS[q]>>>(x->tv, a, rb[q], cur, (int)r, trace);
             const unsigned wgrid = (unsigned)std::min<int64_t>((m + W - 1) / W, (int64_t)x->sm_count * (np == 1 ? 8 : x->rounds_grid[3]));
-            walk_round_kernel<<<wgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
+            if (x->tv.req_ref) walk_round_kernel<true><<<wgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
+            else walk_round_kernel<false><<<wgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
             const unsigned rgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : x->rounds_grid[4]));
             finish_round_kernel<16><<<rgrid, T, sizeof(DetachWarp) * W, sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup >= 2, x->rounds_trace);
             compact_round_kernel<<<(unsigned)((m + kCompactTile - 1) / kCompactTile), kCompactThreads, 0, sS[q]>>>(rb[q], cur, (int)r);
@@ -567,7 +619,8 @@ int launch_score_rounds_plain(kvidx* x, const uint32_t* d_tok, const int64_t* d_
                 continue;
             }
             const unsigned pgrid = (unsigned)std::min<int64_t>((m + plain::kProbeThreads - 1) / plain::kProbeThreads, (int64_t)x->sm_count * per_sm);
-            plain::probe_round_kernel<<<pgrid, plain::kProbeThreads, sizeof(plain::WalkSmem), strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
+            if (x->tv.req_ref) plain::probe_round_kernel<true><<<pgrid, plain::kProbeThreads, sizeof(plain::WalkSmem), strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
+            else plain::probe_round_kernel<false><<<pgrid, plain::kProbeThreads, sizeof(plain::WalkSmem), strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
         }
         x->launches += 2 * nh;
     }
@@ -1076,6 +1129,7 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     t.max_pods = c.max_pods; t.filter_words = (c.max_pods + 63) / 64;
     for (int i = 0; i < 16; ++i) t.weight[i] = (uint32_t)i < c.n_tier_weights ? c.tier_weight[i] : 1.0;
     t.req_stamp = nullptr;
+    t.req_ref = nullptr; t.eng_ref = nullptr;
     // a sharded handle's removal bitmaps (kvidx_shard_remove_pods) follow its request slots: its peers read them through
     // the mapping they already hold, and the in-place compaction rewrites only the slots
     int rc = alloc_tables(x, slots, slots, &t.req, &t.eng, x->stream, shard_bits ? remove_bitmap_bytes(slots) : 0);
@@ -1084,6 +1138,12 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
         if (c.shard_count > 1) return fail(KVIDX_EINVAL, "lru_exact is not supported on a sharded index");
         CK(cudaMalloc((void**)&t.req_stamp, slots * 8));
         CK(cudaMemsetAsync(t.req_stamp, 0, slots * 8, x->stream));
+    }
+    if (c.evict_policy == KVIDX_EVICT_CLOCK) {
+        CK(cudaMalloc((void**)&t.req_ref, slots / 8));
+        CK(cudaMalloc((void**)&t.eng_ref, slots / 8));
+        CK(cudaMemsetAsync(t.req_ref, 0, slots / 8, x->stream));
+        CK(cudaMemsetAsync(t.eng_ref, 0, slots / 8, x->stream));
     }
     CK(cudaMalloc((void**)&x->d_cnt, sizeof(Counters)));
     CK(cudaMemsetAsync(x->d_cnt, 0, sizeof(Counters), x->stream));
@@ -1139,6 +1199,9 @@ int kvidx_create(const kvidx_config_t* cfg_in, kvidx_t** out) {
     if (c.max_pods == 0) c.max_pods = 256;
     if (c.max_pods > KVIDX_MAX_PODS) return fail(KVIDX_ERANGE, "max_pods %u > %u", c.max_pods, KVIDX_MAX_PODS);
     if (c.n_tier_weights > KVIDX_MAX_TIERS) return fail(KVIDX_ERANGE, "n_tier_weights > 16");
+    if (c.evict_policy > KVIDX_EVICT_CLOCK) return fail(KVIDX_EINVAL, "unknown evict_policy %u", c.evict_policy);
+    if (c.evict_policy == KVIDX_EVICT_CLOCK && c.lru_exact) return fail(KVIDX_EINVAL, "evict_policy CLOCK and lru_exact exclude each other");
+    if (c.evict_policy == KVIDX_EVICT_CLOCK && c.shard_count > 1) return fail(KVIDX_EINVAL, "evict_policy CLOCK is not supported on a sharded index");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -1178,6 +1241,9 @@ void kvidx_destroy(kvidx_t* x) {
     if (x->tv.req) cudaFree(x->tv.req);
     if (x->tv.eng) cudaFree(x->tv.eng);
     if (x->tv.req_stamp) cudaFree(x->tv.req_stamp);
+    if (x->tv.req_ref) cudaFree(x->tv.req_ref);
+    if (x->tv.eng_ref) cudaFree(x->tv.eng_ref);
+    x->d_sweep.release();
     if (x->d_cnt) cudaFree(x->d_cnt);
     if (x->h_cnt) cudaFreeHost(x->h_cnt);
     if (x->d_cnt_all) cudaFree(x->d_cnt_all);
@@ -1436,7 +1502,7 @@ int kvidx_add(kvidx_t* x, uint32_t model, const uint64_t* engine, const uint64_t
     rc = refresh_counters(x);
     if (rc) return rc;
     if (x->h_cnt->nospc != nospc_before) return fail(KVIDX_ENOSPC, "%llu inserts refused: the owning shard is full", x->h_cnt->nospc - nospc_before);
-    return enforce_caps(x);
+    return cap_keys(x);
 }
 
 int kvidx_evict(kvidx_t* x, uint32_t model, uint64_t engine, const kvidx_podtier_t* pts, int32_t m) {
@@ -1455,6 +1521,7 @@ int kvidx_evict(kvidx_t* x, uint32_t model, uint64_t engine, const kvidx_podtier
     evict_kernel<<<1, 32, 0, st>>>(x->tv, model, engine, x->d_misc.as<uint16_t>(), m, reserve_stamps(x, 4));
     x->launches += 1;
     CK(cudaGetLastError());
+    if (int rc = clock_sweep(x)) return rc;
     return refresh_counters(x);
 }
 
@@ -1534,6 +1601,7 @@ int kvidx_apply_events_dev(kvidx_t* x, const kvidx_event_t* d_ev_sorted, const i
     cudaStream_t st = wstream(x);
     rc = launch_apply_events(x, d_ev_sorted, d_queue_off, n_queues, n_events, d_hashes, n_hashes, d_tokens, st);
     if (rc) return rc;
+    if ((rc = clock_sweep(x))) return rc;              // asynchronous too: the excess is read on the device
     // events dropped so far on this handle (cumulative, like the counter behind kvidx_apply_events' n_dropped_out)
     if (d_n_dropped) CK(cudaMemcpyAsync(d_n_dropped, &x->d_cnt->dropped_events, sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
     CK(cudaEventRecord(x->ev_write, st));              // reads issued after this call are ordered after the batch
@@ -1599,7 +1667,7 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
     if (rc) return rc;
     if (n_dropped_out) *n_dropped_out = (int64_t)(x->h_cnt->dropped_events - dropped_before);
     if (x->h_cnt->nospc != nospc_before) return fail(KVIDX_ENOSPC, "%llu inserts refused: the owning shard is full", x->h_cnt->nospc - nospc_before);
-    return enforce_caps(x);
+    return cap_keys(x);
 }
 
 }  // extern "C"
@@ -1952,6 +2020,11 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
         CK(cudaMemsetAsync(&x->d_cnt->req_tomb, 0, sizeof(unsigned long long), st));
         CK(cudaMemsetAsync(&x->d_cnt->eng_tomb, 0, sizeof(unsigned long long), st));
     }
+    // restored keys start unreferenced on a CLOCK handle
+    if (x->tv.req_ref) {
+        CK(cudaMemsetAsync(x->tv.req_ref, 0, (x->tv.req_mask + 1) / 8, st));
+        CK(cudaMemsetAsync(x->tv.eng_ref, 0, (x->tv.eng_mask + 1) / 8, st));
+    }
     // 3. insert; recency is kept only by an exact-LRU handle
     const unsigned long long nospc_before = x->h_cnt->nospc, from_req = h_from[0], from_eng = h_from[1];
     if (R) restore_req_kernel<<<snap_ctas(x, R), kSnapThreads, 0, st>>>(x->tv, req_rec, R, keep ? req_st : nullptr, from_req);
@@ -1965,7 +2038,7 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
         while (cur <= stamp_max && !x->clock.compare_exchange_weak(cur, stamp_max + 1)) {}
     }
     release_snap(x);
-    if ((rc = enforce_caps(x))) return rc;            // a no-op after the cut above; kept as the invariant of every write call
+    if ((rc = cap_keys(x))) return rc;                // exact LRU: a no-op after the cut above; CLOCK: the sweep cuts the image
     if (restored_out) { restored_out[0] = x->h_cnt->req_full; restored_out[1] = x->h_cnt->eng_full; }
     return 0;
 }
@@ -2210,6 +2283,24 @@ int kvidx_shard_compact(kvidx_t* x) {
     std::unique_lock<std::shared_mutex> tl(x->tables);
     CK(cudaSetDevice(x->device));
     return rebuild(x, x->tv.shard_bits != 0);
+}
+
+// Counters of the device block read without the write lock, on no stream of the handle: a call never waits behind a write
+// batch in flight (a metrics scrape), and sees the counts of the batches completed so far.
+static int read_device_counters(kvidx* x, size_t off, uint64_t* out, int n) {
+    CK(cudaSetDevice(x->device));
+    CK(cudaMemcpy(out, reinterpret_cast<const uint8_t*>(x->d_cnt) + off, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int kvidx_get_evictions(kvidx_t* x, uint64_t out[2]) {
+    if (!x || !out) return fail(KVIDX_EINVAL, "bad arguments");
+    return read_device_counters(x, offsetof(Counters, cap_evicted), out, 2);
+}
+
+int kvidx_get_sweeps(kvidx_t* x, uint64_t out[2]) {
+    if (!x || !out) return fail(KVIDX_EINVAL, "bad arguments");
+    return read_device_counters(x, offsetof(Counters, sweeps), out, 2);
 }
 
 int kvidx_get_stats(kvidx_t* x, kvidx_stats_t* out) {

@@ -113,6 +113,16 @@ __device__ __forceinline__ bool pair_decides(const uint4& a0, const uint4& b0, c
     if (!hit && meta_state(B.w) != kStateEmpty) { A = a1; B = b1; hit = slot_matches(A, B, key, mdl); }
     return hit || meta_state(B.w) == kStateEmpty;
 }
+// CLOCK mode (t.req_ref set): the slot of a hit that the pair at `slot` decided -- slot 0 if it holds the key, else slot 1
+// -- is marked as referenced.  The Score() kernels mark exactly the blocks their walk looks at: block 0 up to and including
+// the block that empties the active pod set, never a block fetched ahead of the walk's end.  One uniform branch on the
+// pointer; default handles skip it.
+__device__ __forceinline__ uint64_t pair_hit_slot(uint64_t slot, const uint4& a0, const uint4& b0, uint64_t key, uint32_t mdl) {
+    return slot + (slot_matches(a0, b0, key, mdl) ? 0u : 1u);
+}
+__device__ __forceinline__ void mark_hit(const TableView& t, uint64_t slot, const uint4& a0, const uint4& b0, uint64_t key, uint32_t mdl) {
+    if (t.req_ref) ref_touch(t.req_ref, pair_hit_slot(slot, a0, b0, key, mdl));
+}
 __device__ __forceinline__ void ld_slot_pair(const ReqSlot* s, bool peer, uint4& a0, uint4& b0, uint4& a1, uint4& b1) {
     ld_slot(s, peer, a0, b0);
     ld_slot(s + 1, peer, a1, b1);
@@ -155,6 +165,8 @@ struct HomeProbe {
         while (!decide(t, key, mdl, peer, A, B, hit)) load(peer);
         return hit;
     }
+    // after a hit: the slot it was found in (CLOCK marking)
+    __device__ __forceinline__ uint64_t hit_slot(uint64_t key, uint32_t mdl) const { return pair_hit_slot(slot, a0, b0, key, mdl); }
     // both at once, with the loads in one place (every ld_slot is a sequence-lock loop: fewer copies, shorter code)
     __device__ __forceinline__ bool find(const TableView& t, uint64_t key, uint32_t mdl, bool peer, uint4& A, uint4& B) {
         aim(t, key, mdl);
@@ -347,6 +359,11 @@ struct WarpWalk {
             if (present) { sc = __dadd_rn(sc, mx); bt = b; }
         }
         alive = __ballot_sync(0xffffffffu, present);
+    }
+    // CLOCK marking of a warp walk: lane l probed block l of the chunk and found it in slot `hslot`; walk() looked at the
+    // chunk's first j blocks, so exactly those are marked (blocks fetched beyond the walk's end are not)
+    __device__ __forceinline__ static void mark_walked(const TableView& t, int lane, int j, bool hit, uint64_t hslot) {
+        if (t.req_ref && lane < j && hit) ref_touch(t.req_ref, hslot);
     }
     // n blocks that repeat the previous block's pattern: each live pod's addend n times more, in order
     __device__ __forceinline__ void run(const TableView& t, int lane, int n) {

@@ -81,14 +81,21 @@ struct Counters {
     unsigned long long clock;              // recency clock (exact-LRU mode)
     unsigned long long pad;                // work counter of the fused score kernel
     unsigned long long rehashed;           // write path: events whose parent resolved differently from the prediction
-    unsigned long long rsv[7];
+    unsigned long long cap_evicted[2];     // request keys / engine mappings dropped by the capacity bound (CLOCK or exact LRU)
+    unsigned long long hand[2];            // CLOCK mode: the sweep's hand in the request / engine table (a rebuild resets it)
+    unsigned long long sweeps;             // CLOCK mode: sweeps that evicted (both tables) ...
+    unsigned long long turns2;             // ... and those of them that went past a full turn of the hand
+    unsigned long long rsv[1];
 };
+static_assert(sizeof(Counters) == 16 * 8, "counter block layout");
 
 struct TableView {
     ReqSlot* req;
     EngSlot* eng;
     unsigned long long* req_stamp;   // per-request-slot recency stamp: exact-LRU mode only (else nullptr).  Engine
                                      // slots carry their stamp inline.  Larger = more recent (golang-lru front).
+    uint32_t* req_ref;               // CLOCK mode only (else nullptr): a reference bit per request / engine slot, set where
+    uint32_t* eng_ref;               // golang-lru refreshes recency, cleared by the sweep (kernels_clock.cuh)
     uint64_t req_mask, eng_mask;
     uint64_t capacity;
     uint64_t init_hash;
@@ -189,6 +196,14 @@ __device__ __forceinline__ uint32_t slot_ent(const SlotWords& w, int j) {
     return (j & 1) ? (word >> 16) : (word & 0xffffu);
 }
 
+// CLOCK mode: mark slot `slot` as referenced.  The word is read first and the atomic issued only when the bit is clear, so a
+// hot key costs a load, not an atomic, per touch.
+__device__ __forceinline__ void ref_touch(uint32_t* bits, uint64_t slot) {
+    uint32_t* w = bits + (slot >> 5);
+    const uint32_t m = 1u << (slot & 31);
+    if (!(ld_word_relaxed(w, false) & m)) atomicOr(w, m);
+}
+
 // ---- readers ------------------------------------------------------------------------------------------
 
 // Finds the FULL slot holding (model, tag).  Returns false at the first EMPTY slot (or after a full cycle).
@@ -212,7 +227,7 @@ __device__ __forceinline__ bool req_find(const TableView& t, uint32_t model, uin
 
 // engine -> request lookup (GetRequestKey, in_memory.go:264-270).  An engine slot image is {ehash, rhash | meta, pad, stamp}.
 __device__ __forceinline__ bool eng_find(const TableView& t, uint32_t model, uint64_t ehash, uint64_t* rhash, uint64_t* slot_out = nullptr,
-                                         unsigned long long stamp = 0) {
+                                         unsigned long long stamp = 0, bool touch = false) {
     const uint64_t hm = home_of(ehash, model);
     const EngSlot* base = t.eng_peer[shard_of(hm, t.shard_bits)];
     uint64_t i = hm & t.eng_mask & ~1ull;
@@ -227,6 +242,7 @@ __device__ __forceinline__ bool eng_find(const TableView& t, uint32_t model, uin
             *rhash = ((uint64_t)a.w << 32) | a.z;
             if (slot_out) *slot_out = i;
             if (stamp && t.req_stamp) *(volatile uint64_t*)&const_cast<EngSlot*>(s)->stamp = stamp;   // lru Get refreshes recency
+            if (touch && t.eng_ref) ref_touch(t.eng_ref, i);                                        // ... CLOCK: its bit
             return true;
         }
         i = (i + 1) & t.eng_mask;

@@ -336,6 +336,10 @@ int64_t kvhost_metrics_text(kvhost_t* h, char* buf, size_t cap) {
     counter("lookup_requests_total", "Total number of lookup calls", m.lookup_requests_total);
     counter("max_pod_hit_count_total", "Maximum cache hits on a single pod on Lookup()", m.max_pod_hit_count_total);
     counter("lookup_hits_total", "Number of keys found in the cache on Lookup()", m.lookup_hits_total);
+    uint64_t cap_ev[2] = {0, 0};                      // the index's own count (no device: none)
+    if (h->ix && kvidx_get_evictions(h->ix, cap_ev)) cap_ev[0] = cap_ev[1] = 0;   // does not wait for a write batch
+    counter("capacity_evictions_total", "Total number of request keys evicted to hold the index to its capacity", cap_ev[0]);
+    counter("capacity_engine_evictions_total", "Total number of engine-key mappings evicted to hold the index to its capacity", cap_ev[1]);
     s += "# HELP kvcache_index_lookup_latency_seconds Latency of Lookup calls in seconds\n# TYPE kvcache_index_lookup_latency_seconds histogram\n";
     char tmp[96];
     for (int b = 0; b < KVHOST_LATENCY_BUCKETS; ++b) {

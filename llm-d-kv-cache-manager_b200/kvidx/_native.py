@@ -19,6 +19,8 @@ MAX_TIERS = 16
 SCORE_ABSENT = -1.0
 OK, ENOENT, ECUDA, ENOMEM, EINVAL, ENOSPC, ERANGE = 0, -2, -5, -12, -22, -28, -34
 EV_BLOCK_STORED, EV_BLOCK_REMOVED = 0, 1
+EVICT_NONE, EVICT_CLOCK = 0, 1
+_EVICT_POLICIES = {"none": EVICT_NONE, "clock": EVICT_CLOCK}
 
 
 class Config(C.Structure):
@@ -27,7 +29,7 @@ class Config(C.Structure):
                 ("pods_per_key", C.c_uint32), ("init_hash", C.c_uint64), ("capacity", C.c_uint64),
                 ("table_slots", C.c_uint64), ("max_pods", C.c_uint32), ("n_tier_weights", C.c_uint32),
                 ("tier_weight", C.c_double * MAX_TIERS), ("lru_exact", C.c_uint32), ("shard_rank", C.c_uint32),
-                ("shard_count", C.c_uint32), ("reserved", C.c_uint32 * 5)]
+                ("shard_count", C.c_uint32), ("evict_policy", C.c_uint32), ("reserved", C.c_uint32 * 4)]
 
 
 class Stats(C.Structure):
@@ -80,6 +82,8 @@ SYMBOLS = {
     "kvidx_probe_slots_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int64, C.c_void_p]),
     "kvidx_score_slots_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kvidx_get_stats": (C.c_int, [C.c_void_p, C.POINTER(Stats)]),
+    "kvidx_get_evictions": (C.c_int, [C.c_void_p, _u64p]),
+    "kvidx_get_sweeps": (C.c_int, [C.c_void_p, _u64p]),
     "kvidx_shard_export": (C.c_int, [C.c_void_p, C.c_char_p]),
     "kvidx_shard_import": (C.c_int, [C.c_void_p, C.c_uint32, C.c_char_p]),
     "kvidx_shard_attach": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -129,7 +133,10 @@ class Index:
     """One libkvidx handle (== kvblock.Index + TokenProcessor + scorer of the reference, ids not strings)."""
 
     def __init__(self, block_size=16, init_hash=None, hash_seed="", capacity=1 << 20, pods_per_key=10,
-                 tier_weights=(1.0, 0.8), max_pods=256, table_slots=0, device=0, lru_exact=0, shard_rank=0, shard_count=0):
+                 tier_weights=(1.0, 0.8), max_pods=256, table_slots=0, device=0, lru_exact=0, shard_rank=0, shard_count=0,
+                 evict_policy="none"):
+        """evict_policy: "none" (capacity only sizes the table) or "clock" (each map held to `capacity` keys by a CLOCK
+        sweep after every write call, include/kvidx.h); an int is passed to the C ABI as it is."""
         self.L = load()
         cfg = Config()
         self.L.kvidx_config_default(C.byref(cfg))
@@ -145,6 +152,7 @@ class Index:
             cfg.tier_weight[i] = float(w)
         cfg.lru_exact = lru_exact
         cfg.shard_rank, cfg.shard_count = shard_rank, shard_count
+        cfg.evict_policy = _EVICT_POLICIES[evict_policy] if isinstance(evict_policy, str) else int(evict_policy)
         h = C.c_void_p()
         rc = self.L.kvidx_create(C.byref(cfg), C.byref(h))
         if rc:
@@ -186,6 +194,18 @@ class Index:
         s = Stats()
         self._ck(self.L.kvidx_get_stats(self.h, C.byref(s)))
         return {n: getattr(s, n) for n, _ in Stats._fields_}
+
+    def evictions(self) -> tuple:
+        """(request keys, engine mappings) dropped by the capacity bound since the handle was created."""
+        out = np.zeros(2, np.uint64)
+        self._ck(self.L.kvidx_get_evictions(self.h, _p(out, _u64p)))
+        return int(out[0]), int(out[1])
+
+    def sweeps(self) -> tuple:
+        """CLOCK mode: (sweeps that evicted, those that went past a full turn of the hand), both maps together."""
+        out = np.zeros(2, np.uint64)
+        self._ck(self.L.kvidx_get_sweeps(self.h, _p(out, _u64p)))
+        return int(out[0]), int(out[1])
 
     # -- hash-range sharding (one handle per GPU) --
     SHARD_HANDLE_BYTES = 192

@@ -86,12 +86,14 @@ class HostIndexer:
     """kvcache.Indexer + kvblock.Index + kvevents.Pool with strings (pods, tiers, models are names)."""
 
     def __init__(self, block_size=16, hash_seed="", capacity=1 << 20, pods_per_key=10, tiers=(("gpu", 1.0), ("cpu", 0.8)), max_pods=256,
-                 concurrency=4, device=0, no_device=False, lru_exact=0, enable_metrics=False, clear_on_all_blocks_cleared=False):
+                 concurrency=4, device=0, no_device=False, lru_exact=0, enable_metrics=False, clear_on_all_blocks_cleared=False,
+                 evict_policy="none"):
         self.L = _lib()
         cfg = HostConfig()
         self.L.kvhost_config_default(C.byref(cfg))
         cfg.index.block_size, cfg.index.capacity, cfg.index.pods_per_key = block_size, capacity, pods_per_key
         cfg.index.max_pods, cfg.index.device, cfg.index.lru_exact = max_pods, device, lru_exact
+        cfg.index.evict_policy = _native._EVICT_POLICIES[evict_policy] if isinstance(evict_policy, str) else int(evict_policy)
         cfg.concurrency, cfg.n_tiers, cfg.no_device = concurrency, len(tiers), 1 if no_device else 0
         cfg.enable_metrics = 1 if enable_metrics else 0
         cfg.clear_on_all_blocks_cleared = 1 if clear_on_all_blocks_cleared else 0
