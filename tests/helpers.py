@@ -12,6 +12,11 @@ EVENT_DTYPE = np.dtype([("op", "u1"), ("has_parent", "u1"), ("podtier", "<u2"), 
                         ("n_hashes", "<u4"), ("n_tokens", "<u4")])
 
 
+SNAP_REQ_DTYPE = np.dtype([("hash", "<u8"), ("model", "<u2"), ("count", "u1"), ("zero", "u1"), ("ent", "<u2", (10,))])
+SNAP_ENG_DTYPE = np.dtype([("hash", "<u8"), ("request", "<u8"), ("model", "<u2"), ("zero", "V6")])
+assert SNAP_REQ_DTYPE.itemsize == 32 and SNAP_ENG_DTYPE.itemsize == 24
+
+
 def golden(name):
     with open(os.path.join(GOLDEN, name)) as f:
         return json.load(f)
@@ -70,6 +75,80 @@ def scenario_events(sc, pods: Interner, tiers: Interner, model_id=0):
             tokens.extend(e["tokens"])
         ev.append(r)
     return (np.array(ev, EVENT_DTYPE), np.array(hashes, np.uint64), np.array(tokens, np.uint64).astype(np.uint32))
+
+
+def decode_snapshot(img):
+    """A v1 image (include/kvidx.h) -> (request records, engine records) as structured arrays, in image order."""
+    img = bytes(img)
+    assert img[:8] == b"KVIDXSNP"
+    R, E = np.frombuffer(img, "<u8", 2, 32)
+    req = np.frombuffer(img, SNAP_REQ_DTYPE, int(R), 64)
+    eng = np.frombuffer(img, SNAP_ENG_DTYPE, int(E), 64 + 32 * int(R))
+    return req, eng
+
+
+# ---- numpy replica of the table's home slot (csrc/fnv_cbor.cuh home_of, csrc/table.cuh slot_home) ---------------------
+_GOLDEN = np.uint64(0x9E3779B97F4A7C15)
+_MIX = (0xFF51AFD7ED558CCD, 0xC4CEB9FE1A85EC53)
+_UNMIX = tuple(pow(c, -1, 1 << 64) for c in reversed(_MIX))
+
+
+def _home_of(keys, model):
+    x = np.asarray(keys, np.uint64) ^ (np.asarray(model, np.uint64) * _GOLDEN)
+    x = np.atleast_1d(x).copy()
+    x ^= x >> np.uint64(33)
+    x *= np.uint64(_MIX[0])
+    x ^= x >> np.uint64(33)
+    x *= np.uint64(_MIX[1])
+    x ^= x >> np.uint64(33)
+    return x
+
+
+def _slot_home(keys, model, S):
+    return (_home_of(keys, model) & np.uint64((S - 1) & ~1)).astype(np.int64)
+
+
+def keys_homed_at(slots, model, S, rng):
+    """One key per entry of `slots` (even slots of an S-slot table) whose home slot under `model` is that slot.  The mix
+    of _home_of is a bijection (xor-shifts by 33 and odd multipliers), so a random mixed value with the wanted low bits
+    is unmixed into its key."""
+    slots = np.asarray(slots, np.int64)
+    assert not (slots & 1).any()
+    x = rng.integers(0, 1 << 64, len(slots), dtype=np.uint64)
+    x = (x & ~np.uint64((S - 1) & ~1)) | slots.astype(np.uint64)
+    x ^= x >> np.uint64(33)
+    x *= np.uint64(_UNMIX[0])
+    x ^= x >> np.uint64(33)
+    x *= np.uint64(_UNMIX[1])
+    x ^= x >> np.uint64(33)
+    return x ^ np.uint64(int(model) * int(_GOLDEN) & M64)
+
+
+def free_pairs(state):
+    """Even slots s of a table's state array (0 = EMPTY) whose pair s, s + 1 is fully EMPTY."""
+    return np.flatnonzero((state[0::2] == 0) & (state[1::2] == 0)) * 2
+
+
+def keep_free(cands, model, state):
+    """Of the candidate keys (in order), the first one for each home pair that is fully EMPTY in `state`: inserted in one
+    call, each of them lands on its even home slot, wherever the call's inserts run."""
+    cands = np.asarray(cands, np.uint64)
+    home = _slot_home(cands, model, len(state))
+    ok = (state[home] == 0) & (state[home + 1] == 0)
+    _, first = np.unique(home, return_index=True)
+    keep = np.zeros(len(cands), bool)
+    keep[first] = True
+    return cands[ok & keep]
+
+
+def draw_free(state, n, model, rng):
+    """n random keys (no two with one home pair) that keep_free keeps."""
+    out = np.zeros(0, np.uint64)
+    while len(out) < n:
+        c = keep_free(rng.integers(1, 1 << 64, 4 * n + 64, dtype=np.uint64), model, state)
+        c = c[~np.isin(_slot_home(c, model, len(state)), _slot_home(out, model, len(state)))]
+        out = np.concatenate([out, c])
+    return out[:n]
 
 
 def dense_from_map(scores, pods: Interner, P):

@@ -7,7 +7,7 @@ import threading
 import numpy as np
 import pytest
 
-from helpers import EVENT_DTYPE, PATHS, ROUND_PATHS, _index_pair, _select_path, csr, filter_mask
+from helpers import EVENT_DTYPE, PATHS, ROUND_PATHS, _home_of, _index_pair, _select_path, _slot_home, csr, filter_mask
 import kvidx
 from oracle.kvoracle_c import COracle
 
@@ -18,22 +18,6 @@ FNV_OFFSET = 0xCBF29CE484222325
 
 def PT(p, t=0):
     return (p << 4) | t
-
-
-# ---- numpy replica of the table's home slot (csrc/fnv_cbor.cuh home_of, csrc/table.cuh slot_home) ---------------------
-def _home_of(keys, model):
-    x = np.asarray(keys, np.uint64) ^ (np.asarray(model, np.uint64) * np.uint64(0x9E3779B97F4A7C15))
-    x = np.atleast_1d(x).copy()
-    x ^= x >> np.uint64(33)
-    x *= np.uint64(0xFF51AFD7ED558CCD)
-    x ^= x >> np.uint64(33)
-    x *= np.uint64(0xC4CEB9FE1A85EC53)
-    x ^= x >> np.uint64(33)
-    return x
-
-
-def _slot_home(keys, model, S):
-    return (_home_of(keys, model) & np.uint64((S - 1) & ~1)).astype(np.int64)
 
 
 def _check_scores(ix, co, tok, off, model=None, model0=0, fm=None):
