@@ -25,7 +25,7 @@
  *     Add / Evict of that key (table.cuh), which is the guarantee the reference's
  *     per-key mutex gives.  A write call has taken effect when it returns, so a
  *     thread reads its own writes (index_test.go:214-278).  Concurrent host-buffer
- *     kvidx_score_batch* callers are coalesced into one launch;
+ *     kvidx_score_batch* callers are coalesced into one launch (kvidx_score_keys* calls are not);
  *   - there is NO CPU fallback: without a CUDA device kvidx_create fails with
  *     KVIDX_ECUDA.
  */
@@ -167,6 +167,25 @@ int kvidx_score_batch_sparse(kvidx_t* idx, const uint32_t* tok, const int64_t* t
                              const uint32_t* model, uint32_t model0, const uint64_t* filter,
                              uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out);
 
+/* Indexer.GetPodScores steps 3-4 (indexer.go:150-159) for a batch of prompts whose request keys the caller already holds:
+ * LongestPrefixScorer.Score(keys, Index.Lookup(keys, pods)) (kvblock_scorer.go:108-151, in_memory.go:105-146), e.g. a
+ * conversation that kept turn k's keys and hashed only turn k+1's new blocks (kvidx_hash_keys with parent = last key), or
+ * a deployment that keeps its own TokenProcessor.  keys/key_off: CSR, prompt i owns keys[key_off[i] .. key_off[i+1]),
+ * request-key hashes in block order (any list: absent, repeated and other models' keys score as the reference scores
+ * them); key_off[0] may be non-zero.  model, model0, filter, the dense / sparse result rows and KVIDX_SCORE_ABSENT mean what
+ * they mean for kvidx_score_batch; has_keys_out[i] = (prompt i has at least one key) -- no key gives an all-absent row,
+ * the reference's (nil, nil).  One warp per prompt at every batch size and block size; exact-LRU handles stamp every
+ * present key of the prompt, as kvidx_score_batch does.  n_prompts < 0, key_off NULL or not monotone, keys NULL with a
+ * non-zero key count -> KVIDX_EINVAL; n_prompts == 0 -> 0, nothing written.  Host buffers go through the same chunked
+ * copy pipeline as kvidx_score_batch (pinned buffers directly; small calls read pinned keys in place), but calls are NOT
+ * coalesced with other callers: each goes straight through. */
+int kvidx_score_keys(kvidx_t* idx, const uint64_t* keys, const int64_t* key_off, int64_t n_prompts,
+                     const uint32_t* model, uint32_t model0, const uint64_t* filter,
+                     double* scores_out, uint8_t* has_keys_out);
+int kvidx_score_keys_sparse(kvidx_t* idx, const uint64_t* keys, const int64_t* key_off, int64_t n_prompts,
+                            const uint32_t* model, uint32_t model0, const uint64_t* filter,
+                            uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out);
+
 /* ---- write path --------------------------------------------------------------- */
 
 /* Index.Add (index.go:127, in_memory.go:149-209): n (engine,request) key pairs of one model,
@@ -279,6 +298,14 @@ int kvidx_score_batch_dev(kvidx_t* idx, const uint32_t* d_tok, const int64_t* d_
 int kvidx_score_batch_sparse_dev(kvidx_t* idx, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n_prompts,
                                  const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter,
                                  uint16_t* d_pods_out, double* d_scores_out, uint8_t* d_cnt_out, uint8_t* d_has_keys_out);
+/* kvidx_score_keys[_sparse] over device-resident inputs and outputs: one asynchronous kernel on the handle's stream at
+ * every batch size (no wait on the stream), ordered after kvidx_apply_events_dev batches issued before it. */
+int kvidx_score_keys_dev(kvidx_t* idx, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n_prompts,
+                         const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter,
+                         double* d_scores_out, uint8_t* d_has_keys_out);
+int kvidx_score_keys_sparse_dev(kvidx_t* idx, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n_prompts,
+                                const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter,
+                                uint16_t* d_pods_out, double* d_scores_out, uint8_t* d_cnt_out, uint8_t* d_has_keys_out);
 int kvidx_hash_keys_dev(kvidx_t* idx, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n_prompts,
                         const uint64_t* d_parent, const uint8_t* d_parent_valid,
                         const int64_t* d_key_off, uint64_t* d_keys_out);

@@ -8,6 +8,7 @@
  *
  *   kvhost_create            <-> kvcache.NewKVCacheIndexer            pkg/kvcache/indexer.go:75-113
  *   kvhost_get_pod_scores    <-> Indexer.GetPodScores (steps 2-4)     pkg/kvcache/indexer.go:132-166
+ *   kvhost_get_pod_scores_keys <-> GetPodScores steps 3-4 (from keys)  pkg/kvcache/indexer.go:150-159
  *   kvhost_index_*           <-> kvblock.Index Add/Evict/Lookup/GetRequestKey   pkg/kvcache/kvblock/index.go:119-135
  *   kvhost_pool_add_task     <-> kvevents.Pool.AddTask                pkg/kvcache/kvevents/pool.go:132-144
  *   kvhost_pool_process      <-> worker loop: processEvent + digestEvents       pkg/kvcache/kvevents/pool.go:149-338
@@ -53,6 +54,11 @@ kvidx_t* kvhost_index(kvhost_t* h);                      /* Indexer.KVBlockIndex
 int kvhost_get_pod_scores(kvhost_t* h, const uint32_t* tokens, size_t n_tokens, const char* model,
                           const char* const* pods, size_t n_pods, const char** pod_out, double* score_out);
 
+/* Indexer.GetPodScores after step 2 (indexer.go:150-159): the prompt's request keys in block order instead of its tokens
+ * (kvidx_score_keys).  Same filter, results and return values as kvhost_get_pod_scores; -1000 when n_keys == 0. */
+int kvhost_get_pod_scores_keys(kvhost_t* h, const uint64_t* keys, size_t n_keys, const char* model,
+                               const char* const* pods, size_t n_pods, const char** pod_out, double* score_out);
+
 /* kvblock.Index with strings.  entries are (pod, tier) name pairs. */
 int kvhost_index_add(kvhost_t* h, const char* model, const uint64_t* engine, size_t n_engine, const uint64_t* request, size_t n_request,
                      const char* const* pods, const char* const* tiers, size_t n_entries);
@@ -90,7 +96,8 @@ int64_t kvhost_decode_event_batch(kvhost_t* h, const char* pod, const char* mode
  * both max_pod_hit_count and lookup_hits.  The event pool goes through the same Add / Evict (one Evict per removed hash,
  * pool.go:317-330).  With enable_metrics, kvhost_get_pod_scores issues the reference's full-depth Lookup
  * (kvidx_hash_keys + kvidx_lookup on the device) next to the fused score call, because the hit count needs every key of
- * the prompt, not only the consecutive prefix the scorer walks.  All zero when enable_metrics is 0. */
+ * the prompt, not only the consecutive prefix the scorer walks; kvhost_get_pod_scores_keys issues the same Lookup over the
+ * keys it was given.  All zero when enable_metrics is 0. */
 #define KVHOST_LATENCY_BUCKETS 11          /* prometheus.DefBuckets: .005 .01 .025 .05 .1 .25 .5 1 2.5 5 10 (+Inf = count) */
 typedef struct kvhost_metrics {
     uint64_t admissions_total, evictions_total, lookup_requests_total, max_pod_hit_count_total, lookup_hits_total;

@@ -58,23 +58,28 @@ __global__ void lookup_kernel_v1(TableView t, uint32_t model, const uint64_t* __
     cnt_out[i] = (uint8_t)c;
 }
 
-// Indexer.GetPodScores steps 2-4 (indexer.go:141-163): thread per prompt.
-__global__ void score_kernel_v1(TableView t, const uint32_t* __restrict__ tok, const int64_t* __restrict__ tok_off,
-                                int64_t tok_base, int64_t n_prompts, const uint32_t* __restrict__ model, uint32_t model0,
+// Indexer.GetPodScores steps 2-4 (indexer.go:141-163): thread per prompt.  Src is the prompt's source of block keys:
+// uint32_t -- tokens, chained into keys as they are read (steps 2-4); uint64_t -- the request keys themselves (steps 3-4).
+// src_off / src_base: the CSR of that source.
+template <class Src>
+__global__ void score_kernel_v1(TableView t, const Src* __restrict__ src, const int64_t* __restrict__ src_off,
+                                int64_t src_base, int64_t n_prompts, const uint32_t* __restrict__ model, uint32_t model0,
                                 const uint64_t* __restrict__ filter, double* __restrict__ dense_out,
                                 uint16_t* __restrict__ sp_pods, double* __restrict__ sp_scores, uint8_t* __restrict__ sp_cnt,
                                 uint8_t* __restrict__ has_keys, unsigned long long stamp_base = 0, unsigned long long stamp_stride = 0) {
+    constexpr bool kKeys = sizeof(Src) == 8;
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n_prompts) return;
-    const int64_t b = tok_off[i] - tok_base, e = tok_off[i + 1] - tok_base;
-    const int64_t nblk = (e - b) / t.block_size;
+    const int64_t b = src_off[i] - src_base, e = src_off[i + 1] - src_base;
+    const int64_t nblk = kKeys ? e - b : (e - b) / t.block_size;
     const uint32_t mdl = model ? model[i] : model0;
     const uint64_t* frow = filter_row(filter, i, t.filter_words);
     ScoreState s; s.k = 0; s.alive = 0;
     uint64_t h = t.init_hash;
     bool walking = true;
     for (int64_t k = 0; k < nblk; ++k) {
-        h = hash_block_global(h, tok + b + k * t.block_size, t.block_size);
+        if constexpr (kKeys) h = src[b + k];
+        else h = hash_block_global(h, src + b + k * t.block_size, t.block_size);
         SlotWords w;
         uint64_t slot = 0;
         const bool hit = req_find(t, mdl, h, w, &slot);

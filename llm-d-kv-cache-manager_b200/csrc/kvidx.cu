@@ -26,6 +26,7 @@
 #include "kernels_rounds.cuh"
 #include "kernels_rounds_plain.cuh"
 #include "kernels_coop.cuh"
+#include "kernels_keys.cuh"
 #include "kernels_route.cuh"
 #include <cub/device/device_radix_sort.cuh>
 
@@ -666,10 +667,42 @@ int launch_score(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int64_t 
     return 0;
 }
 
-int check_csr(const int64_t* off, int64_t n) {
-    for (int64_t i = 0; i < n; ++i) if (off[i + 1] < off[i]) return fail(KVIDX_EINVAL, "tok_off not monotone at %lld", (long long)i);
+// Score() from request keys over device-resident inputs (GetPodScores steps 3-4): one warp per prompt at every batch
+// size (kernels_keys.cuh).  Ordered after the asynchronous write batches issued before.  Exact-LRU handles, and
+// KVIDX_SCORE_KERNEL=v1 as the cross-check, take the thread-per-prompt kernel, which stamps every present key.
+int launch_score_keys(kvidx* x, const uint64_t* d_keys, const int64_t* d_off, int64_t key_base, int64_t n,
+                      const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, const ScoreOut& o, cudaStream_t st) {
+    if (n <= 0) return 0;
+    if (int rc = check_shards(x)) return rc;
+    CK(cudaStreamWaitEvent(st, x->ev_write, 0));
+    if (x->score_kernel == 1 || x->tv.req_stamp) {
+        const int T = 128;
+        const unsigned long long stride = 1ull << 20;
+        const unsigned long long sb = x->tv.req_stamp ? reserve_stamps(x, (unsigned long long)n * stride) : 0;
+        score_kernel_v1<uint64_t><<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, d_keys, d_off, key_base, n, d_model, model0, d_filter,
+                                                                           o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, sb, stride);
+    } else {
+        ScoreArgs a{nullptr, d_off, key_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
+        const int64_t ctas = std::min<int64_t>((n + kKeysWarps - 1) / kKeysWarps, (int64_t)x->sm_count * kKeysCtasPerSm);
+        score_keys_kernel<<<(unsigned)ctas, kKeysThreads, 0, st>>>(x->tv, d_keys, a);
+    }
+    x->launches += 1;
+    CK(cudaGetLastError());
     return 0;
 }
+
+int check_csr(const int64_t* off, int64_t n, const char* what = "tok_off") {
+    for (int64_t i = 0; i < n; ++i) if (off[i + 1] < off[i]) return fail(KVIDX_EINVAL, "%s not monotone at %lld", what, (long long)i);
+    return 0;
+}
+
+// The prompts of a host-buffer Score() call: tokens (steps 2-4, `p` uint32) or request keys (steps 3-4, `p` uint64).
+// Prompt i owns elements off[i] .. off[i+1] of p.
+struct ScoreIn {
+    const void* p; const int64_t* off; bool keys;
+    size_t elem() const { return keys ? 8 : 4; }
+    const uint8_t* at(int64_t i) const { return static_cast<const uint8_t*>(p) + (size_t)i * elem(); }
+};
 
 // Host-buffer scoring.  Chunks of prompts flow through two slots and three streams so that the H2D copy
 // of chunk c+1, the kernel of chunk c and the D2H of chunk c-1 overlap (two DMA engines + SMs):
@@ -677,19 +710,19 @@ int check_csr(const int64_t* off, int64_t n) {
 //   x->stream   : score kernel                      (waits ev_h2d, records ev_k[slot])
 //   d2h_stream  : results -> pinned host            (waits ev_k, records ev_done[slot])
 // Caller buffers that are already pinned are used directly (no staging memcpy).
-int score_host_locked(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
+int score_host_locked(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, uint32_t model0,
                       const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys);
 
-int score_host(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
+int score_host(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, uint32_t model0,
                const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys) {
-    if (n < 0 || !tok_off) return fail(KVIDX_EINVAL, "bad arguments");
+    if (n < 0 || !in.off) return fail(KVIDX_EINVAL, "bad arguments");
     if (n == 0) return 0;
-    int rc = check_csr(tok_off, n);
+    int rc = check_csr(in.off, n, in.keys ? "key_off" : "tok_off");
     if (rc) return rc;
-    if (tok_off[n] > tok_off[0] && !tok) return fail(KVIDX_EINVAL, "NULL tokens");
+    if (in.off[n] > in.off[0] && !in.p) return fail(KVIDX_EINVAL, in.keys ? "NULL keys" : "NULL tokens");
     ReadGuard g(x);
     CK(cudaSetDevice(x->device));
-    rc = score_host_locked(x, tok, tok_off, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
+    rc = score_host_locked(x, in, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
     if (rc) {
         // an error in the middle of the pipeline: copies may still be reading the caller's buffers and this handle's staging
         // slots -- drain the three streams before the caller gets its buffers back (the error text is kept)
@@ -704,16 +737,19 @@ int score_host(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t n,
 // A handful of prompts (the size of one RPC, or of what the submission queue gathers at low load): no copy engine, no second
 // stream.  The cooperative kernel reads the tokens straight from PINNED HOST memory -- its TMA bulk copies fetch each 2 KB
 // chunk over PCIe one chunk ahead of the chain -- and writes the result rows straight back into pinned host memory; the call
-// is one launch and one stream synchronisation.  (cudaMallocHost memory is device-addressable under UVA.)
-int score_host_zerocopy(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
+// is one launch and one stream synchronisation.  (cudaMallocHost memory is device-addressable under UVA.)  Request keys
+// are read the same way by the key kernel, one coalesced 256-byte read per 32 keys.
+int score_host_zerocopy(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, uint32_t model0,
                         const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys) {
     const uint32_t P = x->tv.max_pods, FW = x->tv.filter_words;
     const bool sparse = sp_cnt != nullptr;
+    const int64_t* tok_off = in.off;
     const int64_t tb = tok_off[0], nt = tok_off[n] - tb;
-    const bool tok_pinned = nt == 0 || is_device_accessible_host(tok);
+    const size_t esz = in.elem();
+    const bool tok_pinned = nt == 0 || is_device_accessible_host(in.p);
     const size_t a8 = 63;
     const size_t in_bytes = (((size_t)(n + 1) * 8 + a8) & ~a8) + (model ? (((size_t)n * 4 + a8) & ~a8) : 0) + (filter ? (((size_t)n * FW * 8 + a8) & ~a8) : 0) +
-                            (tok_pinned ? 0 : (size_t)nt * 4 + 64);
+                            (tok_pinned ? 0 : (size_t)nt * esz + 64);
     CK(x->h_stage[0].need(in_bytes + 64));
     uint8_t* hs = x->h_stage[0].as<uint8_t>();
     size_t o = 0;
@@ -721,8 +757,9 @@ int score_host_zerocopy(kvidx* x, const uint32_t* tok, const int64_t* tok_off, i
     const uint32_t* h_model = nullptr; const uint64_t* h_filter = nullptr;
     if (model) { memcpy(hs + o, model, (size_t)n * 4); h_model = reinterpret_cast<const uint32_t*>(hs + o); o += ((size_t)n * 4 + a8) & ~a8; }
     if (filter) { memcpy(hs + o, filter, (size_t)n * FW * 8); h_filter = reinterpret_cast<const uint64_t*>(hs + o); o += ((size_t)n * FW * 8 + a8) & ~a8; }
-    const uint32_t* h_tok = tok ? tok + tb : nullptr;                     // token of absolute index tb
-    if (!tok_pinned) { memcpy(hs + o, tok + tb, (size_t)nt * 4); h_tok = reinterpret_cast<const uint32_t*>(hs + o); }
+    const uint8_t* h_src = in.p ? in.at(tb) : nullptr;                    // element of absolute index tb
+    if (!tok_pinned) { memcpy(hs + o, in.at(tb), (size_t)nt * esz); h_src = hs + o; }
+    const uint32_t* h_tok = in.keys ? nullptr : reinterpret_cast<const uint32_t*>(h_src);
     // results: straight into the caller's buffers when those are pinned, else through the pinned staging
     const bool out_direct = sparse ? (is_device_accessible_host(sp_pods) && is_device_accessible_host(sp_scores) && is_device_accessible_host(sp_cnt) &&
                                       (!has_keys || is_device_accessible_host(has_keys)))
@@ -737,12 +774,17 @@ int score_host_zerocopy(kvidx* x, const uint32_t* tok, const int64_t* tok_off, i
         if (!sparse) { a.dense = reinterpret_cast<double*>(ho); a.has_keys = ho + (size_t)n * P * 8; }
         else { a.sp_scores = reinterpret_cast<double*>(ho); a.sp_pods = reinterpret_cast<uint16_t*>(ho + (size_t)n * kMaxEnt * 8); a.sp_cnt = ho + (size_t)n * kMaxEnt * 10; a.has_keys = a.sp_cnt + n; }
     }
-    if (int rc = check_shards(x)) return rc;
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
-    const int64_t ctas = std::min<int64_t>((n + kCoopWarps - 1) / kCoopWarps, (int64_t)x->sm_count * 4);
-    coop_score_kernel<16><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem), x->stream>>>(x->tv, a);
-    x->launches += 1;
-    CK(cudaGetLastError());
+    if (in.keys) {
+        const ScoreOut so{a.dense, a.sp_pods, a.sp_scores, a.sp_cnt, a.has_keys};
+        if (int rc = launch_score_keys(x, reinterpret_cast<const uint64_t*>(h_src), h_off, tb, n, h_model, model0, h_filter, so, x->stream)) return rc;
+    } else {
+        if (int rc = check_shards(x)) return rc;
+        CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
+        const int64_t ctas = std::min<int64_t>((n + kCoopWarps - 1) / kCoopWarps, (int64_t)x->sm_count * 4);
+        coop_score_kernel<16><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem), x->stream>>>(x->tv, a);
+        x->launches += 1;
+        CK(cudaGetLastError());
+    }
     CK(cudaStreamSynchronize(x->stream));
     if (!out_direct) {
         if (!sparse) { memcpy(dense, ho, (size_t)n * P * 8); if (has_keys) memcpy(has_keys, ho + (size_t)n * P * 8, (size_t)n); }
@@ -755,20 +797,25 @@ int score_host_zerocopy(kvidx* x, const uint32_t* tok, const int64_t* tok_off, i
     return 0;
 }
 
-int score_host_locked(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
+int score_host_locked(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, uint32_t model0,
                       const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys) {
     int rc = 0;
-    if (n <= x->zerocopy_max && x->tv.block_size == 16 && !x->tv.req_stamp && x->score_kernel != 1 && (x->score_path == 0 || x->score_path == 4) &&
-        tok_off[n] - tok_off[0] <= (4ll << 20))
-        return score_host_zerocopy(x, tok, tok_off, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
+    const int64_t* tok_off = in.off;
+    const size_t esz = in.elem();
+    // the zero-copy and chunk budgets are bytes of input: 4 Mi tokens / 32 Mi tokens (KVIDX_HOST_CHUNK_TOKENS), or as
+    // many bytes of keys
+    const int64_t zc_max = (int64_t)((16ll << 20) / esz);
+    if (n <= x->zerocopy_max && !x->tv.req_stamp && x->score_kernel != 1 && tok_off[n] - tok_off[0] <= zc_max &&
+        (in.keys || (x->tv.block_size == 16 && (x->score_path == 0 || x->score_path == 4))))
+        return score_host_zerocopy(x, in, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
     const uint32_t P = x->tv.max_pods, FW = x->tv.filter_words;
     const bool sparse = sp_cnt != nullptr;
     const size_t out_row = sparse ? (size_t)kMaxEnt * (sizeof(double) + sizeof(uint16_t)) + 2 : (size_t)P * sizeof(double) + 1;
     // chunk = up to 32 Mi tokens (128 MiB): the H2D copy of a chunk must outlast its kernel for the
     // pipeline to be PCIe bound, and smaller chunks leave the fixed cost of a launch exposed.
-    const int64_t kMaxTokChunk = x->host_chunk_tokens;
+    const int64_t kMaxTokChunk = (int64_t)(x->host_chunk_tokens * 4 / (int64_t)esz);
     const int64_t kMaxRowsChunk = std::max<int64_t>(1, (128ll << 20) / (int64_t)out_row);
-    const bool tok_pinned = tok && is_device_accessible_host(tok);
+    const bool tok_pinned = in.p && is_device_accessible_host(in.p);
     const bool out_pinned = !sparse && dense && is_device_accessible_host(dense) && (!has_keys || is_device_accessible_host(has_keys));
     cudaStream_t s_k = x->stream, s_in = x->copy_stream, s_out = x->d2h_stream;
     struct Pending { bool live = false; int64_t i0 = 0, cnt = 0; } pend[2];
@@ -804,10 +851,10 @@ int score_host_locked(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int
         const int64_t c = i1 - i0, tb = tok_off[i0], nt = tok_off[i1] - tb;
         rc = drain(slot);                         // slot's previous results are home; its device buffers are free
         if (rc) return rc;
-        CK(x->d_tok[slot].need((size_t)std::max<int64_t>(nt, 1) * 4 + 64));
+        CK(x->d_tok[slot].need((size_t)std::max<int64_t>(nt, 1) * esz + 64));
         CK(x->d_off[slot].need((size_t)(c + 1) * 8));
         const size_t stage_bytes = (size_t)(c + 1) * 8 + (model ? (size_t)c * 4 : 0) + (filter ? (size_t)c * FW * 8 : 0) +
-                                   (tok_pinned ? 0 : (size_t)nt * 4);
+                                   (tok_pinned ? 0 : (size_t)nt * esz);
         CK(x->h_stage[slot].need(stage_bytes + 64));
         uint8_t* hs = x->h_stage[slot].as<uint8_t>();
         size_t o = 0;
@@ -827,9 +874,9 @@ int score_host_locked(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int
             df = x->d_filter[slot].as<uint64_t>();
         }
         if (nt > 0) {
-            const uint32_t* src = tok + tb;
-            if (!tok_pinned) { memcpy(hs + o, src, (size_t)nt * 4); src = reinterpret_cast<const uint32_t*>(hs + o); }
-            CK(cudaMemcpyAsync(x->d_tok[slot].p, src, (size_t)nt * 4, cudaMemcpyHostToDevice, s_in));
+            const uint8_t* src = in.at(tb);
+            if (!tok_pinned) { memcpy(hs + o, src, (size_t)nt * esz); src = hs + o; }
+            CK(cudaMemcpyAsync(x->d_tok[slot].p, src, (size_t)nt * esz, cudaMemcpyHostToDevice, s_in));
         }
         CK(cudaEventRecord(x->ev_h2d[slot], s_in));
         // kernel
@@ -848,9 +895,13 @@ int score_host_locked(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int
             so.has_keys = dout + q; q += (size_t)c;
         }
         CK(cudaStreamWaitEvent(s_k, x->ev_h2d[slot], 0));
-        int64_t maxb = 0;
-        for (int64_t q = i0; q < i1; ++q) maxb = std::max<int64_t>(maxb, (tok_off[q + 1] - tok_off[q]) / x->tv.block_size);
-        rc = launch_score(x, x->d_tok[slot].as<uint32_t>(), x->d_off[slot].as<int64_t>(), tb, c, dm, model0, df, so, s_k, maxb);
+        if (in.keys) {
+            rc = launch_score_keys(x, x->d_tok[slot].as<uint64_t>(), x->d_off[slot].as<int64_t>(), tb, c, dm, model0, df, so, s_k);
+        } else {
+            int64_t maxb = 0;
+            for (int64_t q = i0; q < i1; ++q) maxb = std::max<int64_t>(maxb, (tok_off[q + 1] - tok_off[q]) / x->tv.block_size);
+            rc = launch_score(x, x->d_tok[slot].as<uint32_t>(), x->d_off[slot].as<int64_t>(), tb, c, dm, model0, df, so, s_k, maxb);
+        }
         if (rc) return rc;
         CK(cudaEventRecord(x->ev_k[slot], s_k));
         // (slot reuse is safe without further stream waits: drain(slot) host-waits on ev_done[slot], which is
@@ -919,7 +970,7 @@ int run_combined(kvidx* x, SubmitQueue* q, const std::vector<SubmitReq*>& batch)
     uint8_t* ho = static_cast<uint8_t*>(q->h_out);
     if (!sparse) {
         double* dense = reinterpret_cast<double*>(ho); uint8_t* has = ho + (size_t)n * P * 8;
-        rc = score_host(x, tok, off, n, model, batch[0]->model0, filter, dense, nullptr, nullptr, nullptr, has);
+        rc = score_host(x, ScoreIn{tok, off, false}, n, model, batch[0]->model0, filter, dense, nullptr, nullptr, nullptr, has);
         if (rc) return rc;
         at = 0;
         for (SubmitReq* r : batch) {
@@ -930,7 +981,7 @@ int run_combined(kvidx* x, SubmitQueue* q, const std::vector<SubmitReq*>& batch)
     } else {
         double* sc = reinterpret_cast<double*>(ho); uint16_t* pods = reinterpret_cast<uint16_t*>(ho + (size_t)n * kMaxEnt * 8);
         uint8_t* cnt = ho + (size_t)n * kMaxEnt * 10; uint8_t* has = cnt + n;
-        rc = score_host(x, tok, off, n, model, batch[0]->model0, filter, nullptr, pods, sc, cnt, has);
+        rc = score_host(x, ScoreIn{tok, off, false}, n, model, batch[0]->model0, filter, nullptr, pods, sc, cnt, has);
         if (rc) return rc;
         at = 0;
         for (SubmitReq* r : batch) {
@@ -950,7 +1001,7 @@ int submit_score(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t 
     SubmitQueue* q = x->queue;
     // big batches and malformed calls go straight through (score_host validates); so does everything when the queue is off
     if (!q || !q->enabled || n <= 0 || !tok_off || n > q->max_prompts / 4)
-        return score_host(x, tok, tok_off, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
+        return score_host(x, ScoreIn{tok, tok_off, false}, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
     if (int rc = check_csr(tok_off, n)) return rc;
     if (tok_off[n] > tok_off[0] && !tok) return fail(KVIDX_EINVAL, "NULL tokens");
     SubmitReq me;
@@ -996,7 +1047,7 @@ int submit_score(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t 
         int rc;
         if (batch.size() == 1) {
             SubmitReq* r = batch[0];
-            rc = score_host(x, r->tok, r->tok_off, r->n, r->model, r->model0, r->filter, r->dense, r->sp_pods, r->sp_scores, r->sp_cnt, r->has_keys);
+            rc = score_host(x, ScoreIn{r->tok, r->tok_off, false}, r->n, r->model, r->model0, r->filter, r->dense, r->sp_pods, r->sp_scores, r->sp_cnt, r->has_keys);
         } else {
             rc = run_combined(x, q, batch);
             q->coalesced += batch.size();
@@ -1409,6 +1460,41 @@ int kvidx_score_batch_sparse_dev(kvidx_t* x, const uint32_t* d_tok, const int64_
     ScoreOut so{};
     so.sp_pods = d_pods_out; so.sp_scores = d_scores_out; so.sp_cnt = d_cnt_out; so.has_keys = d_has_keys_out;
     return launch_score(x, d_tok, d_tok_off, 0, n, d_model, model0, d_filter, so, x->stream);
+}
+
+// ---- Score() from request keys (GetPodScores steps 3-4): not coalesced, every call goes straight through ----
+
+int kvidx_score_keys(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, int64_t n, const uint32_t* model, uint32_t model0,
+                     const uint64_t* filter, double* scores_out, uint8_t* has_keys_out) {
+    if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_host(x, ScoreIn{keys, key_off, true}, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out);
+}
+
+int kvidx_score_keys_sparse(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, int64_t n, const uint32_t* model, uint32_t model0,
+                            const uint64_t* filter, uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out) {
+    if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_host(x, ScoreIn{keys, key_off, true}, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out);
+}
+
+int kvidx_score_keys_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n, const uint32_t* d_model,
+                         uint32_t model0, const uint64_t* d_filter, double* d_scores_out, uint8_t* d_has_keys_out) {
+    if (!x || n < 0 || !d_key_off || !d_scores_out) return fail(KVIDX_EINVAL, "bad arguments");
+    ReadGuard g(x);
+    CK(cudaSetDevice(x->device));
+    ScoreOut so{};
+    so.dense = d_scores_out; so.has_keys = d_has_keys_out;
+    return launch_score_keys(x, d_keys, d_key_off, 0, n, d_model, model0, d_filter, so, x->stream);
+}
+
+int kvidx_score_keys_sparse_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n, const uint32_t* d_model,
+                                uint32_t model0, const uint64_t* d_filter, uint16_t* d_pods_out, double* d_scores_out,
+                                uint8_t* d_cnt_out, uint8_t* d_has_keys_out) {
+    if (!x || n < 0 || !d_key_off || !d_pods_out || !d_scores_out || !d_cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
+    ReadGuard g(x);
+    CK(cudaSetDevice(x->device));
+    ScoreOut so{};
+    so.sp_pods = d_pods_out; so.sp_scores = d_scores_out; so.sp_cnt = d_cnt_out; so.has_keys = d_has_keys_out;
+    return launch_score_keys(x, d_keys, d_key_off, 0, n, d_model, model0, d_filter, so, x->stream);
 }
 
 // ---- routed (all-to-all) form of the sharded Score(): the device steps around the exchange (kernels_route.cuh) ----

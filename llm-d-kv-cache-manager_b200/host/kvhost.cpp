@@ -386,8 +386,10 @@ static bool build_filter(kvhost* h, const char* const* pods, size_t n_pods, std:
     return true;
 }
 
-int kvhost_get_pod_scores(kvhost_t* h, const uint32_t* tokens, size_t n_tokens, const char* model, const char* const* pods, size_t n_pods,
-                          const char** pod_out, double* score_out) {
+// GetPodScores from step 3 on for one prompt given as its tokens (keys == nullptr, n = token count) or as its request
+// keys (n = key count).
+static int pod_scores(kvhost* h, const uint32_t* tokens, const uint64_t* keys, size_t n, const char* model, const char* const* pods, size_t n_pods,
+                      const char** pod_out, double* score_out) {
     if (int rc = need_dev(h)) return rc;
     std::shared_lock<std::shared_mutex> rl(h->read_mu);
     std::vector<uint64_t> mask;
@@ -397,28 +399,43 @@ int kvhost_get_pod_scores(kvhost_t* h, const uint32_t* tokens, size_t n_tokens, 
     if (filtered) {                                 // a filter whose pods all lie outside the mask width selects nothing
         bool any = false; for (uint64_t w : mask) any |= w != 0;
         if (!any) {
-            const bool has_keys = n_tokens >= (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
+            const bool has_keys = keys ? n > 0 : n >= (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
             if (has_keys) observe_lookup(h, 0.0, true, nullptr, nullptr, 0);      // the Lookup still happens; it just finds no listed pod
             return has_keys ? 0 : -1000;
         }
     }
-    const int64_t off[2] = {0, (int64_t)n_tokens};
+    const int64_t off[2] = {0, (int64_t)n};
     uint16_t ids[KVIDX_MAX_PODS_PER_KEY]; double sc[KVIDX_MAX_PODS_PER_KEY]; uint8_t cnt = 0, has = 0;
-    const int rc = kvidx_score_batch_sparse(h->ix, tokens, off, 1, nullptr, (uint32_t)mid, filtered ? mask.data() : nullptr, ids, sc, &cnt, &has);
+    const uint64_t* fm = filtered ? mask.data() : nullptr;
+    const int rc = keys ? kvidx_score_keys_sparse(h->ix, keys, off, 1, nullptr, (uint32_t)mid, fm, ids, sc, &cnt, &has)
+                        : kvidx_score_batch_sparse(h->ix, tokens, off, 1, nullptr, (uint32_t)mid, fm, ids, sc, &cnt, &has);
     if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
     if (!has) return -1000;                         // (nil, nil): no full block (indexer.go:142-146)
     if (h->cfg.enable_metrics) {                    // the instrumented Lookup of indexer.go:150: every key of the prompt
-        const size_t nk = n_tokens / (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
-        std::vector<uint64_t> keys(nk); int64_t koff[2] = {0, 0};
+        const size_t nk = keys ? n : n / (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
+        std::vector<uint64_t> hashed; int64_t koff[2] = {0, 0};
         std::vector<kvidx_podtier_t> pt(nk * KVIDX_MAX_PODS_PER_KEY); std::vector<uint8_t> kc(nk);
-        int r2 = kvidx_hash_keys(h->ix, tokens, off, 1, nullptr, nullptr, keys.data(), koff);
+        int r2 = 0;
+        if (!keys) { hashed.resize(nk); r2 = kvidx_hash_keys(h->ix, tokens, off, 1, nullptr, nullptr, hashed.data(), koff); keys = hashed.data(); }
         const auto t0 = std::chrono::steady_clock::now();
-        if (!r2) r2 = kvidx_lookup(h->ix, (uint32_t)mid, keys.data(), (int64_t)nk, filtered ? mask.data() : nullptr, pt.data(), kc.data());
+        if (!r2) r2 = kvidx_lookup(h->ix, (uint32_t)mid, keys, (int64_t)nk, fm, pt.data(), kc.data());
         observe_lookup(h, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), r2 == 0, pt.data(), kc.data(), nk);
     }
     std::lock_guard<std::mutex> g(h->mu);
     for (int i = 0; i < cnt; ++i) { pod_out[i] = h->pods.name(ids[i]); score_out[i] = sc[i]; }
     return cnt;
+}
+
+int kvhost_get_pod_scores(kvhost_t* h, const uint32_t* tokens, size_t n_tokens, const char* model, const char* const* pods, size_t n_pods,
+                          const char** pod_out, double* score_out) {
+    return pod_scores(h, tokens, nullptr, n_tokens, model, pods, n_pods, pod_out, score_out);
+}
+
+int kvhost_get_pod_scores_keys(kvhost_t* h, const uint64_t* keys, size_t n_keys, const char* model, const char* const* pods, size_t n_pods,
+                               const char** pod_out, double* score_out) {
+    if (n_keys && !keys) return hfail(KVIDX_EINVAL, "NULL keys");
+    static const uint64_t none = 0;
+    return pod_scores(h, nullptr, keys ? keys : &none, n_keys, model, pods, n_pods, pod_out, score_out);
 }
 
 static int entries_of(kvhost* h, const char* const* pods, const char* const* tiers, size_t n, std::vector<kvidx_podtier_t>& out) {

@@ -64,6 +64,10 @@ SYMBOLS = {
     "kvidx_lookup": (C.c_int, [C.c_void_p, C.c_uint32, _u64p, C.c_int64, _u64p, _u16p, _u8p]),
     "kvidx_score_batch": (C.c_int, [C.c_void_p, _u32p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _f64p, _u8p]),
     "kvidx_score_batch_sparse": (C.c_int, [C.c_void_p, _u32p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _u16p, _f64p, _u8p, _u8p]),
+    "kvidx_score_keys": (C.c_int, [C.c_void_p, _u64p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _f64p, _u8p]),
+    "kvidx_score_keys_sparse": (C.c_int, [C.c_void_p, _u64p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _u16p, _f64p, _u8p, _u8p]),
+    "kvidx_score_keys_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kvidx_score_keys_sparse_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kvidx_add": (C.c_int, [C.c_void_p, C.c_uint32, _u64p, _u64p, C.c_int64, _u16p, C.c_int32]),
     "kvidx_evict": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, _u16p, C.c_int32]),
     "kvidx_get_request_key": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, _u64p]),
@@ -289,6 +293,49 @@ class Index:
         """Sparse result rows (<= 10 (pod, score) pairs per prompt) on the device; pointers are device addresses."""
         self._ck(self.L.kvidx_score_batch_sparse_dev(self.h, d_tok, d_tok_off, n, d_model or None, model0, d_filter or None,
                                                      d_pods, d_scores, d_cnt, d_has_keys or None))
+
+    # -- Score() from request keys (GetPodScores steps 3-4): prompt i owns keys[key_off[i] .. key_off[i+1]) --
+    def score_keys(self, keys, key_off, model=None, model0=0, filter_mask=None, out=None):
+        """Dense rows (n, max_pods) and has_keys, as score_batch; `keys` may be a numpy array or a _Raw pinned pointer."""
+        keys = np.ascontiguousarray(keys, np.uint64) if not isinstance(keys, _Raw) else keys
+        key_off = np.ascontiguousarray(key_off, np.int64)
+        n = len(key_off) - 1
+        scores = np.empty((n, self.max_pods), np.float64) if out is None else out
+        has = np.zeros(n, np.uint8)
+        model = None if model is None else np.ascontiguousarray(model, np.uint32)
+        filter_mask = None if filter_mask is None else np.ascontiguousarray(filter_mask, np.uint64)
+        kp = C.cast(keys.ptr, _u64p) if isinstance(keys, _Raw) else _p(keys, _u64p)
+        self._ck(self.L.kvidx_score_keys(self.h, kp, _p(key_off, _i64p), n, _p(model, _u32p), model0,
+                                         _p(filter_mask, _u64p), _p(scores, _f64p), _p(has, _u8p)))
+        return scores, has
+
+    def score_keys_sparse(self, keys, key_off, model=None, model0=0, filter_mask=None, out=None):
+        """Sparse rows as score_batch_sparse; out: optional preallocated (pods, scores, cnt, has)."""
+        keys = np.ascontiguousarray(keys, np.uint64)
+        key_off = np.ascontiguousarray(key_off, np.int64)
+        n = len(key_off) - 1
+        if out is None:
+            pods = np.zeros((n, E), np.uint16)
+            scores = np.zeros((n, E), np.float64)
+            cnt = np.zeros(n, np.uint8)
+            has = np.zeros(n, np.uint8)
+        else:
+            pods, scores, cnt, has = out
+        model = None if model is None else np.ascontiguousarray(model, np.uint32)
+        filter_mask = None if filter_mask is None else np.ascontiguousarray(filter_mask, np.uint64)
+        self._ck(self.L.kvidx_score_keys_sparse(self.h, _p(keys, _u64p), _p(key_off, _i64p), n, _p(model, _u32p), model0,
+                                                _p(filter_mask, _u64p), _p(pods, _u16p), _p(scores, _f64p), _p(cnt, _u8p),
+                                                _p(has, _u8p)))
+        return pods, scores, cnt, has
+
+    def score_keys_dev(self, d_keys, d_key_off, n, d_scores, d_model=0, model0=0, d_filter=0, d_has_keys=0):
+        """All pointers are device addresses (ints).  Asynchronous on the handle's stream."""
+        self._ck(self.L.kvidx_score_keys_dev(self.h, d_keys or None, d_key_off, n, d_model or None, model0, d_filter or None,
+                                             d_scores, d_has_keys or None))
+
+    def score_keys_sparse_dev(self, d_keys, d_key_off, n, d_pods, d_scores, d_cnt, d_model=0, model0=0, d_filter=0, d_has_keys=0):
+        self._ck(self.L.kvidx_score_keys_sparse_dev(self.h, d_keys or None, d_key_off, n, d_model or None, model0, d_filter or None,
+                                                    d_pods, d_scores, d_cnt, d_has_keys or None))
 
     def hash_keys_dev(self, d_tok, d_tok_off, n, d_key_off, d_keys, d_parent=0, d_parent_valid=0):
         self._ck(self.L.kvidx_hash_keys_dev(self.h, d_tok, d_tok_off, n, d_parent or None, d_parent_valid or None, d_key_off, d_keys))

@@ -45,7 +45,8 @@ SYMBOLS = {
     "kvhost_last_error": (C.c_char_p, []),
     "kvhost_index": (C.c_void_p, [C.c_void_p]),
     "kvhost_get_pod_scores": (C.c_int, [C.c_void_p, _u32p, C.c_size_t, C.c_char_p, _cpp, C.c_size_t, _cpp, _f64p]),
-    "kvhost_index_add": (C.c_int, [C.c_void_p, C.c_char_p, _u64p, C.c_size_t, _u64p, C.c_size_t, _cpp, _cpp, C.c_size_t]),
+    "kvhost_get_pod_scores_keys": (C.c_int, [C.c_void_p, _u64p, C.c_size_t, C.c_char_p, _cpp, C.c_size_t, _cpp, _f64p]),
+    "kvhost_index_add":(C.c_int, [C.c_void_p, C.c_char_p, _u64p, C.c_size_t, _u64p, C.c_size_t, _cpp, _cpp, C.c_size_t]),
     "kvhost_index_evict": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, _cpp, _cpp, C.c_size_t]),
     "kvhost_index_get_request_key": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, _u64p]),
     "kvhost_index_lookup": (C.c_int, [C.c_void_p, C.c_char_p, _u64p, C.c_size_t, _cpp, C.c_size_t, _cpp, _cpp, _u8p]),
@@ -126,6 +127,17 @@ class HostIndexer:
         tok = np.ascontiguousarray(tokens, np.uint32)
         po = (C.c_char_p * 10)(); so = (C.c_double * 10)()
         n = self.L.kvhost_get_pod_scores(self.h, tok.ctypes.data_as(_u32p), len(tok), model.encode(), _strs(list(pods)), len(pods), po, so)
+        if n == NO_KEYS:
+            return None
+        if n < 0:
+            raise _native.KvidxError(n, self.err())
+        return {po[i].decode(): so[i] for i in range(n)}
+
+    def get_pod_scores_keys(self, keys, model, pods=()):
+        """GetPodScores from the prompt's request keys (block order) -> dict pod -> score, or None when there are no keys."""
+        k = np.ascontiguousarray(keys, np.uint64)
+        po = (C.c_char_p * 10)(); so = (C.c_double * 10)()
+        n = self.L.kvhost_get_pod_scores_keys(self.h, k.ctypes.data_as(_u64p), len(k), model.encode(), _strs(list(pods)), len(pods), po, so)
         if n == NO_KEYS:
             return None
         if n < 0:

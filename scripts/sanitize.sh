@@ -11,3 +11,5 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_parity.py -x -q -m gpu -k "prefix_tree and rounds2 and not lane"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_snapshot.py -x -q -m gpu -k "golden or error_paths or equal_contents or exact_lru"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_shard_ops.py -x -q -m gpu -k "same-gpu-2 or guards or all_or_nothing or unsharded_handle or (round_trips and coop and same)"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_score_keys.py -x -q -m gpu -k "same_bits or arbitrary or host_buffers or errors"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_score_keys.py -x -q -m gpu -k "arbitrary and 257"
