@@ -225,14 +225,13 @@ inline int score_tuned_init() {
     return 0;
 }
 
-inline int launch_score_tuned(const TableView& t, int sm_count, const uint32_t* d_tok, const int64_t* d_off, int64_t tok_base, int64_t n,
-                              const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, double* dense, uint16_t* sp_pods,
-                              double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys, unsigned long long* d_next, cudaStream_t st,
+// a.next is set to d_next, the work counter this launch zeroes
+inline int launch_score_tuned(const TableView& t, int sm_count, ScoreArgs a, unsigned long long* d_next, cudaStream_t st,
                               uint64_t* launches) {
     if (cudaMemsetAsync(d_next, 0, sizeof(unsigned long long), st) != cudaSuccess) return -1;
-    ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, dense, sp_pods, sp_scores, sp_cnt, has_keys, d_next};
+    a.next = d_next;
     const int64_t lanes_per_cta = kScoreThreads;
-    int64_t ctas = (n + lanes_per_cta - 1) / lanes_per_cta;
+    int64_t ctas = (a.n_prompts + lanes_per_cta - 1) / lanes_per_cta;
     const int64_t max_ctas = (int64_t)sm_count * kScoreCtasPerSm;
     if (ctas > max_ctas) ctas = max_ctas;
     score_kernel_tuned<16><<<(unsigned)ctas, kScoreThreads, sizeof(ScoreSmem<16>), st>>>(t, a);

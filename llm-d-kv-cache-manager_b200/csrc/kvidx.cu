@@ -96,8 +96,7 @@ bool is_device_accessible_host(const void* p) {
 // pipeline and wakes the owners.  No dedicated thread, no artificial delay: a lone caller goes straight through with its
 // own buffers; under load the batch size grows by itself to what arrived during the previous launch.
 struct SubmitReq {
-    const uint32_t* tok; const int64_t* tok_off; int64_t n; const uint32_t* model; uint32_t model0; const uint64_t* filter;
-    double* dense; uint16_t* sp_pods; double* sp_scores; uint8_t* sp_cnt; uint8_t* has_keys;
+    const uint32_t* tok; ScoreArgs a;              // the call in host memory (a.tok unused)
     int rc = 0; bool done = false, promote = false; std::string err;
     std::mutex m; std::condition_variable cv;      // each waiter sleeps on its OWN condition variable: finishing a batch wakes
                                                    // exactly its owners (and the next leader), not every queued thread
@@ -382,11 +381,7 @@ int cap_keys(kvidx* x) {
     return rc ? rc : refresh_counters(x);
 }
 
-struct ScoreOut { double* dense; uint16_t* sp_pods; double* sp_scores; uint8_t* sp_cnt; uint8_t* has_keys; };
-
-int launch_score_rounds_plain(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int64_t tok_base, int64_t n,
-                              const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, const ScoreOut& o, cudaStream_t st,
-                              int64_t max_blocks);
+int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks);
 
 // Batch setup of both round pipelines: clear the counters in r_cnt (part q's list lengths at word 8 * q, the batch's largest
 // block count and the distinct-prefix count as two 64-bit words at word 8 * kMaxParts, part q's four trace counters of the
@@ -420,9 +415,8 @@ int rounds_setup(kvidx* x, const ScoreArgs& a, const PartSizes& ps, cudaStream_t
 // device.  The sorted batch is split into parts that run their rounds on separate streams, so that one part's
 // latency-bound kernels (the serial FNV chain of few representatives, the dependent probes) share the SMs with
 // another part's bandwidth-bound ones.
-int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int64_t tok_base, int64_t n,
-                        const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, const ScoreOut& o, cudaStream_t st,
-                        int64_t max_blocks) {
+int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks) {
+    const int64_t n = a.n_prompts;
     CK(x->r_act0.need((size_t)n * 4)); CK(x->r_act1.need((size_t)n * 4)); CK(x->r_cnt.need(1024));
     CK(x->r_hstate.need((size_t)n * 8)); CK(x->r_keys.need((size_t)n * kRoundBlocks * 8)); CK(x->r_pst.need((size_t)n * sizeof(PromptState) * 2));
     CK(x->r_nbr.need((size_t)n * 4 * 2)); CK(x->r_role.need((size_t)n * 4)); CK(x->r_hl.need((size_t)n * 4 * 2)); CK(x->r_src.need((size_t)n * 4));
@@ -473,7 +467,6 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
         rb[q].grp = rb[q].map + map_slots;
         rb[q].scan = x->r_scan.as<unsigned long long>() + (size_t)q * ctiles;
     }
-    ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
     PartSizes ps{};
     for (int q = 0; q < kMaxParts; ++q) ps.n[q] = (unsigned int)psz[q];
     const uint64_t* fp_sorted = nullptr;
@@ -494,7 +487,7 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
         if (max_blocks < 0) max_blocks = (int64_t)mb[0];
         if (adaptive && (double)mb[1] > (1.0 - x->classes_min_sharing) * (double)n) {
             if (x->rounds_trace) fprintf(stderr, "[kvidx rounds] %llu distinct first blocks among %lld prompts: per-prompt rounds instead\n", mb[1], (long long)n);
-            return launch_score_rounds_plain(x, d_tok, d_off, tok_base, n, d_model, model0, d_filter, o, st, max_blocks);
+            return launch_score_rounds_plain(x, a, st, max_blocks);
         }
     }
     int64_t rounds = (max_blocks + kRoundBlocks - 1) / kRoundBlocks;
@@ -568,9 +561,8 @@ int launch_score_rounds(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, i
 }
 
 // Medium batches: hash / walk rounds, every prompt on its own (kernels_rounds_plain.cuh); two halves on two streams.
-int launch_score_rounds_plain(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int64_t tok_base, int64_t n,
-                        const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, const ScoreOut& o, cudaStream_t st,
-                        int64_t max_blocks) {
+int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks) {
+    const int64_t n = a.n_prompts;
     const bool warp_walk = x->rounds_warp && n <= x->rounds_warp_max;      // kernel P: warp per prompt (batch too small to fill the machine lane per prompt)
     CK(x->r_act0.need((size_t)n * 4)); CK(x->r_act1.need((size_t)n * 4)); CK(x->r_cnt.need(1024));
     CK(x->r_hstate.need((size_t)n * 8)); CK(x->r_keys.need((size_t)n * kRoundBlocks * 8)); CK(x->r_pst.need((size_t)n * sizeof(PromptState)));
@@ -586,7 +578,6 @@ int launch_score_rounds_plain(kvidx* x, const uint32_t* d_tok, const int64_t* d_
         rb[hlf].hstate = x->r_hstate.as<uint64_t>(); rb[hlf].pst = x->r_pst.as<PromptState>();
         rb[hlf].keys = x->r_keys.as<uint64_t>() + (warp_walk ? off * kRoundBlocks : off); rb[hlf].nbr = x->r_nbr.as<uint32_t>() + off;      // prompt-major keys: a half's rows are contiguous
     }
-    ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
     if (int rc = rounds_setup(x, a, PartSizes{{(unsigned int)nA, (unsigned int)nB}}, st, nullptr)) return rc;
     if (max_blocks < 0) {
         unsigned long long mb = 0;
@@ -630,36 +621,65 @@ int launch_score_rounds_plain(kvidx* x, const uint32_t* d_tok, const int64_t* d_
     return 0;
 }
 
-// Launch the score kernel(s) over device-resident inputs.
-int launch_score(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int64_t tok_base, int64_t n,
-                 const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, const ScoreOut& o, cudaStream_t st,
-                 int64_t max_blocks = -1) {
+// The prompts of a Score() call: tokens (steps 2-4, `p` uint32) or request keys (steps 3-4, `p` uint64).  Prompt i owns
+// elements tok_off[i] .. tok_off[i+1] of p, with the offsets and everything else about the call in a ScoreArgs.
+struct ScoreIn {
+    const void* p; bool keys;
+    size_t elem() const { return keys ? 8 : 4; }
+    const uint8_t* at(int64_t i) const { return static_cast<const uint8_t*>(p) + (size_t)i * elem(); }
+};
+
+// Exact-LRU handles take the thread-per-prompt kernel: Lookup must touch every present key of a prompt (no early exit).
+// So do token prompts of every block size but 16, which the other token kernels' staging is written for, and
+// KVIDX_SCORE_KERNEL=v1 as the cross-check.
+bool score_takes_v1(const kvidx* x, bool keys) {
+    return x->score_kernel == 1 || x->tv.req_stamp || (!keys && x->tv.block_size != 16);
+}
+
+// Does a batch of n prompts take a warp-per-prompt kernel: score_keys_kernel (keys, every size) or coop_score_kernel (small
+// token batches)?  Both read their inputs in place, so from pinned host memory as well (score_host_zerocopy).
+bool score_warp_per_prompt(const kvidx* x, bool keys, int64_t n) {
+    return !score_takes_v1(x, keys) && (keys || x->score_path == 4 || (x->score_path == 0 && n <= x->coop_max));
+}
+
+template <class E>
+void launch_score_v1(kvidx* x, const ScoreArgs& a, const E* src, cudaStream_t st) {
+    const int T = 128;
+    const unsigned long long stride = 1ull << 20;
+    const unsigned long long sb = x->tv.req_stamp ? reserve_stamps(x, (unsigned long long)a.n_prompts * stride) : 0;
+    score_kernel_v1<<<(unsigned)((a.n_prompts + T - 1) / T), T, 0, st>>>(x->tv, src, a.tok_off, a.tok_base, a.n_prompts, a.model, a.model0, a.filter,
+                                                                        a.dense, a.sp_pods, a.sp_scores, a.sp_cnt, a.has_keys, sb, stride);
+    x->launches += 1;
+}
+
+// Launch Score() over device-addressable inputs: the prompts' elements at in.p (a.tok is set here), the rest of the call in
+// `a`.  max_blocks: the token batch's largest block count, for the round pipelines; < 0 computes it on the device.  The
+// callers order the launch after the asynchronous write batches issued before (ev_write), once per call.
+int launch_score(kvidx* x, const ScoreIn& in, ScoreArgs a, cudaStream_t st, int64_t max_blocks = -1) {
+    const int64_t n = a.n_prompts;
     if (n <= 0) return 0;
     if (int rc = check_shards(x)) return rc;
-    if (x->score_kernel == 1 || x->tv.req_stamp || x->tv.block_size != 16) {
-        // exact-LRU mode always takes this kernel: Lookup must touch every present key of a prompt (no early exit); so does
-        // every block size but 16, which the other kernels' token staging is written for
-        const int T = 128;
-        const unsigned long long stride = 1ull << 20;
-        const unsigned long long sb = x->tv.req_stamp ? reserve_stamps(x, (unsigned long long)n * stride) : 0;
-        score_kernel_v1<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, d_tok, d_off, tok_base, n, d_model, model0, d_filter,
-                                                                  o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, sb, stride);
+    a.tok = in.keys ? nullptr : static_cast<const uint32_t*>(in.p);
+    if (score_takes_v1(x, in.keys)) {
+        if (in.keys) launch_score_v1(x, a, static_cast<const uint64_t*>(in.p), st);
+        else launch_score_v1(x, a, a.tok, st);
+    } else if (in.keys) {
+        // request keys: one warp per prompt at every batch size (kernels_keys.cuh)
+        const int64_t ctas = std::min<int64_t>((n + kKeysWarps - 1) / kKeysWarps, (int64_t)x->sm_count * kKeysCtasPerSm);
+        score_keys_kernel<<<(unsigned)ctas, kKeysThreads, 0, st>>>(x->tv, static_cast<const uint64_t*>(in.p), a);
         x->launches += 1;
-    } else if (x->score_path == 4 || (x->score_path == 0 && n <= x->coop_max)) {
+    } else if (score_warp_per_prompt(x, false, n)) {
         // small batches: a warp per prompt, warp-cooperative hashing, TMA-staged tokens (kernels_coop.cuh)
-        ScoreArgs a{d_tok, d_off, tok_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
         const int64_t ctas = std::min<int64_t>((n + kCoopWarps - 1) / kCoopWarps, (int64_t)x->sm_count * 4);
         coop_score_kernel<16><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem), st>>>(x->tv, a);
         x->launches += 1;
     } else if (n < (1ll << 31) && ((x->score_path >= 2 && x->score_path <= 3) || (x->score_path == 0 && n >= x->rounds_min))) {
         // path 2: plain rounds, 3: prefix classes; automatic: by batch size (the class pipeline has a fixed cost per round)
         const bool classes = x->score_path == 3 || (x->score_path == 0 && n >= x->classes_min);
-        return classes ? launch_score_rounds(x, d_tok, d_off, tok_base, n, d_model, model0, d_filter, o, st, max_blocks)
-                       : launch_score_rounds_plain(x, d_tok, d_off, tok_base, n, d_model, model0, d_filter, o, st, max_blocks);
+        return classes ? launch_score_rounds(x, a, st, max_blocks) : launch_score_rounds_plain(x, a, st, max_blocks);
     } else {
         uint64_t nl = 0;
-        int rc = launch_score_tuned(x->tv, x->sm_count, d_tok, d_off, tok_base, n, d_model, model0, d_filter,
-                                    o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, &x->d_cnt->pad, st, &nl);
+        int rc = launch_score_tuned(x->tv, x->sm_count, a, &x->d_cnt->pad, st, &nl);
         x->launches += nl;
         if (rc) return fail(KVIDX_ECUDA, "score launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     }
@@ -667,28 +687,12 @@ int launch_score(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int64_t 
     return 0;
 }
 
-// Score() from request keys over device-resident inputs (GetPodScores steps 3-4): one warp per prompt at every batch
-// size (kernels_keys.cuh).  Ordered after the asynchronous write batches issued before.  Exact-LRU handles, and
-// KVIDX_SCORE_KERNEL=v1 as the cross-check, take the thread-per-prompt kernel, which stamps every present key.
-int launch_score_keys(kvidx* x, const uint64_t* d_keys, const int64_t* d_off, int64_t key_base, int64_t n,
-                      const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, const ScoreOut& o, cudaStream_t st) {
-    if (n <= 0) return 0;
-    if (int rc = check_shards(x)) return rc;
-    CK(cudaStreamWaitEvent(st, x->ev_write, 0));
-    if (x->score_kernel == 1 || x->tv.req_stamp) {
-        const int T = 128;
-        const unsigned long long stride = 1ull << 20;
-        const unsigned long long sb = x->tv.req_stamp ? reserve_stamps(x, (unsigned long long)n * stride) : 0;
-        score_kernel_v1<uint64_t><<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, d_keys, d_off, key_base, n, d_model, model0, d_filter,
-                                                                           o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, sb, stride);
-    } else {
-        ScoreArgs a{nullptr, d_off, key_base, n, d_model, model0, d_filter, o.dense, o.sp_pods, o.sp_scores, o.sp_cnt, o.has_keys, nullptr};
-        const int64_t ctas = std::min<int64_t>((n + kKeysWarps - 1) / kKeysWarps, (int64_t)x->sm_count * kKeysCtasPerSm);
-        score_keys_kernel<<<(unsigned)ctas, kKeysThreads, 0, st>>>(x->tv, d_keys, a);
-    }
-    x->launches += 1;
-    CK(cudaGetLastError());
-    return 0;
+// The device-resident entry points: Score() on the handle's stream, after the asynchronous write batches issued before.
+int score_dev(kvidx* x, const ScoreIn& in, const ScoreArgs& a) {
+    ReadGuard g(x);
+    CK(cudaSetDevice(x->device));
+    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
+    return launch_score(x, in, a, x->stream);
 }
 
 int check_csr(const int64_t* off, int64_t n, const char* what = "tok_off") {
@@ -696,33 +700,95 @@ int check_csr(const int64_t* off, int64_t n, const char* what = "tok_off") {
     return 0;
 }
 
-// The prompts of a host-buffer Score() call: tokens (steps 2-4, `p` uint32) or request keys (steps 3-4, `p` uint64).
-// Prompt i owns elements off[i] .. off[i+1] of p.
-struct ScoreIn {
-    const void* p; const int64_t* off; bool keys;
-    size_t elem() const { return keys ? 8 : 4; }
-    const uint8_t* at(int64_t i) const { return static_cast<const uint8_t*>(p) + (size_t)i * elem(); }
+// The result rows of a Score() call with P pods.  A buffer of n rows holds, dense: n x P f64 scores, then n has_keys bytes;
+// sparse: n x kMaxEnt f64 scores, n x kMaxEnt u16 pods, n entry counts, then n has_keys bytes.
+struct RowLayout {
+    uint32_t P; bool sparse;
+    size_t row() const { return sparse ? (size_t)kMaxEnt * (sizeof(double) + sizeof(uint16_t)) + 2 : (size_t)P * sizeof(double) + 1; }
+    // point the outputs of `a` into a buffer of n rows
+    void carve(void* buf, int64_t n, ScoreArgs& a) const {
+        uint8_t* b = static_cast<uint8_t*>(buf);
+        if (!sparse) { a.dense = reinterpret_cast<double*>(b); a.has_keys = b + (size_t)n * P * sizeof(double); return; }
+        a.sp_scores = reinterpret_cast<double*>(b);
+        a.sp_pods = reinterpret_cast<uint16_t*>(b + (size_t)n * kMaxEnt * sizeof(double));
+        a.sp_cnt = reinterpret_cast<uint8_t*>(a.sp_pods + (size_t)n * kMaxEnt);
+        a.has_keys = a.sp_cnt + n;
+    }
+    // the outputs of `a` from row i on
+    ScoreArgs at(ScoreArgs a, int64_t i) const {
+        if (sparse) { a.sp_scores += i * kMaxEnt; a.sp_pods += i * kMaxEnt; a.sp_cnt += i; }
+        else a.dense += i * (int64_t)P;
+        if (a.has_keys) a.has_keys += i;
+        return a;
+    }
+    // copy c rows from the outputs of src to those of dst: memcpy, or with st device to host on *st.  has_keys only when
+    // dst has it.
+    int copy(const ScoreArgs& dst, const ScoreArgs& src, int64_t c, const cudaStream_t* st = nullptr) const {
+        auto cp = [st](void* d, const void* s, size_t bytes) {
+            if (st) return cudaMemcpyAsync(d, s, bytes, cudaMemcpyDeviceToHost, *st);
+            memcpy(d, s, bytes);
+            return cudaSuccess;
+        };
+        if (sparse) {
+            CK(cp(dst.sp_scores, src.sp_scores, (size_t)c * kMaxEnt * sizeof(double)));
+            CK(cp(dst.sp_pods, src.sp_pods, (size_t)c * kMaxEnt * sizeof(uint16_t)));
+            CK(cp(dst.sp_cnt, src.sp_cnt, (size_t)c));
+        } else {
+            CK(cp(dst.dense, src.dense, (size_t)c * P * sizeof(double)));
+        }
+        if (dst.has_keys) CK(cp(dst.has_keys, src.has_keys, (size_t)c));
+        return 0;
+    }
+    // are all of the outputs of `a` pinned host memory?
+    bool pinned(const ScoreArgs& a) const {
+        if (a.has_keys && !is_device_accessible_host(a.has_keys)) return false;
+        return sparse ? is_device_accessible_host(a.sp_pods) && is_device_accessible_host(a.sp_scores) && is_device_accessible_host(a.sp_cnt)
+                      : is_device_accessible_host(a.dense);
+    }
 };
 
-// Host-buffer scoring.  Chunks of prompts flow through two slots and three streams so that the H2D copy
-// of chunk c+1, the kernel of chunk c and the D2H of chunk c-1 overlap (two DMA engines + SMs):
+// The input sections of a host-buffer call over c prompts in one pinned buffer, each 64-byte aligned: the offsets (c + 1),
+// the model ids and the filter rows (when the call has them), then the elements (when they are staged).
+struct StageLayout {
+    size_t model, filter, elem, bytes;            // section starts (the offsets start the buffer) and the total
+    StageLayout(int64_t c, bool has_model, bool has_filter, uint32_t fw, size_t elem_bytes) {
+        auto al = [](size_t b) { return (b + 63) & ~(size_t)63; };
+        model = al((size_t)(c + 1) * 8);
+        filter = model + (has_model ? al((size_t)c * 4) : 0);
+        elem = filter + (has_filter ? al((size_t)c * fw * 8) : 0);
+        bytes = elem + elem_bytes;
+    }
+    // copy the offsets, model ids and filter rows of prompts i0 .. i0+c of the host call `h` into buf: the packed call, with
+    // the outputs of h
+    ScoreArgs pack(uint8_t* buf, const ScoreArgs& h, int64_t i0, int64_t c, uint32_t fw) const {
+        ScoreArgs a = h;
+        a.tok = nullptr; a.tok_off = reinterpret_cast<int64_t*>(buf); a.tok_base = h.tok_off[i0]; a.n_prompts = c;
+        memcpy(buf, h.tok_off + i0, (size_t)(c + 1) * 8);
+        if (h.model) { memcpy(buf + model, h.model + i0, (size_t)c * 4); a.model = reinterpret_cast<const uint32_t*>(buf + model); }
+        if (h.filter) { memcpy(buf + filter, h.filter + i0 * fw, (size_t)c * fw * 8); a.filter = reinterpret_cast<const uint64_t*>(buf + filter); }
+        return a;
+    }
+};
+
+// Host-buffer scoring of the call `h` (host pointers; h.tok unused, the elements are at in.p).  Chunks of prompts flow
+// through two slots and three streams so that the H2D copy of chunk c+1, the kernel of chunk c and the D2H of chunk c-1
+// overlap (two DMA engines + SMs):
 //   copy_stream : staging -> d_tok/d_off/...      (records ev_h2d[slot])
 //   x->stream   : score kernel                      (waits ev_h2d, records ev_k[slot])
 //   d2h_stream  : results -> pinned host            (waits ev_k, records ev_done[slot])
 // Caller buffers that are already pinned are used directly (no staging memcpy).
-int score_host_locked(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, uint32_t model0,
-                      const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys);
+int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h);
 
-int score_host(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, uint32_t model0,
-               const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys) {
-    if (n < 0 || !in.off) return fail(KVIDX_EINVAL, "bad arguments");
+int score_host(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
+    const int64_t n = h.n_prompts;
+    if (n < 0 || !h.tok_off) return fail(KVIDX_EINVAL, "bad arguments");
     if (n == 0) return 0;
-    int rc = check_csr(in.off, n, in.keys ? "key_off" : "tok_off");
+    int rc = check_csr(h.tok_off, n, in.keys ? "key_off" : "tok_off");
     if (rc) return rc;
-    if (in.off[n] > in.off[0] && !in.p) return fail(KVIDX_EINVAL, in.keys ? "NULL keys" : "NULL tokens");
+    if (h.tok_off[n] > h.tok_off[0] && !in.p) return fail(KVIDX_EINVAL, in.keys ? "NULL keys" : "NULL tokens");
     ReadGuard g(x);
     CK(cudaSetDevice(x->device));
-    rc = score_host_locked(x, in, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
+    rc = score_host_locked(x, in, h);
     if (rc) {
         // an error in the middle of the pipeline: copies may still be reading the caller's buffers and this handle's staging
         // slots -- drain the three streams before the caller gets its buffers back (the error text is kept)
@@ -734,89 +800,52 @@ int score_host(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, ui
     return rc;
 }
 
-// A handful of prompts (the size of one RPC, or of what the submission queue gathers at low load): no copy engine, no second
-// stream.  The cooperative kernel reads the tokens straight from PINNED HOST memory -- its TMA bulk copies fetch each 2 KB
-// chunk over PCIe one chunk ahead of the chain -- and writes the result rows straight back into pinned host memory; the call
-// is one launch and one stream synchronisation.  (cudaMallocHost memory is device-addressable under UVA.)  Request keys
-// are read the same way by the key kernel, one coalesced 256-byte read per 32 keys.
-int score_host_zerocopy(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, uint32_t model0,
-                        const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys) {
-    const uint32_t P = x->tv.max_pods, FW = x->tv.filter_words;
-    const bool sparse = sp_cnt != nullptr;
-    const int64_t* tok_off = in.off;
-    const int64_t tb = tok_off[0], nt = tok_off[n] - tb;
-    const size_t esz = in.elem();
-    const bool tok_pinned = nt == 0 || is_device_accessible_host(in.p);
-    const size_t a8 = 63;
-    const size_t in_bytes = (((size_t)(n + 1) * 8 + a8) & ~a8) + (model ? (((size_t)n * 4 + a8) & ~a8) : 0) + (filter ? (((size_t)n * FW * 8 + a8) & ~a8) : 0) +
-                            (tok_pinned ? 0 : (size_t)nt * esz + 64);
-    CK(x->h_stage[0].need(in_bytes + 64));
+// A handful of prompts (the size of one RPC, or of what the submission queue gathers at low load) that take a warp-per-prompt
+// kernel: no copy engine, no second stream.  The cooperative kernel reads the tokens straight from PINNED HOST memory -- its
+// TMA bulk copies fetch each 2 KB chunk over PCIe one chunk ahead of the chain -- and writes the result rows straight back
+// into pinned host memory; the call is one launch and one stream synchronisation.  (cudaMallocHost memory is
+// device-addressable under UVA.)  Request keys are read the same way by the key kernel, one coalesced 256-byte read per 32
+// keys.
+int score_host_zerocopy(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
+    const int64_t n = h.n_prompts, tb = h.tok_off[0], nt = h.tok_off[n] - tb;
+    const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
+    const bool in_pinned = nt == 0 || is_device_accessible_host(in.p);
+    const StageLayout sl(n, h.model != nullptr, h.filter != nullptr, x->tv.filter_words, in_pinned ? 0 : (size_t)nt * in.elem());
+    CK(x->h_stage[0].need(sl.bytes + 64));
     uint8_t* hs = x->h_stage[0].as<uint8_t>();
-    size_t o = 0;
-    int64_t* h_off = reinterpret_cast<int64_t*>(hs); memcpy(h_off, tok_off, (size_t)(n + 1) * 8); o += ((size_t)(n + 1) * 8 + a8) & ~a8;
-    const uint32_t* h_model = nullptr; const uint64_t* h_filter = nullptr;
-    if (model) { memcpy(hs + o, model, (size_t)n * 4); h_model = reinterpret_cast<const uint32_t*>(hs + o); o += ((size_t)n * 4 + a8) & ~a8; }
-    if (filter) { memcpy(hs + o, filter, (size_t)n * FW * 8); h_filter = reinterpret_cast<const uint64_t*>(hs + o); o += ((size_t)n * FW * 8 + a8) & ~a8; }
-    const uint8_t* h_src = in.p ? in.at(tb) : nullptr;                    // element of absolute index tb
-    if (!tok_pinned) { memcpy(hs + o, in.at(tb), (size_t)nt * esz); h_src = hs + o; }
-    const uint32_t* h_tok = in.keys ? nullptr : reinterpret_cast<const uint32_t*>(h_src);
+    ScoreArgs a = sl.pack(hs, h, 0, n, x->tv.filter_words);
+    const uint8_t* src = in.p ? in.at(tb) : nullptr;                    // element of absolute index tb
+    if (!in_pinned) { memcpy(hs + sl.elem, src, (size_t)nt * in.elem()); src = hs + sl.elem; }
     // results: straight into the caller's buffers when those are pinned, else through the pinned staging
-    const bool out_direct = sparse ? (is_device_accessible_host(sp_pods) && is_device_accessible_host(sp_scores) && is_device_accessible_host(sp_cnt) &&
-                                      (!has_keys || is_device_accessible_host(has_keys)))
-                                   : (is_device_accessible_host(dense) && (!has_keys || is_device_accessible_host(has_keys)));
-    ScoreArgs a{h_tok, h_off, tb, n, h_model, model0, h_filter, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    uint8_t* ho = nullptr;
-    if (out_direct) { a.dense = dense; a.sp_pods = sp_pods; a.sp_scores = sp_scores; a.sp_cnt = sp_cnt; a.has_keys = has_keys; }
-    else {
-        const size_t out_bytes = sparse ? (size_t)n * (kMaxEnt * 10 + 2) : (size_t)n * (P * 8 + 1);
-        CK(x->h_out[0].need(out_bytes + 64));
-        ho = x->h_out[0].as<uint8_t>();
-        if (!sparse) { a.dense = reinterpret_cast<double*>(ho); a.has_keys = ho + (size_t)n * P * 8; }
-        else { a.sp_scores = reinterpret_cast<double*>(ho); a.sp_pods = reinterpret_cast<uint16_t*>(ho + (size_t)n * kMaxEnt * 8); a.sp_cnt = ho + (size_t)n * kMaxEnt * 10; a.has_keys = a.sp_cnt + n; }
-    }
-    if (in.keys) {
-        const ScoreOut so{a.dense, a.sp_pods, a.sp_scores, a.sp_cnt, a.has_keys};
-        if (int rc = launch_score_keys(x, reinterpret_cast<const uint64_t*>(h_src), h_off, tb, n, h_model, model0, h_filter, so, x->stream)) return rc;
-    } else {
-        if (int rc = check_shards(x)) return rc;
-        CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
-        const int64_t ctas = std::min<int64_t>((n + kCoopWarps - 1) / kCoopWarps, (int64_t)x->sm_count * 4);
-        coop_score_kernel<16><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem), x->stream>>>(x->tv, a);
-        x->launches += 1;
-        CK(cudaGetLastError());
-    }
-    CK(cudaStreamSynchronize(x->stream));
+    const bool out_direct = rows.pinned(h);
     if (!out_direct) {
-        if (!sparse) { memcpy(dense, ho, (size_t)n * P * 8); if (has_keys) memcpy(has_keys, ho + (size_t)n * P * 8, (size_t)n); }
-        else {
-            memcpy(sp_scores, ho, (size_t)n * kMaxEnt * 8); memcpy(sp_pods, ho + (size_t)n * kMaxEnt * 8, (size_t)n * kMaxEnt * 2);
-            memcpy(sp_cnt, ho + (size_t)n * kMaxEnt * 10, (size_t)n);
-            if (has_keys) memcpy(has_keys, ho + (size_t)n * kMaxEnt * 10 + n, (size_t)n);
-        }
+        CK(x->h_out[0].need((size_t)n * rows.row() + 64));
+        rows.carve(x->h_out[0].p, n, a);
     }
-    return 0;
+    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
+    if (int rc = launch_score(x, ScoreIn{src, in.keys}, a, x->stream)) return rc;
+    CK(cudaStreamSynchronize(x->stream));
+    return out_direct ? 0 : rows.copy(h, a, n);
 }
 
-int score_host_locked(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* model, uint32_t model0,
-                      const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys) {
+int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     int rc = 0;
-    const int64_t* tok_off = in.off;
+    const int64_t n = h.n_prompts;
+    const int64_t* tok_off = h.tok_off;
     const size_t esz = in.elem();
     // the zero-copy and chunk budgets are bytes of input: 4 Mi tokens / 32 Mi tokens (KVIDX_HOST_CHUNK_TOKENS), or as
     // many bytes of keys
     const int64_t zc_max = (int64_t)((16ll << 20) / esz);
-    if (n <= x->zerocopy_max && !x->tv.req_stamp && x->score_kernel != 1 && tok_off[n] - tok_off[0] <= zc_max &&
-        (in.keys || (x->tv.block_size == 16 && (x->score_path == 0 || x->score_path == 4))))
-        return score_host_zerocopy(x, in, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
-    const uint32_t P = x->tv.max_pods, FW = x->tv.filter_words;
-    const bool sparse = sp_cnt != nullptr;
-    const size_t out_row = sparse ? (size_t)kMaxEnt * (sizeof(double) + sizeof(uint16_t)) + 2 : (size_t)P * sizeof(double) + 1;
+    if (n <= x->zerocopy_max && tok_off[n] - tok_off[0] <= zc_max && score_warp_per_prompt(x, in.keys, n)) return score_host_zerocopy(x, in, h);
+    const uint32_t FW = x->tv.filter_words;
+    const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
     // chunk = up to 32 Mi tokens (128 MiB): the H2D copy of a chunk must outlast its kernel for the
     // pipeline to be PCIe bound, and smaller chunks leave the fixed cost of a launch exposed.
     const int64_t kMaxTokChunk = (int64_t)(x->host_chunk_tokens * 4 / (int64_t)esz);
-    const int64_t kMaxRowsChunk = std::max<int64_t>(1, (128ll << 20) / (int64_t)out_row);
+    const int64_t kMaxRowsChunk = std::max<int64_t>(1, (128ll << 20) / (int64_t)rows.row());
     const bool tok_pinned = in.p && is_device_accessible_host(in.p);
-    const bool out_pinned = !sparse && dense && is_device_accessible_host(dense) && (!has_keys || is_device_accessible_host(has_keys));
+    // dense rows are written straight into the caller's buffers when those are pinned; sparse rows are always staged
+    const bool out_pinned = !rows.sparse && rows.pinned(h);
     cudaStream_t s_k = x->stream, s_in = x->copy_stream, s_out = x->d2h_stream;
     struct Pending { bool live = false; int64_t i0 = 0, cnt = 0; } pend[2];
     auto drain = [&](int s) -> int {
@@ -824,19 +853,9 @@ int score_host_locked(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* mo
         CK(cudaEventSynchronize(x->ev_done[s]));
         pend[s].live = false;
         if (out_pinned) return 0;                 // results were written straight into the caller's buffers
-        const int64_t c = pend[s].cnt, b = pend[s].i0;
-        const uint8_t* ho = x->h_out[s].as<uint8_t>();
-        if (!sparse) {
-            memcpy(dense + b * (int64_t)P, ho, (size_t)c * P * sizeof(double));
-            if (has_keys) memcpy(has_keys + b, ho + (size_t)c * P * sizeof(double), (size_t)c);
-        } else {
-            size_t o = 0;
-            memcpy(sp_scores + b * kMaxEnt, ho + o, (size_t)c * kMaxEnt * sizeof(double)); o += (size_t)c * kMaxEnt * sizeof(double);
-            memcpy(sp_pods + b * kMaxEnt, ho + o, (size_t)c * kMaxEnt * sizeof(uint16_t)); o += (size_t)c * kMaxEnt * sizeof(uint16_t);
-            memcpy(sp_cnt + b, ho + o, (size_t)c); o += (size_t)c;
-            if (has_keys) memcpy(has_keys + b, ho + o, (size_t)c);
-        }
-        return 0;
+        ScoreArgs staged{};
+        rows.carve(x->h_out[s].p, pend[s].cnt, staged);
+        return rows.copy(rows.at(h, pend[s].i0), staged, pend[s].cnt);
     };
     // the first chunk must see everything already queued on the handle's stream, and asynchronous write batches issued before
     CK(cudaStreamWaitEvent(s_k, x->ev_write, 0));
@@ -853,55 +872,37 @@ int score_host_locked(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* mo
         if (rc) return rc;
         CK(x->d_tok[slot].need((size_t)std::max<int64_t>(nt, 1) * esz + 64));
         CK(x->d_off[slot].need((size_t)(c + 1) * 8));
-        const size_t stage_bytes = (size_t)(c + 1) * 8 + (model ? (size_t)c * 4 : 0) + (filter ? (size_t)c * FW * 8 : 0) +
-                                   (tok_pinned ? 0 : (size_t)nt * esz);
-        CK(x->h_stage[slot].need(stage_bytes + 64));
+        const StageLayout sl(c, h.model != nullptr, h.filter != nullptr, FW, tok_pinned ? 0 : (size_t)nt * esz);
+        CK(x->h_stage[slot].need(sl.bytes + 64));
         uint8_t* hs = x->h_stage[slot].as<uint8_t>();
-        size_t o = 0;
-        memcpy(hs + o, tok_off + i0, (size_t)(c + 1) * 8);
-        CK(cudaMemcpyAsync(x->d_off[slot].p, hs + o, (size_t)(c + 1) * 8, cudaMemcpyHostToDevice, s_in)); o += (size_t)(c + 1) * 8;
-        const uint32_t* dm = nullptr; const uint64_t* df = nullptr;
-        if (model) {
+        const ScoreArgs hc = sl.pack(hs, h, i0, c, FW);
+        ScoreArgs d = hc;                         // the chunk on the device
+        d.tok_off = x->d_off[slot].as<int64_t>();
+        CK(cudaMemcpyAsync(x->d_off[slot].p, hc.tok_off, (size_t)(c + 1) * 8, cudaMemcpyHostToDevice, s_in));
+        if (hc.model) {
             CK(x->d_model[slot].need((size_t)c * 4));
-            memcpy(hs + o, model + i0, (size_t)c * 4);
-            CK(cudaMemcpyAsync(x->d_model[slot].p, hs + o, (size_t)c * 4, cudaMemcpyHostToDevice, s_in)); o += (size_t)c * 4;
-            dm = x->d_model[slot].as<uint32_t>();
+            CK(cudaMemcpyAsync(x->d_model[slot].p, hc.model, (size_t)c * 4, cudaMemcpyHostToDevice, s_in));
+            d.model = x->d_model[slot].as<uint32_t>();
         }
-        if (filter) {
+        if (hc.filter) {
             CK(x->d_filter[slot].need((size_t)c * FW * 8));
-            memcpy(hs + o, filter + i0 * FW, (size_t)c * FW * 8);
-            CK(cudaMemcpyAsync(x->d_filter[slot].p, hs + o, (size_t)c * FW * 8, cudaMemcpyHostToDevice, s_in)); o += (size_t)c * FW * 8;
-            df = x->d_filter[slot].as<uint64_t>();
+            CK(cudaMemcpyAsync(x->d_filter[slot].p, hc.filter, (size_t)c * FW * 8, cudaMemcpyHostToDevice, s_in));
+            d.filter = x->d_filter[slot].as<uint64_t>();
         }
         if (nt > 0) {
             const uint8_t* src = in.at(tb);
-            if (!tok_pinned) { memcpy(hs + o, src, (size_t)nt * esz); src = hs + o; }
+            if (!tok_pinned) { memcpy(hs + sl.elem, src, (size_t)nt * esz); src = hs + sl.elem; }
             CK(cudaMemcpyAsync(x->d_tok[slot].p, src, (size_t)nt * esz, cudaMemcpyHostToDevice, s_in));
         }
         CK(cudaEventRecord(x->ev_h2d[slot], s_in));
         // kernel
-        CK(x->d_out[slot].need((size_t)c * out_row + 64));
-        if (!out_pinned) CK(x->h_out[slot].need((size_t)c * out_row + 64));
-        uint8_t* dout = x->d_out[slot].as<uint8_t>();
-        ScoreOut so{};
-        if (!sparse) {
-            so.dense = reinterpret_cast<double*>(dout);
-            so.has_keys = dout + (size_t)c * P * sizeof(double);
-        } else {
-            size_t q = 0;
-            so.sp_scores = reinterpret_cast<double*>(dout + q); q += (size_t)c * kMaxEnt * sizeof(double);
-            so.sp_pods = reinterpret_cast<uint16_t*>(dout + q); q += (size_t)c * kMaxEnt * sizeof(uint16_t);
-            so.sp_cnt = dout + q; q += (size_t)c;
-            so.has_keys = dout + q; q += (size_t)c;
-        }
+        CK(x->d_out[slot].need((size_t)c * rows.row() + 64));
+        if (!out_pinned) CK(x->h_out[slot].need((size_t)c * rows.row() + 64));
+        rows.carve(x->d_out[slot].p, c, d);
         CK(cudaStreamWaitEvent(s_k, x->ev_h2d[slot], 0));
-        if (in.keys) {
-            rc = launch_score_keys(x, x->d_tok[slot].as<uint64_t>(), x->d_off[slot].as<int64_t>(), tb, c, dm, model0, df, so, s_k);
-        } else {
-            int64_t maxb = 0;
-            for (int64_t q = i0; q < i1; ++q) maxb = std::max<int64_t>(maxb, (tok_off[q + 1] - tok_off[q]) / x->tv.block_size);
-            rc = launch_score(x, x->d_tok[slot].as<uint32_t>(), x->d_off[slot].as<int64_t>(), tb, c, dm, model0, df, so, s_k, maxb);
-        }
+        int64_t maxb = 0;                         // the round pipelines' block count (tokens)
+        if (!in.keys) for (int64_t q = i0; q < i1; ++q) maxb = std::max<int64_t>(maxb, (tok_off[q + 1] - tok_off[q]) / x->tv.block_size);
+        rc = launch_score(x, ScoreIn{x->d_tok[slot].p, in.keys}, d, s_k, maxb);
         if (rc) return rc;
         CK(cudaEventRecord(x->ev_k[slot], s_k));
         // (slot reuse is safe without further stream waits: drain(slot) host-waits on ev_done[slot], which is
@@ -909,11 +910,9 @@ int score_host_locked(kvidx* x, const ScoreIn& in, int64_t n, const uint32_t* mo
         // read back
         CK(cudaStreamWaitEvent(s_out, x->ev_k[slot], 0));
         if (out_pinned) {
-            CK(cudaMemcpyAsync(dense + i0 * (int64_t)P, so.dense, (size_t)c * P * sizeof(double), cudaMemcpyDeviceToHost, s_out));
-            if (has_keys) CK(cudaMemcpyAsync(has_keys + i0, so.has_keys, (size_t)c, cudaMemcpyDeviceToHost, s_out));
+            if ((rc = rows.copy(rows.at(h, i0), d, c, &s_out))) return rc;
         } else {
-            const size_t total = sparse ? (size_t)c * (kMaxEnt * (sizeof(double) + sizeof(uint16_t)) + 2) : (size_t)c * (P * sizeof(double) + 1);
-            CK(cudaMemcpyAsync(x->h_out[slot].p, dout, total, cudaMemcpyDeviceToHost, s_out));
+            CK(cudaMemcpyAsync(x->h_out[slot].p, x->d_out[slot].p, (size_t)c * rows.row(), cudaMemcpyDeviceToHost, s_out));
         }
         CK(cudaEventRecord(x->ev_done[slot], s_out));
         pend[slot].live = true; pend[slot].i0 = i0; pend[slot].cnt = c;
@@ -939,74 +938,53 @@ int pin_need(void** p, size_t* cap, size_t n) {
 // Several callers' requests as one batch: tokens are gathered into one pinned buffer (CSR rebuilt), per-prompt model ids and
 // filter rows materialised if any request carries them, one pass through score_host, results scattered to the owners.
 int run_combined(kvidx* x, SubmitQueue* q, const std::vector<SubmitReq*>& batch) {
-    const uint32_t P = x->tv.max_pods, FW = x->tv.filter_words;
+    const uint32_t FW = x->tv.filter_words;
+    const ScoreArgs& a0 = batch[0]->a;
     int64_t n = 0, nt = 0;
-    bool any_model = false, any_filter = false, want_has = false;
+    bool any_model = false, any_filter = false;
     for (const SubmitReq* r : batch) {
-        n += r->n; nt += r->tok_off[r->n] - r->tok_off[0];
-        any_model |= r->model != nullptr || r->model0 != batch[0]->model0; any_filter |= r->filter != nullptr; want_has |= r->has_keys != nullptr;
+        n += r->a.n_prompts; nt += r->a.tok_off[r->a.n_prompts] - r->a.tok_off[0];
+        any_model |= r->a.model != nullptr || r->a.model0 != a0.model0; any_filter |= r->a.filter != nullptr;
     }
-    const bool sparse = batch[0]->sp_cnt != nullptr;
-    const size_t in_bytes = (size_t)nt * 4 + 64 + (size_t)(n + 1) * 8 + (any_model ? (size_t)n * 4 : 0) + 64 + (any_filter ? (size_t)n * FW * 8 : 0);
-    const size_t out_bytes = sparse ? (size_t)n * (kMaxEnt * 10 + 2) + 64 : (size_t)n * (P * 8 + 1) + 64;
-    int rc = pin_need(&q->h_in, &q->h_in_cap, in_bytes); if (rc) return rc;
-    rc = pin_need(&q->h_out, &q->h_out_cap, out_bytes); if (rc) return rc;
+    const RowLayout rows{x->tv.max_pods, a0.sp_cnt != nullptr};
+    const StageLayout sl(n, any_model, any_filter, FW, (size_t)nt * 4);
+    int rc = pin_need(&q->h_in, &q->h_in_cap, sl.bytes + 64); if (rc) return rc;
+    rc = pin_need(&q->h_out, &q->h_out_cap, (size_t)n * rows.row() + 64); if (rc) return rc;
     uint8_t* hi = static_cast<uint8_t*>(q->h_in);
-    uint32_t* tok = reinterpret_cast<uint32_t*>(hi); size_t o = ((size_t)nt * 4 + 63) & ~(size_t)63;
-    int64_t* off = reinterpret_cast<int64_t*>(hi + o); o += (size_t)(n + 1) * 8;
-    uint32_t* model = nullptr; uint64_t* filter = nullptr;
-    if (any_model) { model = reinterpret_cast<uint32_t*>(hi + o); o += ((size_t)n * 4 + 63) & ~(size_t)63; }
-    if (any_filter) { filter = reinterpret_cast<uint64_t*>(hi + o); }
+    int64_t* off = reinterpret_cast<int64_t*>(hi);
+    uint32_t* model = any_model ? reinterpret_cast<uint32_t*>(hi + sl.model) : nullptr;
+    uint64_t* filter = any_filter ? reinterpret_cast<uint64_t*>(hi + sl.filter) : nullptr;
+    uint32_t* tok = reinterpret_cast<uint32_t*>(hi + sl.elem);
     int64_t at = 0, tat = 0;
     off[0] = 0;
     for (const SubmitReq* r : batch) {
-        const int64_t tb = r->tok_off[0], rt = r->tok_off[r->n] - tb;
+        const int64_t rn = r->a.n_prompts, tb = r->a.tok_off[0], rt = r->a.tok_off[rn] - tb;
         if (rt > 0) memcpy(tok + tat, r->tok + tb, (size_t)rt * 4);
-        for (int64_t i = 0; i < r->n; ++i) off[at + i + 1] = tat + (r->tok_off[i + 1] - tb);
-        if (model) for (int64_t i = 0; i < r->n; ++i) model[at + i] = r->model ? r->model[i] : r->model0;
-        if (filter) { if (r->filter) memcpy(filter + (size_t)at * FW, r->filter, (size_t)r->n * FW * 8); else memset(filter + (size_t)at * FW, 0, (size_t)r->n * FW * 8); }
-        at += r->n; tat += rt;
+        for (int64_t i = 0; i < rn; ++i) off[at + i + 1] = tat + (r->a.tok_off[i + 1] - tb);
+        if (model) for (int64_t i = 0; i < rn; ++i) model[at + i] = r->a.model ? r->a.model[i] : r->a.model0;
+        if (filter) { if (r->a.filter) memcpy(filter + (size_t)at * FW, r->a.filter, (size_t)rn * FW * 8); else memset(filter + (size_t)at * FW, 0, (size_t)rn * FW * 8); }
+        at += rn; tat += rt;
     }
-    uint8_t* ho = static_cast<uint8_t*>(q->h_out);
-    if (!sparse) {
-        double* dense = reinterpret_cast<double*>(ho); uint8_t* has = ho + (size_t)n * P * 8;
-        rc = score_host(x, ScoreIn{tok, off, false}, n, model, batch[0]->model0, filter, dense, nullptr, nullptr, nullptr, has);
-        if (rc) return rc;
-        at = 0;
-        for (SubmitReq* r : batch) {
-            memcpy(r->dense, dense + (size_t)at * P, (size_t)r->n * P * 8);
-            if (r->has_keys) memcpy(r->has_keys, has + at, (size_t)r->n);
-            at += r->n;
-        }
-    } else {
-        double* sc = reinterpret_cast<double*>(ho); uint16_t* pods = reinterpret_cast<uint16_t*>(ho + (size_t)n * kMaxEnt * 8);
-        uint8_t* cnt = ho + (size_t)n * kMaxEnt * 10; uint8_t* has = cnt + n;
-        rc = score_host(x, ScoreIn{tok, off, false}, n, model, batch[0]->model0, filter, nullptr, pods, sc, cnt, has);
-        if (rc) return rc;
-        at = 0;
-        for (SubmitReq* r : batch) {
-            memcpy(r->sp_scores, sc + (size_t)at * kMaxEnt, (size_t)r->n * kMaxEnt * 8);
-            memcpy(r->sp_pods, pods + (size_t)at * kMaxEnt, (size_t)r->n * kMaxEnt * 2);
-            memcpy(r->sp_cnt, cnt + at, (size_t)r->n);
-            if (r->has_keys) memcpy(r->has_keys, has + at, (size_t)r->n);
-            at += r->n;
-        }
+    ScoreArgs all{nullptr, off, 0, n, model, a0.model0, filter, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    rows.carve(q->h_out, n, all);
+    if ((rc = score_host(x, ScoreIn{tok, false}, all))) return rc;
+    at = 0;
+    for (const SubmitReq* r : batch) {
+        rows.copy(r->a, rows.at(all, at), r->a.n_prompts);
+        at += r->a.n_prompts;
     }
-    (void)want_has;
     return 0;
 }
 
-int submit_score(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
-                 const uint64_t* filter, double* dense, uint16_t* sp_pods, double* sp_scores, uint8_t* sp_cnt, uint8_t* has_keys) {
+int submit_score(kvidx* x, const uint32_t* tok, const ScoreArgs& a) {
     SubmitQueue* q = x->queue;
+    const int64_t n = a.n_prompts;
     // big batches and malformed calls go straight through (score_host validates); so does everything when the queue is off
-    if (!q || !q->enabled || n <= 0 || !tok_off || n > q->max_prompts / 4)
-        return score_host(x, ScoreIn{tok, tok_off, false}, n, model, model0, filter, dense, sp_pods, sp_scores, sp_cnt, has_keys);
-    if (int rc = check_csr(tok_off, n)) return rc;
-    if (tok_off[n] > tok_off[0] && !tok) return fail(KVIDX_EINVAL, "NULL tokens");
+    if (!q || !q->enabled || n <= 0 || !a.tok_off || n > q->max_prompts / 4) return score_host(x, ScoreIn{tok, false}, a);
+    if (int rc = check_csr(a.tok_off, n)) return rc;
+    if (a.tok_off[n] > a.tok_off[0] && !tok) return fail(KVIDX_EINVAL, "NULL tokens");
     SubmitReq me;
-    me.tok = tok; me.tok_off = tok_off; me.n = n; me.model = model; me.model0 = model0; me.filter = filter;
-    me.dense = dense; me.sp_pods = sp_pods; me.sp_scores = sp_scores; me.sp_cnt = sp_cnt; me.has_keys = has_keys;
+    me.tok = tok; me.a = a;
     bool lead;
     {
         std::lock_guard<std::mutex> lk(q->mu);
@@ -1033,21 +1011,20 @@ int submit_score(kvidx* x, const uint32_t* tok, const int64_t* tok_off, int64_t 
                 if (me.rc) g_err = me.err;
                 return me.rc;
             }
-            const bool sparse = q->pending.front()->sp_cnt != nullptr;
+            const bool sparse = q->pending.front()->a.sp_cnt != nullptr;
             int64_t np = 0, ntok = 0;
             for (auto it = q->pending.begin(); it != q->pending.end();) {
                 SubmitReq* r = *it;
-                const int64_t rt = r->tok_off[r->n] - r->tok_off[0];
-                if ((r->sp_cnt != nullptr) != sparse) { ++it; continue; }
-                if (!batch.empty() && (np + r->n > q->max_prompts || ntok + rt > q->max_tokens)) break;
-                batch.push_back(r); np += r->n; ntok += rt;
+                const int64_t rn = r->a.n_prompts, rt = r->a.tok_off[rn] - r->a.tok_off[0];
+                if ((r->a.sp_cnt != nullptr) != sparse) { ++it; continue; }
+                if (!batch.empty() && (np + rn > q->max_prompts || ntok + rt > q->max_tokens)) break;
+                batch.push_back(r); np += rn; ntok += rt;
                 it = q->pending.erase(it);
             }
         }
         int rc;
         if (batch.size() == 1) {
-            SubmitReq* r = batch[0];
-            rc = score_host(x, ScoreIn{r->tok, r->tok_off, false}, r->n, r->model, r->model0, r->filter, r->dense, r->sp_pods, r->sp_scores, r->sp_cnt, r->has_keys);
+            rc = score_host(x, ScoreIn{batch[0]->tok, false}, batch[0]->a);
         } else {
             rc = run_combined(x, q, batch);
             q->coalesced += batch.size();
@@ -1430,36 +1407,26 @@ int kvidx_lookup(kvidx_t* x, uint32_t model, const uint64_t* keys, int64_t n, co
 int kvidx_score_batch(kvidx_t* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
                       const uint64_t* filter, double* scores_out, uint8_t* has_keys_out) {
     if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return submit_score(x, tok, tok_off, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out);
+    return submit_score(x, tok, ScoreArgs{nullptr, tok_off, 0, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out, nullptr});
 }
 
 int kvidx_score_batch_sparse(kvidx_t* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
                              const uint64_t* filter, uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out) {
     if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return submit_score(x, tok, tok_off, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out);
+    return submit_score(x, tok, ScoreArgs{nullptr, tok_off, 0, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out, nullptr});
 }
 
 int kvidx_score_batch_dev(kvidx_t* x, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n, const uint32_t* d_model,
                           uint32_t model0, const uint64_t* d_filter, double* d_scores_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0) return fail(KVIDX_EINVAL, "bad arguments");
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
-    ScoreOut so{};
-    so.dense = d_scores_out; so.has_keys = d_has_keys_out;
-    return launch_score(x, d_tok, d_tok_off, 0, n, d_model, model0, d_filter, so, x->stream);
+    return score_dev(x, ScoreIn{d_tok, false}, ScoreArgs{nullptr, d_tok_off, 0, n, d_model, model0, d_filter, d_scores_out, nullptr, nullptr, nullptr, d_has_keys_out, nullptr});
 }
 
 int kvidx_score_batch_sparse_dev(kvidx_t* x, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n, const uint32_t* d_model,
                                  uint32_t model0, const uint64_t* d_filter, uint16_t* d_pods_out, double* d_scores_out,
                                  uint8_t* d_cnt_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0 || !d_pods_out || !d_scores_out || !d_cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
-    ScoreOut so{};
-    so.sp_pods = d_pods_out; so.sp_scores = d_scores_out; so.sp_cnt = d_cnt_out; so.has_keys = d_has_keys_out;
-    return launch_score(x, d_tok, d_tok_off, 0, n, d_model, model0, d_filter, so, x->stream);
+    return score_dev(x, ScoreIn{d_tok, false}, ScoreArgs{nullptr, d_tok_off, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr});
 }
 
 // ---- Score() from request keys (GetPodScores steps 3-4): not coalesced, every call goes straight through ----
@@ -1467,34 +1434,26 @@ int kvidx_score_batch_sparse_dev(kvidx_t* x, const uint32_t* d_tok, const int64_
 int kvidx_score_keys(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, int64_t n, const uint32_t* model, uint32_t model0,
                      const uint64_t* filter, double* scores_out, uint8_t* has_keys_out) {
     if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_host(x, ScoreIn{keys, key_off, true}, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out);
+    return score_host(x, ScoreIn{keys, true}, ScoreArgs{nullptr, key_off, 0, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out, nullptr});
 }
 
 int kvidx_score_keys_sparse(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, int64_t n, const uint32_t* model, uint32_t model0,
                             const uint64_t* filter, uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out) {
     if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_host(x, ScoreIn{keys, key_off, true}, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out);
+    return score_host(x, ScoreIn{keys, true}, ScoreArgs{nullptr, key_off, 0, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out, nullptr});
 }
 
 int kvidx_score_keys_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n, const uint32_t* d_model,
                          uint32_t model0, const uint64_t* d_filter, double* d_scores_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0 || !d_key_off || !d_scores_out) return fail(KVIDX_EINVAL, "bad arguments");
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    ScoreOut so{};
-    so.dense = d_scores_out; so.has_keys = d_has_keys_out;
-    return launch_score_keys(x, d_keys, d_key_off, 0, n, d_model, model0, d_filter, so, x->stream);
+    return score_dev(x, ScoreIn{d_keys, true}, ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, d_scores_out, nullptr, nullptr, nullptr, d_has_keys_out, nullptr});
 }
 
 int kvidx_score_keys_sparse_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n, const uint32_t* d_model,
                                 uint32_t model0, const uint64_t* d_filter, uint16_t* d_pods_out, double* d_scores_out,
                                 uint8_t* d_cnt_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0 || !d_key_off || !d_pods_out || !d_scores_out || !d_cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    ScoreOut so{};
-    so.sp_pods = d_pods_out; so.sp_scores = d_scores_out; so.sp_cnt = d_cnt_out; so.has_keys = d_has_keys_out;
-    return launch_score_keys(x, d_keys, d_key_off, 0, n, d_model, model0, d_filter, so, x->stream);
+    return score_dev(x, ScoreIn{d_keys, true}, ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr});
 }
 
 // ---- routed (all-to-all) form of the sharded Score(): the device steps around the exchange (kernels_route.cuh) ----
