@@ -25,7 +25,7 @@
  *     Add / Evict of that key (table.cuh), which is the guarantee the reference's
  *     per-key mutex gives.  A write call has taken effect when it returns, so a
  *     thread reads its own writes (index_test.go:214-278).  Concurrent host-buffer
- *     kvidx_score_batch* callers are coalesced into one launch (kvidx_score_keys* calls are not);
+ *     kvidx_score_batch* callers are coalesced into one launch (kvidx_score_keys* and kvidx_score_turn* calls are not);
  *   - there is NO CPU fallback: without a CUDA device kvidx_create fails with
  *     KVIDX_ECUDA.
  */
@@ -186,6 +186,28 @@ int kvidx_score_keys_sparse(kvidx_t* idx, const uint64_t* keys, const int64_t* k
                             const uint32_t* model, uint32_t model0, const uint64_t* filter,
                             uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out);
 
+/* GetPodScores steps 2-4 for a conversation turn, in one call: prompt i is the request keys the caller already holds
+ * (keys[key_off[i] .. key_off[i+1]), block order) followed by new tokens (tok[tok_off[i] .. tok_off[i+1]), whose first
+ * token starts a block).  With K_i = held_i ++ TokensToKVBlockKeys(parent = last held key, or init_hash when prompt i holds
+ * none, new tokens_i), the row is LongestPrefixScorer.Score(K_i, Index.Lookup(K_i, pods)) and has_keys_out[i] = |K_i| > 0.
+ * new_keys_out (may be NULL): the floor(len_i / B) new keys of every prompt, prompt-major; new_key_off_out[n_prompts+1] =
+ * their offsets, from 0 (filled whenever it is given).  A trailing partial block is dropped, as in kvidx_hash_keys: the
+ * caller re-sends it next turn.  Every other argument, KVIDX_SCORE_ABSENT and the result rows mean what they mean for
+ * kvidx_score_keys; key_off[0] and tok_off[0] may be non-zero.  n_prompts < 0, NULL or non-monotone offsets, a NULL
+ * element array with a non-zero count, new_keys_out without new_key_off_out -> KVIDX_EINVAL; n_prompts == 0 -> 0, nothing
+ * written.  Block size 16 on default and CLOCK handles: one fused warp-per-prompt kernel at every batch size (the held keys
+ * are walked, then the new tokens hashed warp-cooperatively from the last held key while the walk goes on).  Other block
+ * sizes, exact-LRU handles and KVIDX_SCORE_KERNEL=v1 hash, concatenate and score the keys (exact-LRU stamps as
+ * kvidx_score_batch).  Host buffers as kvidx_score_keys: pinned ones in place, small calls zero-copy, the rest through the
+ * chunked pipeline; not coalesced with other callers. */
+int kvidx_score_turn(kvidx_t* idx, const uint64_t* keys, const int64_t* key_off, const uint32_t* tok, const int64_t* tok_off,
+                     int64_t n_prompts, const uint32_t* model, uint32_t model0, const uint64_t* filter,
+                     double* scores_out, uint8_t* has_keys_out, uint64_t* new_keys_out, int64_t* new_key_off_out);
+int kvidx_score_turn_sparse(kvidx_t* idx, const uint64_t* keys, const int64_t* key_off, const uint32_t* tok, const int64_t* tok_off,
+                            int64_t n_prompts, const uint32_t* model, uint32_t model0, const uint64_t* filter,
+                            uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out,
+                            uint64_t* new_keys_out, int64_t* new_key_off_out);
+
 /* ---- write path --------------------------------------------------------------- */
 
 /* Index.Add (index.go:127, in_memory.go:149-209): n (engine,request) key pairs of one model,
@@ -306,6 +328,18 @@ int kvidx_score_keys_dev(kvidx_t* idx, const uint64_t* d_keys, const int64_t* d_
 int kvidx_score_keys_sparse_dev(kvidx_t* idx, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n_prompts,
                                 const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter,
                                 uint16_t* d_pods_out, double* d_scores_out, uint8_t* d_cnt_out, uint8_t* d_has_keys_out);
+/* kvidx_score_turn[_sparse] over device-resident inputs and outputs, asynchronous on the handle's stream, ordered after
+ * kvidx_apply_events_dev batches issued before it.  The new keys' offsets are given (d_new_key_off[n_prompts+1], as in
+ * kvidx_hash_keys_dev; may be NULL when d_new_keys_out is).  The fused kernel does not wait on the stream; the composed
+ * path (see kvidx_score_turn) reads the batch's first and last offsets back to size its scratch. */
+int kvidx_score_turn_dev(kvidx_t* idx, const uint64_t* d_keys, const int64_t* d_key_off, const uint32_t* d_tok,
+                         const int64_t* d_tok_off, int64_t n_prompts, const uint32_t* d_model, uint32_t model0,
+                         const uint64_t* d_filter, double* d_scores_out, uint8_t* d_has_keys_out,
+                         const int64_t* d_new_key_off, uint64_t* d_new_keys_out);
+int kvidx_score_turn_sparse_dev(kvidx_t* idx, const uint64_t* d_keys, const int64_t* d_key_off, const uint32_t* d_tok,
+                                const int64_t* d_tok_off, int64_t n_prompts, const uint32_t* d_model, uint32_t model0,
+                                const uint64_t* d_filter, uint16_t* d_pods_out, double* d_scores_out, uint8_t* d_cnt_out,
+                                uint8_t* d_has_keys_out, const int64_t* d_new_key_off, uint64_t* d_new_keys_out);
 int kvidx_hash_keys_dev(kvidx_t* idx, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n_prompts,
                         const uint64_t* d_parent, const uint8_t* d_parent_valid,
                         const int64_t* d_key_off, uint64_t* d_keys_out);

@@ -59,6 +59,14 @@ int kvhost_get_pod_scores(kvhost_t* h, const uint32_t* tokens, size_t n_tokens, 
 int kvhost_get_pod_scores_keys(kvhost_t* h, const uint64_t* keys, size_t n_keys, const char* model,
                                const char* const* pods, size_t n_pods, const char** pod_out, double* score_out);
 
+/* Indexer.GetPodScores for a conversation turn (kvidx_score_turn): the request keys held from earlier turns, then the new
+ * turn's tokens, hashed from the last held key.  new_keys_out (may be NULL) receives the floor(n_tokens / B) new keys.  Same
+ * filter, results and return values as kvhost_get_pod_scores; -1000 when there is no key at all.  With enable_metrics it
+ * counts one Lookup over the held and the new keys. */
+int kvhost_get_pod_scores_turn(kvhost_t* h, const uint64_t* keys, size_t n_keys, const uint32_t* tokens, size_t n_tokens,
+                               const char* model, const char* const* pods, size_t n_pods, const char** pod_out, double* score_out,
+                               uint64_t* new_keys_out);
+
 /* kvblock.Index with strings.  entries are (pod, tier) name pairs. */
 int kvhost_index_add(kvhost_t* h, const char* model, const uint64_t* engine, size_t n_engine, const uint64_t* request, size_t n_request,
                      const char* const* pods, const char* const* tiers, size_t n_entries);

@@ -189,6 +189,91 @@ __device__ __forceinline__ int coop_hash_chunk(const CoopSmem& sm, CoopSmem::War
     return j;                                                                           // blocks hashed
 }
 
+// The CTA's FNV power tables and each warp's two chunk barriers (every thread of the CTA calls this once)
+__device__ __forceinline__ void coop_setup(CoopSmem& sm, CoopSmem::Warp& W, int lane) {
+    for (int i = threadIdx.x; i <= kCoopMaxPayload; i += kCoopThreads) {
+        unsigned long long p = 1;
+        for (int q = 0; q < i; ++q) p *= kFnvPrime;
+        sm.tab.pw[i] = p; sm.tab.c0[i] = kFnvOffset * p;
+    }
+    if (lane == 0) { mbar_init(&W.bar[0], 1); mbar_init(&W.bar[1], 1); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_proxy_async();
+    __syncthreads();
+}
+
+// Chunk c of a prompt's nblk 16-token blocks at tokp -> buffer c & 1: one TMA bulk copy by lane 0 onto the buffer's
+// barrier, or (tokp not 16-byte aligned) loads by every lane
+__device__ __forceinline__ void coop_stage(CoopSmem::Warp& W, const uint32_t* tokp, int nblk, int c, bool aligned, int lane) {
+    constexpr int BS = 16;
+    const int nbc = min(kRoundBlocks, nblk - c * kRoundBlocks);
+    if (nbc <= 0) return;
+    const uint32_t* src = tokp + (size_t)c * kRoundBlocks * BS;
+    if (aligned) {
+        if (lane == 0) { fence_proxy_async(); mbar_expect_tx(&W.bar[c & 1], (uint32_t)nbc * BS * 4); tma_load_1d(W.tok[c & 1], src, (uint32_t)nbc * BS * 4, &W.bar[c & 1]); }
+    } else {
+        for (int x = lane; x < nbc * BS; x += 32) W.tok[c & 1][x] = __ldg(src + x);
+    }
+}
+
+// One chunk of nb <= 32 staged blocks (tk) of a warp-per-prompt token walk, chain seeded with h (left at the chunk's last
+// key): lane j hashes with the warp and probes block j as soon as the eight blocks around it are hashed, a ballot finds the
+// first miss, the hits are walked and marked.  `cont` / `first_block` as for WarpWalk::walk.  Returns the consecutive hits
+// from the chunk's first block (0 when `probe` is false: no slot is read).  `all`: every block of the chunk is hashed (lane
+// j's key in `key`) also once a miss is seen, probes still stop there; else a miss ends the hashing too (`probe` true).
+__device__ __forceinline__ int coop_walk_chunk(const TableView& t, const CoopSmem& sm, CoopSmem::Warp& W, const uint32_t* tk, uint64_t& h, int nb,
+                                               int lane, uint32_t lt, uint32_t mdl, bool peer, bool all, bool probe, WarpWalk& ws, bool cont, bool first_block,
+                                               const uint64_t* filter, int64_t pi, uint64_t& key) {
+    // ---- keys; lane j probes block j as soon as the eight blocks around it are hashed ----
+    uint64_t last = 0;
+    key = 0;
+    uint4 A0 = {0, 0, 0, 0}, B0 = {0, 0, 0, 0}, A1 = {0, 0, 0, 0}, B1 = {0, 0, 0, 0};
+    const ReqSlot* base = t.req; uint64_t slot = 0;
+    bool issued = false, hit = false, decided = false;
+    int nprobe = all && !probe ? 0 : kRoundBlocks;                      // all: the blocks probed before a miss was seen
+    SlotPat mine = {};
+    uint64_t hslot = 0;                                           // CLOCK: slot of this lane's hit
+    auto resolve = [&]() {                                        // the slot pair has (or will have) arrived: hit or miss
+        uint4 A, B;
+        while (!pair_decides(A0, B0, A1, B1, key, mdl, A, B, hit)) {
+            slot = (slot + 2) & t.req_mask;                       // rare: displaced past the home pair
+            ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
+        }
+        if (hit) { mine = SlotPat::of(A, B); if (t.req_ref) hslot = pair_hit_slot(slot, A0, B0, key, mdl); }
+        decided = true;
+    };
+    const int nhashed = coop_hash_chunk(sm, W, tk, h, nb, lane, lt, key, last, [&](int ndone) -> bool {
+        if (all && nprobe < ndone) return false;                            // past a miss (or not probing): hashing only
+        if (lane >= ndone - 8 && lane < ndone) {                  // the eight keys just produced: request their slot pairs
+            const uint64_t hm = home_of(key, mdl);
+            base = t.req_peer[shard_of(hm, t.shard_bits)]; slot = hm & t.req_mask & ~1ull;
+            ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
+            issued = true;
+        }
+        if (ndone < 16) return false;
+        if (lane >= ndone - 16 && lane < ndone - 8) resolve();   // the eight before them have landed: a miss ends the prompt
+        const bool miss = __any_sync(0xffffffffu, decided && !hit);
+        if (all) { if (miss) nprobe = ndone; return false; }
+        return miss;
+    });
+    const int np = all ? min(nhashed, nprobe) : nhashed;         // blocks that are probed
+    // blocks hashed but not yet requested / resolved
+    if (lane < np && !issued) {
+        const uint64_t hm = home_of(key, mdl);
+        base = t.req_peer[shard_of(hm, t.shard_bits)]; slot = hm & t.req_mask & ~1ull;
+        ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
+        issued = true;
+    }
+    if (lane < np && !decided) resolve();
+    const uint32_t hm_ = __ballot_sync(0xffffffffu, hit && lane < np);
+    const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from the chunk's first block
+    // ---- ordered scoring of the hits (kvblock_scorer.go:108-151), lane q owns pod q ----
+    const int nwalked = ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, cont, nhit), first_block, filter, pi, [](int) {});
+    WarpWalk::mark_walked(t, lane, nwalked, hit, hslot);
+    h = last;
+    return nhit;
+}
+
 template <int BS>
 __global__ void __launch_bounds__(kCoopThreads)
 coop_score_kernel(const TableView t, const ScoreArgs a) {
@@ -199,15 +284,7 @@ coop_score_kernel(const TableView t, const ScoreArgs a) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const uint32_t lt = (1u << lane) - 1u;
     CoopSmem::Warp& W = sm.w[wid];
-    for (int i = threadIdx.x; i <= kCoopMaxPayload; i += kCoopThreads) {
-        unsigned long long p = 1;
-        for (int q = 0; q < i; ++q) p *= kFnvPrime;
-        sm.tab.pw[i] = p; sm.tab.c0[i] = kFnvOffset * p;
-    }
-    if (lane == 0) { mbar_init(&W.bar[0], 1); mbar_init(&W.bar[1], 1); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    fence_proxy_async();
-    __syncthreads();
+    coop_setup(sm, W, lane);
     const bool peer = t.shard_bits != 0;
     uint32_t phases = 0;                                                  // bit s: parity the next wait on buffer s uses
     const long long total_warps = (long long)gridDim.x * kCoopWarps;
@@ -219,16 +296,7 @@ coop_score_kernel(const TableView t, const ScoreArgs a) {
         const uint32_t mdl = a.model ? a.model[pi] : a.model0;
         WarpWalk ws;
         uint64_t h = t.init_hash;
-        auto stage = [&](int c) {                                         // chunk c -> buffer c & 1
-            const int nbc = min(kRoundBlocks, nblk - c * kRoundBlocks);
-            if (nbc <= 0) return;
-            const uint32_t* src = tokp + (size_t)c * kRoundBlocks * BS;
-            if (aligned) {
-                if (lane == 0) { fence_proxy_async(); mbar_expect_tx(&W.bar[c & 1], (uint32_t)nbc * BS * 4); tma_load_1d(W.tok[c & 1], src, (uint32_t)nbc * BS * 4, &W.bar[c & 1]); }
-            } else {
-                for (int x = lane; x < nbc * BS; x += 32) W.tok[c & 1][x] = __ldg(src + x);
-            }
-        };
+        auto stage = [&](int c) { coop_stage(W, tokp, nblk, c, aligned, lane); };
         stage(0);
         bool done = nblk == 0;
         const int nchunks = (nblk + kRoundBlocks - 1) / kRoundBlocks;
@@ -241,49 +309,9 @@ coop_score_kernel(const TableView t, const ScoreArgs a) {
             __syncwarp();
             const int nb = min(kRoundBlocks, nblk - c * kRoundBlocks);
             const bool has_more = (c + 1) * kRoundBlocks < nblk;
-            // ---- keys; lane j probes block j as soon as the eight blocks around it are hashed ----
-            uint64_t key = 0, last = 0;
-            uint4 A0 = {0, 0, 0, 0}, B0 = {0, 0, 0, 0}, A1 = {0, 0, 0, 0}, B1 = {0, 0, 0, 0};
-            const ReqSlot* base = t.req; uint64_t slot = 0;
-            bool issued = false, hit = false, decided = false;
-            SlotPat mine = {};
-            uint64_t hslot = 0;                                           // CLOCK: slot of this lane's hit
-            auto resolve = [&]() {                                        // the slot pair has (or will have) arrived: hit or miss
-                uint4 A, B;
-                while (!pair_decides(A0, B0, A1, B1, key, mdl, A, B, hit)) {
-                    slot = (slot + 2) & t.req_mask;                       // rare: displaced past the home pair
-                    ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
-                }
-                if (hit) { mine = SlotPat::of(A, B); if (t.req_ref) hslot = pair_hit_slot(slot, A0, B0, key, mdl); }
-                decided = true;
-            };
-            const int nhashed = coop_hash_chunk(sm, W, W.tok[c & 1], h, nb, lane, lt, key, last, [&](int ndone) -> bool {
-                if (lane >= ndone - 8 && lane < ndone) {                  // the eight keys just produced: request their slot pairs
-                    const uint64_t hm = home_of(key, mdl);
-                    base = t.req_peer[shard_of(hm, t.shard_bits)]; slot = hm & t.req_mask & ~1ull;
-                    ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
-                    issued = true;
-                }
-                if (ndone < 16) return false;
-                if (lane >= ndone - 16 && lane < ndone - 8) resolve();   // the eight before them have landed: a miss ends the prompt
-                const bool miss = __any_sync(0xffffffffu, decided && !hit);
-                return miss;
-            });
-            // blocks hashed but not yet requested / resolved
-            if (lane < nhashed && !issued) {
-                const uint64_t hm = home_of(key, mdl);
-                base = t.req_peer[shard_of(hm, t.shard_bits)]; slot = hm & t.req_mask & ~1ull;
-                ld_slot_pair(base + slot, peer, A0, B0, A1, B1);
-                issued = true;
-            }
-            if (lane < nhashed && !decided) resolve();
-            const uint32_t hm_ = __ballot_sync(0xffffffffu, hit && lane < nhashed);
-            const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from the chunk's first block
-            // ---- ordered scoring of the hits (kvblock_scorer.go:108-151), lane q owns pod q ----
-            const int nwalked = ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, c > 0, nhit), c == 0, a.filter, pi, [](int) {});
-            WarpWalk::mark_walked(t, lane, nwalked, hit, hslot);
+            uint64_t key;
+            const int nhit = coop_walk_chunk(t, sm, W, W.tok[c & 1], h, nb, lane, lt, mdl, peer, false, true, ws, c > 0, c == 0, a.filter, pi, key);
             if (!ws.alive || nhit < nb || !has_more) done = true;
-            h = last;
         }
         // ---- result ----
         warp_write_row(t, a, pi, ws.k, ws.pod, ws.sc, nblk > 0, l2pol);

@@ -30,6 +30,26 @@ __device__ __forceinline__ uint64_t ld_stream_u64(const uint64_t* p, uint64_t po
     return v;
 }
 
+// One chunk of nb <= 32 held keys (lane j: key j): probe, ballot to the first miss, walk, mark.  `cont`: a block was scored
+// before this chunk; `first_block`: the chunk's key 0 is the prompt's block 0.  True while the walk goes on past the chunk.
+__device__ __forceinline__ bool keys_walk_chunk(const TableView& t, WarpWalk& ws, int lane, uint64_t key, int nb, uint32_t mdl, bool peer,
+                                                bool cont, bool first_block, const uint64_t* filter, int64_t pi) {
+    SlotPat mine = {};
+    bool hit = false;
+    uint64_t hslot = 0;                                           // CLOCK: slot of this lane's hit
+    if (lane < nb) {
+        HomeProbe pr;
+        uint4 A, B;
+        hit = pr.find(t, key, mdl, peer, A, B);
+        if (hit) { mine = SlotPat::of(A, B); if (t.req_ref) hslot = pr.hit_slot(key, mdl); }
+    }
+    const uint32_t hm_ = __ballot_sync(0xffffffffu, hit);
+    const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from the chunk's first key
+    const int nwalked = ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, cont, nhit), first_block, filter, pi, [](int) {});
+    WarpWalk::mark_walked(t, lane, nwalked, hit, hslot);
+    return ws.alive && nhit >= nb;                                // else a key not in the index, or no pod left
+}
+
 // a.tok_off / a.tok_base describe the key CSR: prompt i owns keys[a.tok_off[i] - a.tok_base .. a.tok_off[i+1] - a.tok_base)
 __global__ void __launch_bounds__(kKeysThreads, kKeysCtasPerSm)
 score_keys_kernel(const TableView t, const uint64_t* __restrict__ keys, const ScoreArgs a) {
@@ -50,20 +70,7 @@ score_keys_kernel(const TableView t, const uint64_t* __restrict__ keys, const Sc
             // the next chunk's keys, in flight while this chunk is probed and walked
             uint64_t next = 0;
             if (c0 + kKeysChunk + lane < nk) next = ld_stream_u64(kp + c0 + kKeysChunk + lane, l2pol);
-            SlotPat mine = {};
-            bool hit = false;
-            uint64_t hslot = 0;                                           // CLOCK: slot of this lane's hit
-            if (lane < nb) {
-                HomeProbe pr;
-                uint4 A, B;
-                hit = pr.find(t, key, mdl, peer, A, B);
-                if (hit) { mine = SlotPat::of(A, B); if (t.req_ref) hslot = pr.hit_slot(key, mdl); }
-            }
-            const uint32_t hm_ = __ballot_sync(0xffffffffu, hit);
-            const int nhit = hm_ == 0xffffffffu ? 32 : __ffs(~hm_) - 1;   // consecutive hits from the chunk's first key
-            const int nwalked = ws.walk<false>(t, lane, mine, nhit, ws.same_mask(lane, mine, c0 > 0, nhit), c0 == 0, a.filter, pi, [](int) {});
-            WarpWalk::mark_walked(t, lane, nwalked, hit, hslot);
-            if (!ws.alive || nhit < nb) break;                            // a key not in the index, or no pod left
+            if (!keys_walk_chunk(t, ws, lane, key, nb, mdl, peer, c0 > 0, c0 == 0, a.filter, pi)) break;
             key = next;
         }
         warp_write_row(t, a, pi, ws.k, ws.pod, ws.sc, nk > 0, l2pol);

@@ -27,6 +27,7 @@
 #include "kernels_rounds_plain.cuh"
 #include "kernels_coop.cuh"
 #include "kernels_keys.cuh"
+#include "kernels_turn.cuh"
 #include "kernels_route.cuh"
 #include <cub/device/device_radix_sort.cuh>
 
@@ -136,6 +137,7 @@ struct kvidx {
     // read-side scratch (guarded by mu_r)
     DevBuf d_tok[2], d_off[2], d_model[2], d_filter[2], d_out[2], d_aux[2], d_rmisc;
     PinBuf h_stage[2], h_out[2];
+    DevBuf d_turn;                  // a conversation turn on the composed path: the concatenated key CSR and its setup
     // write-side scratch (guarded by mu_w)
     DevBuf d_misc, d_ev, d_hash, d_evtok, d_qoff, d_wkeys, d_wpred, d_wready, d_wmap;
     DevBuf d_sweep;                 // CLOCK sweep scratch: bitmap image, per-tile counts, control block
@@ -623,8 +625,12 @@ int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int
 
 // The prompts of a Score() call: tokens (steps 2-4, `p` uint32) or request keys (steps 3-4, `p` uint64).  Prompt i owns
 // elements tok_off[i] .. tok_off[i+1] of p, with the offsets and everything else about the call in a ScoreArgs.
+// A conversation turn (kvidx_score_turn*) is keys followed by tokens: `t` holds the tokens' CSR and where the new keys go
+// (t.keys unused: the held keys are at p).
 struct ScoreIn {
     const void* p; bool keys;
+    TurnArgs t = {};
+    bool turn() const { return t.tok_off != nullptr; }
     size_t elem() const { return keys ? 8 : 4; }
     const uint8_t* at(int64_t i) const { return static_cast<const uint8_t*>(p) + (size_t)i * elem(); }
 };
@@ -642,6 +648,10 @@ bool score_warp_per_prompt(const kvidx* x, bool keys, int64_t n) {
     return !score_takes_v1(x, keys) && (keys || x->score_path == 4 || (x->score_path == 0 && n <= x->coop_max));
 }
 
+// Does a conversation turn take the fused kernel (score_turn_kernel, one warp per prompt at every batch size, inputs read in
+// place)?  Not where tokens take v1: there it is composed of the hash, a concatenation and Score() from keys.
+bool score_turn_fused(const kvidx* x) { return !score_takes_v1(x, false); }
+
 template <class E>
 void launch_score_v1(kvidx* x, const ScoreArgs& a, const E* src, cudaStream_t st) {
     const int T = 128;
@@ -655,10 +665,13 @@ void launch_score_v1(kvidx* x, const ScoreArgs& a, const E* src, cudaStream_t st
 // Launch Score() over device-addressable inputs: the prompts' elements at in.p (a.tok is set here), the rest of the call in
 // `a`.  max_blocks: the token batch's largest block count, for the round pipelines; < 0 computes it on the device.  The
 // callers order the launch after the asynchronous write batches issued before (ev_write), once per call.
+int launch_turn(kvidx* x, const ScoreIn& in, const ScoreArgs& a, cudaStream_t st);
+
 int launch_score(kvidx* x, const ScoreIn& in, ScoreArgs a, cudaStream_t st, int64_t max_blocks = -1) {
     const int64_t n = a.n_prompts;
     if (n <= 0) return 0;
     if (int rc = check_shards(x)) return rc;
+    if (in.turn()) return launch_turn(x, in, a, st);
     a.tok = in.keys ? nullptr : static_cast<const uint32_t*>(in.p);
     if (score_takes_v1(x, in.keys)) {
         if (in.keys) launch_score_v1(x, a, static_cast<const uint64_t*>(in.p), st);
@@ -685,6 +698,50 @@ int launch_score(kvidx* x, const ScoreIn& in, ScoreArgs a, cudaStream_t st, int6
     }
     CK(cudaGetLastError());
     return 0;
+}
+
+// A conversation turn: a.tok_off / a.tok_base the held keys' CSR (keys at in.p), in.t the tokens and the new keys.  The fused
+// kernel, or (score_turn_fused false) the composed path: its scratch is sized from the batch's key and token counts, read
+// back from the offsets, then hash_keys_kernel_v1 hashes every prompt's new blocks from its last held key straight into
+// the concatenated key CSR, turn_concat_kernel adds the held keys (and hands the new ones out) and Score() runs on the keys.
+int launch_turn(kvidx* x, const ScoreIn& in, const ScoreArgs& a, cudaStream_t st) {
+    const int64_t n = a.n_prompts;
+    TurnArgs ta = in.t;
+    ta.keys = static_cast<const uint64_t*>(in.p);
+    if (score_turn_fused(x)) {
+        const int64_t ctas = std::min<int64_t>((n + kCoopWarps - 1) / kCoopWarps, (int64_t)x->sm_count * 4);
+        score_turn_kernel<<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem), st>>>(x->tv, a, ta);
+        x->launches += 1;
+        CK(cudaGetLastError());
+        return 0;
+    }
+    int64_t e[4];
+    CK(cudaMemcpyAsync(&e[0], a.tok_off, 8, cudaMemcpyDefault, st));
+    CK(cudaMemcpyAsync(&e[1], a.tok_off + n, 8, cudaMemcpyDefault, st));
+    CK(cudaMemcpyAsync(&e[2], ta.tok_off, 8, cudaMemcpyDefault, st));
+    CK(cudaMemcpyAsync(&e[3], ta.tok_off + n, 8, cudaMemcpyDefault, st));
+    CK(cudaStreamSynchronize(st));
+    const uint32_t B = x->tv.block_size;
+    const int64_t cap = (e[1] - e[0]) + (e[3] - e[2]) / B;             // >= the concatenated key count
+    auto al = [](size_t b) { return (b + 63) & ~(size_t)63; };
+    const size_t o_dst = al((size_t)(n + 1) * 8), o_par = o_dst + al((size_t)n * 8), o_pv = o_par + al((size_t)n * 8), o_cat = o_pv + al((size_t)n);
+    CK(x->d_turn.need(o_cat + (size_t)std::max<int64_t>(cap, 1) * 8));
+    uint8_t* d = x->d_turn.as<uint8_t>();
+    int64_t* cat_off = reinterpret_cast<int64_t*>(d);
+    int64_t* new_dst = reinterpret_cast<int64_t*>(d + o_dst);
+    uint64_t* parent = reinterpret_cast<uint64_t*>(d + o_par);
+    uint8_t* pv = d + o_pv;
+    uint64_t* cat = reinterpret_cast<uint64_t*>(d + o_cat);
+    turn_offsets_kernel<<<1, kTurnScanThreads, 0, st>>>(ta.keys, a.tok_off, a.tok_base, ta.tok_off, n, B, cat_off, new_dst, parent, pv);
+    const int T = 128;
+    hash_keys_kernel_v1<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, ta.tok, ta.tok_off, ta.tok_base, n, parent, pv, new_dst, 0, cat);
+    const int64_t cw = std::min<int64_t>((n + 7) / 8, (int64_t)x->sm_count * 8);
+    turn_concat_kernel<<<(unsigned)cw, 256, 0, st>>>(ta.keys, a.tok_off, a.tok_base, cat_off, new_dst, n, cat, ta.new_keys, ta.new_off, ta.new_base);
+    x->launches += 3;
+    CK(cudaGetLastError());
+    ScoreArgs k = a;
+    k.tok_off = cat_off; k.tok_base = 0;
+    return launch_score(x, ScoreIn{cat, true}, k, st);
 }
 
 // The device-resident entry points: Score() on the handle's stream, after the asynchronous write batches issued before.
@@ -749,14 +806,38 @@ struct RowLayout {
 
 // The input sections of a host-buffer call over c prompts in one pinned buffer, each 64-byte aligned: the offsets (c + 1),
 // the model ids and the filter rows (when the call has them), then the elements (when they are staged).
+// A conversation turn adds a second section after them: the tokens' offsets, the new keys' offsets (when the keys are
+// wanted), then the tokens (when they are staged).
 struct StageLayout {
     size_t model, filter, elem, bytes;            // section starts (the offsets start the buffer) and the total
+    size_t off2 = 0, noff = 0, elem2 = 0;         // a turn's second section
+    static size_t al(size_t b) { return (b + 63) & ~(size_t)63; }
     StageLayout(int64_t c, bool has_model, bool has_filter, uint32_t fw, size_t elem_bytes) {
-        auto al = [](size_t b) { return (b + 63) & ~(size_t)63; };
         model = al((size_t)(c + 1) * 8);
         filter = model + (has_model ? al((size_t)c * 4) : 0);
         elem = filter + (has_filter ? al((size_t)c * fw * 8) : 0);
         bytes = elem + elem_bytes;
+    }
+    StageLayout& turn(int64_t c, bool want_keys, size_t tok_bytes) {
+        off2 = al(bytes);
+        noff = off2 + al((size_t)(c + 1) * 8);
+        elem2 = noff + (want_keys ? al((size_t)(c + 1) * 8) : 0);
+        bytes = elem2 + tok_bytes;
+        return *this;
+    }
+    // copy the token and new-key offsets of prompts i0 .. i0+c of the host turn `t` into buf; the packed turn's tok and
+    // new_keys point at the chunk's first token and first new key in the caller's buffers (move them when staged)
+    TurnArgs pack_turn(uint8_t* buf, const TurnArgs& t, int64_t i0, int64_t c) const {
+        TurnArgs r = t;
+        memcpy(buf + off2, t.tok_off + i0, (size_t)(c + 1) * 8);
+        r.tok_off = reinterpret_cast<int64_t*>(buf + off2); r.tok_base = t.tok_off[i0];
+        if (t.tok) r.tok = t.tok + r.tok_base;
+        if (t.new_keys) {
+            memcpy(buf + noff, t.new_off + i0, (size_t)(c + 1) * 8);
+            r.new_off = reinterpret_cast<int64_t*>(buf + noff); r.new_base = t.new_off[i0];
+            r.new_keys = t.new_keys + r.new_base;
+        }
+        return r;
     }
     // copy the offsets, model ids and filter rows of prompts i0 .. i0+c of the host call `h` into buf: the packed call, with
     // the outputs of h
@@ -810,21 +891,34 @@ int score_host_zerocopy(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     const int64_t n = h.n_prompts, tb = h.tok_off[0], nt = h.tok_off[n] - tb;
     const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
     const bool in_pinned = nt == 0 || is_device_accessible_host(in.p);
-    const StageLayout sl(n, h.model != nullptr, h.filter != nullptr, x->tv.filter_words, in_pinned ? 0 : (size_t)nt * in.elem());
+    StageLayout sl(n, h.model != nullptr, h.filter != nullptr, x->tv.filter_words, in_pinned ? 0 : (size_t)nt * in.elem());
+    // a turn: its tokens read in place when pinned, its new keys written in place when pinned, else both staged
+    const TurnArgs& t = in.t;
+    const int64_t nt2 = in.turn() ? t.tok_off[n] - t.tok_off[0] : 0, nnk = t.new_keys ? t.new_off[n] - t.new_off[0] : 0;
+    const bool tok_pinned = nt2 == 0 || is_device_accessible_host(t.tok);
+    const bool nk_pinned = nnk == 0 || is_device_accessible_host(t.new_keys + t.new_off[0]);
+    if (in.turn()) sl.turn(n, t.new_keys != nullptr, tok_pinned ? 0 : (size_t)nt2 * 4);
     CK(x->h_stage[0].need(sl.bytes + 64));
     uint8_t* hs = x->h_stage[0].as<uint8_t>();
     ScoreArgs a = sl.pack(hs, h, 0, n, x->tv.filter_words);
     const uint8_t* src = in.p ? in.at(tb) : nullptr;                    // element of absolute index tb
     if (!in_pinned) { memcpy(hs + sl.elem, src, (size_t)nt * in.elem()); src = hs + sl.elem; }
-    // results: straight into the caller's buffers when those are pinned, else through the pinned staging
-    const bool out_direct = rows.pinned(h);
-    if (!out_direct) {
-        CK(x->h_out[0].need((size_t)n * rows.row() + 64));
-        rows.carve(x->h_out[0].p, n, a);
+    ScoreIn z{src, in.keys};
+    if (in.turn()) {
+        z.t = sl.pack_turn(hs, t, 0, n);
+        if (!tok_pinned) { memcpy(hs + sl.elem2, z.t.tok, (size_t)nt2 * 4); z.t.tok = reinterpret_cast<const uint32_t*>(hs + sl.elem2); }
     }
+    // results: straight into the caller's buffers when those are pinned, else through the pinned staging (new keys after
+    // the rows)
+    const bool out_direct = rows.pinned(h);
+    const size_t nk_at = StageLayout::al((size_t)n * rows.row());
+    if (!out_direct || !nk_pinned) CK(x->h_out[0].need(nk_at + (size_t)nnk * 8 + 64));
+    if (!out_direct) rows.carve(x->h_out[0].p, n, a);
+    if (!nk_pinned) z.t.new_keys = reinterpret_cast<uint64_t*>(x->h_out[0].as<uint8_t>() + nk_at);
     CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
-    if (int rc = launch_score(x, ScoreIn{src, in.keys}, a, x->stream)) return rc;
+    if (int rc = launch_score(x, z, a, x->stream)) return rc;
     CK(cudaStreamSynchronize(x->stream));
+    if (!nk_pinned) memcpy(t.new_keys + t.new_off[0], z.t.new_keys, (size_t)nnk * 8);
     return out_direct ? 0 : rows.copy(h, a, n);
 }
 
@@ -833,10 +927,18 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     const int64_t n = h.n_prompts;
     const int64_t* tok_off = h.tok_off;
     const size_t esz = in.elem();
+    // a turn's second section: its tokens (T: their offsets) and new keys (NK: their offsets, when wanted)
+    const TurnArgs& t = in.t;
+    const int64_t* T = t.tok_off;
+    const int64_t* NK = t.new_keys ? t.new_off : nullptr;
     // the zero-copy and chunk budgets are bytes of input: 4 Mi tokens / 32 Mi tokens (KVIDX_HOST_CHUNK_TOKENS), or as
-    // many bytes of keys
+    // many bytes of keys (of keys and tokens, for a turn)
     const int64_t zc_max = (int64_t)((16ll << 20) / esz);
-    if (n <= x->zerocopy_max && tok_off[n] - tok_off[0] <= zc_max && score_warp_per_prompt(x, in.keys, n)) return score_host_zerocopy(x, in, h);
+    if (in.turn()) {
+        if (n <= x->zerocopy_max && (tok_off[n] - tok_off[0]) * 8 + (T[n] - T[0]) * 4 <= (16ll << 20) && score_turn_fused(x)) return score_host_zerocopy(x, in, h);
+    } else if (n <= x->zerocopy_max && tok_off[n] - tok_off[0] <= zc_max && score_warp_per_prompt(x, in.keys, n)) {
+        return score_host_zerocopy(x, in, h);
+    }
     const uint32_t FW = x->tv.filter_words;
     const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
     // chunk = up to 32 Mi tokens (128 MiB): the H2D copy of a chunk must outlast its kernel for the
@@ -844,6 +946,8 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     const int64_t kMaxTokChunk = (int64_t)(x->host_chunk_tokens * 4 / (int64_t)esz);
     const int64_t kMaxRowsChunk = std::max<int64_t>(1, (128ll << 20) / (int64_t)rows.row());
     const bool tok_pinned = in.p && is_device_accessible_host(in.p);
+    const bool tok2_pinned = t.tok && is_device_accessible_host(t.tok);
+    const bool nk_pinned = NK && is_device_accessible_host(t.new_keys);
     // dense rows are written straight into the caller's buffers when those are pinned; sparse rows are always staged
     const bool out_pinned = !rows.sparse && rows.pinned(h);
     cudaStream_t s_k = x->stream, s_in = x->copy_stream, s_out = x->d2h_stream;
@@ -852,10 +956,13 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
         if (!pend[s].live) return 0;
         CK(cudaEventSynchronize(x->ev_done[s]));
         pend[s].live = false;
+        const int64_t i0 = pend[s].i0, c = pend[s].cnt;
+        if (NK && !nk_pinned && NK[i0 + c] > NK[i0])   // the new keys, staged after the rows
+            memcpy(t.new_keys + NK[i0], x->h_out[s].as<uint8_t>() + StageLayout::al((size_t)c * rows.row()), (size_t)(NK[i0 + c] - NK[i0]) * 8);
         if (out_pinned) return 0;                 // results were written straight into the caller's buffers
         ScoreArgs staged{};
-        rows.carve(x->h_out[s].p, pend[s].cnt, staged);
-        return rows.copy(rows.at(h, pend[s].i0), staged, pend[s].cnt);
+        rows.carve(x->h_out[s].p, c, staged);
+        return rows.copy(rows.at(h, i0), staged, c);
     };
     // the first chunk must see everything already queued on the handle's stream, and asynchronous write batches issued before
     CK(cudaStreamWaitEvent(s_k, x->ev_write, 0));
@@ -865,14 +972,21 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     int slot = 0;
     while (i0 < n) {
         int64_t i1 = i0;
-        while (i1 < n && (i1 - i0) < kMaxRowsChunk && (tok_off[i1 + 1] - tok_off[i0]) <= kMaxTokChunk) ++i1;
+        if (T) {                                  // a turn: keys and tokens share the byte budget
+            while (i1 < n && (i1 - i0) < kMaxRowsChunk && (tok_off[i1 + 1] - tok_off[i0]) * 8 + (T[i1 + 1] - T[i0]) * 4 <= x->host_chunk_tokens * 4) ++i1;
+        } else {
+            while (i1 < n && (i1 - i0) < kMaxRowsChunk && (tok_off[i1 + 1] - tok_off[i0]) <= kMaxTokChunk) ++i1;
+        }
         if (i1 == i0) i1 = i0 + 1;                // a single prompt larger than the chunk budget
         const int64_t c = i1 - i0, tb = tok_off[i0], nt = tok_off[i1] - tb;
+        const int64_t nt2 = T ? T[i1] - T[i0] : 0, nnk = NK ? NK[i1] - NK[i0] : 0;
         rc = drain(slot);                         // slot's previous results are home; its device buffers are free
         if (rc) return rc;
-        CK(x->d_tok[slot].need((size_t)std::max<int64_t>(nt, 1) * esz + 64));
-        CK(x->d_off[slot].need((size_t)(c + 1) * 8));
-        const StageLayout sl(c, h.model != nullptr, h.filter != nullptr, FW, tok_pinned ? 0 : (size_t)nt * esz);
+        const size_t tok2_at = StageLayout::al((size_t)std::max<int64_t>(nt, 1) * esz);   // a turn's tokens after the keys
+        CK(x->d_tok[slot].need(T ? tok2_at + (size_t)nt2 * 4 + 64 : (size_t)std::max<int64_t>(nt, 1) * esz + 64));
+        CK(x->d_off[slot].need((size_t)(c + 1) * 8 * (T ? 3 : 1)));
+        StageLayout sl(c, h.model != nullptr, h.filter != nullptr, FW, tok_pinned ? 0 : (size_t)nt * esz);
+        if (T) sl.turn(c, NK != nullptr, tok2_pinned ? 0 : (size_t)nt2 * 4);
         CK(x->h_stage[slot].need(sl.bytes + 64));
         uint8_t* hs = x->h_stage[slot].as<uint8_t>();
         const ScoreArgs hc = sl.pack(hs, h, i0, c, FW);
@@ -894,15 +1008,39 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
             if (!tok_pinned) { memcpy(hs + sl.elem, src, (size_t)nt * esz); src = hs + sl.elem; }
             CK(cudaMemcpyAsync(x->d_tok[slot].p, src, (size_t)nt * esz, cudaMemcpyHostToDevice, s_in));
         }
+        // output sizes: the rows, then (a turn that wants them) the new keys
+        const size_t nk_at = StageLayout::al((size_t)c * rows.row());
+        const size_t out_bytes = nnk > 0 ? nk_at + (size_t)nnk * 8 + 64 : (size_t)c * rows.row() + 64;
+        TurnArgs dt = {};                         // the chunk's turn on the device
+        if (T) {
+            const TurnArgs ht = sl.pack_turn(hs, t, i0, c);
+            int64_t* doff = x->d_off[slot].as<int64_t>();
+            dt = ht;
+            dt.tok_off = doff + (c + 1);
+            CK(cudaMemcpyAsync(doff + (c + 1), ht.tok_off, (size_t)(c + 1) * 8, cudaMemcpyHostToDevice, s_in));
+            if (NK) {
+                dt.new_off = doff + 2 * (c + 1);
+                CK(cudaMemcpyAsync(doff + 2 * (c + 1), ht.new_off, (size_t)(c + 1) * 8, cudaMemcpyHostToDevice, s_in));
+            }
+            dt.tok = reinterpret_cast<const uint32_t*>(x->d_tok[slot].as<uint8_t>() + tok2_at);
+            if (nt2 > 0) {
+                const uint32_t* src = ht.tok;
+                if (!tok2_pinned) { memcpy(hs + sl.elem2, src, (size_t)nt2 * 4); src = reinterpret_cast<const uint32_t*>(hs + sl.elem2); }
+                CK(cudaMemcpyAsync(const_cast<uint32_t*>(dt.tok), src, (size_t)nt2 * 4, cudaMemcpyHostToDevice, s_in));
+            }
+        }
         CK(cudaEventRecord(x->ev_h2d[slot], s_in));
         // kernel
-        CK(x->d_out[slot].need((size_t)c * rows.row() + 64));
-        if (!out_pinned) CK(x->h_out[slot].need((size_t)c * rows.row() + 64));
+        CK(x->d_out[slot].need(out_bytes));
+        if (!out_pinned || (nnk > 0 && !nk_pinned)) CK(x->h_out[slot].need(out_bytes));
+        if (NK) dt.new_keys = reinterpret_cast<uint64_t*>(x->d_out[slot].as<uint8_t>() + nk_at);
         rows.carve(x->d_out[slot].p, c, d);
         CK(cudaStreamWaitEvent(s_k, x->ev_h2d[slot], 0));
         int64_t maxb = 0;                         // the round pipelines' block count (tokens)
         if (!in.keys) for (int64_t q = i0; q < i1; ++q) maxb = std::max<int64_t>(maxb, (tok_off[q + 1] - tok_off[q]) / x->tv.block_size);
-        rc = launch_score(x, ScoreIn{x->d_tok[slot].p, in.keys}, d, s_k, maxb);
+        ScoreIn din{x->d_tok[slot].p, in.keys};
+        din.t = dt;
+        rc = launch_score(x, din, d, s_k, maxb);
         if (rc) return rc;
         CK(cudaEventRecord(x->ev_k[slot], s_k));
         // (slot reuse is safe without further stream waits: drain(slot) host-waits on ev_done[slot], which is
@@ -914,6 +1052,8 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
         } else {
             CK(cudaMemcpyAsync(x->h_out[slot].p, x->d_out[slot].p, (size_t)c * rows.row(), cudaMemcpyDeviceToHost, s_out));
         }
+        if (nnk > 0) CK(cudaMemcpyAsync(nk_pinned ? static_cast<void*>(t.new_keys + NK[i0]) : static_cast<void*>(x->h_out[slot].as<uint8_t>() + nk_at),
+                                        dt.new_keys, (size_t)nnk * 8, cudaMemcpyDeviceToHost, s_out));
         CK(cudaEventRecord(x->ev_done[slot], s_out));
         pend[slot].live = true; pend[slot].i0 = i0; pend[slot].cnt = c;
         slot ^= 1;
@@ -1204,7 +1344,7 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     if (const char* k = getenv("KVIDX_ROUNDS_OVERLAP_MIN")) x->rounds_overlap_min = atoll(k);
     if (const char* k = getenv("KVIDX_WRITE_PHASE1")) x->write_phase1 = atoi(k);
     x->queue = new_submit_queue();
-    if (rounds_init() || plain::rounds_init() || coop_init()) return fail(KVIDX_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (rounds_init() || plain::rounds_init() || coop_init() || turn_init()) return fail(KVIDX_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaGetLastError()));
     if (score_tuned_init()) return fail(KVIDX_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaGetLastError()));
     return 0;
 }
@@ -1262,7 +1402,7 @@ void kvidx_destroy(kvidx_t* x) {
         if (x->ev_k[i]) cudaEventDestroy(x->ev_k[i]);
     }
     x->r_act0.release(); x->r_act1.release(); x->r_cnt.release(); x->r_hstate.release(); x->r_keys.release(); x->r_pst.release(); x->r_nbr.release(); x->r_fp.release(); x->r_sort.release(); x->r_role.release(); x->r_hl.release(); x->r_map.release(); x->r_src.release(); x->r_fate.release(); x->r_anch.release(); x->r_snap.release(); x->r_rec.release(); x->r_scan.release();
-    x->d_misc.release(); x->d_rmisc.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
+    x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
     x->d_snap.release(); x->h_snap[0].release(); x->h_snap[1].release();
     for (auto& e : x->ev_snap) if (e) cudaEventDestroy(e);
@@ -1454,6 +1594,68 @@ int kvidx_score_keys_sparse_dev(kvidx_t* x, const uint64_t* d_keys, const int64_
                                 uint8_t* d_cnt_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0 || !d_key_off || !d_pods_out || !d_scores_out || !d_cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
     return score_dev(x, ScoreIn{d_keys, true}, ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr});
+}
+
+// ---- Score() for a conversation turn: held keys, then the new turn's tokens; not coalesced either ----
+
+namespace {
+// the host forms: check the token CSR, give the new keys' offsets (from 0), then the host-buffer pipeline
+int score_turn_host(kvidx* x, const uint64_t* keys, const int64_t* key_off, const uint32_t* tok, const int64_t* tok_off, const ScoreArgs& h,
+                    uint64_t* new_keys, int64_t* new_off) {
+    const int64_t n = h.n_prompts;
+    if (n < 0 || !key_off || !tok_off || (new_keys && !new_off)) return fail(KVIDX_EINVAL, "bad arguments");
+    if (n == 0) return 0;
+    int rc = check_csr(tok_off, n);
+    if (rc) return rc;
+    if (tok_off[n] > tok_off[0] && !tok) return fail(KVIDX_EINVAL, "NULL tokens");
+    if (new_off) {
+        const uint32_t B = x->tv.block_size;
+        new_off[0] = 0;
+        for (int64_t i = 0; i < n; ++i) new_off[i + 1] = new_off[i] + (tok_off[i + 1] - tok_off[i]) / B;
+    }
+    ScoreIn in{keys, true};
+    in.t = TurnArgs{nullptr, tok, tok_off, 0, new_keys, new_keys ? new_off : nullptr, 0};
+    return score_host(x, in, h);
+}
+ScoreIn turn_dev(const uint64_t* d_keys, const uint32_t* d_tok, const int64_t* d_tok_off, const int64_t* d_new_off, uint64_t* d_new_keys) {
+    ScoreIn in{d_keys, true};
+    in.t = TurnArgs{nullptr, d_tok, d_tok_off, 0, d_new_keys, d_new_off, 0};
+    return in;
+}
+}  // namespace
+
+int kvidx_score_turn(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, const uint32_t* tok, const int64_t* tok_off, int64_t n,
+                     const uint32_t* model, uint32_t model0, const uint64_t* filter, double* scores_out, uint8_t* has_keys_out,
+                     uint64_t* new_keys_out, int64_t* new_key_off_out) {
+    if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_turn_host(x, keys, key_off, tok, tok_off, ScoreArgs{nullptr, key_off, 0, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out, nullptr},
+                           new_keys_out, new_key_off_out);
+}
+
+int kvidx_score_turn_sparse(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, const uint32_t* tok, const int64_t* tok_off, int64_t n,
+                            const uint32_t* model, uint32_t model0, const uint64_t* filter, uint16_t* pods_out, double* scores_out,
+                            uint8_t* cnt_out, uint8_t* has_keys_out, uint64_t* new_keys_out, int64_t* new_key_off_out) {
+    if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_turn_host(x, keys, key_off, tok, tok_off, ScoreArgs{nullptr, key_off, 0, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out, nullptr},
+                           new_keys_out, new_key_off_out);
+}
+
+int kvidx_score_turn_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n,
+                         const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, double* d_scores_out, uint8_t* d_has_keys_out,
+                         const int64_t* d_new_key_off, uint64_t* d_new_keys_out) {
+    if (!x || n < 0 || !d_key_off || !d_tok_off || !d_scores_out || (d_new_keys_out && !d_new_key_off)) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_dev(x, turn_dev(d_keys, d_tok, d_tok_off, d_new_key_off, d_new_keys_out),
+                     ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, d_scores_out, nullptr, nullptr, nullptr, d_has_keys_out, nullptr});
+}
+
+int kvidx_score_turn_sparse_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, const uint32_t* d_tok, const int64_t* d_tok_off,
+                                int64_t n, const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, uint16_t* d_pods_out,
+                                double* d_scores_out, uint8_t* d_cnt_out, uint8_t* d_has_keys_out, const int64_t* d_new_key_off,
+                                uint64_t* d_new_keys_out) {
+    if (!x || n < 0 || !d_key_off || !d_tok_off || !d_pods_out || !d_scores_out || !d_cnt_out || (d_new_keys_out && !d_new_key_off))
+        return fail(KVIDX_EINVAL, "bad arguments");
+    return score_dev(x, turn_dev(d_keys, d_tok, d_tok_off, d_new_key_off, d_new_keys_out),
+                     ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr});
 }
 
 // ---- routed (all-to-all) form of the sharded Score(): the device steps around the exchange (kernels_route.cuh) ----

@@ -438,6 +438,58 @@ int kvhost_get_pod_scores_keys(kvhost_t* h, const uint64_t* keys, size_t n_keys,
     return pod_scores(h, nullptr, keys ? keys : &none, n_keys, model, pods, n_pods, pod_out, score_out);
 }
 
+int kvhost_get_pod_scores_turn(kvhost_t* h, const uint64_t* keys, size_t n_keys, const uint32_t* tokens, size_t n_tokens, const char* model,
+                               const char* const* pods, size_t n_pods, const char** pod_out, double* score_out, uint64_t* new_keys_out) {
+    if ((n_keys && !keys) || (n_tokens && !tokens)) return hfail(KVIDX_EINVAL, "NULL keys or tokens");
+    if (int rc = need_dev(h)) return rc;
+    std::shared_lock<std::shared_mutex> rl(h->read_mu);
+    std::vector<uint64_t> mask;
+    bool filtered; int mid;
+    { std::lock_guard<std::mutex> g(h->mu); filtered = build_filter(h, pods, n_pods, mask); mid = h->models.id(model, 65536); }
+    if (mid < 0) return hfail(KVIDX_ERANGE, "too many models");
+    const size_t nn = n_tokens / (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
+    static const uint64_t none = 0;
+    static const uint32_t none32 = 0;
+    const uint64_t* kp = keys ? keys : &none;
+    const uint32_t* tp = tokens ? tokens : &none32;
+    const int64_t koff[2] = {0, (int64_t)n_keys}, toff[2] = {0, (int64_t)n_tokens};
+    int64_t noff[2] = {0, 0};
+    std::vector<uint64_t> all(n_keys + std::max<size_t>(nn, 1));     // K = held ++ new keys
+    if (n_keys) memcpy(all.data(), keys, n_keys * 8);
+    uint64_t* nk = all.data() + n_keys;
+    const bool has_keys = n_keys + nn > 0;
+    auto give_keys = [&] { if (new_keys_out && nn) memcpy(new_keys_out, nk, nn * 8); };
+    if (filtered) {                                 // a filter whose pods all lie outside the mask width selects nothing
+        bool any = false; for (uint64_t w : mask) any |= w != 0;
+        if (!any) {
+            if (nn) {                               // the new keys are still the caller's
+                const uint64_t parent = n_keys ? keys[n_keys - 1] : 0;
+                const uint8_t pv = n_keys > 0;
+                if (kvidx_hash_keys(h->ix, tp, toff, 1, &parent, &pv, nk, noff)) { g_herr = kvidx_last_error(h->ix); return KVIDX_EINVAL; }
+            }
+            give_keys();
+            if (has_keys) observe_lookup(h, 0.0, true, nullptr, nullptr, 0);
+            return has_keys ? 0 : -1000;
+        }
+    }
+    uint16_t ids[KVIDX_MAX_PODS_PER_KEY]; double sc[KVIDX_MAX_PODS_PER_KEY]; uint8_t cnt = 0, has = 0;
+    const uint64_t* fm = filtered ? mask.data() : nullptr;
+    const int rc = kvidx_score_turn_sparse(h->ix, kp, koff, tp, toff, 1, nullptr, (uint32_t)mid, fm, ids, sc, &cnt, &has, nk, noff);
+    if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+    give_keys();
+    if (!has) return -1000;                         // (nil, nil): no key at all
+    if (h->cfg.enable_metrics) {                    // the instrumented Lookup of indexer.go:150: every key of K
+        const size_t n = n_keys + nn;
+        std::vector<kvidx_podtier_t> pt(n * KVIDX_MAX_PODS_PER_KEY); std::vector<uint8_t> kc(n);
+        const auto t0 = std::chrono::steady_clock::now();
+        const int r2 = kvidx_lookup(h->ix, (uint32_t)mid, all.data(), (int64_t)n, fm, pt.data(), kc.data());
+        observe_lookup(h, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), r2 == 0, pt.data(), kc.data(), n);
+    }
+    std::lock_guard<std::mutex> g(h->mu);
+    for (int i = 0; i < cnt; ++i) { pod_out[i] = h->pods.name(ids[i]); score_out[i] = sc[i]; }
+    return cnt;
+}
+
 static int entries_of(kvhost* h, const char* const* pods, const char* const* tiers, size_t n, std::vector<kvidx_podtier_t>& out) {
     out.clear();
     for (size_t i = 0; i < n; ++i) {

@@ -68,6 +68,11 @@ SYMBOLS = {
     "kvidx_score_keys_sparse": (C.c_int, [C.c_void_p, _u64p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _u16p, _f64p, _u8p, _u8p]),
     "kvidx_score_keys_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kvidx_score_keys_sparse_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "kvidx_score_turn": (C.c_int, [C.c_void_p, _u64p, _i64p, _u32p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _f64p, _u8p, _u64p, _i64p]),
+    "kvidx_score_turn_sparse": (C.c_int, [C.c_void_p, _u64p, _i64p, _u32p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _u16p, _f64p, _u8p, _u8p,
+                                          _u64p, _i64p]),
+    "kvidx_score_turn_dev": (C.c_int, [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_uint32] + [C.c_void_p] * 5),
+    "kvidx_score_turn_sparse_dev": (C.c_int, [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_uint32] + [C.c_void_p] * 7),
     "kvidx_add": (C.c_int, [C.c_void_p, C.c_uint32, _u64p, _u64p, C.c_int64, _u16p, C.c_int32]),
     "kvidx_evict": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, _u16p, C.c_int32]),
     "kvidx_get_request_key": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, _u64p]),
@@ -336,6 +341,58 @@ class Index:
     def score_keys_sparse_dev(self, d_keys, d_key_off, n, d_pods, d_scores, d_cnt, d_model=0, model0=0, d_filter=0, d_has_keys=0):
         self._ck(self.L.kvidx_score_keys_sparse_dev(self.h, d_keys or None, d_key_off, n, d_model or None, model0, d_filter or None,
                                                     d_pods, d_scores, d_cnt, d_has_keys or None))
+
+    # -- Score() for a conversation turn: prompt i is keys[key_off[i] .. key_off[i+1]) then tok[tok_off[i] .. tok_off[i+1]) --
+    def _turn_args(self, keys, key_off, tok, tok_off, model, filter_mask, want_keys):
+        keys = np.ascontiguousarray(keys, np.uint64) if not isinstance(keys, _Raw) else keys
+        tok = np.ascontiguousarray(tok, np.uint32) if not isinstance(tok, _Raw) else tok
+        key_off = np.ascontiguousarray(key_off, np.int64)
+        tok_off = np.ascontiguousarray(tok_off, np.int64)
+        n = len(key_off) - 1
+        nk = int(((tok_off[1:] - tok_off[:-1]) // self.block_size).sum()) if n > 0 else 0
+        new_keys = np.zeros(max(nk, 1), np.uint64) if want_keys else None
+        new_off = np.zeros(n + 1, np.int64)
+        model = None if model is None else np.ascontiguousarray(model, np.uint32)
+        filter_mask = None if filter_mask is None else np.ascontiguousarray(filter_mask, np.uint64)
+        kp = C.cast(keys.ptr, _u64p) if isinstance(keys, _Raw) else _p(keys, _u64p)
+        tp = C.cast(tok.ptr, _u32p) if isinstance(tok, _Raw) else _p(tok, _u32p)
+        return n, nk, kp, tp, key_off, tok_off, model, filter_mask, new_keys, new_off
+
+    def score_turn(self, keys, key_off, tok, tok_off, model=None, model0=0, filter_mask=None, want_keys=True, out=None):
+        """One conversation turn per prompt: held request keys, then new tokens.  -> (dense rows (n, max_pods), has_keys,
+        new keys (None when want_keys is False), their offsets).  keys / tok may be numpy arrays or _Raw pinned pointers."""
+        n, nk, kp, tp, key_off, tok_off, model, filter_mask, new_keys, new_off = self._turn_args(keys, key_off, tok, tok_off, model, filter_mask, want_keys)
+        scores = np.empty((n, self.max_pods), np.float64) if out is None else out
+        has = np.zeros(n, np.uint8)
+        self._ck(self.L.kvidx_score_turn(self.h, kp, _p(key_off, _i64p), tp, _p(tok_off, _i64p), n, _p(model, _u32p), model0,
+                                         _p(filter_mask, _u64p), _p(scores, _f64p), _p(has, _u8p), _p(new_keys, _u64p), _p(new_off, _i64p)))
+        return scores, has, None if new_keys is None else new_keys[:nk], new_off
+
+    def score_turn_sparse(self, keys, key_off, tok, tok_off, model=None, model0=0, filter_mask=None, want_keys=True, out=None):
+        """Sparse rows as score_keys_sparse -> (pods, scores, cnt, has, new keys, their offsets); out: optional preallocated
+        (pods, scores, cnt, has)."""
+        n, nk, kp, tp, key_off, tok_off, model, filter_mask, new_keys, new_off = self._turn_args(keys, key_off, tok, tok_off, model, filter_mask, want_keys)
+        if out is None:
+            pods, scores = np.zeros((n, E), np.uint16), np.zeros((n, E), np.float64)
+            cnt, has = np.zeros(n, np.uint8), np.zeros(n, np.uint8)
+        else:
+            pods, scores, cnt, has = out
+        self._ck(self.L.kvidx_score_turn_sparse(self.h, kp, _p(key_off, _i64p), tp, _p(tok_off, _i64p), n, _p(model, _u32p), model0,
+                                                _p(filter_mask, _u64p), _p(pods, _u16p), _p(scores, _f64p), _p(cnt, _u8p), _p(has, _u8p),
+                                                _p(new_keys, _u64p), _p(new_off, _i64p)))
+        return pods, scores, cnt, has, None if new_keys is None else new_keys[:nk], new_off
+
+    def score_turn_dev(self, d_keys, d_key_off, d_tok, d_tok_off, n, d_scores, d_model=0, model0=0, d_filter=0, d_has_keys=0,
+                       d_new_key_off=0, d_new_keys=0):
+        """All pointers are device addresses (ints); d_new_keys 0: the new keys are not wanted.  Asynchronous on the handle's stream."""
+        self._ck(self.L.kvidx_score_turn_dev(self.h, d_keys or None, d_key_off, d_tok or None, d_tok_off, n, d_model or None, model0,
+                                             d_filter or None, d_scores, d_has_keys or None, d_new_key_off or None, d_new_keys or None))
+
+    def score_turn_sparse_dev(self, d_keys, d_key_off, d_tok, d_tok_off, n, d_pods, d_scores, d_cnt, d_model=0, model0=0, d_filter=0,
+                              d_has_keys=0, d_new_key_off=0, d_new_keys=0):
+        self._ck(self.L.kvidx_score_turn_sparse_dev(self.h, d_keys or None, d_key_off, d_tok or None, d_tok_off, n, d_model or None, model0,
+                                                    d_filter or None, d_pods, d_scores, d_cnt, d_has_keys or None, d_new_key_off or None,
+                                                    d_new_keys or None))
 
     def hash_keys_dev(self, d_tok, d_tok_off, n, d_key_off, d_keys, d_parent=0, d_parent_valid=0):
         self._ck(self.L.kvidx_hash_keys_dev(self.h, d_tok, d_tok_off, n, d_parent or None, d_parent_valid or None, d_key_off, d_keys))

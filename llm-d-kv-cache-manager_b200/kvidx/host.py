@@ -46,6 +46,7 @@ SYMBOLS = {
     "kvhost_index": (C.c_void_p, [C.c_void_p]),
     "kvhost_get_pod_scores": (C.c_int, [C.c_void_p, _u32p, C.c_size_t, C.c_char_p, _cpp, C.c_size_t, _cpp, _f64p]),
     "kvhost_get_pod_scores_keys": (C.c_int, [C.c_void_p, _u64p, C.c_size_t, C.c_char_p, _cpp, C.c_size_t, _cpp, _f64p]),
+    "kvhost_get_pod_scores_turn": (C.c_int, [C.c_void_p, _u64p, C.c_size_t, _u32p, C.c_size_t, C.c_char_p, _cpp, C.c_size_t, _cpp, _f64p, _u64p]),
     "kvhost_index_add":(C.c_int, [C.c_void_p, C.c_char_p, _u64p, C.c_size_t, _u64p, C.c_size_t, _cpp, _cpp, C.c_size_t]),
     "kvhost_index_evict": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, _cpp, _cpp, C.c_size_t]),
     "kvhost_index_get_request_key": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, _u64p]),
@@ -90,6 +91,7 @@ class HostIndexer:
                  concurrency=4, device=0, no_device=False, lru_exact=0, enable_metrics=False, clear_on_all_blocks_cleared=False,
                  evict_policy="none"):
         self.L = _lib()
+        self.block_size = block_size
         cfg = HostConfig()
         self.L.kvhost_config_default(C.byref(cfg))
         cfg.index.block_size, cfg.index.capacity, cfg.index.pods_per_key = block_size, capacity, pods_per_key
@@ -143,6 +145,22 @@ class HostIndexer:
         if n < 0:
             raise _native.KvidxError(n, self.err())
         return {po[i].decode(): so[i] for i in range(n)}
+
+    def get_pod_scores_turn(self, keys, tokens, model, pods=()):
+        """GetPodScores for a conversation turn: the request keys held from earlier turns, then the new turn's tokens.
+        -> (dict pod -> score, or None when there are no keys at all; the new turn's keys, to hold for the next turn)."""
+        k = np.ascontiguousarray(keys, np.uint64)
+        tok = np.ascontiguousarray(tokens, np.uint32)
+        nk = np.zeros(max(len(tok) // self.block_size, 1), np.uint64)
+        po = (C.c_char_p * 10)(); so = (C.c_double * 10)()
+        n = self.L.kvhost_get_pod_scores_turn(self.h, k.ctypes.data_as(_u64p), len(k), tok.ctypes.data_as(_u32p), len(tok), model.encode(),
+                                              _strs(list(pods)), len(pods), po, so, nk.ctypes.data_as(_u64p))
+        new_keys = nk[:len(tok) // self.block_size]
+        if n == NO_KEYS:
+            return None, new_keys
+        if n < 0:
+            raise _native.KvidxError(n, self.err())
+        return {po[i].decode(): so[i] for i in range(n)}, new_keys
 
     def add(self, model, engine, request, entries):
         e = np.ascontiguousarray(engine, np.uint64); r = np.ascontiguousarray(request, np.uint64)

@@ -13,4 +13,6 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_shard_ops.py -x -q -m gpu -k "same-gpu-2 or guards or all_or_nothing or unsharded_handle or (round_trips and coop and same)"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_score_keys.py -x -q -m gpu -k "same_bits or arbitrary or host_buffers or errors"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_score_keys.py -x -q -m gpu -k "arbitrary and 257"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_score_turn.py -x -q -m gpu -k "identities or arbitrary or chain_edges or block_sizes or host_buffers or errors"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_score_turn.py -x -q -m gpu -k "chain_edges or (arbitrary and 257)"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_host_buffers.py -x -q -m gpu -k "model_filter or exact_lru"
