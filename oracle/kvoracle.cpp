@@ -97,6 +97,13 @@ public:
         if (out) *out = it->second->second;
         return true;
     }
+    bool peek(const K& k, V* out) {   // Peek: no refresh
+        std::lock_guard<std::mutex> g(mu_);
+        auto it = map_.find(k);
+        if (it == map_.end()) return false;
+        *out = it->second->second;
+        return true;
+    }
     bool contains_or_add(const K& k, const V& v) {   // no refresh on hit
         std::lock_guard<std::mutex> g(mu_);
         if (map_.count(k)) return true;
@@ -116,6 +123,10 @@ public:
     template <class F> void keys_oldest_first(F f) {   // Keys(): oldest -> newest
         std::lock_guard<std::mutex> g(mu_);
         for (auto it = list_.rbegin(); it != list_.rend(); ++it) f(it->first);
+    }
+    template <class F> void items_oldest_first(F f) {   // (key, value), oldest -> newest
+        std::lock_guard<std::mutex> g(mu_);
+        for (auto it = list_.rbegin(); it != list_.rend(); ++it) f(it->first, it->second);
     }
 private:
     size_t cap_;
@@ -341,6 +352,12 @@ int ko_get_request_key(void* h, uint32_t model, uint64_t engine, uint64_t* out) 
     if (!static_cast<Oracle*>(h)->engine_to_request.get(Key{model, engine}, &rk)) return KVIDX_ENOENT;
     *out = rk.hash; return 0;
 }
+// GetRequestKey without the recency refresh: what a BlockStored event's parent lookup would find now.
+int ko_peek_request_key(void* h, uint32_t model, uint64_t engine, uint64_t* out) {
+    Key rk{};
+    if (!static_cast<Oracle*>(h)->engine_to_request.peek(Key{model, engine}, &rk)) return KVIDX_ENOENT;
+    *out = rk.hash; return 0;
+}
 uint64_t ko_len_request(void* h) { return static_cast<Oracle*>(h)->data.len(); }
 uint64_t ko_len_engine(void* h) { return static_cast<Oracle*>(h)->engine_to_request.len(); }
 
@@ -411,6 +428,60 @@ int ko_apply_events(void* h, const kvidx_event_t* ev, int64_t n, const uint64_t*
     for (int64_t i = 0; i < n; ++i) if (!o->apply_event(ev[i], hashes, tokens)) ++dropped;
     if (n_dropped) *n_dropped = dropped;
     return 0;
+}
+
+// The v1 index image (include/kvidx.h) of the oracle's contents: request records sorted by (model, hash) with their
+// entries oldest -> newest, engine records sorted by (model, engine hash), stale mappings included.  With recency, one
+// u64 per record: its 1-based position in its LRU (oldest = 1).  Returns the image size; writes nothing unless
+// cap >= size.  Refreshes no recency.
+int64_t ko_snapshot(void* h, int recency, uint8_t* buf, uint64_t cap) {
+    auto* o = static_cast<Oracle*>(h);
+    struct Req { uint32_t model; uint64_t hash; std::vector<uint16_t> ent; uint64_t rank; };
+    struct Eng { uint32_t model; uint64_t hash, request; uint64_t rank; };
+    std::vector<Req> reqs;
+    std::vector<Eng> engs;
+    o->data.items_oldest_first([&](const Key& k, const PodCachePtr& pc) {
+        Req r{k.model, k.hash, {}, reqs.size() + 1};
+        pc->cache.keys_oldest_first([&](uint16_t e) { r.ent.push_back(e); });
+        reqs.push_back(std::move(r));
+    });
+    o->engine_to_request.items_oldest_first([&](const Key& ek, const Key& rk) {
+        engs.push_back(Eng{ek.model, ek.hash, rk.hash, engs.size() + 1});
+    });
+    std::sort(reqs.begin(), reqs.end(), [](const Req& a, const Req& b) { return a.model != b.model ? a.model < b.model : a.hash < b.hash; });
+    std::sort(engs.begin(), engs.end(), [](const Eng& a, const Eng& b) { return a.model != b.model ? a.model < b.model : a.hash < b.hash; });
+    uint32_t pod_span = 0, model_span = 0;
+    for (const Req& r : reqs) {
+        model_span = std::max(model_span, r.model + 1);
+        for (uint16_t e : r.ent) pod_span = std::max<uint32_t>(pod_span, KVIDX_PT_POD(e) + 1u);
+    }
+    for (const Eng& e : engs) model_span = std::max(model_span, e.model + 1);
+    const uint64_t R = reqs.size(), E = engs.size();
+    const uint64_t size = 64 + 32 * R + 24 * E + (recency ? 8 * (R + E) : 0);
+    if (!buf || cap < size) return (int64_t)size;
+    std::memset(buf, 0, size);
+    auto put = [&](uint64_t off, const void* p, size_t n) { std::memcpy(buf + off, p, n); };
+    const uint32_t version = 1, flags = recency ? 1u : 0u, bs = o->block_size, ppk = (uint32_t)o->pod_cache_size;
+    put(0, "KVIDXSNP", 8); put(8, &version, 4); put(12, &flags, 4); put(16, &bs, 4); put(20, &ppk, 4);
+    put(24, &o->init_hash, 8); put(32, &R, 8); put(40, &E, 8); put(48, &pod_span, 4); put(52, &model_span, 4);
+    uint64_t off = 64;
+    for (const Req& r : reqs) {
+        const uint16_t model = (uint16_t)r.model;
+        const uint8_t cnt = (uint8_t)r.ent.size();
+        put(off, &r.hash, 8); put(off + 8, &model, 2); put(off + 10, &cnt, 1);
+        for (size_t j = 0; j < r.ent.size() && j < KVIDX_MAX_PODS_PER_KEY; ++j) put(off + 12 + 2 * j, &r.ent[j], 2);
+        off += 32;
+    }
+    for (const Eng& e : engs) {
+        const uint16_t model = (uint16_t)e.model;
+        put(off, &e.hash, 8); put(off + 8, &e.request, 8); put(off + 16, &model, 2);
+        off += 24;
+    }
+    if (recency) {
+        for (const Req& r : reqs) { put(off, &r.rank, 8); off += 8; }
+        for (const Eng& e : engs) { put(off, &e.rank, 8); off += 8; }
+    }
+    return (int64_t)size;
 }
 
 }  // extern "C"

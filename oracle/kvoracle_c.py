@@ -73,6 +73,9 @@ def lib():
                                      C.POINTER(C.c_double), C.POINTER(C.c_uint8), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
         L.ko_apply_events.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32),
                                       C.POINTER(C.c_int64)]
+        L.ko_peek_request_key.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64, C.POINTER(C.c_uint64)]
+        L.ko_snapshot.restype = C.c_int64
+        L.ko_snapshot.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64]
         _lib = L
     return _lib
 
@@ -134,6 +137,12 @@ class COracle:
         rc = self.L.ko_get_request_key(self.h, model, int(engine), C.byref(out))
         return rc, out.value
 
+    def peek_request_key(self, model, engine):
+        """get_request_key without refreshing the mapping's recency: -> request key, or None on a miss."""
+        out = C.c_uint64(0)
+        rc = self.L.ko_peek_request_key(self.h, model, int(engine), C.byref(out))
+        return out.value if rc == 0 else None
+
     def lookup(self, model, keys, filter_mask=None):
         keys = np.ascontiguousarray(keys, np.uint64)
         n = len(keys)
@@ -173,6 +182,14 @@ class COracle:
         rc = self.L.ko_apply_events(self.h, events.ctypes.data_as(C.c_void_p), len(events), _ptr(hashes, C.c_uint64),
                                     _ptr(tokens, C.c_uint32), C.byref(nd))
         return rc, nd.value
+
+    def snapshot(self, recency=False) -> bytes:
+        """The v1 index image (include/kvidx.h) of the oracle's contents, as kvidx_snapshot writes it.  With recency, each
+        record's value is its 1-based position in its LRU (oldest = 1): compare a library image's by rank."""
+        size = self.L.ko_snapshot(self.h, int(recency), None, 0)
+        buf = (C.c_uint8 * size)()
+        assert self.L.ko_snapshot(self.h, int(recency), buf, size) == size
+        return bytes(buf)
 
     def len_request(self):
         return self.L.ko_len_request(self.h)
