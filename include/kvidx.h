@@ -443,6 +443,37 @@ int kvidx_get_evictions(kvidx_t* idx, uint64_t out[2]);
  * for a write batch in flight: they report the batches completed so far. */
 int kvidx_get_sweeps(kvidx_t* idx, uint64_t out[2]);
 
+/* Pod inventory (no reference counterpart): what the index attributes to each pod, counted by one sweep of the request
+ * table on the device, and -- with KVIDX_INVENTORY_ENGINE -- a second one of the engine table that makes it an exact dry
+ * run of kvidx_remove_pods.  Over the resident request keys k of `model` (a 16-bit id, or KVIDX_ANY_MODEL for all), with
+ * E(k) the key's (pod, tier) entries:
+ *   entries_out[pod * 16 + tier]  keys with (pod, tier) in E(k)                              max_pods * KVIDX_MAX_TIERS u64
+ *   keys_out[pod]                 keys with an entry of the pod on any tier (two tiers of one key count once)   max_pods u64
+ *   sole_out[pod]                 keys all of whose entries belong to the pod                                    max_pods u64
+ *   sole_engine_out[pod]          engine mappings (of `model`) whose request key is resident and counted in sole_out[pod];
+ *                                 all zero without KVIDX_INVENTORY_ENGINE                                        max_pods u64
+ *   totals_out                    {request keys, entries, engine mappings, stale engine mappings}; a mapping is stale when
+ *                                 no resident request key (model, request hash) exists (Evict cleans those up lazily,
+ *                                 in_memory.go:225-230; removal, snapshot and restore keep them, and they count against
+ *                                 `capacity`).  The last two are zero without KVIDX_INVENTORY_ENGINE.
+ * Any output may be NULL.  With KVIDX_ANY_MODEL, kvidx_remove_pods of the single pod p (all tiers) called right after it
+ * returns removed_out = {sum over t of entries_out[p * 16 + t], sole_out[p], sole_engine_out[p]}, and totals_out[0] /
+ * totals_out[2] equal kvidx_get_stats' request_keys / engine_keys.
+ * A READER: it writes no slot, refreshes no recency stamp and sets no CLOCK reference bit, so taking an inventory never
+ * changes what a later eviction picks.  It takes the locks of a read call (not the write side, except on an exact-LRU
+ * handle, where every read call does), so writers and other readers keep running.  Ordered after every write call that has
+ * returned and after the kvidx_apply_events_dev batches issued before it; synchronous.  With no writer running the counts
+ * are exact; beside a writer every key is counted before or after each individual Add / Evict of that key.  Works in all
+ * three capacity modes.  On a sharded handle it reports the request keys and engine mappings THIS rank owns (a mapping's
+ * request key is probed on whichever rank owns it), needs no phases and no barrier, and the results of all ranks sum to
+ * the unsharded answer (kvidx.dist.pod_inventory_shards).
+ * All outputs NULL, or a flag other than KVIDX_INVENTORY_ENGINE -> KVIDX_EINVAL; model neither KVIDX_ANY_MODEL nor
+ * <= 65535 -> KVIDX_ERANGE. */
+#define KVIDX_ANY_MODEL        0xFFFFFFFFu
+#define KVIDX_INVENTORY_ENGINE 1u
+int kvidx_pod_inventory(kvidx_t* idx, uint32_t model, uint32_t flags, uint64_t* entries_out, uint64_t* keys_out,
+                        uint64_t* sole_out, uint64_t* sole_engine_out, uint64_t totals_out[4]);
+
 #ifdef __cplusplus
 }
 #endif

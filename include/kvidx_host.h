@@ -15,6 +15,7 @@
  *   kvhost_decode_event_batch<-> processEvent's msgpack decoding      pkg/kvcache/kvevents/pool.go:177-244, events.go:38-96
  *   kvhost_remove_pod        <-> (no counterpart) drop a departed pod's entries and free its id (kvidx_remove_pods)
  *   kvhost_snapshot / _restore <-> (no counterpart) names + index image, warm start of a fresh mirror (kvidx_snapshot)
+ *   kvhost_pod_inventory / kvhost_inventory_text <-> (no counterpart) what each pod holds, by name (kvidx_pod_inventory)
  *   kvhost_prefix_store_*    <-> prefixstore.LRUTokenStore            pkg/tokenization/prefixstore/lru_store.go:54-190
  *   kvhost_get_metrics / _text <-> InstrumentedIndex + collectors      pkg/kvcache/kvblock/instrumented_index.go:30-92, metrics/collector.go:28-59
  */
@@ -163,6 +164,31 @@ int kvhost_remove_pod(kvhost_t* h, const char* pod, const char* const* tiers, si
  * goes through kvidx_restore and its error codes; on any error the target is left as it was. */
 int kvhost_snapshot(kvhost_t* h, void* buf, uint64_t cap, uint64_t* size_out);
 int kvhost_restore(kvhost_t* h, const void* buf, uint64_t len);
+
+/* Pod inventory with names (no counterpart; kvidx_pod_inventory): for every interned pod its name and id, the request keys
+ * it holds, those it alone holds (what kvhost_remove_pod of it would remove), with `engine` != 0 the engine mappings that
+ * would go with them, and its entries per tier id.  model: a model name, or NULL for all models; a name never seen counts
+ * nothing (it is not interned).  Pod ids freed by kvhost_remove_pod are skipped.  tier_names_out (may be NULL): the name of
+ * every interned tier id, NULL for the others; name pointers stay valid for the life of the handle.  totals_out (may be
+ * NULL): {request keys, entries, engine mappings, stale engine mappings}, the last two only with `engine`.
+ * Writes at most `cap` rows, in pod id order, and returns the number of interned pods (call again with more room if it
+ * exceeds cap), or a negative KVIDX_E* code.  Serialised with kvhost_remove_pod and kvhost_restore (it holds the write side
+ * shared), so ids and names agree; read calls, index_add / index_evict and kvhost_pool_process keep running, and a pod
+ * interned while the device counts is reported with whatever the device saw of it.  A no_device instance answers with
+ * all-zero counts. */
+typedef struct kvhost_pod_row {
+    const char* pod;
+    uint32_t pod_id, reserved;
+    uint64_t keys, sole_keys, sole_engine_keys;
+    uint64_t entries[KVIDX_MAX_TIERS];           /* by tier id */
+} kvhost_pod_row_t;
+int64_t kvhost_pod_inventory(kvhost_t* h, const char* model, int32_t engine, kvhost_pod_row_t* rows, size_t cap,
+                             const char** tier_names_out /* KVIDX_MAX_TIERS */, uint64_t totals_out[4]);
+/* The inventory over all models, engine pass included, in Prometheus text format, apart from kvhost_metrics_text (whose
+ * output is the reference's metric set): gauges kvcache_index_pod_entries{pod,tier} (non-zero ones),
+ * kvcache_index_pod_keys{pod}, kvcache_index_pod_sole_keys{pod}, kvcache_index_pod_sole_engine_keys{pod},
+ * kvcache_index_stale_engine_keys.  Buffer conventions of kvhost_metrics_text; a negative KVIDX_E* code on failure. */
+int64_t kvhost_inventory_text(kvhost_t* h, char* buf, size_t cap);
 
 /* interning introspection.  Model and tier ids are never reused; a pod id is freed by kvhost_remove_pod (all tiers) and
  * reused lowest first.  Name pointers returned by the calls above stay valid for the life of the handle. */

@@ -22,6 +22,7 @@
 #include "kernels_clock.cuh"
 #include "kernels_remove.cuh"
 #include "kernels_snapshot.cuh"
+#include "kernels_inventory.cuh"
 #include "kernels_score.cuh"
 #include "kernels_rounds.cuh"
 #include "kernels_rounds_plain.cuh"
@@ -138,6 +139,7 @@ struct kvidx {
     DevBuf d_tok[2], d_off[2], d_model[2], d_filter[2], d_out[2], d_aux[2], d_rmisc;
     PinBuf h_stage[2], h_out[2];
     DevBuf d_turn;                  // a conversation turn on the composed path: the concatenated key CSR and its setup
+    DevBuf d_inv; PinBuf h_inv;     // kvidx_pod_inventory: the 64-bit histograms on the device and their pinned copy
     // write-side scratch (guarded by mu_w)
     DevBuf d_misc, d_ev, d_hash, d_evtok, d_qoff, d_wkeys, d_wpred, d_wready, d_wmap;
     DevBuf d_sweep;                 // CLOCK sweep scratch: bitmap image, per-tile counts, control block
@@ -1402,7 +1404,7 @@ void kvidx_destroy(kvidx_t* x) {
         if (x->ev_k[i]) cudaEventDestroy(x->ev_k[i]);
     }
     x->r_act0.release(); x->r_act1.release(); x->r_cnt.release(); x->r_hstate.release(); x->r_keys.release(); x->r_pst.release(); x->r_nbr.release(); x->r_fp.release(); x->r_sort.release(); x->r_role.release(); x->r_hl.release(); x->r_map.release(); x->r_src.release(); x->r_fate.release(); x->r_anch.release(); x->r_snap.release(); x->r_rec.release(); x->r_scan.release();
-    x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
+    x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_inv.release(); x->h_inv.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
     x->d_snap.release(); x->h_snap[0].release(); x->h_snap[1].release();
     for (auto& e : x->ev_snap) if (e) cudaEventDestroy(e);
@@ -2561,6 +2563,40 @@ int kvidx_get_stats(kvidx_t* x, kvidx_stats_t* out) {
     out->request_slots = x->tv.req_mask + 1; out->engine_slots = x->tv.eng_mask + 1;
     out->rebuilds = x->rebuilds; out->kernel_launches = x->launches.load();
     out->rehashed_events = x->h_cnt->rehashed; out->coalesced_calls = x->queue ? submit_queue_coalesced(x->queue) : 0;
+    return 0;
+}
+
+// What each pod holds (kernels_inventory.cuh).  A read call: the read side's locks, stream and scratch.
+//   d_inv: entries[P * 16] | keys[P] | sole[P] | sole_engine[P] | totals[4], all u64, zeroed by every call
+int kvidx_pod_inventory(kvidx_t* x, uint32_t model, uint32_t flags, uint64_t* entries_out, uint64_t* keys_out, uint64_t* sole_out,
+                        uint64_t* sole_engine_out, uint64_t totals_out[4]) {
+    if (!x) return fail(KVIDX_EINVAL, "NULL handle");
+    if (!entries_out && !keys_out && !sole_out && !sole_engine_out && !totals_out) return fail(KVIDX_EINVAL, "every output is NULL");
+    if (flags & ~KVIDX_INVENTORY_ENGINE) return fail(KVIDX_EINVAL, "unknown inventory flags 0x%x", flags);
+    if (model != KVIDX_ANY_MODEL && model > 0xffffu) return fail(KVIDX_ERANGE, "model id %u > 65535", model);
+    ReadGuard g(x);
+    CK(cudaSetDevice(x->device));
+    if (int rc0 = check_shards(x)) return rc0;
+    const size_t P = x->tv.max_pods, n_ent = P * KVIDX_MAX_TIERS, words = n_ent + 3 * P + 4;
+    CK(x->d_inv.need(words * 8));
+    CK(x->h_inv.need(words * 8));
+    unsigned long long* d = x->d_inv.as<unsigned long long>();
+    InvArgs ia{model, d, d + n_ent, d + n_ent + P, d + n_ent + 2 * P, d + n_ent + 3 * P};
+    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
+    CK(cudaMemsetAsync(d, 0, words * 8, x->stream));
+    auto ctas = [&](uint64_t slots) { return (unsigned)std::min<uint64_t>((slots + kInvThreads - 1) / kInvThreads, (uint64_t)x->sm_count * 8); };
+    inventory_req_kernel<<<ctas(x->tv.req_mask + 1), kInvThreads, inv_req_smem(x->tv.max_pods), x->stream>>>(x->tv, ia);
+    if (flags & KVIDX_INVENTORY_ENGINE) inventory_eng_kernel<<<ctas(x->tv.eng_mask + 1), kInvThreads, P * 4, x->stream>>>(x->tv, ia);
+    x->launches += (flags & KVIDX_INVENTORY_ENGINE) ? 2 : 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(x->h_inv.p, d, words * 8, cudaMemcpyDeviceToHost, x->stream));
+    CK(cudaStreamSynchronize(x->stream));
+    const uint64_t* h = x->h_inv.as<uint64_t>();
+    if (entries_out) memcpy(entries_out, h, n_ent * 8);
+    if (keys_out) memcpy(keys_out, h + n_ent, P * 8);
+    if (sole_out) memcpy(sole_out, h + n_ent + P, P * 8);
+    if (sole_engine_out) memcpy(sole_engine_out, h + n_ent + 2 * P, P * 8);
+    if (totals_out) memcpy(totals_out, h + n_ent + 3 * P, 4 * 8);
     return 0;
 }
 

@@ -817,6 +817,78 @@ int kvhost_restore(kvhost_t* h, const void* buf, uint64_t len) {
     return 0;
 }
 
+int64_t kvhost_pod_inventory(kvhost_t* h, const char* model, int32_t engine, kvhost_pod_row_t* rows, size_t cap, const char** tier_names_out,
+                             uint64_t totals_out[4]) {
+    if (!h || (cap && !rows)) return hfail(KVIDX_EINVAL, "bad arguments");
+    std::shared_lock<std::shared_mutex> wl(h->write_mu);     // no kvhost_remove_pod / kvhost_restore meanwhile: no id changes its name
+    const size_t P = h->pod_cap;
+    std::vector<uint64_t> ent(P * KVIDX_MAX_TIERS, 0), keys(P, 0), sole(P, 0), sole_eng(P, 0);
+    uint64_t totals[4] = {0, 0, 0, 0};
+    int mid = -1;
+    if (model) { std::lock_guard<std::mutex> g(h->mu); mid = h->models.find(model); }
+    if (h->ix && (!model || mid >= 0)) {
+        const int rc = kvidx_pod_inventory(h->ix, model ? (uint32_t)mid : KVIDX_ANY_MODEL, engine ? KVIDX_INVENTORY_ENGINE : 0u, ent.data(),
+                                           keys.data(), sole.data(), sole_eng.data(), totals);
+        if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+    }
+    // names after the counts: a writer interns a pod before it writes the pod's entries, so every id the device saw has its name
+    std::lock_guard<std::mutex> g(h->mu);
+    size_t n = 0;
+    for (uint32_t id = 0; id < h->pods.names.size(); ++id) {
+        if (!h->pods.names[id]) continue;                        // freed by kvhost_remove_pod
+        if (n < cap) {
+            kvhost_pod_row_t& r = rows[n];
+            r = kvhost_pod_row_t{};
+            r.pod = h->pods.name(id); r.pod_id = id;
+            if (id < P) {                                        // ids from pod_cap up (filter-only names) own no entries
+                r.keys = keys[id]; r.sole_keys = sole[id]; r.sole_engine_keys = sole_eng[id];
+                memcpy(r.entries, &ent[(size_t)id * KVIDX_MAX_TIERS], sizeof r.entries);
+            }
+        }
+        ++n;
+    }
+    if (tier_names_out)
+        for (uint32_t t = 0; t < KVIDX_MAX_TIERS; ++t) tier_names_out[t] = t < h->tiers.names.size() ? h->tiers.name(t) : nullptr;
+    if (totals_out) memcpy(totals_out, totals, sizeof totals);
+    return (int64_t)n;
+}
+
+int64_t kvhost_inventory_text(kvhost_t* h, char* buf, size_t cap) {
+    if (!h) return hfail(KVIDX_EINVAL, "bad arguments");
+    std::vector<kvhost_pod_row_t> rows(KVIDX_MAX_PODS);
+    const char* tier[KVIDX_MAX_TIERS];
+    uint64_t totals[4];
+    const int64_t n = kvhost_pod_inventory(h, nullptr, 1, rows.data(), rows.size(), tier, totals);
+    if (n < 0) return n;
+    auto label = [](const char* v) {                             // label value escaping of the text format
+        std::string o;
+        for (; *v; ++v) { if (*v == '\\' || *v == '"') o += '\\'; if (*v == '\n') { o += "\\n"; continue; } o += *v; }
+        return o;
+    };
+    std::string s;
+    auto gauge = [&](const char* name, const char* help) {
+        s += "# HELP kvcache_index_"; s += name; s += " "; s += help; s += "\n# TYPE kvcache_index_"; s += name; s += " gauge\n";
+    };
+    gauge("pod_entries", "Request keys the index holds for a pod on a device tier");
+    for (int64_t i = 0; i < n; ++i)
+        for (uint32_t t = 0; t < KVIDX_MAX_TIERS; ++t)
+            if (rows[i].entries[t])
+                s += "kvcache_index_pod_entries{pod=\"" + label(rows[i].pod) + "\",tier=\"" + (tier[t] ? label(tier[t]) : std::to_string(t)) + "\"} " +
+                     std::to_string(rows[i].entries[t]) + "\n";
+    auto per_pod = [&](const char* name, const char* help, uint64_t kvhost_pod_row_t::*field) {
+        gauge(name, help);
+        for (int64_t i = 0; i < n; ++i)
+            s += std::string("kvcache_index_") + name + "{pod=\"" + label(rows[i].pod) + "\"} " + std::to_string(rows[i].*field) + "\n";
+    };
+    per_pod("pod_keys", "Request keys with an entry of the pod on any tier", &kvhost_pod_row_t::keys);
+    per_pod("pod_sole_keys", "Request keys held by the pod alone (removed with it)", &kvhost_pod_row_t::sole_keys);
+    per_pod("pod_sole_engine_keys", "Engine-key mappings of the request keys held by the pod alone", &kvhost_pod_row_t::sole_engine_keys);
+    gauge("stale_engine_keys", "Engine-key mappings whose request key is not resident");
+    s += "kvcache_index_stale_engine_keys " + std::to_string(totals[3]) + "\n";
+    if (buf && cap) { const size_t m = std::min(cap - 1, s.size()); memcpy(buf, s.data(), m); buf[m] = 0; }
+    return (int64_t)s.size();
+}
+
 int64_t kvhost_decode_event_batch(kvhost_t* h, const char* pod, const char* model, const void* payload, size_t len, kvidx_event_t* ev_out,
                                   size_t ev_cap, uint64_t* hash_out, size_t hash_cap, size_t* n_hash_out, uint32_t* tok_out, size_t tok_cap,
                                   size_t* n_tok_out) {

@@ -20,6 +20,7 @@ SCORE_ABSENT = -1.0
 OK, ENOENT, ECUDA, ENOMEM, EINVAL, ENOSPC, ERANGE = 0, -2, -5, -12, -22, -28, -34
 EV_BLOCK_STORED, EV_BLOCK_REMOVED = 0, 1
 EVICT_NONE, EVICT_CLOCK = 0, 1
+ANY_MODEL, INVENTORY_ENGINE = 0xFFFFFFFF, 1
 _EVICT_POLICIES = {"none": EVICT_NONE, "clock": EVICT_CLOCK}
 
 
@@ -93,6 +94,7 @@ SYMBOLS = {
     "kvidx_get_stats": (C.c_int, [C.c_void_p, C.POINTER(Stats)]),
     "kvidx_get_evictions": (C.c_int, [C.c_void_p, _u64p]),
     "kvidx_get_sweeps": (C.c_int, [C.c_void_p, _u64p]),
+    "kvidx_pod_inventory": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, _u64p, _u64p, _u64p, _u64p, _u64p]),
     "kvidx_shard_export": (C.c_int, [C.c_void_p, C.c_char_p]),
     "kvidx_shard_import": (C.c_int, [C.c_void_p, C.c_uint32, C.c_char_p]),
     "kvidx_shard_attach": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
@@ -215,6 +217,19 @@ class Index:
         out = np.zeros(2, np.uint64)
         self._ck(self.L.kvidx_get_sweeps(self.h, _p(out, _u64p)))
         return int(out[0]), int(out[1])
+
+    def pod_inventory(self, model=None, engine=False) -> dict:
+        """kvidx_pod_inventory: what each pod holds, counted on the device without touching recency.  model None = all models.
+        -> {"entries" (max_pods, 16), "keys", "sole" (max_pods,), "sole_engine" (max_pods,) or None without `engine`,
+        "totals" [request keys, entries, engine mappings, stale engine mappings] (the last two only with `engine`)}, uint64.
+        remove_pods([p]) right after an all-model inventory removes entries[p].sum() entries, sole[p] request keys and
+        sole_engine[p] engine keys.  On a sharded handle: this rank's share (kvidx.dist.pod_inventory_shards sums them)."""
+        ent = np.zeros((self.max_pods, MAX_TIERS), np.uint64)
+        keys, sole, totals = np.zeros(self.max_pods, np.uint64), np.zeros(self.max_pods, np.uint64), np.zeros(4, np.uint64)
+        sole_eng = np.zeros(self.max_pods, np.uint64) if engine else None
+        self._ck(self.L.kvidx_pod_inventory(self.h, ANY_MODEL if model is None else int(model), INVENTORY_ENGINE if engine else 0,
+                                            _p(ent, _u64p), _p(keys, _u64p), _p(sole, _u64p), _p(sole_eng, _u64p), _p(totals, _u64p)))
+        return {"entries": ent, "keys": keys, "sole": sole, "sole_engine": sole_eng, "totals": totals}
 
     # -- hash-range sharding (one handle per GPU) --
     SHARD_HANDLE_BYTES = 192

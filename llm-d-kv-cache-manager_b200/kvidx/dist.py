@@ -5,7 +5,8 @@ scores its own contiguous slice of the batch, and no data-path collective is nee
 the write path: every rank must apply the same KV events, in the same per-pod order.  `broadcast_event_batch` does
 that from the ingesting rank; `shard_range` splits a batch; `max_over_ranks` is the timing reduction bench.py uses.
 The hash-range sharded mode has its own helpers: `connect_shards`, and the collective maintenance calls
-`compact_shards`, `remove_pods_shards`, `snapshot_shards` and `restore_shards`, which put the barriers around them.
+`compact_shards`, `remove_pods_shards`, `snapshot_shards` and `restore_shards`, which put the barriers around them,
+and `pod_inventory_shards`, a read that needs none.
 """
 from __future__ import annotations
 
@@ -259,3 +260,20 @@ def restore_shards(ix, image=None, src: int = 0, device=None) -> dict:
     got = _collective_step(lambda: ix.shard_restore(image), "the shard restore", device)
     tot = _sum_over_ranks([got["request_keys"], got["engine_keys"]], device)
     return {"request_keys": tot[0], "engine_keys": tot[1]}
+
+
+def pod_inventory_shards(ix, model=None, engine=False, device=None) -> dict:
+    """kvidx_pod_inventory over a hash-range sharded index: every rank counts the request keys and engine mappings it owns
+    and the arrays are summed with one all-reduce, so every rank gets the answer an unsharded index with the same contents
+    gives.  A read: writers may run, and nothing but the all-reduce keeps the ranks together."""
+    inv = ix.pod_inventory(model, engine)
+    names = [k for k in ("entries", "keys", "sole", "sole_engine", "totals") if inv[k] is not None]
+    flat = torch.from_numpy(np.concatenate([inv[k].reshape(-1) for k in names]).view(np.int64).copy())
+    if device is not None:
+        flat = flat.to(device)
+    dist.all_reduce(flat)
+    flat, out, at = flat.cpu().numpy().view(np.uint64), dict(inv), 0
+    for k in names:
+        out[k] = flat[at:at + inv[k].size].reshape(inv[k].shape).copy()
+        at += inv[k].size
+    return out

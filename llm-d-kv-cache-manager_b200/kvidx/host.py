@@ -28,6 +28,12 @@ class HostMetrics(C.Structure):
                 ("lookup_latency_count", C.c_uint64), ("lookup_latency_sum", C.c_double)]
 
 
+class PodRow(C.Structure):
+    """kvhost_pod_row_t."""
+    _fields_ = [("pod", C.c_char_p), ("pod_id", C.c_uint32), ("reserved", C.c_uint32), ("keys", C.c_uint64), ("sole_keys", C.c_uint64),
+                ("sole_engine_keys", C.c_uint64), ("entries", C.c_uint64 * MAX_TIERS)]
+
+
 _cpp = C.POINTER(C.c_char_p)
 _u64p, _u32p, _u8p, _f64p = C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint8), C.POINTER(C.c_double)
 SYMBOLS = {
@@ -57,6 +63,8 @@ SYMBOLS = {
     "kvhost_remove_pod": (C.c_int, [C.c_void_p, C.c_char_p, _cpp, C.c_size_t]),
     "kvhost_snapshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
     "kvhost_restore": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64]),
+    "kvhost_pod_inventory": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_int32, C.POINTER(PodRow), C.c_size_t, _cpp, _u64p]),
+    "kvhost_inventory_text": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_size_t]),
     "kvhost_decode_event_batch": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, _u64p, C.c_size_t,
                                               C.POINTER(C.c_size_t), _u32p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "kvhost_pod_id": (C.c_int, [C.c_void_p, C.c_char_p]),
@@ -238,6 +246,33 @@ class HostIndexer:
         rc = self.L.kvhost_restore(self.h, image, len(image))
         if rc:
             raise _native.KvidxError(rc, self.err())
+
+    def pod_inventory(self, model=None, engine=False, totals=False):
+        """kvhost_pod_inventory: {pod name: {"id", "keys", "sole_keys", "sole_engine_keys" (None without `engine`), "entries":
+        {tier name: count, non-zero tiers only}}} for every interned pod; model None = all models.  With `totals`, a pair of
+        that and [request keys, entries, engine mappings, stale engine mappings] (the last two only with `engine`)."""
+        cap = 256
+        while True:
+            rows, tiers, tot = (PodRow * cap)(), (C.c_char_p * MAX_TIERS)(), (C.c_uint64 * 4)()
+            n = self.L.kvhost_pod_inventory(self.h, None if model is None else model.encode(), 1 if engine else 0, rows, cap, tiers, tot)
+            if n < 0:
+                raise _native.KvidxError(int(n), self.err())
+            if n <= cap:
+                break
+            cap = int(n)
+        pods = {r.pod.decode(): {"id": r.pod_id, "keys": r.keys, "sole_keys": r.sole_keys, "sole_engine_keys": r.sole_engine_keys if engine else None,
+                                 "entries": {(tiers[t].decode() if tiers[t] is not None else str(t)): r.entries[t]
+                                             for t in range(MAX_TIERS) if r.entries[t]}} for r in rows[:n]}
+        return (pods, [int(v) for v in tot]) if totals else pods
+
+    def inventory_text(self) -> str:
+        """kvhost_inventory_text: the all-model inventory as Prometheus gauges (kvcache_index_pod_* and stale_engine_keys)."""
+        n = self.L.kvhost_inventory_text(self.h, None, 0)
+        if n < 0:
+            raise _native.KvidxError(int(n), self.err())
+        buf = C.create_string_buffer(int(n) + 4096)          # pods may join between the two calls
+        self.L.kvhost_inventory_text(self.h, buf, len(buf))
+        return buf.value.decode()
 
     def decode(self, pod, model, payload: bytes, cap=4096):
         ev = np.zeros(cap, EVENT_DTYPE); hs = np.zeros(cap * 64, np.uint64); tk = np.zeros(cap * 1024, np.uint32)

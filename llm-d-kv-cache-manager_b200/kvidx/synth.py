@@ -171,3 +171,22 @@ class Workload:
             ok = (m > 0) & (pods[:, j] >= 0)
             out[rows[ok], pods[ok, j]] = seq[tier[ok], L[ok]]
         return out
+
+    def expected_inventory(self):
+        """Closed form of the pod inventory (kvidx_pod_inventory, all models, engine pass) of the fill above: block b of a
+        document is held by its pods j with depth_j > b, so pod j adds depth_j keys and entries (on its pair's tier), the
+        deepest pod alone holds the blocks past the second deepest's depth, and every block has one engine mapping and
+        none is stale.  Documents are random, so no two blocks share a key.  Same arrays as kvidx.Index.pod_inventory."""
+        pods = self.doc_pods(0, self.D)
+        k = min(4, self.P)
+        ent = np.zeros((self.P, 16), np.uint64)
+        keys, sole = np.zeros(self.P, np.uint64), np.zeros(self.P, np.uint64)
+        docs = np.arange(self.D, dtype=np.int64)
+        for j in range(k):
+            tier = ((docs * 4 + j) % 8 == 7).astype(np.int64)
+            np.add.at(ent, (pods[:, j], tier), np.uint64(self.depth(j)))
+            np.add.at(keys, pods[:, j], np.uint64(self.depth(j)))
+        np.add.at(sole, pods[:, k - 1], np.uint64(self.depth(k - 1) - (self.depth(k - 2) if k > 1 else 0)))
+        stored = self.D * self.depth(k - 1)
+        return {"entries": ent, "keys": keys, "sole": sole, "sole_engine": sole.copy(),
+                "totals": np.array([stored, int(keys.sum()), stored, 0], np.uint64)}

@@ -16,3 +16,5 @@ compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/tes
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_score_turn.py -x -q -m gpu -k "identities or arbitrary or chain_edges or block_sizes or host_buffers or errors"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_score_turn.py -x -q -m gpu -k "chain_edges or (arbitrary and 257)"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_host_buffers.py -x -q -m gpu -k "model_filter or exact_lru"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_inventory.py -x -q -m gpu -k "max_pods or removing_each_pod or high_load or shard_inventories or errors"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_inventory.py -x -q -m gpu -k "max_pods and (257 or 513)"
