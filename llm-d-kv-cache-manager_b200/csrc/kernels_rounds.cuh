@@ -21,6 +21,10 @@
 //                            walk their own blocks
 //   C   compact_round_kernel next round's live list: the prompts that continue, in the order of this round's list
 //
+// What a prompt carries between rounds (position, chain state, where its walk state is) lives in a LiveRec per LIVE SLOT
+// and moves with the slot; the walk states are stored by the slot of the round that wrote them.  So every kernel reads a
+// live slot's state in list order, and the prompt id is only needed for the result row and the model / filter rows.
+//
 // Every round pays a fixed cost of short latency-bound kernels (hidden by running the batch as independent parts
 // on separate streams), so medium batches use kernels_rounds_plain.cuh instead (see kvidx.cu: launch_score).
 #pragma once
@@ -49,14 +53,39 @@ struct __align__(8) PromptState {        // walk state carried between rounds (o
 
 constexpr int kMaxParts = 16;             // the sorted batch runs as up to this many independent parts on their own streams
 
+// What a live prompt carries from round to round, stored by LIVE SLOT: kernel C moves it into the next list together with
+// the slot.  The kernels read one coalesced record per slot instead of gathering each field by prompt id.
+struct __align__(16) LiveRec {
+    int64_t tok;                         // token index of the prompt's next chunk (relative to tok_base)
+    uint32_t left;                       // full blocks from there to the end of the prompt
+    uint32_t src;                        // live slot of the previous round whose PromptState is this prompt's walk state:
+                                         // its own, or its class representative's (round 0: kRoleSelf)
+    uint64_t hstate;                     // chain hash after the last block of the previous round (round 0: the initial hash)
+    uint32_t srcp;                       // the prompt in slot src (round 0: kRoleSelf).  Same state <=> same srcp; the class
+                                         // election key hashes it
+    uint32_t p;                          // prompt id: only for its result row, has_keys, model and filter row
+};
+static_assert(sizeof(LiveRec) == 32, "two 16-byte halves");
+__device__ __forceinline__ LiveRec live_load(const LiveRec* r) {
+    const uint4 u = __ldg(reinterpret_cast<const uint4*>(r)), v = __ldg(reinterpret_cast<const uint4*>(r) + 1);
+    LiveRec L;
+    L.tok = (int64_t)(((uint64_t)u.y << 32) | u.x); L.left = u.z; L.src = u.w;
+    L.hstate = ((uint64_t)v.y << 32) | v.x; L.srcp = v.z; L.p = v.w;
+    return L;
+}
+// the record of a prompt that continues next round: tok / left advanced, walk state in slot src (prompt srcp), chain state h
+__device__ __forceinline__ void live_store(LiveRec* r, int64_t tok, uint32_t left, uint32_t src, uint64_t h, uint32_t srcp, uint32_t p) {
+    uint4* d = reinterpret_cast<uint4*>(r);
+    d[0] = make_uint4((uint32_t)(uint64_t)tok, (uint32_t)((uint64_t)tok >> 32), left, src);
+    d[1] = make_uint4((uint32_t)h, (uint32_t)(h >> 32), srcp, p);
+}
+
 struct RoundBufs {
-    uint32_t* act[2];                    // live prompt lists (ping-pong)
+    LiveRec* live[2];                    // live lists (ping-pong): one record per live slot, in the order of the round-0 sort
     unsigned int* n_act;                 // [2] list lengths
-    uint64_t* hstate;                    // per prompt: chain hash after the last block of the previous round
-    uint32_t* pos;                       // per prompt: first block of its next chunk (32 x round unless it walked part of a chunk alone)
-    uint32_t* src;                       // per prompt: the prompt whose PromptState (previous round's buffer) is this prompt's
-                                         // walk state -- itself, or the representative of the class it was in
-    PromptState* pst[2];                 // per prompt, by round parity (round r reads [r&1 ^ 1], writes [r&1])
+    uint32_t* nmap;                      // [n_act] written by kernel C: live slot of this round -> its slot next round (prompts that continue)
+    PromptState* pst[2];                 // by live slot of the round that wrote it, by round parity (round r reads [r&1 ^ 1] at
+                                         // LiveRec::src, writes [r&1])
     uint64_t* keys;                      // [kRoundBlocks][n_prompts] keys of the current round, block-major, by position in
                                          // the representative list: key of block j of entry a at keys[j * n_prompts + a]
     uint32_t* nbr;                       // [n_act] per live slot: blocks in this round | (more blocks follow) << 8
@@ -67,8 +96,7 @@ struct RoundBufs {
     uint8_t* fate;                       // [n_act] kFateMore (continues next round) / kFateDone, for every live slot: written by
                                          // kernel P for representatives, R for followers, D for partial followers; read by C
     uint32_t* hl;                        // [n_act] representative list (live slots), compacted
-    uint32_t* fl;                        // [n_act] follower list (live slots), compacted
-    uint32_t* dl;                        // [n_act] partial-follower list (live slots), compacted
+    uint2* fl;                           // [n_act] follower list {live slot, its representative's live slot}, compacted
     unsigned int* n_hl;                  // [0] representatives, [1] followers, [2] partial followers (zeroed before every round)
     unsigned int* stat;                  // with KVIDX_ROUNDS_TRACE=1, running totals of the batch: [0] chunks kernel G streams,
                                          // [1] election losers that read two chunks again in G, [2] chunk compares in G2,
@@ -81,10 +109,9 @@ struct RoundBufs {
     uint32_t* anch;                      // [n_act] live slot of the representative it could share a chunk prefix with
     uint8_t* dmin;                       // [n_act] ... and the number of leading blocks it shares (0: none)
     uint32_t* apos;                      // [n_act] live slot -> position in the representative list
-    uint32_t* lslot;                     // per prompt: its slot in the current live list (written when the list is built)
     unsigned long long* scan;            // [tiles of kernel C] per tile: round + 1 << 32 | prefix done << 31 | live slots (zeroed per batch)
     uint4* rec;                          // [n_hl] per representative {prompt, live slot, nbr word, src}: one load instead of a chain
-    uint4* drec;                         // [n_dl] per partial follower {prompt, representative's live slot, shared blocks << 16 | nbr word, representative's prompt}
+    uint4* drec;                         // [n_dl] per partial follower {live slot, representative's live slot, shared blocks << 16 | nbr word, prompt}
     uint32_t* grp;                       // [n_act] by live slot of last round's representative R: a class of this round whose members
                                          // had R's state (kRoleSelf: none); cleared with the map
     uint8_t* nwalk;                      // [n_hl] blocks of the round after which the representative's walk was still alive
@@ -149,17 +176,14 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         int nb = 0; bool more = false;
         uint64_t hprev = t.init_hash;
         const uint32_t* tp = a.tok;
-        int64_t first = 0;
         if (have) {
-            p = rb.act[cur][i];
-            if (round > 0) first = rb.pos[p];
-            const int64_t b = a.tok_off[p] - a.tok_base, e = a.tok_off[p + 1] - a.tok_base;
-            const int64_t nblk = (e - b) / BS;
-            nb = (int)max((int64_t)0, min((int64_t)kRoundBlocks, nblk - first));
-            more = first + nb < nblk;
+            const LiveRec L = live_load(rb.live[cur] + i);
+            p = L.p;
+            nb = (int)min(L.left, (uint32_t)kRoundBlocks);
+            more = L.left > (uint32_t)nb;
             rb.nbr[i] = (uint32_t)nb | (more ? 0x100u : 0u);
-            tp = a.tok + b + first * BS;
-            if (round > 0) { srcp = rb.src[p]; hprev = rb.hstate[p]; }
+            tp = a.tok + L.tok;
+            srcp = L.srcp; hprev = L.hstate;
             if (a.model) mdl = a.model[p];
         }
         const bool cls = have && nb > 0 && dedup;
@@ -285,17 +309,15 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         bool okm = false;
         const uint32_t* lp = a.tok;
         if (cand != kRoleSelf) {
-            const uint32_t pl = rb.act[cur][cand];
-            const int64_t bl = a.tok_off[pl] - a.tok_base, el = a.tok_off[pl + 1] - a.tok_base;
-            const int64_t nblk_l = (el - bl) / BS;
-            const int nbl = (int)max((int64_t)0, min((int64_t)kRoundBlocks, nblk_l - first));
-            okm = nbl == nb && (first + nbl < nblk_l) == more && (a.model ? a.model[pl] : a.model0) == mdl;
-            if (round > 0) okm = okm && rb.src[pl] == srcp && rb.hstate[pl] == hprev;
+            const LiveRec Lc = live_load(rb.live[cur] + cand);      // (same state source => same position in the prompt)
+            const int nbl = (int)min(Lc.left, (uint32_t)kRoundBlocks);
+            okm = nbl == nb && (Lc.left > (uint32_t)nbl) == more && (a.model ? a.model[Lc.p] : a.model0) == mdl;
+            if (round > 0) okm = okm && Lc.srcp == srcp && Lc.hstate == hprev;
             else if (a.filter) {
-                const uint64_t* fa = a.filter + (int64_t)p * t.filter_words; const uint64_t* fb = a.filter + (int64_t)pl * t.filter_words;
+                const uint64_t* fa = a.filter + (int64_t)p * t.filter_words; const uint64_t* fb = a.filter + (int64_t)Lc.p * t.filter_words;
                 for (uint32_t x = 0; x < t.filter_words; ++x) okm = okm && fa[x] == fb[x];
             }
-            lp = a.tok + bl + first * BS;
+            lp = a.tok + Lc.tok;
         }
         // ... and the tokens warp-wide
         bool shared = false;
@@ -325,8 +347,8 @@ group_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         }
         if (have) { rb.role[i] = shared ? cand : kRoleSelf; if (shared) rb.nfol[cand] = 1; }
         // Every member of a class tells the prompts that shared its state last round (same src) where the class lives:
-        // kernel G2 points the ones that stayed alone at this class.
-        if (shared && round > 0) rb.grp[rb.lslot[srcp]] = cand;
+        // kernel G2 points the ones that stayed alone at this class.  (grp is by the state owner's slot in this round's list.)
+        if (shared && round > 0) rb.grp[rb.nmap[rb.live[cur][i].src]] = cand;
         {
             const int hl_ = hlane >= 0 ? hlane : lane;
             const uint32_t cand_h = __shfl_sync(0xffffffffu, cand, hl_);
@@ -364,14 +386,13 @@ group_lists_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
             kind = rb.role[i] == kRoleSelf ? 0 : 1;
             const int nb = (int)(rb.nbr[i] & 63u);
             if (kind == 0 && partial && nb > 0 && !rb.nfol[i]) {
-                const uint32_t p = rb.act[cur][i];
+                const LiveRec L = live_load(rb.live[cur] + i);
                 // (Last round's representatives never become partial followers: the prompts that shared their state may be
                 //  attaching to them right now.)
                 bool allow = true;
                 if (round > 0) {
-                    const uint32_t srcp = rb.src[p];
-                    allow = srcp != p;
-                    if (allow) { const uint32_t rs = rb.lslot[srcp]; const uint32_t g = rb.grp[rs]; target = g != kRoleSelf ? g : rs; }
+                    allow = L.srcp != L.p;
+                    if (allow) { const uint32_t rs = rb.nmap[L.src]; const uint32_t g = rb.grp[rs]; target = g != kRoleSelf ? g : rs; }
                 }
                 const uint32_t hint = rb.dmin[i];                  // kernel G: shared blocks with a neighbour's class | 0x80 if exact
                 // a hinted class is only safe to lean on if it has followers (then its representative stays one)
@@ -379,14 +400,12 @@ group_lists_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
                 if (target != kRoleSelf && rb.role[target] != kRoleSelf) target = rb.role[target];   // someone with the same chunk represents it
                 if (target == i) target = kRoleSelf;
                 if (target != kRoleSelf) {
-                    const uint32_t pl = rb.act[cur][target];
-                    const int64_t first = round > 0 ? (int64_t)rb.pos[p] : 0;      // the class's too: same state
-                    const int64_t b = a.tok_off[p] - a.tok_base;
-                    const int64_t bl = a.tok_off[pl] - a.tok_base, el = a.tok_off[pl + 1] - a.tok_base;
-                    nbc = min(nb, (int)max((int64_t)0, min((int64_t)kRoundBlocks, (el - bl) / BS - first)));
-                    tp = a.tok + b + first * BS; rp = a.tok + bl + first * BS;
+                    const LiveRec Lt = live_load(rb.live[cur] + target);
+                    nbc = min(nb, (int)min(Lt.left, (uint32_t)kRoundBlocks));
+                    tp = a.tok + L.tok; rp = a.tok + Lt.tok;
                     // same walk state, model and filter as the class?  (grp / src: by construction; the neighbour hint: checked by kernel G)
-                    if (round > 0 && !(rb.src[pl] == rb.src[p] && rb.hstate[pl] == rb.hstate[p])) nbc = 0;
+                    // (same state source => same position in the prompt, so the two chunks start at the same block)
+                    if (round > 0 && !(Lt.srcp == L.srcp && Lt.hstate == L.hstate)) nbc = 0;
                     // kernel G compared this prompt with a member of exactly this class already: no need to read the chunks again
                     if (nbc > 0 && (hint & 0x80u) && rb.anch[i] == target) { dknown = min((int)(hint & 0x7fu), nbc); nbc = 0; }
                 }
@@ -422,15 +441,10 @@ group_lists_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, con
         const uint32_t below = (1u << lane) - 1u;
         if (kind == 0) {
             const unsigned int ap = b0 + __popc(m0 & below);
-            const uint32_t p = rb.act[cur][i];
             rb.hl[ap] = i; rb.apos[i] = ap;
-            rb.rec[ap] = make_uint4(p, i, rb.nbr[i], round > 0 ? rb.src[p] : p);
-        } else if (kind == 1) rb.fl[b1 + __popc(m1 & below)] = i;
-        else if (kind == 2) {
-            const unsigned int dp = b2 + __popc(m2 & below);
-            rb.dl[dp] = i;
-            rb.drec[dp] = make_uint4(rb.act[cur][i], target, ((uint32_t)dshare << 16) | rb.nbr[i], rb.act[cur][target]);
-        }
+            rb.rec[ap] = make_uint4(rb.live[cur][i].p, i, rb.nbr[i], rb.live[cur][i].src);
+        } else if (kind == 1) rb.fl[b1 + __popc(m1 & below)] = make_uint2(i, rb.role[i]);
+        else if (kind == 2) rb.drec[b2 + __popc(m2 & below)] = make_uint4(i, target, ((uint32_t)dshare << 16) | rb.nbr[i], rb.live[cur][i].p);
     }
 }
 
@@ -456,19 +470,21 @@ hash_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
     for (unsigned int w = blockIdx.x * (blockDim.x / 32) + wid; w * 32u < n_hl; w += total_warps) {
         const unsigned int i = w * 32u + lane;                            // position in the representative list
         const bool have = i < n_hl;
-        const uint32_t p = have ? rb.act[cur][rb.hl[i]] : 0u;
         int nb = 0;                                                      // blocks of this prompt in this round
         const uint32_t* src = nullptr;
         bool aligned = true;
         uint64_t h = 0;
         if (have) {
-            const int64_t b = a.tok_off[p] - a.tok_base, e = a.tok_off[p + 1] - a.tok_base;
-            const int64_t nblk = (e - b) / BS;
-            const int64_t first = round > 0 ? (int64_t)rb.pos[p] : 0;
-            nb = (int)max((int64_t)0, min((int64_t)kRoundBlocks, nblk - first));
-            src = a.tok + b + first * BS;
+            const uint32_t li = rb.hl[i];
+            const LiveRec L = live_load(rb.live[cur] + li);
+            nb = (int)min(L.left, (uint32_t)kRoundBlocks);
+            src = a.tok + L.tok;
             aligned = (reinterpret_cast<uintptr_t>(src) & 15u) == 0;
-            h = round == 0 ? t.init_hash : rb.hstate[p];
+            h = L.hstate;                                                // (round 0: the initial hash)
+            // the first half of its record for the next round, in case it continues: past this chunk, walk state in its own
+            // slot (kernel P writes the other half).  Nothing reads a representative's position after this kernel.
+            reinterpret_cast<uint4*>(rb.live[cur] + li)[0] = make_uint4((uint32_t)(uint64_t)(L.tok + (int64_t)nb * BS),
+                                                                        (uint32_t)((uint64_t)(L.tok + (int64_t)nb * BS) >> 32), L.left - (uint32_t)nb, li);
         }
         const int nb_max = __reduce_max_sync(0xffffffffu, nb);
         if (trace) { const unsigned int nbs = __reduce_add_sync(0xffffffffu, (unsigned int)nb); if (lane == 0 && nbs) atomicAdd(&rb.stat[3], nbs); }
@@ -534,7 +550,7 @@ walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
         const uint32_t mdl = a.model ? a.model[p] : a.model0;
         const bool snapf = rb.need_snap[li];
         WarpWalk ws;
-        if (round > 0) ws.load(pst_prev[rc.w], lane);
+        if (round > 0) ws.load(pst_prev[rc.w], lane);       // by last round's live slot
         // probe: lane j looks up block j's key
         SlotPat mine = {};
         bool hit = false;
@@ -565,22 +581,22 @@ walk_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, cons
         }
         const bool done = nb == 0 || nhit < nb || !ws.alive;   // no block, a block of the round is not in the index, or no pod left
         const bool more = !done && has_more;
-        PromptState& ps = pst_cur[p];
+        PromptState& ps = pst_cur[li];
         ws.store_lane(ps, lane);
         if (lane == 0) {
             ws.store_uniform(ps);
             rb.fate[li] = more ? kFateMore : kFateDone; rb.nwalk[i] = (uint8_t)nwalk;
-            if (more) { rb.src[p] = p; rb.pos[p] = (round > 0 ? rb.pos[p] : 0u) + (uint32_t)nb; }
         }
-        if (more) { if (lane == nb - 1) rb.hstate[p] = key; }   // chain state for the next round: key of the round's last block
-        else warp_write_row(t, a, p, ws.k, ws.pod, ws.sc, round > 0 || nb > 0, l2pol);
+        if (more) {           // chain state for the next round: key of the round's last block; its own walk state from here
+            if (lane == nb - 1) reinterpret_cast<uint4*>(rb.live[cur] + li)[1] = make_uint4((uint32_t)key, (uint32_t)(key >> 32), p, p);
+        } else warp_write_row(t, a, p, ws.k, ws.pod, ws.sc, round > 0 || nb > 0, l2pol);
         __syncwarp();
     }
 }
 
 // ---- kernel R: followers take their representative's outcome --------------------------------------------------
 // Lane per follower.  Representative continues: so does the follower, with the representative's chain state, and its
-// walk state stays where the representative left it (src).  Representative finished: same pods, same scores -- the warp
+// walk state stays where the representative left it (src: the representative's slot).  Representative finished: same pods, same scores -- the warp
 // writes the follower's result from the representative's final state.  Either way the follower's slot takes the
 // representative's fate, for kernel C.
 __device__ __forceinline__ void resolve_round(const TableView& t, const ScoreArgs& a, const RoundBufs& rb, const int cur, const int round,
@@ -596,22 +612,27 @@ __device__ __forceinline__ void resolve_round(const TableView& t, const ScoreArg
     for (unsigned int w = bid * (blockDim.x / 32) + (threadIdx.x >> 5); w * 32u < n_fl; w += total_warps) {
         const unsigned int f = w * 32u + lane;
         const bool have = f < n_fl;
-        uint32_t p = 0, pl = 0; uint8_t ft = 0;
+        uint32_t p = 0, lj = 0; uint8_t ft = 0;
         if (have) {
-            const unsigned int li = rb.fl[f], lj = rb.role[li];
-            p = rb.act[cur][li]; pl = rb.act[cur][lj]; ft = rb.fate[lj];
+            const uint2 fr = rb.fl[f];
+            const unsigned int li = fr.x;
+            lj = fr.y;
+            ft = rb.fate[lj];
+            const LiveRec L = live_load(rb.live[cur] + li);
+            const uint4 rs = __ldg(reinterpret_cast<const uint4*>(rb.live[cur] + lj) + 1);    // the representative's {hstate, srcp} as kernel P left them
+            p = L.p;
             rb.fate[li] = ft;
+            if (ft == kFateMore) {        // same chunk length as the representative: advance by the same blocks
+                const uint32_t nb = rb.nbr[li] & 63u;
+                live_store(rb.live[cur] + li, L.tok + (int64_t)nb * t.block_size, L.left - nb, lj, ((uint64_t)rs.y << 32) | rs.x, rs.z, p);
+            }
         }
         const bool more = have && ft == kFateMore;
-        if (more) {
-            rb.src[p] = pl;
-            rb.hstate[p] = rb.hstate[pl]; rb.pos[p] = rb.pos[pl];
-        }
         uint32_t dm = __ballot_sync(0xffffffffu, have && !more);
         while (dm) {
             const int l = __ffs(dm) - 1; dm &= dm - 1;
             const uint32_t pp = __shfl_sync(0xffffffffu, p, l);
-            const PromptState& ps = pst_cur[__shfl_sync(0xffffffffu, pl, l)];
+            const PromptState& ps = pst_cur[__shfl_sync(0xffffffffu, lj, l)];
             const uint32_t pk = ps.k;
             const bool in = (uint32_t)lane < pk;
             warp_write_row(t, a, pp, pk, in ? ps.pod[lane] : 0u, in ? ps.sc[lane] : 0.0, true, l2pol);   // followers always have a block in the round
@@ -654,20 +675,20 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
     for (unsigned int w = bid * (blockDim.x / 32) + wid; w * 32u < n_dl; w += total_warps) {
         const unsigned int f = w * 32u + lane;
         const bool have = f < n_dl;
-        uint32_t p = 0, meta = 0;
+        uint32_t p = 0, meta = 0, li = 0;
         bool more = false;
         ScoreState s; s.k = 0; s.alive = 0;
         uint64_t h = 0;
-        uint32_t pos0 = 0, adv = 0;
+        uint32_t adv = 0;
+        uint4 pos0 = make_uint4(0, 0, 0, 0);                     // its LiveRec's {tok, left, src}
         if (have) {
             const uint4 rc = __ldg(rb.drec + f);
-            p = rc.x; meta = rc.z & 0xffffu;
+            li = rc.x; p = rc.w; meta = rc.z & 0xffffu;
             const unsigned int lr = rc.y;
             const int d = (int)(rc.z >> 16);
-            const uint32_t pl = rc.w;
             const unsigned int ar = rb.apos[lr];
             const int nb = (int)(meta & 63u);
-            const PromptState& R = pst_rd[pl];
+            const PromptState& R = pst_rd[lr];
             s.k = R.k;
             for (uint32_t q = 0; q < s.k; ++q) s.pod[q] = R.pod[q];
             if ((int)rb.nwalk[ar] < d) {                       // R stopped inside the shared blocks: same stop, same scores
@@ -686,8 +707,8 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
                 }
                 h = rb.keys[(size_t)(d - 1) * kstride + ar];
                 const uint32_t mdl = a.model ? a.model[p] : a.model0;
-                pos0 = round > 0 ? rb.pos[p] : 0u;
-                const uint32_t* tk = a.tok + (a.tok_off[p] - a.tok_base) + (int64_t)pos0 * BS;
+                pos0 = __ldg(reinterpret_cast<const uint4*>(rb.live[cur] + li));
+                const uint32_t* tk = a.tok + (int64_t)(((uint64_t)pos0.y << 32) | pos0.x);
                 bool walking = true;
                 const int bend = min(nb, d + kDetachBlocks);          // walk at most this far alone; the rest waits for the next round
                 uint64_t hk = d < nb ? hash_block16(h, tk + (size_t)d * BS) : 0ull;       // key of the first block of its own
@@ -710,10 +731,10 @@ __device__ __forceinline__ void detach_round(const TableView& t, const ScoreArgs
             }
         }
         // continue on its own next round, or write the result
-        if (have) rb.fate[rb.dl[f]] = more ? kFateMore : kFateDone;
+        if (have) rb.fate[li] = more ? kFateMore : kFateDone;
         if (more) {
-            rb.hstate[p] = h; rb.src[p] = p; rb.pos[p] = pos0 + adv;
-            PromptState& ps = pst_cur[p];
+            live_store(rb.live[cur] + li, (int64_t)(((uint64_t)pos0.y << 32) | pos0.x) + (int64_t)adv * BS, pos0.z - adv, li, h, p, p);
+            PromptState& ps = pst_cur[li];
             ps.k = (uint8_t)s.k; ps.alive = (uint16_t)s.alive;
             ps.pat[5] = 0xffffffffu;                        // no cached slot pattern: the next block is scored the long way
             for (uint32_t q = 0; q < s.k; ++q) { ps.sc[q] = s.sc[q]; ps.pod[q] = s.pod[q]; ps.bt[q] = 0xffu; }
@@ -753,6 +774,7 @@ finish_round_kernel(const TableView t, const ScoreArgs a, const RoundBufs rb, co
 // G's anchor takes them without the election and its second read of two chunks.  One pass: a CTA counts its tile, publishes
 // the count, adds up its predecessors' published counts (decoupled look-back) and writes its prompts from there.  A tile's
 // status word carries round + 1 in its upper half, so a word of an earlier round of the batch reads as not yet published.
+// Each continuing slot's LiveRec is copied to its place in the next list, and nmap records where it went.
 constexpr int kCompactThreads = 256;
 constexpr int kCompactItems = 8;                           // consecutive live slots per thread
 constexpr int kCompactTile = kCompactThreads * kCompactItems;
@@ -815,12 +837,13 @@ compact_round_kernel(const RoundBufs rb, const int cur, const int round) {
     }
     __syncthreads();
     unsigned int at = s_base + wbase + incl - c;
-    const uint32_t* act = rb.act[cur];
-    uint32_t* nxt = rb.act[cur ^ 1];
-    while (m) {
+    const uint4* lv = reinterpret_cast<const uint4*>(rb.live[cur]);
+    uint4* nxt = reinterpret_cast<uint4*>(rb.live[cur ^ 1]);
+    while (m) {                                            // the slot's record moves with it
         const int k = __ffs(m) - 1; m &= m - 1;
-        const uint32_t p = act[s0 + k];
-        nxt[at] = p; rb.lslot[p] = at; ++at;
+        const uint4 u = lv[2 * (s0 + k)], v = lv[2 * (s0 + k) + 1];
+        nxt[2 * at] = u; nxt[2 * at + 1] = v;
+        rb.nmap[s0 + k] = at; ++at;
     }
     if (threadIdx.x == 0 && (n_act == 0 || (n_act - 1) / (unsigned)kCompactTile == tile)) rb.n_act[cur ^ 1] = s_base + agg;
 }
@@ -862,6 +885,16 @@ __global__ void count_distinct_prefixes_kernel(const uint64_t* __restrict__ fp_s
     const bool edge = i < n && (i == 0 || (fp_sorted[i] >> 32) != (fp_sorted[i - 1] >> 32));
     const unsigned int m = __ballot_sync(0xffffffffu, edge);
     if ((threadIdx.x & 31) == 0 && m) atomicAdd(out, (unsigned long long)__popc(m));
+}
+
+// Round 0's live records, in the sorted order: slot i of the batch-wide list (part q's slots start at its offset) takes
+// prompt idx[i].
+__global__ void live_init_kernel(const ScoreArgs a, uint32_t block_size, const uint32_t* __restrict__ idx, LiveRec* live, uint64_t init_hash) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= a.n_prompts) return;
+    const uint32_t p = idx[i];
+    const int64_t b = a.tok_off[p] - a.tok_base, e = a.tok_off[p + 1] - a.tok_base;
+    live_store(live + i, b, (uint32_t)max((int64_t)0, (e - b) / block_size), kRoleSelf, init_hash, kRoleSelf, p);
 }
 
 inline int rounds_init() {

@@ -168,7 +168,7 @@ struct kvidx {
     int64_t rounds_min = 2048;     // batches at least this large (and above coop_max) use the round pipeline
     int64_t classes_min = 131072;  // ... and at least this large, the prefix-class round pipeline
     double classes_min_sharing = 0.85;   // ... if at least this fraction of the batch follows a representative in round 0
-    DevBuf r_act0, r_act1, r_cnt, r_hstate, r_keys, r_pst, r_nbr, r_fp, r_sort, r_role, r_hl, r_map, r_src, r_fate, r_anch, r_snap, r_rec, r_scan;
+    DevBuf r_act0, r_act1, r_cnt, r_hstate, r_keys, r_pst, r_nbr, r_fp, r_sort, r_role, r_hl, r_map, r_live, r_fate, r_anch, r_snap, r_rec, r_scan;
     int64_t host_chunk_tokens = 32ll << 20;   // tokens per H2D chunk of the host-buffer pipeline
     int rounds_trace = 0;
     int rounds_grid[5] = {2, 4, 2, 4, 4};   // CTAs per SM a part's group / lists / hash / walk / finish kernel may occupy (multi-part runs)
@@ -421,12 +421,13 @@ int rounds_setup(kvidx* x, const ScoreArgs& a, const PartSizes& ps, cudaStream_t
 // another part's bandwidth-bound ones.
 int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks) {
     const int64_t n = a.n_prompts;
-    CK(x->r_act0.need((size_t)n * 4)); CK(x->r_act1.need((size_t)n * 4)); CK(x->r_cnt.need(1024));
-    CK(x->r_hstate.need((size_t)n * 8)); CK(x->r_keys.need((size_t)n * kRoundBlocks * 8)); CK(x->r_pst.need((size_t)n * sizeof(PromptState) * 2));
-    CK(x->r_nbr.need((size_t)n * 4 * 2)); CK(x->r_role.need((size_t)n * 4)); CK(x->r_hl.need((size_t)n * 4 * 2)); CK(x->r_src.need((size_t)n * 4));
+    CK(x->r_act0.need((size_t)n * 4)); CK(x->r_cnt.need(1024));
+    CK(x->r_keys.need((size_t)n * kRoundBlocks * 8)); CK(x->r_pst.need((size_t)n * sizeof(PromptState) * 2));
+    CK(x->r_nbr.need((size_t)n * 4)); CK(x->r_role.need((size_t)n * 4)); CK(x->r_hl.need((size_t)n * (8 + 4)));
+    CK(x->r_live.need((size_t)n * sizeof(LiveRec) * 2));
     const int64_t n_al = (n + 63) & ~63ll;
     CK(x->r_fate.need((size_t)n_al * 4 + 64 * kMaxParts));      // fate, dmin, then per part nfol | need_snap
-    CK(x->r_anch.need((size_t)n * 4 * 4));  // anch, apos, dl, lslot
+    CK(x->r_anch.need((size_t)n * 4 * 3));  // anch, apos, nmap
     CK(x->r_rec.need((size_t)n * 16 * 2));  // rec, drec
     CK(x->r_snap.need((size_t)n * (kRoundBlocks * kMaxEnt * 8 + kRoundBlocks * 2 + 1 + kRoundBlocks + kRoundBlocks * kMaxEnt)));
     int np = 1;
@@ -447,18 +448,17 @@ int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t m
     RoundBufs rb[kMaxParts]{};
     for (int q = 0; q < np; ++q) {
         const int64_t off = poff[q];
-        rb[q].act[0] = x->r_act0.as<uint32_t>() + off; rb[q].act[1] = x->r_act1.as<uint32_t>() + off;
+        rb[q].live[0] = x->r_live.as<LiveRec>() + off; rb[q].live[1] = x->r_live.as<LiveRec>() + n + off;
         rb[q].n_act = cnt + 8 * q;
         rb[q].n_hl = cnt + 8 * q + 2;
         rb[q].stat = cnt + 8 * kMaxParts + 4 + 4 * q;
-        rb[q].hstate = x->r_hstate.as<uint64_t>(); rb[q].src = x->r_src.as<uint32_t>();
-        rb[q].pst[0] = x->r_pst.as<PromptState>(); rb[q].pst[1] = x->r_pst.as<PromptState>() + n;
-        rb[q].keys = x->r_keys.as<uint64_t>() + off; rb[q].nbr = x->r_nbr.as<uint32_t>() + off; rb[q].pos = x->r_nbr.as<uint32_t>() + n;
+        rb[q].pst[0] = x->r_pst.as<PromptState>() + off; rb[q].pst[1] = x->r_pst.as<PromptState>() + n + off;
+        rb[q].keys = x->r_keys.as<uint64_t>() + off; rb[q].nbr = x->r_nbr.as<uint32_t>() + off;
         rb[q].role = x->r_role.as<uint32_t>() + off; rb[q].fate = x->r_fate.as<uint8_t>() + off;
         rb[q].part_size = (uint32_t)((psz[q] + 31) & ~31ll);
         rb[q].nfol = x->r_fate.as<uint8_t>() + 2 * n_al + 2 * off + 64 * q; rb[q].need_snap = rb[q].nfol + rb[q].part_size;
         rb[q].dmin = x->r_fate.as<uint8_t>() + n_al + off;
-        rb[q].anch = x->r_anch.as<uint32_t>() + off; rb[q].apos = x->r_anch.as<uint32_t>() + n + off; rb[q].dl = x->r_anch.as<uint32_t>() + 2 * n + off; rb[q].lslot = x->r_anch.as<uint32_t>() + 3 * n;
+        rb[q].anch = x->r_anch.as<uint32_t>() + off; rb[q].apos = x->r_anch.as<uint32_t>() + n + off; rb[q].nmap = x->r_anch.as<uint32_t>() + 2 * n + off;
         rb[q].rec = x->r_rec.as<uint4>() + off; rb[q].drec = x->r_rec.as<uint4>() + n + off;
         rb[q].snap_sc = x->r_snap.as<double>() + (size_t)off * kRoundBlocks * kMaxEnt;
         rb[q].snap_alive = reinterpret_cast<uint16_t*>(x->r_snap.as<double>() + (size_t)n * kRoundBlocks * kMaxEnt) + (size_t)off * kRoundBlocks;
@@ -466,7 +466,7 @@ int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t m
         rb[q].nwalk = snap_bytes + off;
         rb[q].snap_run = snap_bytes + n + (size_t)off * kRoundBlocks;
         rb[q].snap_bt = snap_bytes + n + (size_t)n * kRoundBlocks + (size_t)off * kRoundBlocks * kMaxEnt;
-        rb[q].hl = x->r_hl.as<uint32_t>() + off; rb[q].fl = x->r_hl.as<uint32_t>() + n + off;
+        rb[q].fl = x->r_hl.as<uint2>() + off; rb[q].hl = reinterpret_cast<uint32_t*>(x->r_hl.as<uint2>() + n) + off;
         rb[q].map = x->r_map.as<uint32_t>() + (size_t)q * gstride; rb[q].map_mask = (uint32_t)(map_slots - 1);
         rb[q].grp = rb[q].map + map_slots;
         rb[q].scan = x->r_scan.as<unsigned long long>() + (size_t)q * ctiles;
@@ -497,6 +497,8 @@ int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t m
     int64_t rounds = (max_blocks + kRoundBlocks - 1) / kRoundBlocks;
     if (x->rounds_dedup >= 2) rounds += 1;            // a prompt that left its class mid-chunk runs unaligned from there: one more round
     if (rounds < 1) rounds = 1;                       // round 0 also retires the prompts that have no full block
+    live_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, x->tv.block_size, x->r_act0.as<uint32_t>(), x->r_live.as<LiveRec>(), x->tv.init_hash);
+    x->launches += 1;
     cudaStream_t strm[kMaxParts];
     strm[0] = st;
     for (int q = 1; q < kMaxParts; ++q) strm[q] = x->aux_stream[q - 1];
@@ -1403,7 +1405,7 @@ void kvidx_destroy(kvidx_t* x) {
         if (x->ev_done[i]) cudaEventDestroy(x->ev_done[i]);
         if (x->ev_k[i]) cudaEventDestroy(x->ev_k[i]);
     }
-    x->r_act0.release(); x->r_act1.release(); x->r_cnt.release(); x->r_hstate.release(); x->r_keys.release(); x->r_pst.release(); x->r_nbr.release(); x->r_fp.release(); x->r_sort.release(); x->r_role.release(); x->r_hl.release(); x->r_map.release(); x->r_src.release(); x->r_fate.release(); x->r_anch.release(); x->r_snap.release(); x->r_rec.release(); x->r_scan.release();
+    x->r_act0.release(); x->r_act1.release(); x->r_cnt.release(); x->r_hstate.release(); x->r_keys.release(); x->r_pst.release(); x->r_nbr.release(); x->r_fp.release(); x->r_sort.release(); x->r_role.release(); x->r_hl.release(); x->r_map.release(); x->r_live.release(); x->r_fate.release(); x->r_anch.release(); x->r_snap.release(); x->r_rec.release(); x->r_scan.release();
     x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_inv.release(); x->h_inv.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
     x->d_snap.release(); x->h_snap[0].release(); x->h_snap[1].release();

@@ -95,6 +95,32 @@ for t, d, i in pts:
         live.add(i)
     else:
         live.discard(i)
+
+
+def part_streams(trace_path):
+    """Class pipeline, second step of the trace: per part (its kernel-G stream and its short-kernel stream, paired by launch
+    order), the time within the part's own span when neither stream runs a kernel, in all and per round."""
+    kern = [e for e in json.load(open(trace_path))["traceEvents"] if e.get("cat") == "kernel"]
+    kern.sort(key=lambda e: e["args"]["correlation"])
+    kern = kern[len(kern) // 2:]
+    pair, out = {}, {}
+    for a, b in zip(kern, kern[1:]):
+        if "group_round" in a["name"] and "group_lists" in b["name"]:
+            pair.setdefault(a["args"]["stream"], b["args"]["stream"])
+    for q, (sg, ss) in enumerate(pair.items()):
+        iv = sorted((e["ts"], e["ts"] + e["dur"]) for e in kern if e["args"]["stream"] in (sg, ss))
+        rounds = sum(1 for e in kern if e["args"]["stream"] == sg and "group_round" in e["name"])
+        busy, end = 0.0, iv[0][0]
+        for s, e in iv:
+            if e > end:
+                busy += e - max(s, end)
+                end = e
+        span = iv[-1][1] - iv[0][0]
+        out["part%d" % q] = {"span_ms": round(span / 1e3, 3), "idle_ms": round((span - busy) / 1e3, 3), "rounds": rounds,
+                             "idle_us_per_round": round((span - busy) / max(rounds, 1), 1)}
+    return out
+
+
 res = {
     "what": "second of two profiled Score() steps, %d prompts, %d-block index (CUPTI via torch.profiler)" % (nq, wl.n_blocks),
     "unprofiled_step_ms": round(plain_ms, 3), "profiled_span_ms": round(span / 1e3, 3), "launches": len(ev),
@@ -102,6 +128,7 @@ res = {
                 for k, v in sorted(agg.items(), key=lambda kv: -kv[1][1])},
     "ms_with_k_kernels_in_flight": {str(k): round(v / 1e3, 3) for k, v in sorted(conc.items())},
     "top_mixes_ms": {k or "idle": round(v / 1e3, 3) for k, v in mix.most_common(14)},
+    "part_streams_idle": part_streams(out.replace('.json', '_trace.json')),
 }
 exp = wl.expected_scores(doc[:2048], m[:2048])
 assert np.array_equal(d_sc[:2048].cpu().numpy(), exp)
