@@ -127,6 +127,23 @@ struct RoundBufs {
 };
 constexpr uint8_t kFateMore = 1, kFateDone = 2;
 
+// The counters of a round-pipeline batch, cleared by one memset per batch.  Part q's RoundBufs::n_act, n_hl and stat point
+// into part[q] and stat[q] (the per-prompt rounds' two halves are parts 0 and 1); rounds_init_kernel sets the first list
+// lengths and max_blocks.
+struct RoundCounters {
+    struct Part {
+        unsigned int n_act[2];           // RoundBufs::n_act
+        unsigned int n_hl[4];            // RoundBufs::n_hl; [3]: with KVIDX_ROUNDS_TRACE=1, blocks partial followers walked alone
+        unsigned int unused[2];
+    } part[kMaxParts];
+    unsigned long long max_blocks;       // full blocks of the batch's longest prompt
+    unsigned long long distinct;         // distinct first-block fingerprints (count_distinct_prefixes_kernel)
+    unsigned int stat[kMaxParts][4];     // RoundBufs::stat
+};
+static_assert(sizeof(RoundCounters::Part) == 32 && offsetof(RoundCounters, max_blocks) == 4 * 8 * kMaxParts &&
+              offsetof(RoundCounters, distinct) == offsetof(RoundCounters, max_blocks) + 8 &&
+              offsetof(RoundCounters, stat) == 4 * (8 * kMaxParts + 4), "counter words: part q at 8 q, then max_blocks, distinct, stat");
+
 template <int BS> struct HashSmem {
     static constexpr int kRow = BS * 4 + 16;                 // 80 B: the four LDS.128 of a block stay conflict free
     unsigned char tok[kHashThreads / 32][kHashStages][32 * kRow];     // [warps of the CTA]: a launch with fewer warps passes that much less
@@ -853,8 +870,8 @@ compact_round_kernel(const RoundBufs rb, const int cur, const int round) {
 // load unit merges within a warp and L2 serves across warps.  (Any order gives the same results; this one lets the
 // prefix sharing the system exists for -- system prompts, shared documents -- show up as memory locality.)
 struct PartSizes { unsigned int n[kMaxParts]; };
-__global__ void rounds_init_kernel(const ScoreArgs a, uint32_t block_size, unsigned long long* max_blocks, uint64_t* fp, uint32_t* idx,
-                                   unsigned int* cnt, const PartSizes ps) {
+__global__ void rounds_init_kernel(const ScoreArgs a, uint32_t block_size, RoundCounters* cnt, uint64_t* fp, uint32_t* idx,
+                                   const PartSizes ps) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     unsigned long long nb = 0;
     if (i < a.n_prompts) {
@@ -875,8 +892,8 @@ __global__ void rounds_init_kernel(const ScoreArgs a, uint32_t block_size, unsig
         fp[i] = f; idx[i] = (uint32_t)i;
     }
     nb = __reduce_max_sync(0xffffffffu, (unsigned)min(nb, 0xffffffffull));
-    if ((threadIdx.x & 31) == 0 && nb) atomicMax(max_blocks, nb);
-    if (i == 0) for (int q = 0; q < kMaxParts; ++q) { cnt[8 * q] = ps.n[q]; cnt[8 * q + 1] = 0; }      // live-list lengths per part
+    if ((threadIdx.x & 31) == 0 && nb) atomicMax(&cnt->max_blocks, nb);
+    if (i == 0) for (int q = 0; q < kMaxParts; ++q) { cnt->part[q].n_act[0] = ps.n[q]; cnt->part[q].n_act[1] = 0; }      // live-list lengths per part
 }
 
 // Distinct values among the sorted fingerprints (the sort orders by the top 32 bits, so those are compared).

@@ -168,17 +168,15 @@ struct kvidx {
     int64_t rounds_min = 2048;     // batches at least this large (and above coop_max) use the round pipeline
     int64_t classes_min = 131072;  // ... and at least this large, the prefix-class round pipeline
     double classes_min_sharing = 0.85;   // ... if at least this fraction of the batch follows a representative in round 0
-    DevBuf r_act0, r_act1, r_cnt, r_hstate, r_keys, r_pst, r_nbr, r_fp, r_sort, r_role, r_hl, r_map, r_live, r_fate, r_anch, r_snap, r_rec, r_scan;
+    DevBuf d_rounds;               // the round pipelines' scratch, carved per batch (ClassPlan / PlainPlan)
     int64_t host_chunk_tokens = 32ll << 20;   // tokens per H2D chunk of the host-buffer pipeline
     int rounds_trace = 0;
-    int rounds_grid[5] = {2, 4, 2, 4, 4};   // CTAs per SM a part's group / lists / hash / walk / finish kernel may occupy (multi-part runs)
     int rounds_parts = 8;          // parts (streams) a large batch is split into
     int rounds_dedup = 2;          // round pipeline: 0 every prompt on its own, 1 prefix classes, 2 + partial followers
     int sort_prefix = 1;           // sort the batch by first-block fingerprint before the rounds
-    int rounds_overlap = 1;        // run the two halves of a large batch on two streams
-    int64_t rounds_overlap_min = 65536;
+    int64_t rounds_overlap_min = 65536;   // batches from this size run as several parts (per-prompt rounds: two halves)
     cudaStream_t aux_stream[kMaxParts - 1] = {}; cudaEvent_t ev_fork = nullptr, ev_join[kMaxParts - 1] = {};
-    int rounds_warp = 1; int64_t rounds_warp_max = 131072;      // per-prompt rounds: kernel P warp per prompt up to this many prompts
+    int64_t rounds_warp_max = 131072;      // per-prompt rounds: kernel P warp per prompt up to this many prompts
                                    // (faster than the lane-per-prompt kernel P at every size swept up to 131 072)
     // multi-part class pipeline: a part's kernel G on a low-priority stream, its short kernels (G2, H, P, R) on a high-priority one
     cudaStream_t hp_stream[kMaxParts] = {}, lp_stream[kMaxParts] = {}; cudaEvent_t ev_g[kMaxParts] = {}, ev_r[kMaxParts] = {};
@@ -387,31 +385,144 @@ int cap_keys(kvidx* x) {
 
 int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks);
 
-// Batch setup of both round pipelines: clear the counters in r_cnt (part q's list lengths at word 8 * q, the batch's largest
-// block count and the distinct-prefix count as two 64-bit words at word 8 * kMaxParts, part q's four trace counters of the
-// class pipeline at word 8 * kMaxParts + 4 + 4 * q), fingerprint every prompt's first
-// block and set the parts' first list lengths (rounds_init_kernel), and with sort_prefix order the batch by fingerprint into
-// r_act0.  *fp_sorted (if not null): the sorted fingerprints.
-int rounds_setup(kvidx* x, const ScoreArgs& a, const PartSizes& ps, cudaStream_t st, const uint64_t** fp_sorted) {
+// ---- Round-pipeline batch plans ------------------------------------------------------------------------------------
+// Both round pipelines take a batch's scratch from one device arena, kvidx::d_rounds.  A plan lays out its sections with a
+// Carver twice: over a null base to size the arena, then over the arena itself, so each section's size is written once.
+// Sections start on 256-byte boundaries, as a cudaMalloc of their own would, and parts start on kPartSlots boundaries:
+// the kernels' vector accesses of a part's slice stay aligned (kernel C reads fate 8 slots at a time; kernels H and P clear
+// nfol and need_snap by words, map and grp by 4 words).
+struct Carver {
+    static constexpr size_t kAlign = 256;
+    uintptr_t base = 0; size_t at = 0;
+    template <class T> T* take(size_t count) {
+        static_assert(kAlign % alignof(T) == 0, "a section is aligned for its elements");
+        T* p = reinterpret_cast<T*>(base + at);
+        at += (count * sizeof(T) + kAlign - 1) & ~(kAlign - 1);
+        return p;
+    }
+};
+
+// A batch of n prompts in np parts: part q holds slots off[q] .. off[q] + size[q] of the sorted batch.  Every part but the
+// last ones holds ceil(n / np) prompts rounded up to kPartSlots; the last ones hold fewer, or none.
+constexpr int64_t kPartSlots = 32;
+static_assert(kPartSlots % 8 == 0, "per-slot arrays are read 8 bytes and cleared 4 words at a time");
+struct PartSplit {
+    int np;
+    int64_t per, off[kMaxParts] = {}, size[kMaxParts] = {};
+    PartSplit(int64_t n, int parts) : np(parts), per(((n + parts - 1) / parts + kPartSlots - 1) / kPartSlots * kPartSlots) {
+        for (int q = 0; q < np; ++q) { off[q] = std::min(n, q * per); size[q] = std::min(per, n - off[q]); }
+    }
+    PartSizes sizes() const { PartSizes ps{}; for (int q = 0; q < kMaxParts; ++q) ps.n[q] = (unsigned int)size[q]; return ps; }
+};
+
+// rounds_setup's sections, the first of both plans
+struct SetupBufs {
+    RoundCounters* cnt;
+    uint32_t* order;                     // the batch's prompts in sorted order: round 0's list
+    uint64_t* fp; uint64_t* fp_sorted; uint32_t* idx;    // first-block fingerprints by prompt, the same sorted, the prompt ids
+    void* sort; size_t sort_bytes = 0;   // cub's scratch (sort_prefix)
+    void carve(Carver& c, int64_t n) {
+        cnt = c.take<RoundCounters>(1); order = c.take<uint32_t>(n);
+        fp = c.take<uint64_t>(n); fp_sorted = c.take<uint64_t>(n); idx = c.take<uint32_t>(n);
+        sort = c.take<uint8_t>(sort_bytes);
+    }
+};
+
+// The class pipeline: `b` holds the batch-wide per-slot arrays (part q's slice starts at its offset) and, back to back, every
+// part's election map and grp, nfol and need_snap, and kernel C's tile words.
+struct ClassPlan {
+    int64_t n; PartSplit s;
+    int64_t ctiles;                      // kernel C's tiles per part (part 0 is the largest)
+    uint64_t map_slots;                  // a part's election map: 4 buckets per prompt, at least 1024
+    SetupBufs su{};
+    RoundBufs b{};
+    ClassPlan(int64_t n, int np) : n(n), s(n, np), ctiles((s.size[0] + kCompactTile - 1) / kCompactTile),
+                                   map_slots(pow2ceil((uint64_t)std::max<int64_t>(4 * ((n + np - 1) / np), 1024))) {}
+    size_t map_words() const { return (size_t)s.np * (map_slots + s.per); }      // each part's map, then its grp
+    size_t flag_bytes() const { return (size_t)s.np * 2 * s.per; }               // each part's nfol, then its need_snap
+    size_t scan_words() const { return (size_t)s.np * ctiles; }
+    void carve(Carver& c) {
+        su.carve(c, n);
+        b.live[0] = c.take<LiveRec>(n); b.live[1] = c.take<LiveRec>(n);
+        b.pst[0] = c.take<PromptState>(n); b.pst[1] = c.take<PromptState>(n);
+        b.keys = c.take<uint64_t>((size_t)n * kRoundBlocks);
+        b.nbr = c.take<uint32_t>(n); b.role = c.take<uint32_t>(n);
+        b.fate = c.take<uint8_t>(n); b.dmin = c.take<uint8_t>(n);
+        b.hl = c.take<uint32_t>(n); b.fl = c.take<uint2>(n);
+        b.anch = c.take<uint32_t>(n); b.apos = c.take<uint32_t>(n); b.nmap = c.take<uint32_t>(n);
+        b.rec = c.take<uint4>(n); b.drec = c.take<uint4>(n);
+        b.nwalk = c.take<uint8_t>(n);
+        b.snap_run = c.take<uint8_t>((size_t)n * kRoundBlocks); b.snap_alive = c.take<uint16_t>((size_t)n * kRoundBlocks);
+        b.snap_bt = c.take<uint8_t>((size_t)n * kRoundBlocks * kMaxEnt); b.snap_sc = c.take<double>((size_t)n * kRoundBlocks * kMaxEnt);
+        b.map = c.take<uint32_t>(map_words());
+        b.nfol = c.take<uint8_t>(flag_bytes());
+        b.scan = c.take<unsigned long long>(scan_words());
+    }
+    RoundBufs part(int q) const {
+        const int64_t o = s.off[q];
+        RoundBufs r = b;
+        r.live[0] += o; r.live[1] += o; r.pst[0] += o; r.pst[1] += o;
+        r.keys += o; r.nbr += o; r.role += o; r.fate += o; r.dmin += o; r.hl += o; r.fl += o;
+        r.anch += o; r.apos += o; r.nmap += o; r.rec += o; r.drec += o; r.nwalk += o;
+        r.snap_run += o * kRoundBlocks; r.snap_alive += o * kRoundBlocks;
+        r.snap_bt += o * kRoundBlocks * kMaxEnt; r.snap_sc += o * kRoundBlocks * kMaxEnt;
+        r.part_size = (uint32_t)((s.size[q] + kPartSlots - 1) / kPartSlots * kPartSlots);
+        r.map = b.map + q * (map_slots + s.per); r.map_mask = (uint32_t)(map_slots - 1); r.grp = r.map + map_slots;
+        r.nfol = b.nfol + q * 2 * s.per; r.need_snap = r.nfol + s.per;
+        r.scan = b.scan + q * ctiles;
+        r.n_act = su.cnt->part[q].n_act; r.n_hl = su.cnt->part[q].n_hl; r.stat = su.cnt->stat[q];
+        return r;
+    }
+};
+
+// The per-prompt rounds.  Keys are prompt-major for the warp-per-prompt kernel P (pm: a half's rows start at its offset
+// times kRoundBlocks), block-major for the lane-per-prompt one.
+struct PlainPlan {
+    int64_t n; PartSplit s; bool pm;
+    SetupBufs su{};
+    plain::RoundBufs b{};
+    PlainPlan(int64_t n, int np, bool pm) : n(n), s(n, np), pm(pm) {}
+    void carve(Carver& c) {
+        su.carve(c, n);
+        b.act[0] = su.order; b.act[1] = c.take<uint32_t>(n);
+        b.hstate = c.take<uint64_t>(n); b.pst = c.take<PromptState>(n);
+        b.keys = c.take<uint64_t>((size_t)n * kRoundBlocks); b.nbr = c.take<uint32_t>(n);
+    }
+    plain::RoundBufs part(int q) const {
+        const int64_t o = s.off[q];
+        plain::RoundBufs r = b;
+        r.act[0] += o; r.act[1] += o; r.keys += pm ? o * kRoundBlocks : o; r.nbr += o;
+        r.n_act = su.cnt->part[q].n_act;
+        return r;
+    }
+};
+
+// Sizes d_rounds for plan p (growing it as DevBuf::need does; what it held is dropped) and carves p's sections from it.
+template <class Plan> int carve_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, Plan& p) {
+    if (x->sort_prefix)
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, p.su.sort_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const uint32_t*)nullptr,
+                                           (uint32_t*)nullptr, (int)a.n_prompts, 32, 64, st));
+    Carver size;
+    p.carve(size);
+    CK(x->d_rounds.need(size.at));
+    Carver c{reinterpret_cast<uintptr_t>(x->d_rounds.p)};
+    p.carve(c);
+    return 0;
+}
+
+// Batch setup of both round pipelines: clear the counters, fingerprint every prompt's first block and set the parts' first
+// list lengths (rounds_init_kernel), and with sort_prefix order the batch by fingerprint into su.order.
+int rounds_setup(kvidx* x, const ScoreArgs& a, const SetupBufs& su, const PartSizes& ps, cudaStream_t st) {
     const int64_t n = a.n_prompts;
-    unsigned int* cnt = x->r_cnt.as<unsigned int>();
-    CK(cudaMemsetAsync(cnt, 0, 1024, st));
-    CK(x->r_fp.need((size_t)n * 8 * 2 + (size_t)n * 4));
-    uint64_t* fp_in = x->r_fp.as<uint64_t>(); uint64_t* fp_out = fp_in + n;
-    uint32_t* idx_in = reinterpret_cast<uint32_t*>(fp_out + n);
-    uint32_t* act0 = x->r_act0.as<uint32_t>();
-    rounds_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, x->tv.block_size, reinterpret_cast<unsigned long long*>(cnt + 8 * kMaxParts), fp_in,
-                                                                    x->sort_prefix ? idx_in : act0, cnt, ps);
+    CK(cudaMemsetAsync(su.cnt, 0, sizeof(RoundCounters), st));
+    rounds_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, x->tv.block_size, su.cnt, su.fp, x->sort_prefix ? su.idx : su.order, ps);
     x->launches += 1;
     CK(cudaGetLastError());
     if (x->sort_prefix) {
-        size_t tmp = 0;
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, fp_in, fp_out, idx_in, act0, (int)n, 32, 64, st));
-        CK(x->r_sort.need(tmp));
-        CK(cub::DeviceRadixSort::SortPairs(x->r_sort.p, tmp, fp_in, fp_out, idx_in, act0, (int)n, 32, 64, st));
+        size_t tmp = su.sort_bytes;
+        CK(cub::DeviceRadixSort::SortPairs(su.sort, tmp, su.fp, su.fp_sorted, su.idx, su.order, (int)n, 32, 64, st));
         x->launches += 5;     // cub: histogram + 4 onesweep passes (the top 32 fingerprint bits order the groups well enough)
     }
-    if (fp_sorted) *fp_sorted = fp_out;
     return 0;
 }
 
@@ -421,72 +532,24 @@ int rounds_setup(kvidx* x, const ScoreArgs& a, const PartSizes& ps, cudaStream_t
 // another part's bandwidth-bound ones.
 int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks) {
     const int64_t n = a.n_prompts;
-    CK(x->r_act0.need((size_t)n * 4)); CK(x->r_cnt.need(1024));
-    CK(x->r_keys.need((size_t)n * kRoundBlocks * 8)); CK(x->r_pst.need((size_t)n * sizeof(PromptState) * 2));
-    CK(x->r_nbr.need((size_t)n * 4)); CK(x->r_role.need((size_t)n * 4)); CK(x->r_hl.need((size_t)n * (8 + 4)));
-    CK(x->r_live.need((size_t)n * sizeof(LiveRec) * 2));
-    const int64_t n_al = (n + 63) & ~63ll;
-    CK(x->r_fate.need((size_t)n_al * 4 + 64 * kMaxParts));      // fate, dmin, then per part nfol | need_snap
-    CK(x->r_anch.need((size_t)n * 4 * 3));  // anch, apos, nmap
-    CK(x->r_rec.need((size_t)n * 16 * 2));  // rec, drec
-    CK(x->r_snap.need((size_t)n * (kRoundBlocks * kMaxEnt * 8 + kRoundBlocks * 2 + 1 + kRoundBlocks + kRoundBlocks * kMaxEnt)));
-    int np = 1;
-    if (x->rounds_overlap && n >= x->rounds_overlap_min) np = std::max(1, std::min(kMaxParts, x->rounds_parts));
-    int64_t psz[kMaxParts] = {}, poff[kMaxParts] = {};
-    {
-        const int64_t per = ((n + np - 1) / np + 31) & ~31ll;
-        int64_t at = 0;
-        for (int q = 0; q < np; ++q) { poff[q] = at; psz[q] = std::max<int64_t>(0, std::min(per, n - at)); at += psz[q]; }
-    }
-    const int64_t ctiles = (psz[0] + kCompactTile - 1) / kCompactTile;      // kernel C's tiles per part (part 0 is the largest)
-    CK(x->r_scan.need((size_t)std::max<int64_t>(ctiles, 1) * np * 8));
-    const uint64_t map_slots = pow2ceil((uint64_t)std::max<int64_t>(4 * ((n + np - 1) / np), 1024));
-    const size_t gstride = map_slots + (size_t)((((n + np - 1) / np) + 32 + 3) & ~3ll);      // election map + grp per part, cleared together
-    CK(x->r_map.need(gstride * 4 * np));
-    unsigned int* cnt = x->r_cnt.as<unsigned int>();
-    unsigned long long* d_maxb = reinterpret_cast<unsigned long long*>(cnt + 8 * kMaxParts);
+    ClassPlan p(n, n >= x->rounds_overlap_min ? std::max(1, std::min(kMaxParts, x->rounds_parts)) : 1);
+    if (int rc = carve_rounds(x, a, st, p)) return rc;
+    const int np = p.s.np;
     RoundBufs rb[kMaxParts]{};
-    for (int q = 0; q < np; ++q) {
-        const int64_t off = poff[q];
-        rb[q].live[0] = x->r_live.as<LiveRec>() + off; rb[q].live[1] = x->r_live.as<LiveRec>() + n + off;
-        rb[q].n_act = cnt + 8 * q;
-        rb[q].n_hl = cnt + 8 * q + 2;
-        rb[q].stat = cnt + 8 * kMaxParts + 4 + 4 * q;
-        rb[q].pst[0] = x->r_pst.as<PromptState>() + off; rb[q].pst[1] = x->r_pst.as<PromptState>() + n + off;
-        rb[q].keys = x->r_keys.as<uint64_t>() + off; rb[q].nbr = x->r_nbr.as<uint32_t>() + off;
-        rb[q].role = x->r_role.as<uint32_t>() + off; rb[q].fate = x->r_fate.as<uint8_t>() + off;
-        rb[q].part_size = (uint32_t)((psz[q] + 31) & ~31ll);
-        rb[q].nfol = x->r_fate.as<uint8_t>() + 2 * n_al + 2 * off + 64 * q; rb[q].need_snap = rb[q].nfol + rb[q].part_size;
-        rb[q].dmin = x->r_fate.as<uint8_t>() + n_al + off;
-        rb[q].anch = x->r_anch.as<uint32_t>() + off; rb[q].apos = x->r_anch.as<uint32_t>() + n + off; rb[q].nmap = x->r_anch.as<uint32_t>() + 2 * n + off;
-        rb[q].rec = x->r_rec.as<uint4>() + off; rb[q].drec = x->r_rec.as<uint4>() + n + off;
-        rb[q].snap_sc = x->r_snap.as<double>() + (size_t)off * kRoundBlocks * kMaxEnt;
-        rb[q].snap_alive = reinterpret_cast<uint16_t*>(x->r_snap.as<double>() + (size_t)n * kRoundBlocks * kMaxEnt) + (size_t)off * kRoundBlocks;
-        uint8_t* snap_bytes = reinterpret_cast<uint8_t*>(reinterpret_cast<uint16_t*>(x->r_snap.as<double>() + (size_t)n * kRoundBlocks * kMaxEnt) + (size_t)n * kRoundBlocks);
-        rb[q].nwalk = snap_bytes + off;
-        rb[q].snap_run = snap_bytes + n + (size_t)off * kRoundBlocks;
-        rb[q].snap_bt = snap_bytes + n + (size_t)n * kRoundBlocks + (size_t)off * kRoundBlocks * kMaxEnt;
-        rb[q].fl = x->r_hl.as<uint2>() + off; rb[q].hl = reinterpret_cast<uint32_t*>(x->r_hl.as<uint2>() + n) + off;
-        rb[q].map = x->r_map.as<uint32_t>() + (size_t)q * gstride; rb[q].map_mask = (uint32_t)(map_slots - 1);
-        rb[q].grp = rb[q].map + map_slots;
-        rb[q].scan = x->r_scan.as<unsigned long long>() + (size_t)q * ctiles;
-    }
-    PartSizes ps{};
-    for (int q = 0; q < kMaxParts; ++q) ps.n[q] = (unsigned int)psz[q];
-    const uint64_t* fp_sorted = nullptr;
-    if (int rc = rounds_setup(x, a, ps, st, &fp_sorted)) return rc;
+    for (int q = 0; q < np; ++q) rb[q] = p.part(q);
+    if (int rc = rounds_setup(x, a, p.su, p.s.sizes(), st)) return rc;
     // Is the batch worth it?  The class pipeline pays a token pass and five kernels per round; with few prompts per distinct
     // prefix the per-prompt rounds are faster.  The sorted first-block
     // fingerprints tell before anything is spent: count the distinct ones, and hand the batch over if more than 15 % of the
     // prompts start differently from their neighbour.  (The device-resident entry point waits for the block count here anyway.)
     const bool adaptive = x->score_path == 0 && x->rounds_dedup && x->sort_prefix && x->classes_min_sharing > 0.0;
     if (adaptive) {
-        count_distinct_prefixes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(fp_sorted, n, d_maxb + 1);
+        count_distinct_prefixes_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(p.su.fp_sorted, n, &p.su.cnt->distinct);
         x->launches += 1;
     }
     if (max_blocks < 0 || adaptive) {
-        unsigned long long mb[2] = {0, 0};
-        CK(cudaMemcpyAsync(mb, d_maxb, sizeof mb, cudaMemcpyDeviceToHost, st));
+        unsigned long long mb[2] = {0, 0};           // max_blocks, distinct
+        CK(cudaMemcpyAsync(mb, &p.su.cnt->max_blocks, sizeof mb, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         if (max_blocks < 0) max_blocks = (int64_t)mb[0];
         if (adaptive && (double)mb[1] > (1.0 - x->classes_min_sharing) * (double)n) {
@@ -497,14 +560,14 @@ int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t m
     int64_t rounds = (max_blocks + kRoundBlocks - 1) / kRoundBlocks;
     if (x->rounds_dedup >= 2) rounds += 1;            // a prompt that left its class mid-chunk runs unaligned from there: one more round
     if (rounds < 1) rounds = 1;                       // round 0 also retires the prompts that have no full block
-    live_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, x->tv.block_size, x->r_act0.as<uint32_t>(), x->r_live.as<LiveRec>(), x->tv.init_hash);
+    live_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, x->tv.block_size, p.su.order, p.b.live[0], x->tv.init_hash);
     x->launches += 1;
     cudaStream_t strm[kMaxParts];
     strm[0] = st;
     for (int q = 1; q < kMaxParts; ++q) strm[q] = x->aux_stream[q - 1];
-    CK(cudaMemsetAsync(x->r_map.p, 0xff, gstride * 4 * np, st));
-    CK(cudaMemsetAsync(x->r_fate.as<uint8_t>() + 2 * n_al, 0, (size_t)n_al * 2 + 64 * kMaxParts, st));     // nfol, need_snap
-    CK(cudaMemsetAsync(x->r_scan.p, 0, (size_t)ctiles * np * 8, st));     // kernel C's tile words: nothing published
+    CK(cudaMemsetAsync(p.b.map, 0xff, p.map_words() * 4, st));
+    CK(cudaMemsetAsync(p.b.nfol, 0, p.flag_bytes(), st));
+    CK(cudaMemsetAsync(p.b.scan, 0, p.scan_words() * 8, st));     // kernel C's tile words: nothing published
     if (np > 1) {
         CK(cudaEventRecord(x->ev_fork, st));
         for (int q = 1; q < np; ++q) CK(cudaStreamWaitEvent(strm[q], x->ev_fork, 0));
@@ -520,40 +583,42 @@ int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t m
     constexpr int T = 256, W = T / 32;                // threads / warps of the short kernels' CTAs
     const int trace = x->rounds_trace == 1;           // count the token work of every round (kernels_rounds.cuh: RoundBufs::stat)
     unsigned int stat0[kMaxParts][4] = {};            // ... the counts up to the last round, to print each round's own
+    // The grids below are capped at CTAs per SM: what fills the machine with one part (two for the list and finish kernels),
+    // less with more parts sharing it.
     for (int64_t r = 0; r < rounds; ++r) {
         const int cur = (int)(r & 1);
         for (int q = 0; q < np; ++q) {
-            const int64_t m = psz[q];
+            const int64_t m = p.s.size[q];
             if (m <= 0) continue;
-            const unsigned ggrid = (unsigned)std::min<int64_t>((m + kGroupThreads / 32 * kGroupTile - 1) / (kGroupThreads / 32 * kGroupTile), (int64_t)x->sm_count * (np == 1 ? 3 : x->rounds_grid[0]));
+            const unsigned ggrid = (unsigned)std::min<int64_t>((m + kGroupThreads / 32 * kGroupTile - 1) / (kGroupThreads / 32 * kGroupTile), (int64_t)x->sm_count * (np == 1 ? 3 : 2));
             if (prio && r > 0) CK(cudaStreamWaitEvent(sG[q], x->ev_r[q], 0));       // this part's previous round has built the live list
             group_round_kernel<16><<<ggrid, kGroupThreads, sizeof(GroupSmem), sG[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup, trace);
             if (prio) { CK(cudaEventRecord(x->ev_g[q], sG[q])); CK(cudaStreamWaitEvent(sS[q], x->ev_g[q], 0)); }
-            const unsigned lgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : x->rounds_grid[1]));
+            const unsigned lgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : 4));
             group_lists_kernel<16><<<lgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup >= 2, trace);
         }
         for (int q = 0; q < np; ++q) {
-            const int64_t m = psz[q];
+            const int64_t m = p.s.size[q];
             if (m <= 0) continue;
-            const unsigned hgrid = (unsigned)std::min<int64_t>((m + kHashThreads - 1) / kHashThreads, (int64_t)x->sm_count * (np == 1 ? 4 : x->rounds_grid[2]));
+            const unsigned hgrid = (unsigned)std::min<int64_t>((m + kHashThreads - 1) / kHashThreads, (int64_t)x->sm_count * (np == 1 ? 4 : 2));
             hash_round_kernel<16><<<hgrid, kHashThreads, sizeof(HashSmem<16>), sS[q]>>>(x->tv, a, rb[q], cur, (int)r, trace);
-            const unsigned wgrid = (unsigned)std::min<int64_t>((m + W - 1) / W, (int64_t)x->sm_count * (np == 1 ? 8 : x->rounds_grid[3]));
+            const unsigned wgrid = (unsigned)std::min<int64_t>((m + W - 1) / W, (int64_t)x->sm_count * (np == 1 ? 8 : 4));
             if (x->tv.req_ref) walk_round_kernel<true><<<wgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
             else walk_round_kernel<false><<<wgrid, T, 0, sS[q]>>>(x->tv, a, rb[q], cur, (int)r);
-            const unsigned rgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : x->rounds_grid[4]));
+            const unsigned rgrid = (unsigned)std::min<int64_t>((m + T - 1) / T, (int64_t)x->sm_count * (np <= 2 ? 8 : 4));
             finish_round_kernel<16><<<rgrid, T, sizeof(DetachWarp) * W, sS[q]>>>(x->tv, a, rb[q], cur, (int)r, x->rounds_dedup >= 2, x->rounds_trace);
             compact_round_kernel<<<(unsigned)((m + kCompactTile - 1) / kCompactTile), kCompactThreads, 0, sS[q]>>>(rb[q], cur, (int)r);
             if (prio && r + 1 < rounds) CK(cudaEventRecord(x->ev_r[q], sS[q]));
             x->launches += 6;
             if (trace) {      // debugging aid: list sizes and token work of this round (synchronises)
-                unsigned int c[256];
-                CK(cudaMemcpyAsync(c, cnt, sizeof c, cudaMemcpyDeviceToHost, sS[q]));
+                RoundCounters c;
+                CK(cudaMemcpyAsync(&c, p.su.cnt, sizeof c, cudaMemcpyDeviceToHost, sS[q]));
                 CK(cudaStreamSynchronize(sS[q]));
-                const unsigned int* l = c + 8 * q;
-                const unsigned int* s = c + (rb[q].stat - cnt);
+                const RoundCounters::Part& l = c.part[q];
+                const unsigned int* s = c.stat[q];
                 fprintf(stderr, "[kvidx rounds] round %lld part %d: live %u -> representatives %u, followers %u, partial %u (%u blocks walked alone) -> next %u;"
                         " G streamed %u chunks, %u losers re-read, G2 compared %u, H hashed %u blocks\n",
-                        (long long)r, q, l[cur], l[2], l[3], l[4], l[5], l[cur ^ 1], s[0] - stat0[q][0], s[1] - stat0[q][1], s[2] - stat0[q][2], s[3] - stat0[q][3]);
+                        (long long)r, q, l.n_act[cur], l.n_hl[0], l.n_hl[1], l.n_hl[2], l.n_hl[3], l.n_act[cur ^ 1], s[0] - stat0[q][0], s[1] - stat0[q][1], s[2] - stat0[q][2], s[3] - stat0[q][3]);
                 for (int k = 0; k < 4; ++k) stat0[q][k] = s[k];
             }
         }
@@ -569,38 +634,27 @@ int launch_score_rounds(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t m
 // Medium batches: hash / walk rounds, every prompt on its own (kernels_rounds_plain.cuh); two halves on two streams.
 int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks) {
     const int64_t n = a.n_prompts;
-    const bool warp_walk = x->rounds_warp && n <= x->rounds_warp_max;      // kernel P: warp per prompt (batch too small to fill the machine lane per prompt)
-    CK(x->r_act0.need((size_t)n * 4)); CK(x->r_act1.need((size_t)n * 4)); CK(x->r_cnt.need(1024));
-    CK(x->r_hstate.need((size_t)n * 8)); CK(x->r_keys.need((size_t)n * kRoundBlocks * 8)); CK(x->r_pst.need((size_t)n * sizeof(PromptState)));
-    CK(x->r_nbr.need((size_t)n * 4));
-    const bool overlap = x->rounds_overlap && n >= x->rounds_overlap_min;
-    const int64_t nA = overlap ? ((n / 2 + 31) & ~31ll) : n, nB = n - nA;
-    unsigned int* cnt = x->r_cnt.as<unsigned int>();
-    plain::RoundBufs rb[2]{};
-    for (int hlf = 0; hlf < 2; ++hlf) {
-        const int64_t off = hlf ? nA : 0;
-        rb[hlf].act[0] = x->r_act0.as<uint32_t>() + off; rb[hlf].act[1] = x->r_act1.as<uint32_t>() + off;
-        rb[hlf].n_act = cnt + 8 * hlf;                // the halves are parts 0 and 1 of rounds_setup's counters
-        rb[hlf].hstate = x->r_hstate.as<uint64_t>(); rb[hlf].pst = x->r_pst.as<PromptState>();
-        rb[hlf].keys = x->r_keys.as<uint64_t>() + (warp_walk ? off * kRoundBlocks : off); rb[hlf].nbr = x->r_nbr.as<uint32_t>() + off;      // prompt-major keys: a half's rows are contiguous
-    }
-    if (int rc = rounds_setup(x, a, PartSizes{{(unsigned int)nA, (unsigned int)nB}}, st, nullptr)) return rc;
+    const bool warp_walk = n <= x->rounds_warp_max;      // kernel P: warp per prompt (batch too small to fill the machine lane per prompt)
+    PlainPlan p(n, n >= x->rounds_overlap_min ? 2 : 1, warp_walk);
+    if (int rc = carve_rounds(x, a, st, p)) return rc;
+    const plain::RoundBufs rb[2] = {p.part(0), p.part(1)};
+    if (int rc = rounds_setup(x, a, p.su, p.s.sizes(), st)) return rc;
     if (max_blocks < 0) {
         unsigned long long mb = 0;
-        CK(cudaMemcpyAsync(&mb, cnt + 8 * kMaxParts, sizeof mb, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(&mb, &p.su.cnt->max_blocks, sizeof mb, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         max_blocks = (int64_t)mb;
     }
     int64_t rounds = (max_blocks + kRoundBlocks - 1) / kRoundBlocks;
     if (rounds < 1) rounds = 1;                       // round 0 also retires the prompts that have no full block
-    const int nh = nB > 0 ? 2 : 1;
+    const int nh = p.s.size[1] > 0 ? 2 : 1;
     const int per_sm = nh == 2 ? 2 : 4;               // CTAs per SM of a half's lane-per-prompt kernels H and P
     cudaStream_t strm[2] = {st, x->aux_stream[0]};
     if (nh == 2) { CK(cudaEventRecord(x->ev_fork, st)); CK(cudaStreamWaitEvent(x->aux_stream[0], x->ev_fork, 0)); }
     for (int64_t r = 0; r < rounds; ++r) {
         const int cur = (int)(r & 1);
         for (int hlf = 0; hlf < nh; ++hlf) {
-            const int64_t m = hlf ? nB : nA;
+            const int64_t m = p.s.size[hlf];
             if (warp_walk) {      // 128-thread CTAs, three stages: 55 KB, four CTAs per SM
                 const unsigned hg = (unsigned)std::min<int64_t>((m + 127) / 128, (int64_t)x->sm_count * 4);
                 plain::hash_round_kernel<16, true><<<hg, 128, 4 * 3 * 32 * HashSmem<16>::kRow, strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
@@ -610,7 +664,7 @@ int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int
             }
         }
         for (int hlf = 0; hlf < nh; ++hlf) {
-            const int64_t m = hlf ? nB : nA;
+            const int64_t m = p.s.size[hlf];
             if (warp_walk) {      // warp per prompt: 8 prompts per CTA iteration
                 const unsigned pgrid = (unsigned)std::min<int64_t>((m + 7) / 8, (int64_t)x->sm_count * 8);
                 plain::probe_round_warp_kernel<<<pgrid, plain::kProbeThreads, 0, strm[hlf]>>>(x->tv, a, rb[hlf], cur, (int)r);
@@ -1336,13 +1390,10 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     if (const char* k = getenv("KVIDX_CLASSES_MIN")) x->classes_min = atoll(k);
     if (const char* k = getenv("KVIDX_CLASSES_SHARING")) x->classes_min_sharing = atof(k);
     if (const char* k = getenv("KVIDX_SORT_PREFIX")) x->sort_prefix = atoi(k) != 0;
-    if (const char* k = getenv("KVIDX_ROUNDS_OVERLAP")) x->rounds_overlap = atoi(k) != 0;
-    if (const char* k = getenv("KVIDX_ROUNDS_GRID")) sscanf(k, "%d,%d,%d,%d,%d", &x->rounds_grid[0], &x->rounds_grid[1], &x->rounds_grid[2], &x->rounds_grid[3], &x->rounds_grid[4]);
     if (const char* k = getenv("KVIDX_HOST_CHUNK_TOKENS")) x->host_chunk_tokens = std::max<int64_t>(1 << 16, atoll(k));
     if (const char* k = getenv("KVIDX_ROUNDS_TRACE")) x->rounds_trace = atoi(k);
     if (const char* k = getenv("KVIDX_ROUNDS_PARTS")) x->rounds_parts = atoi(k);
     if (const char* k = getenv("KVIDX_PEER_PAIR")) x->tv.peer_pair = atoi(k) != 0;
-    if (const char* k = getenv("KVIDX_ROUNDS_WARP")) x->rounds_warp = atoi(k) != 0;
     if (const char* k = getenv("KVIDX_ROUNDS_WARP_MAX")) x->rounds_warp_max = atoll(k);
     if (const char* k = getenv("KVIDX_ROUNDS_DEDUP")) x->rounds_dedup = atoi(k);
     if (const char* k = getenv("KVIDX_ROUNDS_OVERLAP_MIN")) x->rounds_overlap_min = atoll(k);
@@ -1405,7 +1456,7 @@ void kvidx_destroy(kvidx_t* x) {
         if (x->ev_done[i]) cudaEventDestroy(x->ev_done[i]);
         if (x->ev_k[i]) cudaEventDestroy(x->ev_k[i]);
     }
-    x->r_act0.release(); x->r_act1.release(); x->r_cnt.release(); x->r_hstate.release(); x->r_keys.release(); x->r_pst.release(); x->r_nbr.release(); x->r_fp.release(); x->r_sort.release(); x->r_role.release(); x->r_hl.release(); x->r_map.release(); x->r_live.release(); x->r_fate.release(); x->r_anch.release(); x->r_snap.release(); x->r_rec.release(); x->r_scan.release();
+    x->d_rounds.release();
     x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_inv.release(); x->h_inv.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
     x->d_snap.release(); x->h_snap[0].release(); x->h_snap[1].release();

@@ -192,8 +192,8 @@ def _select_path(monkeypatch, path):
     if parts:
         monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP_MIN", "64")
         monkeypatch.setenv("KVIDX_ROUNDS_PARTS", parts)
-    else:
-        monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP", "0")
+    else:                                    # no batch is large enough to be split
+        monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP_MIN", str(1 << 62))
     if var == "nosort":
         monkeypatch.setenv("KVIDX_SORT_PREFIX", "0")
     elif var == "nodedup":
@@ -201,7 +201,7 @@ def _select_path(monkeypatch, path):
     elif var == "whole":
         monkeypatch.setenv("KVIDX_ROUNDS_DEDUP", "1")
     elif var == "lane":                      # per-prompt rounds with the lane-per-prompt kernel P (what batches above 131 072 take)
-        monkeypatch.setenv("KVIDX_ROUNDS_WARP", "0")
+        monkeypatch.setenv("KVIDX_ROUNDS_WARP_MAX", "0")
 
 
 ROUND_PATHS = ["rounds", "rounds2", "rounds-nosort", "rounds2-nosort", "rounds-lane", "rounds2-lane", "classes", "classes2", "classes8",

@@ -540,6 +540,31 @@ def test_automatic_fallback_by_sharing(monkeypatch, capfd):
         assert np.array_equal(s_t, s_o)
 
 
+def test_round_scratch_grows_and_shrinks_through_both_pipelines(monkeypatch, capfd):
+    """One handle scores batches that grow and shrink while they alternate between the class pipeline and the per-prompt
+    rounds (directly, or handed over by the class pipeline after its setup), so both pipelines carve their scratch from
+    the same arena as it grows and is reused at smaller sizes.  Bit-exact vs the oracle every time."""
+    _select_path(monkeypatch, "auto")
+    monkeypatch.setenv("KVIDX_ROUNDS_TRACE", "2")
+    wl = synth.Workload(10, 512, 1 << 17, 32)                # 4096 documents of 32 blocks
+    ix, co = _index_pair(capacity=1 << 18, max_pods=32)
+    ev, hs, tk = wl.fill_events(0, wl.D)
+    assert ix.apply_events(ev, hs, tk)[0] == 0 and co.apply_events(ev, hs, tk)[0] == 0
+    toks, doc, _ = wl.queries(0, 20000)
+    few = np.concatenate([toks[doc < 16]] * 80)              # prompts on 16 documents: the class pipeline keeps them
+    many = toks                                              # on all 4096: too few share their first block, handed over
+    for batch, handed_over in ((few[:300], False), (many[:3000], True), (few[:5000], False), (many[:40], False),
+                               (few[:700], False), (many[:1500], True)):
+        off = np.arange(0, (len(batch) + 1) * wl.T, wl.T, dtype=np.int64)
+        capfd.readouterr()
+        s_t, h_t = ix.score_batch(batch.reshape(-1), off)
+        err = capfd.readouterr().err
+        assert ("per-prompt rounds instead" in err) == handed_over, (len(batch), err)
+        s_o, h_o, _, _ = co.score_batch(batch.reshape(-1), off, n_threads=4)
+        assert np.array_equal(h_t, h_o) and np.array_equal(s_t, s_o), (len(batch), np.argwhere(s_t != s_o)[:5])
+        assert (s_o.max(axis=1) > 0).any()
+
+
 def test_config5_scores_while_the_write_path_runs():
     """BASELINE config #5 in miniature: one thread keeps storing and removing documents through apply_events while another
     scores prompts of documents the writer never touches.  Calls on one handle serialise, so every Score() sees the index
