@@ -195,9 +195,9 @@ int kvidx_score_keys_sparse(kvidx_t* idx, const uint64_t* keys, const int64_t* k
  * caller re-sends it next turn.  Every other argument, KVIDX_SCORE_ABSENT and the result rows mean what they mean for
  * kvidx_score_keys; key_off[0] and tok_off[0] may be non-zero.  n_prompts < 0, NULL or non-monotone offsets, a NULL
  * element array with a non-zero count, new_keys_out without new_key_off_out -> KVIDX_EINVAL; n_prompts == 0 -> 0, nothing
- * written.  Block size 16 on default and CLOCK handles: one fused warp-per-prompt kernel at every batch size (the held keys
- * are walked, then the new tokens hashed warp-cooperatively from the last held key while the walk goes on).  Other block
- * sizes, exact-LRU handles and KVIDX_SCORE_KERNEL=v1 hash, concatenate and score the keys (exact-LRU stamps as
+ * written.  Block size 16, 32, 64 or 128 on default and CLOCK handles: one fused warp-per-prompt kernel at every batch size
+ * (the held keys are walked, then the new tokens hashed warp-cooperatively from the last held key while the walk goes on).
+ * Other block sizes, exact-LRU handles and KVIDX_SCORE_KERNEL=v1 hash, concatenate and score the keys (exact-LRU stamps as
  * kvidx_score_batch).  Host buffers as kvidx_score_keys: pinned ones in place, small calls zero-copy, the rest through the
  * chunked pipeline; not coalesced with other callers. */
 int kvidx_score_turn(kvidx_t* idx, const uint64_t* keys, const int64_t* key_off, const uint32_t* tok, const int64_t* tok_off,

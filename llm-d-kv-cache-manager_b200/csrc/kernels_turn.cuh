@@ -9,9 +9,10 @@
 //     the keys are walked;
 //   * token phase: the coop kernel's chunk (coop_walk_chunk), chain seeded with the last held key, the walk state carried
 //     on.  Probes stop where the walk stops, in either phase; the hashing goes on to the prompt's last full block only when
-//     the new keys are wanted (lane j stores key j: one 256-byte store per chunk).
-// Composed path (block size != 16, exact-LRU handles, KVIDX_SCORE_KERNEL=v1): hash_keys_kernel_v1 with each prompt's
-// parent read on the device, turn_concat_kernel, then Score() from the concatenated keys.
+//     the new keys are wanted (lane j stores the key of the chunk's block j: one store of 512 / B keys per chunk).
+// Built for block sizes B = 16, 32, 64 and 128, as the coop kernel.  Composed path (other block sizes, exact-LRU handles,
+// KVIDX_SCORE_KERNEL=v1): hash_keys_kernel_v1 with each prompt's parent read on the device, turn_concat_kernel, then
+// Score() from the concatenated keys.
 #pragma once
 #include <cuda_runtime.h>
 #include "score_common.cuh"
@@ -29,16 +30,17 @@ struct TurnArgs {
     uint64_t* new_keys; const int64_t* new_off; int64_t new_base;
 };
 
-__global__ void __launch_bounds__(kCoopThreads)
+template <int BS>
+__global__ void __launch_bounds__(kCoopThreads, CoopGeom<BS>::kMinCtas)
 score_turn_kernel(const TableView t, const ScoreArgs a, const TurnArgs ta) {
-    constexpr int BS = 16;
+    constexpr int NB = CoopGeom<BS>::kBlocks;
     const uint64_t l2pol = l2_policy_stream();
     extern __shared__ __align__(128) unsigned char smem_raw_t[];
-    CoopSmem& sm = *reinterpret_cast<CoopSmem*>(smem_raw_t);
+    CoopSmem<BS>& sm = *reinterpret_cast<CoopSmem<BS>*>(smem_raw_t);
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const uint32_t lt = (1u << lane) - 1u;
-    CoopSmem::Warp& W = sm.w[wid];
-    coop_setup(sm, W, lane);
+    typename CoopSmem<BS>::Warp& W = sm.w[wid];
+    coop_setup<BS>(sm, W, lane);
     const bool peer = t.shard_bits != 0;
     uint32_t phases = 0;                                                  // bit s: parity the next wait on buffer s uses
     const long long total_warps = (long long)gridDim.x * kCoopWarps;
@@ -52,7 +54,7 @@ score_turn_kernel(const TableView t, const ScoreArgs a, const TurnArgs ta) {
         uint64_t* nkp = ta.new_keys ? ta.new_keys + (ta.new_off[pi] - ta.new_base) : nullptr;
         const uint64_t* kp = ta.keys + kb;
         uint64_t h = nk > 0 ? __ldg(kp + nk - 1) : t.init_hash;          // the chain's parent: the last held key
-        coop_stage(W, tokp, nblk, 0, aligned, lane);                      // lands while the held keys are walked
+        coop_stage<BS>(W, tokp, nblk, 0, aligned, lane);                  // lands while the held keys are walked
         WarpWalk ws;
         // ---- held keys ----
         bool walking = true;
@@ -66,18 +68,18 @@ score_turn_kernel(const TableView t, const ScoreArgs a, const TurnArgs ta) {
             key = next;
         }
         // ---- new tokens: hashed while the walk goes on, and to the end when the keys are wanted ----
-        const int nchunks = (nblk + kRoundBlocks - 1) / kRoundBlocks;
+        const int nchunks = (nblk + NB - 1) / NB;
         int consumed = 0;                                                 // chunks waited for (at most one more is in flight)
         for (int c = 0; c < nchunks && (walking || nkp); ++c) {
             __syncwarp();                                                 // every lane is done with buffer (c+1)&1 (chunk c-1)
-            coop_stage(W, tokp, nblk, c + 1, aligned, lane);
+            coop_stage<BS>(W, tokp, nblk, c + 1, aligned, lane);
             if (aligned) { mbar_wait(&W.bar[c & 1], (phases >> (c & 1)) & 1u); phases ^= 1u << (c & 1); }
             consumed = c + 1;
             __syncwarp();
-            const int nb = min(kRoundBlocks, nblk - c * kRoundBlocks);
+            const int nb = min(NB, nblk - c * NB);
             const bool first = nk == 0 && c == 0;
-            const int nhit = coop_walk_chunk(t, sm, W, W.tok[c & 1], h, nb, lane, lt, mdl, peer, nkp != nullptr, walking, ws, !first, first, a.filter, pi, key);
-            if (nkp && lane < nb) nkp[c * kRoundBlocks + lane] = key;
+            const int nhit = coop_walk_chunk<BS>(t, sm, W, W.tok[c & 1], h, nb, lane, lt, mdl, peer, nkp != nullptr, walking, ws, !first, first, a.filter, pi, key);
+            if (nkp && lane < nb) nkp[c * NB + lane] = key;               // lane j: block j of the chunk
             if (!ws.alive || nhit < nb) walking = false;
         }
         warp_write_row(t, a, pi, ws.k, ws.pod, ws.sc, nk + nblk > 0, l2pol);
@@ -138,8 +140,12 @@ __global__ void turn_concat_kernel(const uint64_t* __restrict__ keys, const int6
     }
 }
 
+template <int BS>
+inline bool turn_init_one() {
+    return cudaFuncSetAttribute(score_turn_kernel<BS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CoopSmem<BS>)) == cudaSuccess;
+}
 inline int turn_init() {
-    return cudaFuncSetAttribute(score_turn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CoopSmem)) == cudaSuccess ? 0 : -1;
+    return turn_init_one<16>() && turn_init_one<32>() && turn_init_one<64>() && turn_init_one<128>() ? 0 : -1;
 }
 
 }  // namespace kvx

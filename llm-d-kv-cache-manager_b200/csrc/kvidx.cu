@@ -694,21 +694,26 @@ struct ScoreIn {
 };
 
 // Exact-LRU handles take the thread-per-prompt kernel: Lookup must touch every present key of a prompt (no early exit).
-// So do token prompts of every block size but 16, which the other token kernels' staging is written for, and
-// KVIDX_SCORE_KERNEL=v1 as the cross-check.
-bool score_takes_v1(const kvidx* x, bool keys) {
-    return x->score_kernel == 1 || x->tv.req_stamp || (!keys && x->tv.block_size != 16);
+// So does KVIDX_SCORE_KERNEL=v1 as the cross-check, and so do token prompts of a block size the other token kernels' staging
+// is not written for: every size but 16, 32, 64 and 128.  At 32, 64 and 128 only the warp-per-prompt kernel
+// (coop_score_kernel) is built, so a token batch of n prompts takes it where it would at 16 (n <= coop_max, or
+// KVIDX_SCORE_PATH=coop) and v1 otherwise; the round pipelines and the fused kernel are 16-token only.
+bool score_takes_v1(const kvidx* x, bool keys, int64_t n) {
+    if (x->score_kernel == 1 || x->tv.req_stamp) return true;
+    if (keys || x->tv.block_size == 16) return false;
+    return !coop_block_size(x->tv.block_size) || !(x->score_path == 4 || (x->score_path == 0 && n <= x->coop_max));
 }
 
 // Does a batch of n prompts take a warp-per-prompt kernel: score_keys_kernel (keys, every size) or coop_score_kernel (small
 // token batches)?  Both read their inputs in place, so from pinned host memory as well (score_host_zerocopy).
 bool score_warp_per_prompt(const kvidx* x, bool keys, int64_t n) {
-    return !score_takes_v1(x, keys) && (keys || x->score_path == 4 || (x->score_path == 0 && n <= x->coop_max));
+    return !score_takes_v1(x, keys, n) && (keys || x->score_path == 4 || (x->score_path == 0 && n <= x->coop_max));
 }
 
 // Does a conversation turn take the fused kernel (score_turn_kernel, one warp per prompt at every batch size, inputs read in
-// place)?  Not where tokens take v1: there it is composed of the hash, a concatenation and Score() from keys.
-bool score_turn_fused(const kvidx* x) { return !score_takes_v1(x, false); }
+// place)?  At every block size the kernel is built for, on default and CLOCK handles; elsewhere it is composed of the hash,
+// a concatenation and Score() from keys.
+bool score_turn_fused(const kvidx* x) { return x->score_kernel != 1 && !x->tv.req_stamp && coop_block_size(x->tv.block_size); }
 
 template <class E>
 void launch_score_v1(kvidx* x, const ScoreArgs& a, const E* src, cudaStream_t st) {
@@ -731,7 +736,7 @@ int launch_score(kvidx* x, const ScoreIn& in, ScoreArgs a, cudaStream_t st, int6
     if (int rc = check_shards(x)) return rc;
     if (in.turn()) return launch_turn(x, in, a, st);
     a.tok = in.keys ? nullptr : static_cast<const uint32_t*>(in.p);
-    if (score_takes_v1(x, in.keys)) {
+    if (score_takes_v1(x, in.keys, n)) {
         if (in.keys) launch_score_v1(x, a, static_cast<const uint64_t*>(in.p), st);
         else launch_score_v1(x, a, a.tok, st);
     } else if (in.keys) {
@@ -742,7 +747,9 @@ int launch_score(kvidx* x, const ScoreIn& in, ScoreArgs a, cudaStream_t st, int6
     } else if (score_warp_per_prompt(x, false, n)) {
         // small batches: a warp per prompt, warp-cooperative hashing, TMA-staged tokens (kernels_coop.cuh)
         const int64_t ctas = std::min<int64_t>((n + kCoopWarps - 1) / kCoopWarps, (int64_t)x->sm_count * 4);
-        coop_score_kernel<16><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem), st>>>(x->tv, a);
+        coop_dispatch(x->tv.block_size, [&](auto bs) {
+            coop_score_kernel<bs.value><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem<bs.value>), st>>>(x->tv, a);
+        });
         x->launches += 1;
     } else if (n < (1ll << 31) && ((x->score_path >= 2 && x->score_path <= 3) || (x->score_path == 0 && n >= x->rounds_min))) {
         // path 2: plain rounds, 3: prefix classes; automatic: by batch size (the class pipeline has a fixed cost per round)
@@ -768,7 +775,9 @@ int launch_turn(kvidx* x, const ScoreIn& in, const ScoreArgs& a, cudaStream_t st
     ta.keys = static_cast<const uint64_t*>(in.p);
     if (score_turn_fused(x)) {
         const int64_t ctas = std::min<int64_t>((n + kCoopWarps - 1) / kCoopWarps, (int64_t)x->sm_count * 4);
-        score_turn_kernel<<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem), st>>>(x->tv, a, ta);
+        coop_dispatch(x->tv.block_size, [&](auto bs) {
+            score_turn_kernel<bs.value><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem<bs.value>), st>>>(x->tv, a, ta);
+        });
         x->launches += 1;
         CK(cudaGetLastError());
         return 0;

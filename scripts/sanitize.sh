@@ -1,6 +1,6 @@
 #!/bin/bash
-# compute-sanitizer passes (run on a GPU box; minutes): the class pipeline, the cooperative kernel (TMA + mbarrier), the
-# two-phase write path with its slot-ownership protocol.
+# compute-sanitizer passes (run on a GPU box; minutes): the class pipeline, the cooperative kernel (TMA + mbarrier, at 16-
+# and 64-token blocks), the two-phase write path with its slot-ownership protocol.
 set -x
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_parity.py -x -q -m gpu -k "prefix_tree and classes8"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_parity.py -x -q -m gpu -k "alphabet and classes8 and 1"
@@ -18,3 +18,5 @@ compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/tes
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_host_buffers.py -x -q -m gpu -k "model_filter or exact_lru"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_inventory.py -x -q -m gpu -k "max_pods or removing_each_pod or high_load or shard_inventories or errors"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_inventory.py -x -q -m gpu -k "max_pods and (257 or 513)"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_block_sizes.py -x -q -m gpu -k "payloads_and_shapes and 64-None"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_block_sizes.py -x -q -m gpu -k "payloads_and_shapes and 64-None"
