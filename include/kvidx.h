@@ -88,7 +88,19 @@ typedef struct kvidx_config {
     uint32_t lru_exact;        /* 1: track key recency (a stamp per slot, written by Lookup / Score / Add / Evict /
                                   GetRequestKey exactly where golang-lru refreshes) and evict the least recently used
                                   request / engine keys when a write call leaves more than `capacity` of them
-                                  (in_memory.go:59,64,118,163,170).  Exact at call granularity.  Score() then probes
+                                  (in_memory.go:59,64,118,163,170).  A key touched several times in one call ranks
+                                  as of its last touch in the order the reference applies the call:
+                                    kvidx_lookup        keys in array order;
+                                    Score() (batch, keys, turn; host and _dev)  prompt after prompt, and within a
+                                                        prompt every present key in block order, also past the end
+                                                        of the walk;
+                                    kvidx_add           pairs in order, each one's engine mapping before its request key;
+                                    apply_events[_dev]  each pod's events in array order, pods in ascending id (one of
+                                                        the orders the reference's per-pod workers allow);
+                                  every touch of a call gets its own stamp, however many keys a prompt or event holds.
+                                  What stays at call granularity is eviction: it runs after the call, not inside it,
+                                  so a call that takes a map past `capacity` may still see a key the reference would
+                                  have evicted part way through it.  Score() probes
                                   every key of a prompt (the reference's Lookup has no early exit), so it is the slow,
                                   semantics-first mode.  0 (default): recency is not tracked and `capacity` only sizes
                                   the table -- right whenever the fleet's block count stays below Size (default 1e8). */

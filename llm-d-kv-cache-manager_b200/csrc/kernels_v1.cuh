@@ -45,7 +45,7 @@ __global__ void lookup_kernel_v1(TableView t, uint32_t model, const uint64_t* __
     uint32_t c = 0;
     uint64_t slot = 0;
     if (req_find(t, model, keys[i], w, &slot)) {
-        if (t.req_stamp) t.req_stamp[slot] = stamp_base + (unsigned long long)i;      // data.Get refreshes recency (in_memory.go:118)
+        if (t.req_stamp) stamp_touch(t.req_stamp + slot, stamp_base + (unsigned long long)i);   // data.Get refreshes recency (in_memory.go:118)
         if (t.req_ref) ref_touch(t.req_ref, slot);
         const uint32_t cnt = meta_count(w.b.w);
         if (cnt == 0) atomicMin(cut_out, (int)min(i, (int64_t)0x7fffffff));
@@ -60,13 +60,15 @@ __global__ void lookup_kernel_v1(TableView t, uint32_t model, const uint64_t* __
 
 // Indexer.GetPodScores steps 2-4 (indexer.go:141-163): thread per prompt.  Src is the prompt's source of block keys:
 // uint32_t -- tokens, chained into keys as they are read (steps 2-4); uint64_t -- the request keys themselves (steps 3-4).
-// src_off / src_base: the CSR of that source.
+// src_off / src_base: the CSR of that source.  Exact-LRU mode: block k of prompt i is stamped
+// stamp_base + (src_off[i] - src_off[0]) + k -- unique within the call and in prompt-then-block order, since k is below the
+// prompt's element count -- so the call reserves src_off[n] - src_off[0] stamps.
 template <class Src>
 __global__ void score_kernel_v1(TableView t, const Src* __restrict__ src, const int64_t* __restrict__ src_off,
                                 int64_t src_base, int64_t n_prompts, const uint32_t* __restrict__ model, uint32_t model0,
                                 const uint64_t* __restrict__ filter, double* __restrict__ dense_out,
                                 uint16_t* __restrict__ sp_pods, double* __restrict__ sp_scores, uint8_t* __restrict__ sp_cnt,
-                                uint8_t* __restrict__ has_keys, unsigned long long stamp_base = 0, unsigned long long stamp_stride = 0) {
+                                uint8_t* __restrict__ has_keys, unsigned long long stamp_base = 0) {
     constexpr bool kKeys = sizeof(Src) == 8;
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n_prompts) return;
@@ -85,7 +87,7 @@ __global__ void score_kernel_v1(TableView t, const Src* __restrict__ src, const 
         const bool hit = req_find(t, mdl, h, w, &slot);
         // exact-LRU mode: the reference's Lookup touches EVERY key of the prompt that is present, also past the end of
         // the consecutive prefix (in_memory.go:117-139), so the probe loop runs to the last block and stamps them.
-        if (hit && t.req_stamp) t.req_stamp[slot] = stamp_base + (unsigned long long)i * stamp_stride + (unsigned long long)k;
+        if (hit && t.req_stamp) stamp_touch(t.req_stamp + slot, stamp_base + (unsigned long long)(b + src_base - src_off[0] + k));
         if (walking) {
             if (!hit) walking = false;
             else {

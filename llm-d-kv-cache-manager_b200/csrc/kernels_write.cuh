@@ -39,10 +39,14 @@ __device__ __forceinline__ void do_add(const TableView& t, uint32_t model, uint6
         if (!es) atomicAdd(&t.cnt->nospc, 1ull);
         else {
             a.z = (uint32_t)rhash; a.w = (uint32_t)(rhash >> 32);
-            if (t.req_stamp) { b.z = (uint32_t)stamp; b.w = (uint32_t)(stamp >> 32); }       // lru Add: insert or refresh
             if (t.eng_ref) ref_touch(t.eng_ref, es - t.eng);
             if (created) atomicAdd_system(&cnt_of(t, ehash, model)->eng_full, 1ull);
-            eng_publish(es, a, b, make_meta(kStateFull, 0, model));
+            if (t.req_stamp) {                         // lru Add: insert or refresh (an EMPTY slot's stamp word is 0)
+                eng_stamp_touch(es, stamp);
+                eng_publish_lru(es, a, b, make_meta(kStateFull, 0, model));
+            } else {
+                eng_publish(es, a, b, make_meta(kStateFull, 0, model));
+            }
         }
     }
     if (do_request) {                                 // 2. get-or-create the PodCache and add the entries    (in_memory.go:170-203)
@@ -52,7 +56,7 @@ __device__ __forceinline__ void do_add(const TableView& t, uint32_t model, uint6
         EntList L; L.unpack(a, b);
         for (int j = 0; j < m; ++j) count = L.add(count, pts[j], t.pods_per_key);
         L.pack(a, b);
-        if (t.req_stamp) t.req_stamp[rs - t.req] = stamp + 1;                             // data.Get refresh / ContainsOrAdd insert
+        if (t.req_stamp) stamp_touch(t.req_stamp + (rs - t.req), stamp + 1);              // data.Get refresh / ContainsOrAdd insert
         if (t.req_ref) ref_touch(t.req_ref, rs - t.req);
         if (created) atomicAdd_system(&cnt_of(t, rhash, model)->req_full, 1ull);
         req_publish(rs, a, b, make_meta(kStateFull, count, model));
@@ -72,7 +76,7 @@ __device__ __forceinline__ void do_evict(const TableView& t, uint32_t model, uin
         drop_engine = true;                                              // :225-230 stale engine mapping
     } else {
         uint32_t count = meta_count(b.w);
-        if (t.req_stamp) t.req_stamp[rs - t.req] = stamp + 1;                         // data.Get (:225)
+        if (t.req_stamp) stamp_touch(t.req_stamp + (rs - t.req), stamp + 1);          // data.Get (:225)
         if (t.req_ref) ref_touch(t.req_ref, rs - t.req);
         EntList L; L.unpack(a, b);
         for (int j = 0; j < m; ++j) count = L.remove(count, pts[j]);
@@ -253,10 +257,13 @@ hash_events_kernel(const TableView t, const kvidx_event_t* __restrict__ ev, int6
 //   ev        events stably sorted by pod; queue q owns ev[queue_off[q] .. queue_off[q+1])
 //   keys/pred phase 1's request keys (indexed like `hashes`) and the parent key each event's chain was started from;
 //             nullptr: hash here (small batches skip phase 1)
+//   stamp_*   exact-LRU mode: event e owns the stamps [stamp_base + e * stamp_stride, + stamp_stride), the parent lookup
+//             first, then two per block, so stamp_stride = 2 + 2 x the batch's largest n_hashes; the pod-sorted order of
+//             the batch is the order its stamps give
 __global__ void apply_events_kernel(TableView t, const kvidx_event_t* __restrict__ ev, const int64_t* __restrict__ queue_off,
                                     int64_t n_queues, const uint64_t* __restrict__ hashes, const uint32_t* __restrict__ tokens,
                                     const uint64_t* __restrict__ keys, const uint64_t* __restrict__ pred,
-                                    unsigned long long stamp_base) {
+                                    unsigned long long stamp_base, unsigned long long stamp_stride) {
     const int lane = threadIdx.x & 31;
     const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     if (q >= n_queues) return;
@@ -264,8 +271,7 @@ __global__ void apply_events_kernel(TableView t, const kvidx_event_t* __restrict
     for (int64_t e = queue_off[q]; e < queue_off[q + 1]; ++e) {
         const kvidx_event_t evt = ev[e];
         const uint16_t pt = evt.podtier;
-        // exact-LRU mode: event e owns the stamp range [sb, sb + 2^20): parent lookup first, then two stamps per block
-        const unsigned long long sb = stamp_base + ((unsigned long long)e << 20);
+        const unsigned long long sb = stamp_base + (unsigned long long)e * stamp_stride;     // exact-LRU: this event's stamps
         if (evt.op == KVIDX_EV_BLOCK_STORED) {
             // parent request key: GetRequestKey(parent engine key); a miss restarts at the seed (pool.go:279-294)
             uint64_t h = t.init_hash;
@@ -317,6 +323,12 @@ __global__ void apply_events_kernel(TableView t, const kvidx_event_t* __restrict
         }
         __syncwarp();
     }
+}
+
+// exact-LRU mode, kvidx_apply_events_dev: the largest n_hashes of a device-resident batch (sizes apply_events_kernel's stamp_stride)
+__global__ void max_event_hashes_kernel(const kvidx_event_t* __restrict__ ev, int64_t n_ev, unsigned long long* out) {
+    const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (e < n_ev) atomicMax(out, (unsigned long long)ev[e].n_hashes);
 }
 
 // ---- exact key-LRU (InMemoryIndexConfig.Size, in_memory.go:59,64): evict the least recently used key -----------

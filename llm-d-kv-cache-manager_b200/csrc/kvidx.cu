@@ -131,7 +131,6 @@ struct kvidx {
     Counters* h_cnt_all = nullptr;
     uint64_t rebuilds = 0;
     std::atomic<uint64_t> launches{0};
-    int64_t last_batch_events = 1 << 20;   // events in the batch being applied (sizes the stamp range)
     std::atomic<unsigned long long> clock{1};   // exact-LRU mode: recency stamps handed to kernels
     std::mutex mu_r, mu_w;          // read-side / write-side scratch and stream
     std::shared_mutex tables;       // shared: any call that launches on the tables; exclusive: rebuild swaps them
@@ -716,13 +715,22 @@ bool score_warp_per_prompt(const kvidx* x, bool keys, int64_t n) {
 bool score_turn_fused(const kvidx* x) { return x->score_kernel != 1 && !x->tv.req_stamp && coop_block_size(x->tv.block_size); }
 
 template <class E>
-void launch_score_v1(kvidx* x, const ScoreArgs& a, const E* src, cudaStream_t st) {
+int launch_score_v1(kvidx* x, const ScoreArgs& a, const E* src, cudaStream_t st) {
     const int T = 128;
-    const unsigned long long stride = 1ull << 20;
-    const unsigned long long sb = x->tv.req_stamp ? reserve_stamps(x, (unsigned long long)a.n_prompts * stride) : 0;
+    unsigned long long sb = 0;
+    if (x->tv.req_stamp) {
+        // exact-LRU: a stamp per element of the call (score_kernel_v1), counted from the offsets.  They may be device memory
+        // (the _dev entry points, the host pipeline's chunks): read back -- this mode serialises its calls anyway
+        int64_t e[2];
+        CK(cudaMemcpyAsync(&e[0], a.tok_off, 8, cudaMemcpyDefault, st));
+        CK(cudaMemcpyAsync(&e[1], a.tok_off + a.n_prompts, 8, cudaMemcpyDefault, st));
+        CK(cudaStreamSynchronize(st));
+        sb = reserve_stamps(x, (unsigned long long)(e[1] - e[0]));
+    }
     score_kernel_v1<<<(unsigned)((a.n_prompts + T - 1) / T), T, 0, st>>>(x->tv, src, a.tok_off, a.tok_base, a.n_prompts, a.model, a.model0, a.filter,
-                                                                        a.dense, a.sp_pods, a.sp_scores, a.sp_cnt, a.has_keys, sb, stride);
+                                                                        a.dense, a.sp_pods, a.sp_scores, a.sp_cnt, a.has_keys, sb);
     x->launches += 1;
+    return 0;
 }
 
 // Launch Score() over device-addressable inputs: the prompts' elements at in.p (a.tok is set here), the rest of the call in
@@ -737,8 +745,8 @@ int launch_score(kvidx* x, const ScoreIn& in, ScoreArgs a, cudaStream_t st, int6
     if (in.turn()) return launch_turn(x, in, a, st);
     a.tok = in.keys ? nullptr : static_cast<const uint32_t*>(in.p);
     if (score_takes_v1(x, in.keys, n)) {
-        if (in.keys) launch_score_v1(x, a, static_cast<const uint64_t*>(in.p), st);
-        else launch_score_v1(x, a, a.tok, st);
+        const int rc = in.keys ? launch_score_v1(x, a, static_cast<const uint64_t*>(in.p), st) : launch_score_v1(x, a, a.tok, st);
+        if (rc) return rc;
     } else if (in.keys) {
         // request keys: one warp per prompt at every batch size (kernels_keys.cuh)
         const int64_t ctas = std::min<int64_t>((n + kKeysWarps - 1) / kKeysWarps, (int64_t)x->sm_count * kKeysCtasPerSm);
@@ -1858,9 +1866,25 @@ int kvidx_get_request_key(kvidx_t* x, uint32_t model, uint64_t engine, uint64_t*
 
 namespace {
 // Both phases of a device-resident, pod-sorted event batch on the write stream (kernels_write.cuh).  Caller holds mu_w and
-// `tables` shared.
+// `tables` shared.  max_ev_hashes: the batch's largest n_hashes (exact-LRU stamp stride), < 0: found on the device.
 int launch_apply_events(kvidx* x, const kvidx_event_t* d_ev_sorted, const int64_t* d_queue_off, int64_t n_queues, int64_t n_events,
-                        const uint64_t* d_hashes, int64_t n_hashes, const uint32_t* d_tokens, cudaStream_t st) {
+                        const uint64_t* d_hashes, int64_t n_hashes, const uint32_t* d_tokens, cudaStream_t st, int64_t max_ev_hashes) {
+    unsigned long long sb = 0, stride = 0;
+    if (x->tv.req_stamp) {
+        if (max_ev_hashes < 0) {                      // read back: this mode serialises its calls anyway
+            CK(x->d_misc.need(8));
+            unsigned long long* d_max = x->d_misc.as<unsigned long long>();
+            unsigned long long h_max = 0;
+            CK(cudaMemsetAsync(d_max, 0, 8, st));
+            max_event_hashes_kernel<<<(unsigned)((n_events + 255) / 256), 256, 0, st>>>(d_ev_sorted, n_events, d_max);
+            x->launches += 1;
+            CK(cudaMemcpyAsync(&h_max, d_max, 8, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            max_ev_hashes = (int64_t)h_max;
+        }
+        stride = 2ull + 2ull * (unsigned long long)max_ev_hashes;
+        sb = reserve_stamps(x, stride * (unsigned long long)n_events);
+    }
     const uint64_t* d_keys = nullptr; const uint64_t* d_pred = nullptr;
     const bool phase1 = x->write_phase1 == 1 || (x->write_phase1 < 0 && n_hashes >= x->write_phase1_min);
     if (phase1 && n_hashes > 0) {
@@ -1891,7 +1915,7 @@ int launch_apply_events(kvidx* x, const kvidx_event_t* d_ev_sorted, const int64_
     }
     const int T = 128;   // 4 queues per CTA
     apply_events_kernel<<<(unsigned)((n_queues * 32 + T - 1) / T), T, 0, st>>>(x->tv, d_ev_sorted, d_queue_off, n_queues, d_hashes, d_tokens, d_keys, d_pred,
-                                                                               x->tv.req_stamp ? reserve_stamps(x, (1ull << 20) * (unsigned long long)std::max<int64_t>(n_events, 1)) : 0);
+                                                                               sb, stride);
     x->launches += 1;
     CK(cudaGetLastError());
     return 0;
@@ -1910,7 +1934,7 @@ int kvidx_apply_events_dev(kvidx_t* x, const kvidx_event_t* d_ev_sorted, const i
     if (rc) return rc;
     std::shared_lock<std::shared_mutex> tl(x->tables);
     cudaStream_t st = wstream(x);
-    rc = launch_apply_events(x, d_ev_sorted, d_queue_off, n_queues, n_events, d_hashes, n_hashes, d_tokens, st);
+    rc = launch_apply_events(x, d_ev_sorted, d_queue_off, n_queues, n_events, d_hashes, n_hashes, d_tokens, st, -1);
     if (rc) return rc;
     if ((rc = clock_sweep(x))) return rc;              // asynchronous too: the excess is read on the device
     // events dropped so far on this handle (cumulative, like the counter behind kvidx_apply_events' n_dropped_out)
@@ -1928,8 +1952,10 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
     // validate + stable counting sort by pod -> per-pod FIFO queues (pool.go:129-144)
     std::vector<int64_t> qcount(KVIDX_MAX_PODS + 1, 0);
     uint64_t new_keys = 0;
+    int64_t max_ev_hashes = 0;
     for (int64_t i = 0; i < n; ++i) {
         const kvidx_event_t& e = ev[i];
+        max_ev_hashes = std::max<int64_t>(max_ev_hashes, e.n_hashes);
         if (e.op > KVIDX_EV_BLOCK_REMOVED) return fail(KVIDX_EINVAL, "event %lld: unknown op %u", (long long)i, e.op);
         if (e.model > 0xffffu) return fail(KVIDX_ERANGE, "event %lld: model id %u > 65535", (long long)i, e.model);
         if (KVIDX_PT_POD(e.podtier) >= x->tv.max_pods) return fail(KVIDX_ERANGE, "event %lld: pod id %u >= max_pods %u", (long long)i, KVIDX_PT_POD(e.podtier), x->tv.max_pods);
@@ -1970,9 +1996,8 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
     if (n_hashes > 0) CK(cudaMemcpyAsync(x->d_hash.p, hashes, (size_t)n_hashes * 8, cudaMemcpyHostToDevice, st));
     if (n_tokens > 0) CK(cudaMemcpyAsync(x->d_evtok.p, tokens, (size_t)n_tokens * 4, cudaMemcpyHostToDevice, st));
     const unsigned long long dropped_before = x->h_cnt->dropped_events, nospc_before = x->h_cnt->nospc;
-    x->last_batch_events = n;
     rc = launch_apply_events(x, x->d_ev.as<kvidx_event_t>(), x->d_qoff.as<int64_t>(), nq, n, x->d_hash.as<uint64_t>(), n_hashes,
-                             x->d_evtok.as<uint32_t>(), st);
+                             x->d_evtok.as<uint32_t>(), st, max_ev_hashes);
     if (rc) return rc;
     rc = refresh_counters(x);
     if (rc) return rc;

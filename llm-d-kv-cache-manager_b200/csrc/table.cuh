@@ -204,6 +204,18 @@ __device__ __forceinline__ void ref_touch(uint32_t* bits, uint64_t slot) {
     if (!(ld_word_relaxed(w, false) & m)) atomicOr(w, m);
 }
 
+// Exact-LRU mode: a touch of a slot's recency stamp.  One call may touch a key many times from many threads (prompts that
+// share a prefix, pods that store the same block); every touch carries a stamp unique within the call and ordered as the
+// reference applies the call, so the largest stamp is the last touch, whichever thread stores last.
+__device__ __forceinline__ void stamp_touch(unsigned long long* p, unsigned long long stamp) { atomicMax(p, stamp); }
+// An engine slot's stamp word is NOT part of the image an exact-LRU writer publishes (eng_publish_lru): eng_find touches it
+// without owning the slot, and a publish of the whole half b would put back the stamp read when the writer acquired the
+// slot.  Readers still see whole images: what they read is {ehash, rhash, meta}, checked by the meta word's sequence lock
+// as before, and no reader uses the stamp -- only the LRU cut and the snapshot read it, after the call.
+__device__ __forceinline__ void eng_stamp_touch(EngSlot* s, unsigned long long stamp) {
+    stamp_touch(reinterpret_cast<unsigned long long*>(&s->stamp), stamp);
+}
+
 // ---- readers ------------------------------------------------------------------------------------------
 
 // Finds the FULL slot holding (model, tag).  Returns false at the first EMPTY slot (or after a full cycle).
@@ -241,7 +253,7 @@ __device__ __forceinline__ bool eng_find(const TableView& t, uint32_t model, uin
         if (st == kStateFull && meta_model(b.x) == model && a.x == elo && a.y == ehi) {
             *rhash = ((uint64_t)a.w << 32) | a.z;
             if (slot_out) *slot_out = i;
-            if (stamp && t.req_stamp) *(volatile uint64_t*)&const_cast<EngSlot*>(s)->stamp = stamp;   // lru Get refreshes recency
+            if (stamp && t.req_stamp) eng_stamp_touch(const_cast<EngSlot*>(s), stamp);               // lru Get refreshes recency
             if (touch && t.eng_ref) ref_touch(t.eng_ref, i);                                        // ... CLOCK: its bit
             return true;
         }
@@ -376,6 +388,12 @@ __device__ __forceinline__ EngSlot* eng_acquire(const TableView& t, uint32_t mod
 __device__ __forceinline__ void eng_publish(EngSlot* s, uint4& a, uint4& b, uint32_t new_meta) {
     b.x = published_meta(b.x, new_meta);
     st_slot(s, a, b);
+}
+// exact-LRU mode: the same publish without the stamp word (eng_stamp_touch): half a, then meta and pad as one 8-byte release
+__device__ __forceinline__ void eng_publish_lru(EngSlot* s, uint4& a, uint4& b, uint32_t new_meta) {
+    b.x = published_meta(b.x, new_meta);
+    st_half_release(s, a);
+    asm volatile("st.release.sys.global.v2.u32 [%2], {%0,%1};" :: "r"(b.x), "r"(b.y), "l"(&s->meta) : "memory");
 }
 
 __device__ __forceinline__ Counters* cnt_of(const TableView& t, uint64_t hash, uint32_t model) {

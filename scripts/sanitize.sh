@@ -20,3 +20,4 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_inventory.py -x -q -m gpu -k "max_pods and (257 or 513)"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_block_sizes.py -x -q -m gpu -k "payloads_and_shapes and 64-None"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_block_sizes.py -x -q -m gpu -k "payloads_and_shapes and 64-None"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_lru_recency.py -x -q -m gpu -k "lookup or add or events or (shared_prefixes and 16 and (dense or dev or keys or turn))"

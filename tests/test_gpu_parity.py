@@ -658,7 +658,8 @@ def test_index_size_cap_exact_lru():
 
 def test_exact_lru_random_stream_vs_oracle():
     """Size-capped index under a random single-block event stream with lookups and Score() calls in between (both refresh
-    recency in the reference).  One call = one oracle operation, so call-granular exactness is full exactness here."""
+    recency in the reference).  Score() calls of several prompts that share documents, and lookups that repeat keys: the
+    last touch of a key in the call's order (prompt after prompt, key after key) decides its recency."""
     rng = np.random.default_rng(41)
     BS, P, CAP = 16, 12, 40
     ix = kvidx.Index(block_size=BS, capacity=CAP, pods_per_key=3, max_pods=16, lru_exact=1)
@@ -679,16 +680,18 @@ def test_exact_lru_random_stream_vs_oracle():
             hs = np.array([d * 1000 + b], np.uint64); tk = np.zeros(0, np.uint32)
         assert ix.apply_events(r, hs, tk)[0] == 0 and co.apply_events(r, hs, tk)[0] == 0
         if step % 5 == 4:
-            q = docs[int(rng.integers(0, len(docs)))]
-            q = q[:BS * int(rng.integers(0, len(q) // BS + 1))] + rng.integers(0, 128256, size=int(rng.integers(0, 20))).tolist()
-            tok, off = csr([q])
+            qs = []
+            for _ in range(int(rng.integers(1, 5))):
+                q = docs[int(rng.integers(0, 4))]                 # a few documents: the prompts of one call overlap
+                qs.append(q[:BS * int(rng.integers(0, len(q) // BS + 1))] + rng.integers(0, 128256, size=int(rng.integers(0, 20))).tolist())
+            tok, off = csr(qs)
             s1, h1 = ix.score_batch(tok, off)
             s2, h2, _, _ = co.score_batch(tok, off)
             assert np.array_equal(s1, s2) and np.array_equal(h1, h2), step
         if step % 7 == 6:
             d2 = docs[int(rng.integers(0, len(docs)))]
             keys, _ = co.hash_keys(np.array(d2, np.uint32), [0, len(d2)])
-            uk = np.unique(keys)
+            uk = np.concatenate([keys, keys[::-2], keys[:1]])      # repeated keys: the last position touches last
             r1 = ix.lookup(0, uk); r2 = co.lookup(0, uk)
             assert np.array_equal(r1[2], r2[2]), step
             for i in range(len(uk)):

@@ -356,7 +356,7 @@ def test_other_block_sizes(B):
 # ---- exact-LRU and CLOCK ----------------------------------------------------------------------------------------------
 def test_exact_lru_stamps_every_present_key():
     """After score_keys, a capped write evicts exactly what the reference evicts: Lookup refreshed every present key of
-    every prompt (no early exit), prompt after prompt."""
+    every prompt (no early exit), prompt after prompt, so a key held by several prompts ranks by the last of them."""
     rng = np.random.default_rng(21)
     CAP, P = 200, 16
     ix = kvidx.Index(capacity=CAP, pods_per_key=3, max_pods=P, lru_exact=1)
@@ -367,10 +367,12 @@ def test_exact_lru_stamps_every_present_key():
             assert t.add(0, allk[i:i + 10] ^ np.uint64(0x55), allk[i:i + 10], [PT(i % 7), PT(9, 1)]) == 0
     absent = rng.integers(1, 1 << 63, 20, dtype=np.uint64)
     lists = []
-    perm = rng.permutation(allk[:120])                           # disjoint prompts: stamps of one call are ordered
+    perm = rng.permutation(allk[:120])
     for i in range(12):
         ks = perm[10 * i:10 * (i + 1)]
         ks = np.concatenate([ks, ks[:: 1 + i % 4]])               # repeats: the later one refreshes again
+        if i % 4 == 3:
+            ks = np.concatenate([ks, perm[:5 * i:7]])             # keys of earlier prompts: they rank as of this one
         if i % 3 == 0:
             ks = np.concatenate([absent[i:i + 1], ks])            # the walk ends at block 0; Lookup still touches the rest
         elif i % 3 == 1:

@@ -229,16 +229,23 @@ def test_crowded_small_table_with_rebuild(monkeypatch):
 
 @pytest.mark.parametrize("capped", [False, True])
 def test_exact_lru_recency_ranks(capped, monkeypatch):
-    """Exact-LRU handles, one event per call (so call-granular exactness is full exactness): recency ranks of every
-    request key and engine mapping equal the oracle's, with the capacity above the contents and with it capped."""
+    """Exact-LRU handles: recency ranks of every request key and engine mapping equal the oracle's.  Capacity above the
+    contents: whole batches of four pods, replayed on the oracle in the order their stamps give (each pod's events in
+    order, pods in ascending id).  Capped: one event per call, so that eviction after each call is eviction in order."""
     _phase1_env(monkeypatch, None)
     B = 4
     cap = 150 if capped else 1 << 14
-    s = _stream(B, "a1", 41 + capped)
+    s = _stream(B, "a1" if capped else "a", 41 + capped)
     ix, co = _pair(B, capacity=cap, oracle_size=cap, lru_exact=1)
     for r in range(3):
-        for e in s.batch(80):
-            _apply(ix, co, [e], B, SEED_HASH, None)
+        if capped:
+            for e in s.batch(80):
+                _apply(ix, co, [e], B, SEED_HASH, None)
+        else:
+            batch = s.batch(80)
+            exp_drop, _ = ws.expect_batch(co, sorted(batch, key=lambda e: e.pod), B, SEED_HASH, False)
+            assert ix.apply_events(*ws.pack(batch)) == (0, exp_drop)
+            assert len({e.pod for e in batch}) > 1
         got = ix.snapshot()
         assert ws.recency_ranks(got) == co.snapshot(recency=True)
     if capped:
