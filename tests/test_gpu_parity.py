@@ -567,9 +567,10 @@ def test_round_scratch_grows_and_shrinks_through_both_pipelines(monkeypatch, cap
 
 def test_config5_scores_while_the_write_path_runs():
     """BASELINE config #5 in miniature: one thread keeps storing and removing documents through apply_events while another
-    scores prompts of documents the writer never touches.  Calls on one handle serialise, so every Score() sees the index
-    between two event batches; the untouched documents' scores must be exact in every call, and the final index must equal
-    the oracle's after the same event sequence."""
+    scores prompts of documents the writer never touches.  Reads and writes on one handle do not serialise (they take
+    different host locks and run on different streams): a Score() may run while an event batch is being applied.  The
+    untouched documents' scores must be exact in every call, and the final index must equal the oracle's after the same
+    event sequence.  Reads of keys the writer changes are checked in tests/test_gpu_reads_beside_writes.py."""
     import threading
     wl = synth.Workload(5, 1024, 1 << 14, 32)
     ix, co = _index_pair(capacity=1 << 16, max_pods=32)
