@@ -220,6 +220,66 @@ int kvidx_score_turn_sparse(kvidx_t* idx, const uint64_t* keys, const int64_t* k
                             uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out,
                             uint64_t* new_keys_out, int64_t* new_key_off_out);
 
+/* ---- prefix store and Score() from text (tokenization.Pool.processTask, pool.go:198-237) ------------------------------
+ * prefixstore.LRUTokenStore (lru_store.go:54-190) on the device, one per handle: cached tokenizations, so that a prompt
+ * whose text repeats an earlier prompt's is scored without going back to the tokenizer.  Text is cut into block_bytes-byte
+ * blocks; a partial last block is never stored or looked up.  Block b's key is XXH64 (seed 0) of the previous block's key
+ * (little-endian u64; 0 for block 0) followed by the block's bytes -- the host store's chain (kvhost_xxhash64).  A block
+ * holds the tokens whose END offset is <= the block's end and that no earlier block took (zero-width tokens included).
+ * One map, no model in the key.  Add inserts or replaces a block's tokens and refreshes it; Find walks the blocks up to
+ * the first miss, refreshes each hit, and returns their tokens with ratio = (end of the last hit block) / text length
+ * (0.0 when nothing hits).  Exact LRU over cache_blocks keys.
+ * A call holds many prompts (text / text_off: CSR of bytes, prompt i owns text[text_off[i] .. text_off[i+1]); text_off[0]
+ * may be non-zero) and equals the host store applying them one after another in array order: an add's touches run prompt
+ * by prompt, block by block, the last add of a key wins its tokens, and the eviction down to the cache_blocks most recently
+ * touched keys runs once, after the add call (every touch of an add is an insert or an update, so the resident set and
+ * every later find equal the sequential store's).  Finds never evict.
+ * Store calls serialise on the store's own lock; the store is independent of the index's read and write sides, of its
+ * capacity mode and of sharding (on a sharded handle it is rank-local).  Host buffers: pinned ones are copied in place,
+ * pageable ones through pinned chunks.  Errors: NULL handle, negative n_prompts, NULL or non-monotone offsets, NULL arrays
+ * with non-zero counts, a store call before kvidx_text_store_init, a second init, cache_blocks or block_bytes <= 0
+ * -> KVIDX_EINVAL; a device allocation that fails -> KVIDX_ENOMEM.  n_prompts == 0 -> 0, nothing written.
+ *
+ * kvidx_text_store_init: NewLRUTokenStore (defaults there: cache_blocks 500000, block_bytes 256, lru_store.go:30-33).
+ * kvidx_text_store_add: AddTokenization of every prompt.  tok / tok_off: CSR of the prompts' token ids (tok_off[0] may be
+ *   non-zero); tok_span[2 t], tok_span[2 t + 1]: token t's [low, high) byte offsets in its prompt's text.  A prompt with no
+ *   text or no tokens adds nothing (lru_store.go:96-98).
+ * kvidx_text_store_find: FindLongestContainedTokens of every prompt.  tok_off_out[n_prompts + 1] (from 0) is always
+ *   filled; tok_out NULL or tok_cap below the total -> KVIDX_ENOSPC, and the find refreshes nothing.  ratio_out may be NULL.
+ * kvidx_text_store_len: keys resident.
+ * kvidx_text_hash_keys: the block keys of every prompt at block_bytes (prompt-major, key_off_out[n_prompts + 1] from 0), as
+ *   the store computes them; needs an initialised store (its stream and staging), whose contents it does not touch.
+ * kvidx_score_text[_sparse]: processTask + GetPodScores steps 2-4.  One find over the batch (refreshing as above); prompt i
+ *   is scored from its contained tokens when ratio_i >= min_ratio (the reference's `overlapRatio < min` test, negated),
+ *   with the kvidx_score_batch dispatch at the batch's size, so its row equals kvidx_score_batch's of the same tokens on
+ *   every handle mode.  Otherwise its row is all-absent, has_keys 0 and tokenize_out[i] = 1: the caller tokenizes it,
+ *   adds it and scores it.  model, model0, filter and the result rows mean what they mean for kvidx_score_batch;
+ *   has_keys_out, tokenize_out and ratio_out may be NULL.  min_ratio < 0 or NaN -> KVIDX_EINVAL.
+ * kvidx_score_text[_sparse]_dev: the same over device-resident inputs and outputs, on the handle's stream.  It waits on the
+ *   stream twice to size its scratch (the batch's block total, then its token totals), and is asynchronous after that. */
+int kvidx_text_store_init(kvidx_t* idx, int64_t cache_blocks, int32_t block_bytes);
+int kvidx_text_store_add(kvidx_t* idx, const uint8_t* text, const int64_t* text_off, int64_t n_prompts,
+                         const uint32_t* tok, const uint64_t* tok_span, const int64_t* tok_off);
+int kvidx_text_store_find(kvidx_t* idx, const uint8_t* text, const int64_t* text_off, int64_t n_prompts,
+                          uint32_t* tok_out, int64_t tok_cap, int64_t* tok_off_out, double* ratio_out);
+int kvidx_text_store_len(kvidx_t* idx, int64_t* blocks_out);
+int kvidx_text_hash_keys(kvidx_t* idx, const uint8_t* text, const int64_t* text_off, int64_t n_prompts, int32_t block_bytes,
+                         uint64_t* keys_out, int64_t* key_off_out);
+int kvidx_score_text(kvidx_t* idx, const uint8_t* text, const int64_t* text_off, int64_t n_prompts,
+                     const uint32_t* model, uint32_t model0, const uint64_t* filter, double min_ratio,
+                     double* scores_out, uint8_t* has_keys_out, uint8_t* tokenize_out, double* ratio_out);
+int kvidx_score_text_sparse(kvidx_t* idx, const uint8_t* text, const int64_t* text_off, int64_t n_prompts,
+                            const uint32_t* model, uint32_t model0, const uint64_t* filter, double min_ratio,
+                            uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out,
+                            uint8_t* tokenize_out, double* ratio_out);
+int kvidx_score_text_dev(kvidx_t* idx, const uint8_t* d_text, const int64_t* d_text_off, int64_t n_prompts,
+                         const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, double min_ratio,
+                         double* d_scores_out, uint8_t* d_has_keys_out, uint8_t* d_tokenize_out, double* d_ratio_out);
+int kvidx_score_text_sparse_dev(kvidx_t* idx, const uint8_t* d_text, const int64_t* d_text_off, int64_t n_prompts,
+                                const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, double min_ratio,
+                                uint16_t* d_pods_out, double* d_scores_out, uint8_t* d_cnt_out, uint8_t* d_has_keys_out,
+                                uint8_t* d_tokenize_out, double* d_ratio_out);
+
 /* ---- write path --------------------------------------------------------------- */
 
 /* Index.Add (index.go:127, in_memory.go:149-209): n (engine,request) key pairs of one model,

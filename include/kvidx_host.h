@@ -68,6 +68,21 @@ int kvhost_get_pod_scores_turn(kvhost_t* h, const uint64_t* keys, size_t n_keys,
                                const char* model, const char* const* pods, size_t n_pods, const char** pod_out, double* score_out,
                                uint64_t* new_keys_out);
 
+/* GetPodScores for a batch of prompts (model and pod filter shared by the batch), read_mu held from the filter to the pod
+ * names as in kvhost_get_pod_scores.  Results: pod_out / score_out hold n * KVIDX_MAX_PODS_PER_KEY entries, prompt i's at
+ * i * KVIDX_MAX_PODS_PER_KEY; cnt_out[i] = its entry count, or -1 for (nil, nil) (no full block).  With enable_metrics each
+ * scored prompt counts one Lookup, as kvhost_get_pod_scores does.
+ * kvhost_get_pod_scores_text: prompt i is text[text_off[i] .. text_off[i+1]), looked up in the device prefix store of the
+ *   index (kvidx_text_store_init on kvhost_index(h) first) and scored by kvidx_score_text_sparse: a prompt whose cached
+ *   prefix covers less than min_ratio of its text gets cnt_out[i] = -1 and tokenize_out[i] = 1 (tokenize it,
+ *   kvidx_text_store_add it, and score it with kvhost_get_pod_scores_batch).
+ * kvhost_get_pod_scores_batch: prompt i is tokens[tok_off[i] .. tok_off[i+1]). */
+int kvhost_get_pod_scores_text(kvhost_t* h, const uint8_t* text, const int64_t* text_off, size_t n, const char* model,
+                               const char* const* pods, size_t n_pods, double min_ratio, const char** pod_out, double* score_out,
+                               int32_t* cnt_out, uint8_t* tokenize_out);
+int kvhost_get_pod_scores_batch(kvhost_t* h, const uint32_t* tokens, const int64_t* tok_off, size_t n, const char* model,
+                                const char* const* pods, size_t n_pods, const char** pod_out, double* score_out, int32_t* cnt_out);
+
 /* kvblock.Index with strings.  entries are (pod, tier) name pairs. */
 int kvhost_index_add(kvhost_t* h, const char* model, const uint64_t* engine, size_t n_engine, const uint64_t* request, size_t n_request,
                      const char* const* pods, const char* const* tiers, size_t n_entries);

@@ -30,7 +30,9 @@
 #include "kernels_keys.cuh"
 #include "kernels_turn.cuh"
 #include "kernels_route.cuh"
+#include "kernels_text.cuh"
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 using namespace kvx;
 
@@ -179,6 +181,9 @@ struct kvidx {
                                    // (faster than the lane-per-prompt kernel P at every size swept up to 131 072)
     // multi-part class pipeline: a part's kernel G on a low-priority stream, its short kernels (G2, H, P, R) on a high-priority one
     cudaStream_t hp_stream[kMaxParts] = {}, lp_stream[kMaxParts] = {}; cudaEvent_t ev_g[kMaxParts] = {}, ev_r[kMaxParts] = {};
+    // the device prefix store (kvidx_text_store_*): its own lock, independent of the read and write sides
+    std::mutex mu_text;
+    struct TextStore* text = nullptr;
 };
 
 namespace {
@@ -1277,6 +1282,8 @@ int launch_hash_keys(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int6
     return 0;
 }
 
+void delete_text_store(TextStore* s);
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------
@@ -1465,6 +1472,7 @@ void kvidx_destroy(kvidx_t* x) {
     if (!x) return;
     cudaSetDevice(x->device);
     cudaDeviceSynchronize();
+    delete_text_store(x->text);
     if (x->queue) { delete_submit_queue(x->queue); x->queue = nullptr; }
     for (int i = 0; i < 2; ++i) {
         x->d_tok[i].release(); x->d_off[i].release(); x->d_model[i].release(); x->d_filter[i].release();
@@ -2120,43 +2128,43 @@ void release_snap(kvidx* x) { x->d_snap.release(); }
 
 // device -> caller's buffer: directly if it is pinned, else through the two pinned chunks (the copy engine fills one while
 // the host empties the other)
-int stage_d2h(kvidx* x, void* dst, const void* src, size_t n, cudaStream_t st) {
+int stage_d2h(PinBuf* hb, cudaEvent_t* ev, void* dst, const void* src, size_t n, cudaStream_t st) {
     if (n == 0) return 0;
     if (is_device_accessible_host(dst)) {             // a pinned caller buffer: one copy, no staging
         CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         return 0;
     }
-    CK(x->h_snap[0].need(kSnapChunk));
-    CK(x->h_snap[1].need(kSnapChunk));
+    CK(hb[0].need(kSnapChunk));
+    CK(hb[1].need(kSnapChunk));
     const size_t nc = (n + kSnapChunk - 1) / kSnapChunk;
     for (size_t k = 0; k <= nc; ++k) {
         if (k < nc) {
             const size_t off = k * kSnapChunk, len = std::min(kSnapChunk, n - off);
-            CK(cudaMemcpyAsync(x->h_snap[k & 1].p, static_cast<const char*>(src) + off, len, cudaMemcpyDeviceToHost, st));
-            CK(cudaEventRecord(x->ev_snap[k & 1], st));
+            CK(cudaMemcpyAsync(hb[k & 1].p, static_cast<const char*>(src) + off, len, cudaMemcpyDeviceToHost, st));
+            CK(cudaEventRecord(ev[k & 1], st));
         }
         if (k > 0) {
             const size_t j = k - 1, off = j * kSnapChunk, len = std::min(kSnapChunk, n - off);
-            CK(cudaEventSynchronize(x->ev_snap[j & 1]));
-            memcpy(static_cast<char*>(dst) + off, x->h_snap[j & 1].p, len);
+            CK(cudaEventSynchronize(ev[j & 1]));
+            memcpy(static_cast<char*>(dst) + off, hb[j & 1].p, len);
         }
     }
     return 0;
 }
 // caller's buffer -> device, the same way round
-int stage_h2d(kvidx* x, void* dst, const void* src, size_t n, cudaStream_t st) {
+int stage_h2d(PinBuf* hb, cudaEvent_t* ev, void* dst, const void* src, size_t n, cudaStream_t st) {
     if (n == 0) return 0;
     if (is_device_accessible_host(src)) { CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, st)); return 0; }
-    CK(x->h_snap[0].need(kSnapChunk));
-    CK(x->h_snap[1].need(kSnapChunk));
+    CK(hb[0].need(kSnapChunk));
+    CK(hb[1].need(kSnapChunk));
     const size_t nc = (n + kSnapChunk - 1) / kSnapChunk;
     for (size_t k = 0; k < nc; ++k) {
         const size_t off = k * kSnapChunk, len = std::min(kSnapChunk, n - off);
-        if (k >= 2) CK(cudaEventSynchronize(x->ev_snap[k & 1]));          // the copy out of this chunk two steps ago is done
-        memcpy(x->h_snap[k & 1].p, static_cast<const char*>(src) + off, len);
-        CK(cudaMemcpyAsync(static_cast<char*>(dst) + off, x->h_snap[k & 1].p, len, cudaMemcpyHostToDevice, st));
-        CK(cudaEventRecord(x->ev_snap[k & 1], st));
+        CK(cudaEventSynchronize(ev[k & 1]));          // the copy out of this chunk two steps (or one call) ago is done
+        memcpy(hb[k & 1].p, static_cast<const char*>(src) + off, len);
+        CK(cudaMemcpyAsync(static_cast<char*>(dst) + off, hb[k & 1].p, len, cudaMemcpyHostToDevice, st));
+        CK(cudaEventRecord(ev[k & 1], st));
     }
     return 0;
 }
@@ -2257,7 +2265,7 @@ int snapshot_impl(kvidx* x, void* buf, uint64_t R, uint64_t E, bool rec) {
     hd.pod_span = x->h_misc.as<SnapMisc>()->pod_span;
     hd.model_span = std::max(model_span_req, model_span_eng);
     memcpy(buf, &hd, sizeof hd);
-    return stage_d2h(x, static_cast<char*>(buf) + kSnapHeaderBytes, out, body, st);
+    return stage_d2h(x->h_snap, x->ev_snap, static_cast<char*>(buf) + kSnapHeaderBytes, out, body, st);
 }
 
 int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t restored_out[2]) {
@@ -2280,7 +2288,7 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
     CK(cudaMemsetAsync(&d_chk[0].first_bad, 0xff, 8, st));
     CK(cudaMemsetAsync(&d_chk[1].first_bad, 0xff, 8, st));
     uint8_t* dbody = d + body_off;
-    int rc = stage_h2d(x, dbody, body, nbody, st);
+    int rc = stage_h2d(x->h_snap, x->ev_snap, dbody, body, nbody, st);
     if (rc) return rc;
     const uint4* req_rec = reinterpret_cast<const uint4*>(dbody);
     const unsigned long long* eng_rec = reinterpret_cast<const unsigned long long*>(dbody + 32 * R);
@@ -2685,6 +2693,527 @@ int kvidx_pod_inventory(kvidx_t* x, uint32_t model, uint32_t flags, uint64_t* en
     if (sole_engine_out) memcpy(sole_engine_out, h + n_ent + 2 * P, P * 8);
     if (totals_out) memcpy(totals_out, h + n_ent + 3 * P, 4 * 8);
     return 0;
+}
+
+}  // extern "C"
+
+// ---- the device prefix store (kvidx_text_store_*, kernels_text.cuh) -----------------------------------------------------
+struct TextStore {
+    int64_t cap_blocks = 0; uint32_t B = 0;
+    cudaStream_t stream = nullptr;            // kvidx_text_store_add / _find (Score() from text runs on the handle's stream)
+    cudaEvent_t ev_last = nullptr;            // the end of the last store call, on whichever stream it ran: the next one waits
+    cudaEvent_t ev_stage[2] = {nullptr, nullptr};
+    PinBuf h_stage[2];                        // pinned chunks for pageable host buffers
+    PinBuf h_misc;
+    TextTable t{};
+    void* tab = nullptr;                      // the table's arrays, one allocation
+    uint32_t* arena = nullptr; int64_t arena_cap = 0, arena_used = 0;
+    int64_t resident = 0;
+    unsigned long long clock = 0;             // recency stamps handed out so far
+    DevBuf d_in, d_blk, d_scr, d_tok, d_cub, d_out;
+};
+
+namespace {
+
+constexpr int64_t kTextLaneMax = 16384;       // batches below this many prompts hash with 4 lanes per prompt, larger ones with 1
+
+void delete_text_store(TextStore* s) {
+    if (!s) return;
+    if (s->tab) cudaFree(s->tab);
+    if (s->arena) cudaFree(s->arena);
+    s->d_in.release(); s->d_blk.release(); s->d_scr.release(); s->d_tok.release(); s->d_cub.release(); s->d_out.release();
+    s->h_stage[0].release(); s->h_stage[1].release(); s->h_misc.release();
+    for (auto& e : s->ev_stage) if (e) cudaEventDestroy(e);
+    if (s->ev_last) cudaEventDestroy(s->ev_last);
+    if (s->stream) cudaStreamDestroy(s->stream);
+    delete s;
+}
+
+int nomem(cudaError_t e, const char* what) {
+    cudaGetLastError();
+    return fail(e == cudaErrorMemoryAllocation ? KVIDX_ENOMEM : KVIDX_ECUDA, "prefix store: %s: %s", what, cudaGetErrorString(e));
+}
+#define TK(call, what) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return nomem(e_, what); } while (0)
+
+unsigned text_grid(kvidx* x, int64_t threads) {
+    return (unsigned)std::max<int64_t>(1, std::min<int64_t>((threads + kTextThreads - 1) / kTextThreads, (int64_t)x->sm_count * 16));
+}
+
+// a fresh, empty table of `slots` slots
+int text_table_alloc(TextStore* s, uint64_t slots, TextTable* t, void** mem, cudaStream_t st) {
+    const size_t bytes = (size_t)slots * (8 + 8 + 8 + 8 + 4);
+    TK(cudaMalloc(mem, bytes), "table");
+    uint8_t* p = static_cast<uint8_t*>(*mem);
+    t->key = reinterpret_cast<uint64_t*>(p);
+    t->stamp = reinterpret_cast<unsigned long long*>(p + slots * 8);
+    t->off = reinterpret_cast<int64_t*>(p + slots * 16);
+    t->len = reinterpret_cast<int64_t*>(p + slots * 24);
+    t->state = reinterpret_cast<uint32_t*>(p + slots * 32);
+    t->mask = slots - 1;
+    CK(cudaMemsetAsync(*mem, 0, bytes, st));
+    return 0;
+}
+
+// Move the full slots whose stamp is >= keep_from into a fresh table of `slots` slots (growth: keep_from 0; eviction: the
+// cut).  Records stay where they are in the arena.
+int text_rebuild(kvidx* x, TextStore* s, uint64_t slots, unsigned long long keep_from, cudaStream_t st) {
+    TextTable nt{}; void* mem = nullptr;
+    if (int rc = text_table_alloc(s, slots, &nt, &mem, st)) return rc;
+    text_rebuild_kernel<<<text_grid(x, (int64_t)s->t.mask + 1), kTextThreads, 0, st>>>(s->t, nt, keep_from);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    cudaFree(s->tab);
+    s->tab = mem; s->t = nt;
+    return 0;
+}
+
+// in-place inclusive sum of a[1 .. n] (a[0] = 0): CSR offsets from counts
+int text_scan(kvidx* x, TextStore* s, int64_t* a, int64_t n, cudaStream_t st) {
+    if (n <= 0) return 0;
+    if (n >= (1ll << 31)) return fail(KVIDX_EINVAL, "prefix store: %lld elements in one call", (long long)n);
+    size_t tb = 0;
+    CK(cub::DeviceScan::InclusiveSum(nullptr, tb, a + 1, a + 1, (int)n, st));
+    TK(s->d_cub.need(tb), "scan scratch");
+    CK(cub::DeviceScan::InclusiveSum(s->d_cub.p, tb, a + 1, a + 1, (int)n, st));
+    x->launches += 1;
+    return 0;
+}
+
+// read n int64 values from the device (synchronises st)
+int text_read(TextStore* s, const int64_t* const* src, int n, int64_t* out, cudaStream_t st) {
+    CK(s->h_misc.need(64));
+    int64_t* h = s->h_misc.as<int64_t>();
+    for (int i = 0; i < n; ++i) CK(cudaMemcpyAsync(h + i, src[i], 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int i = 0; i < n; ++i) out[i] = h[i];
+    return 0;
+}
+
+// Block offsets of the call (d_blk: n + 1 int64, scanned) and their total.  tok_off (an add call): prompts without tokens
+// have no blocks.
+int text_blocks(kvidx* x, TextStore* s, const int64_t* text_off, const int64_t* tok_off, int64_t n, int64_t* nblk, cudaStream_t st) {
+    TK(s->d_blk.need((size_t)(n + 1) * 8), "block offsets");
+    int64_t* bo = s->d_blk.as<int64_t>();
+    CK(cudaMemsetAsync(bo, 0, 8, st));
+    text_block_counts_kernel<<<text_grid(x, n), kTextThreads, 0, st>>>(text_off, tok_off, n, s->B, bo);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    if (int rc = text_scan(x, s, bo, n, st)) return rc;
+    const int64_t* p = bo + n;
+    return text_read(s, &p, 1, nblk, st);
+}
+
+// Make room for `incoming` more tokens in the arena: compact the live records (into a larger arena when live + incoming
+// would fill more than half of it).
+int text_arena_room(kvidx* x, TextStore* s, int64_t incoming, cudaStream_t st) {
+    if (s->arena_used + incoming <= s->arena_cap) return 0;
+    const uint64_t slots = s->t.mask + 1;
+    TK(s->d_scr.need((slots + 1) * 8 + 64), "compaction scratch");
+    int64_t* newoff = s->d_scr.as<int64_t>();
+    CK(cudaMemsetAsync(newoff, 0, 8, st));
+    text_rec_len_kernel<<<text_grid(x, (int64_t)slots), kTextThreads, 0, st>>>(s->t, newoff);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    if (int rc = text_scan(x, s, newoff, (int64_t)slots, st)) return rc;
+    int64_t live = 0;
+    const int64_t* p = newoff + slots;
+    if (int rc = text_read(s, &p, 1, &live, st)) return rc;
+    const int64_t cap = std::max<int64_t>(s->arena_cap, 2 * (live + incoming));
+    uint32_t* na = nullptr;
+    TK(cudaMalloc((void**)&na, (size_t)std::max<int64_t>(cap, 1) * 4), "token arena");
+    text_compact_kernel<<<text_grid(x, (int64_t)slots * 32), kTextThreads, 0, st>>>(s->t, newoff, s->arena, na);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    cudaFree(s->arena);
+    s->arena = na; s->arena_cap = cap; s->arena_used = live;
+    return 0;
+}
+
+// scratch carved from one DevBuf, 256-byte aligned sections
+struct TextCarve {
+    uint8_t* base; size_t at = 0;
+    template <class T> T* take(int64_t n) { T* p = reinterpret_cast<T*>(base + at); at += ((size_t)std::max<int64_t>(n, 1) * sizeof(T) + 255) & ~(size_t)255; return p; }
+};
+
+// The device inputs of a store call: text (prompt i at text + text_off[i] - text_base) and its offsets.
+struct TextIn { const uint8_t* text; const int64_t* off; int64_t base; int64_t n; };
+
+template <class K> void text_launch_lanes(kvidx* x, int64_t n, K k) {
+    if (n < kTextLaneMax) k(std::integral_constant<int, 4>{}, text_grid(x, n * 4));
+    else k(std::integral_constant<int, 1>{}, text_grid(x, n));
+}
+
+// Find, pass one, for the call `in`: block offsets, hit slots, token counts (tok_off: n + 1, scanned), ratios; with
+// min_ratio >= 0 also the Score() CSR counts (score_off, scanned) and tokenize flags.  totals = {tokens, score tokens}.
+struct FindScratch { int64_t nblk = 0; uint32_t* hit = nullptr; int64_t* nhit = nullptr; int64_t* tok_off = nullptr; int64_t* score_off = nullptr;
+                     double* ratio = nullptr; uint8_t* tokenize = nullptr; int64_t totals[2] = {0, 0}; };
+int text_find_pass1(kvidx* x, TextStore* s, const TextIn& in, double min_ratio, FindScratch& f, cudaStream_t st) {
+    const int64_t n = in.n;
+    if (int rc = text_blocks(x, s, in.off, nullptr, n, &f.nblk, st)) return rc;
+    TextCarve c{nullptr};
+    c.take<uint32_t>(f.nblk); c.take<int64_t>(n); c.take<int64_t>(n + 1); c.take<int64_t>(n + 1); c.take<double>(n); c.take<uint8_t>(n);
+    TK(s->d_scr.need(c.at), "find scratch");
+    c = TextCarve{s->d_scr.as<uint8_t>()};
+    f.hit = c.take<uint32_t>(f.nblk); f.nhit = c.take<int64_t>(n); f.tok_off = c.take<int64_t>(n + 1); f.score_off = c.take<int64_t>(n + 1);
+    f.ratio = c.take<double>(n); f.tokenize = c.take<uint8_t>(n);
+    CK(cudaMemsetAsync(f.tok_off, 0, 8, st));
+    CK(cudaMemsetAsync(f.score_off, 0, 8, st));
+    const bool score = min_ratio >= 0;
+    const int64_t* bo = s->d_blk.as<int64_t>();
+    text_launch_lanes(x, n, [&](auto L, unsigned grid) {
+        text_find_kernel<L.value><<<grid, kTextThreads, 0, st>>>(s->t, in.text, in.off, in.base, n, s->B, bo, f.hit, f.nhit, f.tok_off,
+                                                                 f.ratio, min_ratio, score ? f.score_off : nullptr, f.tokenize);
+    });
+    x->launches += 1;
+    CK(cudaGetLastError());
+    if (int rc = text_scan(x, s, f.tok_off, n, st)) return rc;
+    if (score) { if (int rc = text_scan(x, s, f.score_off, n, st)) return rc; }
+    const int64_t* p[2] = {f.tok_off + n, f.score_off + n};
+    return text_read(s, p, score ? 2 : 1, f.totals, st);
+}
+
+// Find, pass two: refresh every hit in call order and copy tokens to out (offsets out_off; gate: skip prompts flagged for
+// the tokenizer; out NULL: refresh only).
+int text_find_pass2(kvidx* x, TextStore* s, int64_t n, const FindScratch& f, const int64_t* out_off, const uint8_t* gate, uint32_t* out,
+                    cudaStream_t st) {
+    const unsigned long long base = s->clock + 1;
+    s->clock += (unsigned long long)f.nblk + 1;
+    text_gather_kernel<<<text_grid(x, n * 32), kTextThreads, 0, st>>>(s->t, s->arena, n, s->d_blk.as<int64_t>(), f.hit, f.nhit, base,
+                                                                      out_off, gate, out);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// AddTokenization for every prompt of the call, in array order; then the cut down to cap_blocks keys.
+int text_add(kvidx* x, TextStore* s, const TextIn& in, const uint32_t* tok, const uint64_t* span, const int64_t* tok_off, int64_t tok_base,
+             cudaStream_t st) {
+    const int64_t n = in.n;
+    int64_t nblk = 0;
+    if (int rc = text_blocks(x, s, in.off, tok_off, n, &nblk, st)) return rc;
+    if (nblk == 0) return 0;
+    // room for every key of the call at load <= 1/2 before the cut
+    const uint64_t want = pow2ceil((uint64_t)std::max<int64_t>(2 * (s->resident + nblk), 1024));
+    if (want > s->t.mask + 1) { if (int rc = text_rebuild(x, s, want, 0, st)) return rc; }
+    TextCarve c{nullptr};
+    c.take<uint64_t>(nblk); c.take<int64_t>(nblk); c.take<int64_t>(nblk + 1); c.take<uint32_t>(nblk); c.take<unsigned long long>(1);
+    TK(s->d_out.need(c.at), "add scratch");
+    c = TextCarve{s->d_out.as<uint8_t>()};
+    uint64_t* key = c.take<uint64_t>(nblk);
+    int64_t* src = c.take<int64_t>(nblk);
+    int64_t* pos = c.take<int64_t>(nblk + 1);
+    uint32_t* slot_of = c.take<uint32_t>(nblk);
+    unsigned long long* inserted = c.take<unsigned long long>(1);
+    const int64_t* bo = s->d_blk.as<int64_t>();
+    text_launch_lanes(x, n, [&](auto L, unsigned grid) {
+        text_hash_kernel<L.value><<<grid, kTextThreads, 0, st>>>(in.text, in.off, in.base, n, s->B, bo, key);
+    });
+    CK(cudaMemsetAsync(pos, 0, 8, st));
+    text_add_ranges_kernel<<<text_grid(x, n), kTextThreads, 0, st>>>(tok_off, tok_base, span, n, s->B, bo, src, pos);
+    x->launches += 2;
+    CK(cudaGetLastError());
+    if (int rc = text_scan(x, s, pos, nblk, st)) return rc;
+    int64_t ntok = 0;
+    const int64_t* pp = pos + nblk;
+    if (int rc = text_read(s, &pp, 1, &ntok, st)) return rc;
+    if (int rc = text_arena_room(x, s, ntok, st)) return rc;
+    const unsigned long long base = s->clock + 1;
+    s->clock += (unsigned long long)nblk + 1;
+    CK(cudaMemsetAsync(inserted, 0, 8, st));
+    if (ntok > 0) text_add_copy_kernel<<<text_grid(x, nblk * 32), kTextThreads, 0, st>>>(tok, src, pos, nblk, s->arena_used, s->arena);
+    text_add_touch_kernel<<<text_grid(x, nblk), kTextThreads, 0, st>>>(s->t, key, nblk, base, slot_of, inserted);
+    text_add_commit_kernel<<<text_grid(x, nblk), kTextThreads, 0, st>>>(s->t, nblk, base, slot_of, pos, s->arena_used);
+    x->launches += 3;
+    CK(cudaGetLastError());
+    s->arena_used += ntok;
+    CK(cudaMemcpyAsync(s->h_misc.p, inserted, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    s->resident += (int64_t)*s->h_misc.as<unsigned long long>();
+    if (s->resident <= s->cap_blocks) return 0;
+    // the cut: keep the cap_blocks most recently touched keys (stamps are distinct: one sort finds the threshold)
+    const int64_t R = s->resident;
+    size_t tb = 0;
+    CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)R, 0, 64, st));
+    TK(s->d_scr.need(((size_t)R * 16 + 511) & ~(size_t)255), "eviction scratch");
+    TK(s->d_cub.need(tb), "eviction sort scratch");
+    unsigned long long* st0 = s->d_scr.as<unsigned long long>();
+    unsigned long long* st1 = st0 + R;
+    CK(cudaMemsetAsync(inserted, 0, 8, st));
+    text_stamps_kernel<<<text_grid(x, (int64_t)s->t.mask + 1), kTextThreads, 0, st>>>(s->t, st0, inserted, nullptr);
+    CK(cub::DeviceRadixSort::SortKeys(s->d_cub.p, tb, st0, st1, (int)R, 0, 64, st));
+    x->launches += 5;
+    const int64_t* tp = reinterpret_cast<const int64_t*>(st1 + (R - s->cap_blocks));
+    int64_t thr = 0;
+    if (int rc = text_read(s, &tp, 1, &thr, st)) return rc;
+    // the kept keys go into a table sized for them (load <= 1/2), not for this call: one large add does not leave a large table
+    const uint64_t keep_slots = pow2ceil((uint64_t)std::max<int64_t>(2 * s->cap_blocks, 1024));
+    if (int rc = text_rebuild(x, s, std::min<uint64_t>(keep_slots, s->t.mask + 1), (unsigned long long)thr, st)) return rc;
+    s->resident = s->cap_blocks;
+    return 0;
+}
+
+int text_check(kvidx* x, int64_t n, const void* text, const int64_t* text_off) {
+    if (!x) return fail(KVIDX_EINVAL, "NULL handle");
+    if (n < 0 || (n > 0 && !text_off)) return fail(KVIDX_EINVAL, "bad arguments");
+    if (!x->text) return fail(KVIDX_EINVAL, "prefix store not initialised (kvidx_text_store_init)");
+    if (n == 0) return 0;
+    if (int rc = check_csr(text_off, n, "text_off")) return rc;
+    if (text_off[n] > text_off[0] && !text) return fail(KVIDX_EINVAL, "NULL text");
+    return 0;
+}
+
+// Upload a host call's text and offsets to d_in: text at 0, offsets after it.  -> the device view.
+int text_upload(kvidx* x, TextStore* s, const uint8_t* text, const int64_t* text_off, int64_t n, size_t extra, TextIn* out, size_t* extra_at,
+                cudaStream_t st) {
+    const int64_t tb = text_off[0], nb = text_off[n] - tb;
+    const size_t off_at = ((size_t)nb + 255) & ~(size_t)255;
+    *extra_at = off_at + (((size_t)(n + 1) * 8 + 255) & ~(size_t)255);
+    TK(s->d_in.need(*extra_at + extra + 64), "input buffer");
+    uint8_t* d = s->d_in.as<uint8_t>();
+    if (int rc = stage_h2d(s->h_stage, s->ev_stage, d, text + tb, (size_t)nb, st)) return rc;
+    if (int rc = stage_h2d(s->h_stage, s->ev_stage, d + off_at, text_off, (size_t)(n + 1) * 8, st)) return rc;
+    *out = TextIn{d, reinterpret_cast<const int64_t*>(d + off_at), tb, n};
+    return 0;
+}
+
+// A store call: the store's lock, the device, and the order after the previous store call on stream st.
+struct TextCall {
+    std::unique_lock<std::mutex> lk;
+    TextStore* s; cudaStream_t st;
+    TextCall(kvidx* x, cudaStream_t stream) : lk(x->mu_text), s(x->text), st(stream) {}
+    int begin(kvidx* x) { CK(cudaSetDevice(x->device)); CK(cudaStreamWaitEvent(st, s->ev_last, 0)); return 0; }
+    // after an error: let nothing of this call run on past the return (the caller's buffers, the store's scratch)
+    int end(int rc) {
+        if (rc) { const std::string keep = g_err; cudaStreamSynchronize(st); cudaGetLastError(); g_err = keep; }
+        cudaEventRecord(s->ev_last, st);
+        return rc;
+    }
+};
+
+// Score() from text: find with the min_ratio gate, then the Score() dispatch on the contained tokens of the passing prompts.
+// `a` carries the model, filter and the result rows (device pointers); tokenize / ratio: device outputs (may be NULL).
+int score_text_run(kvidx* x, TextStore* s, const TextIn& in, double min_ratio, ScoreArgs a, uint8_t* tokenize, double* ratio, cudaStream_t st) {
+    FindScratch f;
+    if (int rc = text_find_pass1(x, s, in, min_ratio, f, st)) return rc;
+    TK(s->d_tok.need((size_t)std::max<int64_t>(f.totals[1], 1) * 4 + 64), "token buffer");
+    if (int rc = text_find_pass2(x, s, in.n, f, f.score_off, f.tokenize, s->d_tok.as<uint32_t>(), st)) return rc;
+    if (tokenize) CK(cudaMemcpyAsync(tokenize, f.tokenize, (size_t)in.n, cudaMemcpyDeviceToDevice, st));
+    if (ratio) CK(cudaMemcpyAsync(ratio, f.ratio, (size_t)in.n * 8, cudaMemcpyDeviceToDevice, st));
+    a.tok_off = f.score_off; a.tok_base = 0; a.n_prompts = in.n;
+    ReadGuard g(x);
+    CK(cudaStreamWaitEvent(st, x->ev_write, 0));
+    return launch_score(x, ScoreIn{s->d_tok.p, false}, a, st);
+}
+
+int score_text_host(kvidx* x, const uint8_t* text, const int64_t* text_off, int64_t n, const uint32_t* model, uint32_t model0,
+                    const uint64_t* filter, double min_ratio, const ScoreArgs& h, uint8_t* tokenize_out, double* ratio_out) {
+    if (int rc = text_check(x, n, text, text_off)) return rc;
+    if (n == 0) return 0;
+    if (!(min_ratio >= 0)) return fail(KVIDX_EINVAL, "min_ratio must be >= 0");
+    TextCall c(x, x->stream);
+    if (int rc = c.begin(x)) return rc;
+    TextStore* s = c.s;
+    const uint32_t FW = x->tv.filter_words;
+    const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
+    const size_t model_b = model ? (size_t)n * 4 : 0, filter_b = filter ? (size_t)n * FW * 8 : 0;
+    const size_t out_b = (size_t)n * rows.row() + (size_t)n * 9;
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    TextIn in; size_t at = 0;
+    int rc = text_upload(x, s, text, text_off, n, al(model_b) + al(filter_b) + al(out_b) + 512, &in, &at, c.st);
+    if (rc) return c.end(rc);
+    uint8_t* d = s->d_in.as<uint8_t>() + at;
+    ScoreArgs a{nullptr, nullptr, 0, n, nullptr, model0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    if (model) { a.model = reinterpret_cast<const uint32_t*>(d); rc = stage_h2d(s->h_stage, s->ev_stage, d, model, model_b, c.st); }
+    if (!rc && filter) { a.filter = reinterpret_cast<const uint64_t*>(d + al(model_b)); rc = stage_h2d(s->h_stage, s->ev_stage, d + al(model_b), filter, filter_b, c.st); }
+    if (rc) return c.end(rc);
+    uint8_t* o = d + al(model_b) + al(filter_b);
+    rows.carve(o, n, a);
+    double* d_ratio = reinterpret_cast<double*>(o + al((size_t)n * rows.row()));
+    uint8_t* d_tokz = reinterpret_cast<uint8_t*>(d_ratio + n);
+    rc = score_text_run(x, s, in, min_ratio, a, d_tokz, d_ratio, c.st);
+    auto back = [&](void* dst, const void* src, size_t b) { return dst && !rc ? (rc = stage_d2h(s->h_stage, s->ev_stage, dst, src, b, c.st)) : rc; };
+    if (rows.sparse) {
+        back(h.sp_scores, a.sp_scores, (size_t)n * kMaxEnt * 8); back(h.sp_pods, a.sp_pods, (size_t)n * kMaxEnt * 2); back(h.sp_cnt, a.sp_cnt, (size_t)n);
+    } else {
+        back(h.dense, a.dense, (size_t)n * rows.P * 8);
+    }
+    back(h.has_keys, a.has_keys, (size_t)n);
+    back(tokenize_out, d_tokz, (size_t)n);
+    back(ratio_out, d_ratio, (size_t)n * 8);
+    if (!rc) { CK(cudaStreamSynchronize(c.st)); }
+    return c.end(rc);
+}
+
+int score_text_dev(kvidx* x, const uint8_t* d_text, const int64_t* d_text_off, int64_t n, double min_ratio, const ScoreArgs& a,
+                   uint8_t* d_tokenize, double* d_ratio) {
+    if (!x) return fail(KVIDX_EINVAL, "NULL handle");
+    if (n < 0 || (n > 0 && !d_text_off)) return fail(KVIDX_EINVAL, "bad arguments");
+    if (!x->text) return fail(KVIDX_EINVAL, "prefix store not initialised (kvidx_text_store_init)");
+    if (n == 0) return 0;
+    if (!(min_ratio >= 0)) return fail(KVIDX_EINVAL, "min_ratio must be >= 0");
+    TextCall c(x, x->stream);
+    if (int rc = c.begin(x)) return rc;
+    return c.end(score_text_run(x, c.s, TextIn{d_text, d_text_off, 0, n}, min_ratio, a, d_tokenize, d_ratio, c.st));
+}
+
+}  // namespace
+
+extern "C" {
+
+int kvidx_text_store_init(kvidx_t* x, int64_t cache_blocks, int32_t block_bytes) {
+    if (!x) return fail(KVIDX_EINVAL, "NULL handle");
+    if (cache_blocks <= 0) return fail(KVIDX_EINVAL, "failed to initialize in-memory index: must provide a positive size");   // lru.New
+    if (block_bytes <= 0) return fail(KVIDX_EINVAL, "block size must be positive");
+    std::lock_guard<std::mutex> g(x->mu_text);
+    if (x->text) return fail(KVIDX_EINVAL, "prefix store already initialised on this handle");
+    CK(cudaSetDevice(x->device));
+    TextStore* s = new TextStore();
+    s->cap_blocks = cache_blocks; s->B = (uint32_t)block_bytes;
+    auto bail = [&](int rc) { delete_text_store(s); return rc; };
+    if (cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&s->ev_last, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&s->ev_stage[0], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&s->ev_stage[1], cudaEventDisableTiming) != cudaSuccess)
+        return bail(fail(KVIDX_ECUDA, "prefix store: stream / event creation failed"));
+    if (int rc = text_table_alloc(s, 1024, &s->t, &s->tab, s->stream)) return bail(rc);
+    s->arena_cap = 1 << 16;
+    if (cudaError_t e = cudaMalloc((void**)&s->arena, (size_t)s->arena_cap * 4)) return bail(nomem(e, "token arena"));
+    if (s->h_misc.need(64) != cudaSuccess) return bail(fail(KVIDX_ENOMEM, "prefix store: pinned scratch"));
+    if (cudaEventRecord(s->ev_last, s->stream) != cudaSuccess || cudaStreamSynchronize(s->stream) != cudaSuccess)
+        return bail(fail(KVIDX_ECUDA, "prefix store: initialisation failed"));
+    x->text = s;
+    return 0;
+}
+
+int kvidx_text_store_len(kvidx_t* x, int64_t* blocks_out) {
+    if (!x || !blocks_out) return fail(KVIDX_EINVAL, "bad arguments");
+    std::lock_guard<std::mutex> g(x->mu_text);
+    if (!x->text) return fail(KVIDX_EINVAL, "prefix store not initialised (kvidx_text_store_init)");
+    *blocks_out = x->text->resident;
+    return 0;
+}
+
+int kvidx_text_store_add(kvidx_t* x, const uint8_t* text, const int64_t* text_off, int64_t n, const uint32_t* tok, const uint64_t* tok_span,
+                         const int64_t* tok_off) {
+    if (int rc = text_check(x, n, text, text_off)) return rc;
+    if (n == 0) return 0;
+    if (!tok_off) return fail(KVIDX_EINVAL, "NULL tok_off");
+    if (int rc = check_csr(tok_off, n)) return rc;
+    const int64_t tb = tok_off[0], nt = tok_off[n] - tb;
+    if (nt > 0 && (!tok || !tok_span)) return fail(KVIDX_EINVAL, "NULL tokens or spans");
+    TextCall c(x, nullptr);
+    c.st = c.s->stream;
+    if (int rc = c.begin(x)) return rc;
+    TextStore* s = c.s;
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t toff_b = al((size_t)(n + 1) * 8), tok_b = al((size_t)nt * 4);
+    TextIn in; size_t at = 0;
+    int rc = text_upload(x, s, text, text_off, n, toff_b + tok_b + (size_t)nt * 16, &in, &at, c.st);
+    if (rc) return c.end(rc);
+    uint8_t* d = s->d_in.as<uint8_t>() + at;
+    int64_t* d_toff = reinterpret_cast<int64_t*>(d);
+    uint32_t* d_tok = reinterpret_cast<uint32_t*>(d + toff_b);
+    uint64_t* d_span = reinterpret_cast<uint64_t*>(d + toff_b + tok_b);
+    rc = stage_h2d(s->h_stage, s->ev_stage, d_toff, tok_off, (size_t)(n + 1) * 8, c.st);
+    if (!rc && nt > 0) rc = stage_h2d(s->h_stage, s->ev_stage, d_tok, tok + tb, (size_t)nt * 4, c.st);
+    if (!rc && nt > 0) rc = stage_h2d(s->h_stage, s->ev_stage, d_span, tok_span + 2 * tb, (size_t)nt * 16, c.st);
+    if (!rc) rc = text_add(x, s, in, d_tok, d_span, d_toff, tb, c.st);
+    if (!rc) { CK(cudaStreamSynchronize(c.st)); }
+    return c.end(rc);
+}
+
+int kvidx_text_store_find(kvidx_t* x, const uint8_t* text, const int64_t* text_off, int64_t n, uint32_t* tok_out, int64_t tok_cap,
+                          int64_t* tok_off_out, double* ratio_out) {
+    if (int rc = text_check(x, n, text, text_off)) return rc;
+    if (n == 0) return 0;
+    if (!tok_off_out) return fail(KVIDX_EINVAL, "NULL tok_off_out");
+    TextCall c(x, nullptr);
+    c.st = c.s->stream;
+    if (int rc = c.begin(x)) return rc;
+    TextStore* s = c.s;
+    TextIn in; size_t at = 0;
+    int rc = text_upload(x, s, text, text_off, n, 0, &in, &at, c.st);
+    FindScratch f;
+    if (!rc) rc = text_find_pass1(x, s, in, -1.0, f, c.st);
+    if (!rc) rc = stage_d2h(s->h_stage, s->ev_stage, tok_off_out, f.tok_off, (size_t)(n + 1) * 8, c.st);
+    if (!rc && ratio_out) rc = stage_d2h(s->h_stage, s->ev_stage, ratio_out, f.ratio, (size_t)n * 8, c.st);
+    if (rc) return c.end(rc);
+    if (f.totals[0] > 0 && (!tok_out || tok_cap < f.totals[0]))       // nothing refreshed: the find has not happened
+        return c.end(fail(KVIDX_ENOSPC, "tok_out holds %lld tokens, the find returns %lld", (long long)(tok_out ? tok_cap : 0), (long long)f.totals[0]));
+    TK(s->d_tok.need((size_t)std::max<int64_t>(f.totals[0], 1) * 4 + 64), "token buffer");
+    rc = text_find_pass2(x, s, n, f, f.tok_off, nullptr, s->d_tok.as<uint32_t>(), c.st);
+    if (!rc && f.totals[0] > 0) rc = stage_d2h(s->h_stage, s->ev_stage, tok_out, s->d_tok.p, (size_t)f.totals[0] * 4, c.st);
+    if (!rc) { CK(cudaStreamSynchronize(c.st)); }
+    return c.end(rc);
+}
+
+int kvidx_text_hash_keys(kvidx_t* x, const uint8_t* text, const int64_t* text_off, int64_t n, int32_t block_bytes, uint64_t* keys_out,
+                         int64_t* key_off_out) {
+    if (!x || n < 0 || (n > 0 && (!text_off || !key_off_out))) return fail(KVIDX_EINVAL, "bad arguments");
+    if (block_bytes <= 0) return fail(KVIDX_EINVAL, "block size must be positive");
+    if (n == 0) return 0;
+    if (int rc = check_csr(text_off, n, "text_off")) return rc;
+    if (text_off[n] > text_off[0] && !text) return fail(KVIDX_EINVAL, "NULL text");
+    int64_t nk = 0;
+    for (int64_t i = 0; i < n; ++i) { key_off_out[i] = nk; nk += (text_off[i + 1] - text_off[i]) / block_bytes; }
+    key_off_out[n] = nk;
+    if (nk == 0) return 0;
+    if (!keys_out) return fail(KVIDX_EINVAL, "NULL keys_out");
+    TextCall c(x, nullptr);
+    if (!c.s) return fail(KVIDX_EINVAL, "prefix store not initialised (kvidx_text_store_init)");
+    c.st = c.s->stream;
+    if (int rc = c.begin(x)) return rc;
+    TextStore* s = c.s;
+    TextIn in; size_t at = 0;
+    int rc = text_upload(x, s, text, text_off, n, (size_t)(n + 1) * 8 + (size_t)nk * 8 + 256, &in, &at, c.st);
+    if (rc) return c.end(rc);
+    int64_t* d_koff = reinterpret_cast<int64_t*>(s->d_in.as<uint8_t>() + at);
+    uint64_t* d_keys = reinterpret_cast<uint64_t*>(d_koff + ((n + 1 + 31) & ~(int64_t)31));
+    CK(cudaMemcpyAsync(d_koff, key_off_out, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, c.st));
+    const uint32_t B = (uint32_t)block_bytes;
+    text_launch_lanes(x, n, [&](auto L, unsigned grid) {
+        text_hash_kernel<L.value><<<grid, kTextThreads, 0, c.st>>>(in.text, in.off, in.base, n, B, d_koff, d_keys);
+    });
+    x->launches += 1;
+    rc = cudaGetLastError() == cudaSuccess ? 0 : fail(KVIDX_ECUDA, "text hash launch failed");
+    if (!rc) rc = stage_d2h(s->h_stage, s->ev_stage, keys_out, d_keys, (size_t)nk * 8, c.st);
+    if (!rc) { CK(cudaStreamSynchronize(c.st)); }
+    return c.end(rc);
+}
+
+int kvidx_score_text(kvidx_t* x, const uint8_t* text, const int64_t* text_off, int64_t n, const uint32_t* model, uint32_t model0,
+                     const uint64_t* filter, double min_ratio, double* scores_out, uint8_t* has_keys_out, uint8_t* tokenize_out, double* ratio_out) {
+    if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_text_host(x, text, text_off, n, model, model0, filter, min_ratio,
+                           ScoreArgs{nullptr, nullptr, 0, n, nullptr, model0, nullptr, scores_out, nullptr, nullptr, nullptr, has_keys_out, nullptr},
+                           tokenize_out, ratio_out);
+}
+
+int kvidx_score_text_sparse(kvidx_t* x, const uint8_t* text, const int64_t* text_off, int64_t n, const uint32_t* model, uint32_t model0,
+                            const uint64_t* filter, double min_ratio, uint16_t* pods_out, double* scores_out, uint8_t* cnt_out,
+                            uint8_t* has_keys_out, uint8_t* tokenize_out, double* ratio_out) {
+    if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_text_host(x, text, text_off, n, model, model0, filter, min_ratio,
+                           ScoreArgs{nullptr, nullptr, 0, n, nullptr, model0, nullptr, nullptr, pods_out, scores_out, cnt_out, has_keys_out, nullptr},
+                           tokenize_out, ratio_out);
+}
+
+int kvidx_score_text_dev(kvidx_t* x, const uint8_t* d_text, const int64_t* d_text_off, int64_t n, const uint32_t* d_model, uint32_t model0,
+                         const uint64_t* d_filter, double min_ratio, double* d_scores_out, uint8_t* d_has_keys_out, uint8_t* d_tokenize_out,
+                         double* d_ratio_out) {
+    if (!x || !d_scores_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_text_dev(x, d_text, d_text_off, n, min_ratio,
+                          ScoreArgs{nullptr, nullptr, 0, n, d_model, model0, d_filter, d_scores_out, nullptr, nullptr, nullptr, d_has_keys_out, nullptr},
+                          d_tokenize_out, d_ratio_out);
+}
+
+int kvidx_score_text_sparse_dev(kvidx_t* x, const uint8_t* d_text, const int64_t* d_text_off, int64_t n, const uint32_t* d_model, uint32_t model0,
+                                const uint64_t* d_filter, double min_ratio, uint16_t* d_pods_out, double* d_scores_out, uint8_t* d_cnt_out,
+                                uint8_t* d_has_keys_out, uint8_t* d_tokenize_out, double* d_ratio_out) {
+    if (!x || !d_pods_out || !d_scores_out || !d_cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
+    return score_text_dev(x, d_text, d_text_off, n, min_ratio,
+                          ScoreArgs{nullptr, nullptr, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr},
+                          d_tokenize_out, d_ratio_out);
 }
 
 }  // extern "C"

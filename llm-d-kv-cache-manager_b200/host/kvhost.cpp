@@ -386,6 +386,21 @@ static bool build_filter(kvhost* h, const char* const* pods, size_t n_pods, std:
     return true;
 }
 
+// With enable_metrics: the instrumented Lookup of indexer.go:150 over every key of one prompt, given as its tokens
+// (keys == nullptr, n = token count) or its request keys (n = key count).
+static void observe_prompt(kvhost* h, const uint32_t* tokens, const uint64_t* keys, size_t n, uint32_t mid, const uint64_t* fm) {
+    if (!h->cfg.enable_metrics) return;
+    const int64_t off[2] = {0, (int64_t)n};
+    const size_t nk = keys ? n : n / (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
+    std::vector<uint64_t> hashed; int64_t koff[2] = {0, 0};
+    std::vector<kvidx_podtier_t> pt(nk * KVIDX_MAX_PODS_PER_KEY); std::vector<uint8_t> kc(nk);
+    int r2 = 0;
+    if (!keys) { hashed.resize(nk); r2 = kvidx_hash_keys(h->ix, tokens, off, 1, nullptr, nullptr, hashed.data(), koff); keys = hashed.data(); }
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!r2) r2 = kvidx_lookup(h->ix, mid, keys, (int64_t)nk, fm, pt.data(), kc.data());
+    observe_lookup(h, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), r2 == 0, pt.data(), kc.data(), nk);
+}
+
 // GetPodScores from step 3 on for one prompt given as its tokens (keys == nullptr, n = token count) or as its request
 // keys (n = key count).
 static int pod_scores(kvhost* h, const uint32_t* tokens, const uint64_t* keys, size_t n, const char* model, const char* const* pods, size_t n_pods,
@@ -411,19 +426,77 @@ static int pod_scores(kvhost* h, const uint32_t* tokens, const uint64_t* keys, s
                         : kvidx_score_batch_sparse(h->ix, tokens, off, 1, nullptr, (uint32_t)mid, fm, ids, sc, &cnt, &has);
     if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
     if (!has) return -1000;                         // (nil, nil): no full block (indexer.go:142-146)
-    if (h->cfg.enable_metrics) {                    // the instrumented Lookup of indexer.go:150: every key of the prompt
-        const size_t nk = keys ? n : n / (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
-        std::vector<uint64_t> hashed; int64_t koff[2] = {0, 0};
-        std::vector<kvidx_podtier_t> pt(nk * KVIDX_MAX_PODS_PER_KEY); std::vector<uint8_t> kc(nk);
-        int r2 = 0;
-        if (!keys) { hashed.resize(nk); r2 = kvidx_hash_keys(h->ix, tokens, off, 1, nullptr, nullptr, hashed.data(), koff); keys = hashed.data(); }
-        const auto t0 = std::chrono::steady_clock::now();
-        if (!r2) r2 = kvidx_lookup(h->ix, (uint32_t)mid, keys, (int64_t)nk, fm, pt.data(), kc.data());
-        observe_lookup(h, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), r2 == 0, pt.data(), kc.data(), nk);
-    }
+    observe_prompt(h, tokens, keys, n, (uint32_t)mid, fm);
     std::lock_guard<std::mutex> g(h->mu);
     for (int i = 0; i < cnt; ++i) { pod_out[i] = h->pods.name(ids[i]); score_out[i] = sc[i]; }
     return cnt;
+}
+
+// GetPodScores for a batch: prompt texts through the device prefix store (text != nullptr; tokenize_out flags the prompts
+// whose cached prefix is too short) or a token CSR.  Like pod_scores, read_mu is held from the filter through the device
+// call to the id -> name mapping, so a pod id freed and reused meanwhile cannot lend its new name to the old pod's entries.
+static int batch_scores(kvhost* h, const uint8_t* text, const int64_t* text_off, const uint32_t* tok, const int64_t* tok_off, size_t n,
+                        const char* model, const char* const* pods, size_t n_pods, double min_ratio, const char** pod_out, double* score_out,
+                        int32_t* cnt_out, uint8_t* tokenize_out) {
+    if (int rc = need_dev(h)) return rc;
+    if (!model || !pod_out || !score_out || !cnt_out || (text_off ? !tokenize_out : !tok_off) || (n_pods && !pods))
+        return hfail(KVIDX_EINVAL, "bad arguments");
+    if (n == 0) return 0;
+    std::shared_lock<std::shared_mutex> rl(h->read_mu);
+    std::vector<uint64_t> mask;
+    bool filtered; int mid;
+    { std::lock_guard<std::mutex> g(h->mu); filtered = build_filter(h, pods, n_pods, mask); mid = h->models.id(model, 65536); }
+    if (mid < 0) return hfail(KVIDX_ERANGE, "too many models");
+    bool none = filtered;                           // a filter whose pods all lie outside the mask width selects nothing
+    for (uint64_t w : mask) none = none && w == 0;
+    std::vector<uint64_t> rows;
+    if (filtered && !none) { rows.resize(n * h->filter_words); for (size_t i = 0; i < n; ++i) memcpy(&rows[i * h->filter_words], mask.data(), h->filter_words * 8); }
+    const uint64_t* fm = rows.empty() ? nullptr : rows.data();
+    std::vector<uint16_t> ids(n * KVIDX_MAX_PODS_PER_KEY); std::vector<double> sc(n * KVIDX_MAX_PODS_PER_KEY);
+    std::vector<uint8_t> cnt(n), has(n);
+    int rc = text ? kvidx_score_text_sparse(h->ix, text, text_off, (int64_t)n, nullptr, (uint32_t)mid, fm, min_ratio, ids.data(), sc.data(),
+                                            cnt.data(), has.data(), tokenize_out, nullptr)
+                  : kvidx_score_batch_sparse(h->ix, tok, tok_off, (int64_t)n, nullptr, (uint32_t)mid, fm, ids.data(), sc.data(), cnt.data(), has.data());
+    if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+    if (h->cfg.enable_metrics) {                    // one instrumented Lookup per scored prompt, as pod_scores counts them
+        std::vector<uint32_t> found;
+        std::vector<int64_t> foff(n + 1, 0);
+        const int64_t* to = tok_off;
+        if (text) {
+            // the tokens the score used: a second find over the same prompts touches the same keys in the same order, so the
+            // store's recency order comes out as after one find
+            rc = kvidx_text_store_find(h->ix, text, text_off, (int64_t)n, nullptr, 0, foff.data(), nullptr);
+            if (rc == KVIDX_ENOSPC) { found.resize((size_t)foff[n]); rc = kvidx_text_store_find(h->ix, text, text_off, (int64_t)n, found.data(), foff[n], foff.data(), nullptr); }
+            if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+            to = foff.data();
+        }
+        const uint32_t* tb = text ? found.data() : tok;
+        for (size_t i = 0; i < n; ++i) {
+            if (!has[i]) continue;
+            if (none) observe_lookup(h, 0.0, true, nullptr, nullptr, 0);
+            else observe_prompt(h, tb + (to[i] - to[0]), nullptr, (size_t)(to[i + 1] - to[i]), (uint32_t)mid, fm);
+        }
+    }
+    std::lock_guard<std::mutex> g(h->mu);
+    for (size_t i = 0; i < n; ++i) {
+        cnt_out[i] = !has[i] ? -1 : none ? 0 : cnt[i];
+        for (int j = 0; j < cnt_out[i]; ++j) {
+            pod_out[i * KVIDX_MAX_PODS_PER_KEY + j] = h->pods.name(ids[i * KVIDX_MAX_PODS_PER_KEY + j]);
+            score_out[i * KVIDX_MAX_PODS_PER_KEY + j] = sc[i * KVIDX_MAX_PODS_PER_KEY + j];
+        }
+    }
+    return 0;
+}
+
+int kvhost_get_pod_scores_text(kvhost_t* h, const uint8_t* text, const int64_t* text_off, size_t n, const char* model, const char* const* pods,
+                               size_t n_pods, double min_ratio, const char** pod_out, double* score_out, int32_t* cnt_out, uint8_t* tokenize_out) {
+    if (!text_off && n) return hfail(KVIDX_EINVAL, "NULL text_off");
+    return batch_scores(h, text, text_off, nullptr, nullptr, n, model, pods, n_pods, min_ratio, pod_out, score_out, cnt_out, tokenize_out);
+}
+
+int kvhost_get_pod_scores_batch(kvhost_t* h, const uint32_t* tokens, const int64_t* tok_off, size_t n, const char* model, const char* const* pods,
+                                size_t n_pods, const char** pod_out, double* score_out, int32_t* cnt_out) {
+    return batch_scores(h, nullptr, nullptr, tokens, tok_off, n, model, pods, n_pods, 0.0, pod_out, score_out, cnt_out, nullptr);
 }
 
 int kvhost_get_pod_scores(kvhost_t* h, const uint32_t* tokens, size_t n_tokens, const char* model, const char* const* pods, size_t n_pods,

@@ -102,6 +102,18 @@ SYMBOLS = {
     "kvidx_shard_snapshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
     "kvidx_snapshot_merge": (C.c_int, [C.POINTER(C.c_char_p), _u64p, C.c_uint32, C.c_void_p, C.c_uint64, _u64p]),
     "kvidx_shard_restore": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, _u64p]),
+    "kvidx_text_store_init": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32]),
+    "kvidx_text_store_add": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, _u64p, _i64p]),
+    "kvidx_text_store_find": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, C.c_int64, _i64p, _f64p]),
+    "kvidx_text_store_len": (C.c_int, [C.c_void_p, _i64p]),
+    "kvidx_text_hash_keys": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, C.c_int32, _u64p, _i64p]),
+    "kvidx_score_text": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, C.c_double, _f64p, _u8p, _u8p, _f64p]),
+    "kvidx_score_text_sparse": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, C.c_double, _u16p, _f64p, _u8p, _u8p,
+                                          _u8p, _f64p]),
+    "kvidx_score_text_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_double]
+                             + [C.c_void_p] * 4),
+    "kvidx_score_text_sparse_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_double]
+                                    + [C.c_void_p] * 6),
 }
 
 _lib = None
@@ -130,6 +142,18 @@ class KvidxError(RuntimeError):
 
 def _p(a, t):
     return None if a is None else a.ctypes.data_as(t)
+
+
+def _u8(text):
+    return np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray)) else np.ascontiguousarray(text, np.uint8)
+
+
+def pack_text(prompts):
+    """Prompts (str or bytes; str as UTF-8) -> (text bytes as uint8, offsets (n+1)): the CSR the text calls take."""
+    raw = [p.encode("utf-8") if isinstance(p, str) else bytes(p) for p in prompts]
+    off = np.zeros(len(raw) + 1, np.int64)
+    off[1:] = np.cumsum([len(r) for r in raw])
+    return np.frombuffer(b"".join(raw), np.uint8) if raw else np.zeros(0, np.uint8), off
 
 
 def fnv64a(data: bytes) -> int:
@@ -173,8 +197,20 @@ class Index:
         self.filter_words = (max_pods + 63) // 64
         self.lru_exact = bool(lru_exact)
 
+    @classmethod
+    def borrow(cls, handle: int, block_size=16, max_pods=256) -> "Index":
+        """An Index over a handle that another owner created and destroys (kvhost_index of a HostIndexer)."""
+        self = cls.__new__(cls)
+        self.L, self.h, self._borrowed = load(), C.c_void_p(handle), True
+        self.block_size, self.max_pods = block_size, max_pods
+        self.filter_words = (max_pods + 63) // 64
+        self.lru_exact = False
+        return self
+
     # -- plumbing --
     def close(self):
+        if getattr(self, "_borrowed", False):
+            self.h = None
         if getattr(self, "h", None):
             self.L.kvidx_destroy(self.h)
             self.h = None
@@ -425,6 +461,90 @@ class Index:
         """Device-resident, pod-sorted event batch; asynchronous on the handle's write stream."""
         self._ck(self.L.kvidx_apply_events_dev(self.h, d_ev_sorted, d_queue_off, n_queues, n_events, d_hashes, n_hashes, d_tokens,
                                                d_n_dropped or None))
+
+    # -- the device prefix store and Score() from text: prompt i is text[text_off[i] .. text_off[i+1]) (pack_text) --
+    def text_store_init(self, cache_blocks=500000, block_bytes=256):
+        """NewLRUTokenStore on this handle (once)."""
+        self._ck(self.L.kvidx_text_store_init(self.h, cache_blocks, block_bytes))
+
+    def text_store_add(self, text, text_off, tok, tok_span, tok_off):
+        """AddTokenization of every prompt, in order.  tok / tok_off: the prompts' token CSR; tok_span (n_tok, 2): each
+        token's [low, high) byte offsets in its prompt."""
+        text, text_off = _u8(text), np.ascontiguousarray(text_off, np.int64)
+        tok, tok_off = np.ascontiguousarray(tok, np.uint32), np.ascontiguousarray(tok_off, np.int64)
+        span = np.ascontiguousarray(tok_span, np.uint64).reshape(-1)
+        self._ck(self.L.kvidx_text_store_add(self.h, _p(text, _u8p), _p(text_off, _i64p), len(text_off) - 1, _p(tok, _u32p),
+                                             _p(span, _u64p), _p(tok_off, _i64p)))
+
+    def text_store_find_into(self, text, text_off, tok_out, tok_off_out, ratio_out=None) -> int:
+        """One kvidx_text_store_find into caller arrays; returns the code (ENOSPC: tok_out too small, nothing refreshed)."""
+        text, text_off = _u8(text), np.ascontiguousarray(text_off, np.int64)
+        return self.L.kvidx_text_store_find(self.h, _p(text, _u8p), _p(text_off, _i64p), len(text_off) - 1, _p(tok_out, _u32p),
+                                            0 if tok_out is None else len(tok_out), _p(tok_off_out, _i64p), _p(ratio_out, _f64p))
+
+    def text_store_find(self, text, text_off):
+        """FindLongestContainedTokens of every prompt -> (tokens, their offsets (n+1), ratios)."""
+        n = len(text_off) - 1
+        off, ratio = np.zeros(n + 1, np.int64), np.zeros(max(n, 0), np.float64)
+        tok = np.zeros(0, np.uint32)
+        while True:                           # ENOSPC refreshes nothing: size the buffer from the offsets and find again
+            rc = self.text_store_find_into(text, text_off, tok if len(tok) else None, off, ratio)
+            if rc != ENOSPC:
+                break
+            tok = np.zeros(int(off[-1]), np.uint32)
+        self._ck(rc)
+        return tok[:int(off[-1])], off, ratio
+
+    def text_store_len(self) -> int:
+        out = C.c_int64(0)
+        self._ck(self.L.kvidx_text_store_len(self.h, C.byref(out)))
+        return out.value
+
+    def text_hash_keys(self, text, text_off, block_bytes):
+        """The store's block keys of every prompt at block_bytes -> (keys, their offsets)."""
+        text, text_off = _u8(text), np.ascontiguousarray(text_off, np.int64)
+        n = len(text_off) - 1
+        nk = int(((text_off[1:] - text_off[:-1]) // block_bytes).sum()) if n > 0 else 0
+        keys, koff = np.zeros(max(nk, 1), np.uint64), np.zeros(n + 1, np.int64)
+        self._ck(self.L.kvidx_text_hash_keys(self.h, _p(text, _u8p), _p(text_off, _i64p), n, block_bytes, _p(keys, _u64p), _p(koff, _i64p)))
+        return keys[:nk], koff
+
+    def _text_args(self, text, text_off, model, filter_mask):
+        text, text_off = _u8(text), np.ascontiguousarray(text_off, np.int64)
+        model = None if model is None else np.ascontiguousarray(model, np.uint32)
+        filter_mask = None if filter_mask is None else np.ascontiguousarray(filter_mask, np.uint64)
+        n = len(text_off) - 1
+        return n, text, text_off, model, filter_mask, np.zeros(n, np.uint8), np.zeros(n, np.uint8), np.zeros(n, np.float64)
+
+    def score_text(self, text, text_off, model=None, model0=0, filter_mask=None, min_ratio=0.8):
+        """Score() from text -> (dense rows (n, max_pods), has_keys, tokenize flags, ratios).  A prompt whose cached prefix
+        covers less than min_ratio of its text gets an all-absent row and tokenize 1."""
+        n, text, text_off, model, filter_mask, has, tokz, ratio = self._text_args(text, text_off, model, filter_mask)
+        scores = np.empty((n, self.max_pods), np.float64)
+        self._ck(self.L.kvidx_score_text(self.h, _p(text, _u8p), _p(text_off, _i64p), n, _p(model, _u32p), model0, _p(filter_mask, _u64p),
+                                         float(min_ratio), _p(scores, _f64p), _p(has, _u8p), _p(tokz, _u8p), _p(ratio, _f64p)))
+        return scores, has, tokz, ratio
+
+    def score_text_sparse(self, text, text_off, model=None, model0=0, filter_mask=None, min_ratio=0.8):
+        """Sparse rows as score_batch_sparse -> (pods, scores, cnt, has, tokenize flags, ratios)."""
+        n, text, text_off, model, filter_mask, has, tokz, ratio = self._text_args(text, text_off, model, filter_mask)
+        pods, scores, cnt = np.zeros((n, E), np.uint16), np.zeros((n, E), np.float64), np.zeros(n, np.uint8)
+        self._ck(self.L.kvidx_score_text_sparse(self.h, _p(text, _u8p), _p(text_off, _i64p), n, _p(model, _u32p), model0,
+                                                _p(filter_mask, _u64p), float(min_ratio), _p(pods, _u16p), _p(scores, _f64p),
+                                                _p(cnt, _u8p), _p(has, _u8p), _p(tokz, _u8p), _p(ratio, _f64p)))
+        return pods, scores, cnt, has, tokz, ratio
+
+    def score_text_dev(self, d_text, d_text_off, n, d_scores, d_model=0, model0=0, d_filter=0, min_ratio=0.8, d_has_keys=0,
+                       d_tokenize=0, d_ratio=0):
+        """All pointers are device addresses (ints).  On the handle's stream."""
+        self._ck(self.L.kvidx_score_text_dev(self.h, d_text or None, d_text_off, n, d_model or None, model0, d_filter or None,
+                                             float(min_ratio), d_scores, d_has_keys or None, d_tokenize or None, d_ratio or None))
+
+    def score_text_sparse_dev(self, d_text, d_text_off, n, d_pods, d_scores, d_cnt, d_model=0, model0=0, d_filter=0, min_ratio=0.8,
+                              d_has_keys=0, d_tokenize=0, d_ratio=0):
+        self._ck(self.L.kvidx_score_text_sparse_dev(self.h, d_text or None, d_text_off, n, d_model or None, model0, d_filter or None,
+                                                    float(min_ratio), d_pods, d_scores, d_cnt, d_has_keys or None, d_tokenize or None,
+                                                    d_ratio or None))
 
     # -- write path --
     def add(self, model, engine, request, podtiers):

@@ -35,6 +35,7 @@ class PodRow(C.Structure):
 
 
 _cpp = C.POINTER(C.c_char_p)
+_i64p = C.POINTER(C.c_int64)
 _u64p, _u32p, _u8p, _f64p = C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint8), C.POINTER(C.c_double)
 SYMBOLS = {
     "kvhost_config_default": (None, [C.POINTER(HostConfig)]),
@@ -70,6 +71,10 @@ SYMBOLS = {
     "kvhost_pod_id": (C.c_int, [C.c_void_p, C.c_char_p]),
     "kvhost_tier_id": (C.c_int, [C.c_void_p, C.c_char_p]),
     "kvhost_model_id": (C.c_int, [C.c_void_p, C.c_char_p]),
+    "kvhost_get_pod_scores_text": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_size_t, C.c_char_p, _cpp, C.c_size_t, C.c_double, _cpp,
+                                             C.POINTER(C.c_double), C.POINTER(C.c_int32), _u8p]),
+    "kvhost_get_pod_scores_batch": (C.c_int, [C.c_void_p, _u32p, _i64p, C.c_size_t, C.c_char_p, _cpp, C.c_size_t, _cpp,
+                                              C.POINTER(C.c_double), C.POINTER(C.c_int32)]),
 }
 _bound = False
 
@@ -99,7 +104,7 @@ class HostIndexer:
                  concurrency=4, device=0, no_device=False, lru_exact=0, enable_metrics=False, clear_on_all_blocks_cleared=False,
                  evict_policy="none"):
         self.L = _lib()
-        self.block_size = block_size
+        self.block_size, self.max_pods = block_size, max_pods
         cfg = HostConfig()
         self.L.kvhost_config_default(C.byref(cfg))
         cfg.index.block_size, cfg.index.capacity, cfg.index.pods_per_key = block_size, capacity, pods_per_key
@@ -142,6 +147,33 @@ class HostIndexer:
         if n < 0:
             raise _native.KvidxError(n, self.err())
         return {po[i].decode(): so[i] for i in range(n)}
+
+    def _batch_rows(self, n, rc, po, so, cnt):
+        if rc:
+            raise _native.KvidxError(rc, self.err())
+        return [None if cnt[i] < 0 else {po[i * 10 + j].decode(): so[i * 10 + j] for j in range(cnt[i])} for i in range(n)]
+
+    def get_pod_scores_text(self, text, text_off, model, pods=(), min_ratio=0.8):
+        """GetPodScores for a batch of prompt texts through the device prefix store (kvhost_get_pod_scores_text).
+        -> (per prompt a dict pod -> score, or None; tokenize flags: the prompts whose cached prefix was too short)."""
+        text = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray)) else np.ascontiguousarray(text, np.uint8)
+        off = np.ascontiguousarray(text_off, np.int64)
+        n = len(off) - 1
+        po = (C.c_char_p * (10 * max(n, 1)))(); so = (C.c_double * (10 * max(n, 1)))(); cnt = (C.c_int32 * max(n, 1))()
+        tz = np.zeros(max(n, 1), np.uint8)
+        rc = self.L.kvhost_get_pod_scores_text(self.h, text.ctypes.data_as(_u8p), off.ctypes.data_as(_i64p), n, model.encode(),
+                                               _strs(list(pods)), len(pods), float(min_ratio), po, so, cnt, tz.ctypes.data_as(_u8p))
+        return self._batch_rows(n, rc, po, so, cnt), tz[:n]
+
+    def get_pod_scores_batch(self, tokens, tok_off, model, pods=()):
+        """GetPodScores for a batch of token prompts (CSR) -> per prompt a dict pod -> score, or None."""
+        tok = np.ascontiguousarray(tokens, np.uint32)
+        off = np.ascontiguousarray(tok_off, np.int64)
+        n = len(off) - 1
+        po = (C.c_char_p * (10 * max(n, 1)))(); so = (C.c_double * (10 * max(n, 1)))(); cnt = (C.c_int32 * max(n, 1))()
+        rc = self.L.kvhost_get_pod_scores_batch(self.h, tok.ctypes.data_as(_u32p), off.ctypes.data_as(_i64p), n, model.encode(),
+                                                _strs(list(pods)), len(pods), po, so, cnt)
+        return self._batch_rows(n, rc, po, so, cnt)
 
     def get_pod_scores_keys(self, keys, model, pods=()):
         """GetPodScores from the prompt's request keys (block order) -> dict pod -> score, or None when there are no keys."""
@@ -299,6 +331,7 @@ class PrefixStore:
 
     def __init__(self, cache_size=500000, block_size=256):
         self.L = _lib()
+        self.cache_size, self.block_size = cache_size, block_size
         h = C.c_void_p()
         rc = self.L.kvhost_prefix_store_create(cache_size, block_size, C.byref(h))
         if rc:

@@ -103,15 +103,59 @@ class TokenizationPool:
 
 # ---- Indexer over the host mirror --------------------------------------------------------------------------------------
 class Indexer:
-    """kvcache.Indexer (indexer.go:132-166): Tokenize -> (TokensToKVBlockKeys -> Lookup -> Score on the device)."""
+    """kvcache.Indexer (indexer.go:132-166): Tokenize -> (TokensToKVBlockKeys -> Lookup -> Score on the device).
 
-    def __init__(self, host_indexer, tokenization: TokenizationPool):
+    get_pod_scores serves one prompt through the TokenizationPool's host prefix store (a device round trip costs more than
+    the host store's lookup for a single prompt).  get_pod_scores_batch serves a batch through a prefix store on the device
+    (kvidx_text_store_*, created on first use with text_cache_blocks / text_block_bytes): one Score() from text, the
+    tokenizer for the prompts whose cached prefix is too short, one add and one Score() for those."""
+
+    def __init__(self, host_indexer, tokenization: TokenizationPool, text_cache_blocks: int = 500000, text_block_bytes: int = 256):
         self.host = host_indexer
         self.tok = tokenization
+        self.text_cache_blocks, self.text_block_bytes = text_cache_blocks, text_block_bytes
+        self._dev = None
+        self._dev_mu = threading.Lock()
 
     def get_pod_scores(self, prompt: str, model_name: str, pod_identifiers: Sequence[str] = ()) -> Optional[Dict[str, float]]:
         tokens = self.tok.tokenize(prompt)
         return self.host.get_pod_scores(np.asarray(tokens, np.uint32), model_name, list(pod_identifiers))
+
+    def _device_store(self):
+        with self._dev_mu:
+            if self._dev is None:
+                from ._native import Index
+                ix = Index.borrow(self.host.L.kvhost_index(self.host.h), self.host.block_size, self.host.max_pods)
+                ix.text_store_init(self.text_cache_blocks, self.text_block_bytes)
+                self._dev = ix
+            return self._dev
+
+    def get_pod_scores_batch(self, prompts: Sequence[str], model_name: str,
+                             pod_identifiers: Sequence[str] = ()) -> List[Optional[Dict[str, float]]]:
+        """GetPodScores for every prompt of a batch, on the device prefix store.  -> per prompt a dict pod -> score, or None
+        for the reference's (nil, nil) (no full block).  The batch's finds all run before its adds, so a prompt is not served
+        from the tokenization of another prompt of the same batch."""
+        from ._native import pack_text
+        ix = self._device_store()
+        if not prompts:
+            return []
+        pods = list(pod_identifiers)
+        text, text_off = pack_text(prompts)
+        out, tokz = self.host.get_pod_scores_text(text, text_off, model_name, pods, self.tok.ratio)
+        redo = np.flatnonzero(tokz)
+        if len(redo):
+            enc = [self.tok._encode(prompts[i]) for i in redo]
+            with self.tok._mu:
+                self.tok.encodes += len(redo)
+            r_text, r_off = pack_text([prompts[i] for i in redo])
+            tok_off = np.zeros(len(redo) + 1, np.int64)
+            tok_off[1:] = np.cumsum([len(ids) for ids, _ in enc])
+            tok = np.concatenate([np.asarray(ids, np.uint32) for ids, _ in enc]) if tok_off[-1] else np.zeros(0, np.uint32)
+            span = np.concatenate([np.asarray(offs, np.uint64).reshape(-1, 2) for _, offs in enc]) if tok_off[-1] else np.zeros((0, 2), np.uint64)
+            ix.text_store_add(r_text, r_off, tok, span, tok_off)
+            for i, row in zip(redo, self.host.get_pod_scores_batch(tok, tok_off, model_name, pods)):
+                out[i] = row
+        return out
 
 
 # ---- gRPC --------------------------------------------------------------------------------------------------------------
