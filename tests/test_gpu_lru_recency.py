@@ -12,6 +12,7 @@ keys than its capacity (nothing is evicted inside the call, so exact per call is
   * the recency section of the handle's image, rank by rank, against the oracle's LRU order, with no stamp repeated,
   * after one capped add of fresh keys on both sides, the whole image again: the same keys were evicted.
 Two more cases touch more keys in one prompt or one event than a fixed-width stamp range per prompt or event would hold.
+Score() from text must leave exactly the recency score_batch of the tokens it finds leaves.
 """
 import struct
 
@@ -357,3 +358,42 @@ def test_event_past_2_19_blocks():
         assert t.apply_events(ev, hs, tk) == (0, 0)
     img = check_recency(ix, co)
     _restores(img, B, cap)
+
+
+# ---- Score() from text: the same touches as score_batch of the tokens it finds ------------------------------------------
+def test_score_text_leaves_score_batch_recency():
+    """Twin exact-LRU handles on the shared-prefix documents, the prompts' text in a device prefix store on one of them:
+    Score() from text there, score_batch of the same token CSR (the host store's find, gated at 0.8) on the twin and on
+    the oracle.  The images, which carry recency, are byte-equal right after the call and again after a capped add."""
+    from kvidx import pack_text
+    from kvidx.host import PrefixStore
+    from test_gpu_text_store_scale import _text_of, _want
+    B = 16
+    twins = [_score_setup(B, np.random.default_rng(140)) for _ in range(2)]
+    (a, co, docs), (b, _, _) = twins
+    rng = np.random.default_rng(141)
+    tok, off = _prompts(B, rng, docs, 4096)
+    a.text_store_init(500000, 64)
+    hs = PrefixStore(500000, 64)
+    texts = [_text_of(d) for d in docs]
+    dtext, doff = pack_text(texts)
+    spans = np.concatenate([np.stack([np.arange(len(d)) * 4, np.arange(len(d)) * 4 + 4], axis=1) for d in docs]).astype(np.uint64)
+    a.text_store_add(dtext, doff, np.concatenate(docs), spans, np.concatenate([[0], np.cumsum([len(d) for d in docs])]))
+    for t, d in zip(texts, docs):
+        hs.add_tokenization(t, d, np.stack([np.arange(len(d)) * 4, np.arange(len(d)) * 4 + 4], axis=1))
+    q = [_text_of(tok[off[i]:off[i + 1]]) for i in range(len(off) - 1)]
+    tq, soff, passing, _ = _want(hs, q, 0.8)
+    assert passing.any() and not passing.all()
+    got = a.score_text(*pack_text(q), min_ratio=0.8)[0]
+    want_b = b.score_batch(tq, soff)[0]
+    want_o = co.score_batch(tq, soff, n_threads=1)[0]
+    assert got.tobytes() == want_b.tobytes() == want_o.tobytes()
+    check_recency(a, co)
+    _same(a.snapshot(), b.snapshot(), "images after score_text and score_batch")
+    assert a.evictions() == (0, 0)
+    new = rng.integers(1, 1 << 63, a.stats()["request_keys"] // 3, dtype=np.uint64)
+    for t in (a, b, co):
+        assert t.add(0, new ^ np.uint64(0x3C3C), new, [PT(13)]) == 0
+    assert a.evictions()[0] > 0
+    check_recency(a, co)
+    _same(a.snapshot(), b.snapshot(), "images after the capped add")

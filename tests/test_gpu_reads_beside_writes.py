@@ -14,7 +14,9 @@ shared system prompts (prefix classes with followers and partial followers), on 
 every block that no writer touches; churn pods 1..8 on tiers weighted 1.0, 0.8, 1/3 and 0.1 (at most 9 churn entries a
 key, so the 10-entry pod LRU never drops the anchor); a pod filter on a quarter of the prompts; and a hot document, outside
 the prompt pool, whose first 8 blocks one event batch stores and removes 32 times while Lookup reads each of their slots
-256 times a call."""
+256 times a call.
+
+Score() from text reads the same documents through a device prefix store that holds their text (4 bytes a token)."""
 import threading
 import time
 
@@ -713,3 +715,122 @@ def test_clock_handle_below_its_contents_beside_the_writer():
                 assert why is None, "spec %d: %s" % (spec, why)
     assert {"add", "remove_pods"} <= evidence["kinds"]
     _quiescent(work, hist, [ix], clock=True)
+
+
+def test_score_text_beside_the_writer():
+    """Score() from text -- dense, sparse and _dev at 4096 prompts, dense at 131 072 -- while the writer runs, and a store
+    thread adds and finds text disjoint from the queried prompts (its calls serialise with the readers' on the store's
+    lock).  Every document's text is in the store before the race (4 bytes a token, 64-byte blocks: one store block per
+    index block) and the cache evicts nothing, so each prompt's find is exactly its whole index blocks: the history
+    oracle checks the rows as it checks score_batch rows."""
+    import torch
+    from kvidx import pack_text
+    from kvidx.host import PrefixStore
+    from test_gpu_text_store import host_find
+    from test_gpu_text_store_scale import _text_of
+    work = Work(71)
+    ix = _handle(work)
+    ix.text_store_init(1 << 22, 64)
+    hs = PrefixStore(1 << 22, 64)
+    dtext = [_text_of(d) for d in work.docs]
+    spans = [np.stack([np.arange(len(d)) * 4, np.arange(len(d)) * 4 + 4], axis=1).astype(np.uint64) for d in work.docs]
+    t, o = pack_text(dtext)
+    ix.text_store_add(t, o, np.concatenate(work.docs), np.concatenate(spans), np.concatenate([[0], np.cumsum([len(d) for d in work.docs])]))
+    for x, d, sp in zip(dtext, work.docs, spans):
+        hs.add_tokenization(x, d, sp)
+    reads = Reads()
+    writer = Writer(work, [ix], np.random.default_rng(15), ALL_KINDS)
+    dev = torch.device("cuda", 0)
+    readers_left = [4]
+    lock = threading.Lock()
+
+    def prompt_text(s, mb):
+        d, nb, tail, _ = work.specs[s]
+        nb = nb if mb is None else min(nb, mb)
+        return dtext[d][:4 * (work.BS * nb + tail)], nb
+
+    def text_reader(how, n, until, seed, max_blocks=None):
+        rng = np.random.default_rng(seed)
+        batches = []
+        for _ in range(2 if n > 4096 else 4):
+            idx, _, _, model, fm = work.batch(rng, n, max_blocks)
+            q, nb = zip(*[prompt_text(int(s), max_blocks) for s in idx])
+            text, off = pack_text(q)
+            ratio = (np.array(nb, np.int64) * 64).astype(np.float64) / (off[1:] - off[:-1]).astype(np.float64)
+            if n <= 4096:                                       # the host store's find: the prompt's whole index blocks
+                ftok, foff, fr = host_find(hs, q)
+                assert np.array_equal(foff[1:] - foff[:-1], np.array(nb) * work.BS) and fr.tobytes() == ratio.tobytes()
+            d_in = [torch.from_numpy(x).to(dev) for x in (text.copy(), off, model.view(np.int32), fm.view(np.int64))] if how == "dev" else None
+            batches.append((idx, text, off, model, fm, ratio, d_in))
+        torch.cuda.synchronize()
+
+        def run(stop):
+            try:
+                while until.more() and not stop.is_set():
+                    idx, text, off, model, fm, ratio, d_in = batches[until.k % len(batches)]
+                    s = time.monotonic_ns()
+                    if how == "dense":
+                        rows, has, tz, r = ix.score_text(text, off, model=model, filter_mask=fm, min_ratio=0.0)
+                        e = time.monotonic_ns()
+                    elif how == "sparse":
+                        pods, sc, cnt, has, tz, r = ix.score_text_sparse(text, off, model=model, filter_mask=fm, min_ratio=0.0)
+                        e = time.monotonic_ns()
+                        rows = np.full((n, P), -1.0)
+                        for i in range(n):
+                            rows[i, pods[i, :cnt[i]]] = sc[i, :cnt[i]]
+                    else:
+                        out = [torch.empty((n, P), dtype=torch.float64, device=dev), torch.empty(n, dtype=torch.uint8, device=dev),
+                               torch.empty(n, dtype=torch.uint8, device=dev), torch.empty(n, dtype=torch.float64, device=dev)]
+                        ix.score_text_dev(d_in[0].data_ptr(), d_in[1].data_ptr(), n, out[0].data_ptr(), d_model=d_in[2].data_ptr(),
+                                          d_filter=d_in[3].data_ptr(), min_ratio=0.0, d_has_keys=out[1].data_ptr(),
+                                          d_tokenize=out[2].data_ptr(), d_ratio=out[3].data_ptr())
+                        ix.synchronize()
+                        e = time.monotonic_ns()
+                        rows, has, tz, r = (x.cpu().numpy() for x in out)
+                    assert not tz.any() and r.tobytes() == ratio.tobytes(), "a queried prompt's find changed"
+                    reads.add("score", 0, s, e, (idx, rows, has, max_blocks))
+                    until.saw(s, e)
+            finally:
+                with lock:
+                    readers_left[0] -= 1
+        return run
+
+    store_calls = []
+
+    def store_thread(stop):
+        """adds and finds of random text (no block of it is a document's) until the text readers are done, two calls at least"""
+        rng = np.random.default_rng(16)
+        k = 0
+        while (readers_left[0] > 0 or k < 2) and not stop.is_set():
+            ps = [rng.bytes(int(rng.integers(0, 900))) for _ in range(512)]
+            text, off = pack_text(ps)
+            s = time.monotonic_ns()
+            if k % 2 == 0:
+                toks = [(rng.integers(0, 1 << 31, len(p) // 8 + 1), [(min(8 * j, len(p)), min(8 * j + 8, len(p))) for j in range(len(p) // 8 + 1)]) for p in ps]
+                toff = np.concatenate([[0], np.cumsum([len(x[0]) for x in toks])])
+                ix.text_store_add(text, off, np.concatenate([x[0] for x in toks]), np.array([sp for x in toks for sp in x[1]], np.uint64), toff)
+                for p, (ti, ts) in zip(ps, toks):
+                    hs.add_tokenization(p, ti, ts)
+            else:
+                got, want = ix.text_store_find(text, off), host_find(hs, ps)
+                assert all(np.array_equal(g, w) for g, w in zip(got, want)) and got[2].tobytes() == want[2].tobytes()
+            store_calls.append((s, time.monotonic_ns()))
+            k += 1
+
+    readers = [text_reader("dense", 4096, Until(writer, 0, 3, KINDS, rebuild=True), 1),
+               text_reader("sparse", 4096, Until(writer, 0, 3, KINDS), 2),
+               text_reader("dev", 4096, Until(writer, 0, 3, KINDS), 3),
+               text_reader("dense", 131072, Until(writer, 0, 2, ["add"], cap=3), 4, max_blocks=40),
+               store_thread]
+    _race(work, writer, readers, 60)
+    hist = writer.history(work)
+    evidence = {}
+    _check_scores(work, writer, hist, reads, Checker(hist, W), evidence)
+    _evidence_ok(evidence, 1, KINDS)
+    spans_r = [(s, e) for _, _, s, e, _ in reads.calls]
+    assert len(store_calls) >= 2 and any(s < e1 and s1 < e for s, e in store_calls for s1, e1 in spans_r), "no store call ran during a read"
+    assert ix.text_store_len() == len(hs)
+    q = [prompt_text(s, None)[0] for s in range(len(work.specs))]
+    got, want = ix.text_store_find(*pack_text(q)), host_find(hs, q)
+    assert all(np.array_equal(g, w) for g, w in zip(got, want))
+    _quiescent(work, hist, [ix])

@@ -33,13 +33,26 @@ def rand_text(rng, n):
 
 
 def tokenize(rng, text: bytes):
-    """Random tokens over the text: monotone ends, zero-width tokens, tokens across block edges and in the tail."""
+    """Random tokens over the text with the spans tokenizers really report: mostly monotone ends, zero-width tokens,
+    tokens across block edges and in the tail; special tokens reported as (0, 0) after later tokens, ends that decrease,
+    ends past the end of the text, and runs of tokens that end on one byte."""
     ids, spans, pos = [], [], 0
     while pos < len(text):
         w = int(rng.choice([0, 1, 2, 3, 5, 9, 17]))
         w = min(w, len(text) - pos)
         ids.append(int(rng.integers(0, 1 << 32, dtype=np.uint64)))
         spans.append((pos, pos + w))
+        r = rng.random()
+        if r < 0.04:
+            spans.append((0, 0))                                                # a special token after later tokens
+        elif r < 0.07:
+            e = max(pos + w - int(rng.integers(1, 24)), 0)                      # an end below the previous one
+            spans.append((e, e))
+        elif r < 0.08:
+            spans.append((pos, len(text) + int(rng.integers(1, 40))))           # past the end of the text
+        elif r < 0.12:
+            spans.extend([(pos, pos + w)] * int(rng.integers(1, 6)))            # more tokens ending on the same byte
+        ids.extend(int(x) for x in rng.integers(0, 1 << 32, len(spans) - len(ids), dtype=np.uint64))
         pos += w if w else (1 if rng.random() < 0.5 else 0)
     return ids, spans
 
@@ -69,18 +82,93 @@ def dev_store(cache_blocks, bb, **kw):
 
 
 # ---- hash chains -----------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("bb", [1, 3, 8, 31, 32, 256, 1000])
-@pytest.mark.parametrize("n", [1, 37, 20000])                    # 4 lanes per prompt below 16384 prompts, 1 lane above
-def test_hash_chains_match_the_host_store(bb, n):
+_XP = [np.uint64(x) for x in (0x9E3779B185EBCA87, 0xC2B2AE3D27D4EB4F, 0x165667B19E3779F9, 0x85EBCA77C2B2AE63, 0x27D4EB2F165667C5)]
+
+
+def _rotl(x, r):
+    return (x << np.uint64(r)) | (x >> np.uint64(64 - r))
+
+
+def _xround(acc, w):
+    return _rotl(acc + w * _XP[1], 31) * _XP[0]
+
+
+def xxh64_rows(msg):
+    """XXH64 (seed 0) of every row of msg (m, M) uint8, in numpy: the spec's stripes of four 8-byte lanes, then the 8-,
+    4- and 1-byte tails, then the avalanche."""
+    m, M = msg.shape
+    P1, P2, P3, P4, P5 = _XP
+    w8 = np.ascontiguousarray(msg[:, :M // 8 * 8]).view("<u8")
+    k = 0
+    if M >= 32:
+        v = [np.full(m, P1 + P2), np.full(m, P2), np.zeros(m, np.uint64), np.full(m, np.uint64(0) - P1)]
+        while k + 32 <= M:
+            for j in range(4):
+                v[j] = _xround(v[j], w8[:, k // 8 + j])
+            k += 32
+        h = _rotl(v[0], 1) + _rotl(v[1], 7) + _rotl(v[2], 12) + _rotl(v[3], 18)
+        for j in range(4):
+            h = (h ^ _xround(np.uint64(0), v[j])) * P1 + P4
+    else:
+        h = np.full(m, P5)
+    h = h + np.uint64(M)
+    while k + 8 <= M:
+        h = _rotl(h ^ _xround(np.uint64(0), w8[:, k // 8]), 27) * P1 + P4
+        k += 8
+    if k + 4 <= M:
+        h = _rotl(h ^ (np.ascontiguousarray(msg[:, k:k + 4]).view("<u4")[:, 0].astype(np.uint64) * P1), 23) * P2 + P3
+        k += 4
+    while k < M:
+        h = _rotl(h ^ (msg[:, k].astype(np.uint64) * P5), 11) * P1
+        k += 1
+    h ^= h >> np.uint64(33)
+    h *= P2
+    h ^= h >> np.uint64(29)
+    h *= P3
+    h ^= h >> np.uint64(32)
+    return h
+
+
+def chains(text, off, bb):
+    """Every prompt's chain of bb-byte block keys (numpy, block b of every prompt at once) -> (keys, key offsets)"""
+    nb = (off[1:] - off[:-1]) // bb
+    koff = np.zeros(len(nb) + 1, np.int64)
+    koff[1:] = np.cumsum(nb)
+    keys = np.zeros(int(koff[-1]), np.uint64)
+    prev = np.zeros(len(nb), np.uint64)
+    for b in range(int(nb.max()) if len(nb) else 0):
+        act = np.flatnonzero(nb > b)
+        at = (off[act] + b * bb)[:, None] + np.arange(bb)
+        msg = np.concatenate([prev[act].view(np.uint8).reshape(-1, 8), text[at]], axis=1)
+        prev[act] = xxh64_rows(msg)
+        keys[koff[act] + b] = prev[act]
+    return keys, koff
+
+
+@pytest.fixture(scope="module")
+def hash_ix():
+    return dev_store(10, 4)
+
+
+@pytest.mark.parametrize("bb", list(range(1, 73)) + [255, 256, 257, 1000, 1024, 4096])      # every XXH64 tail layout
+@pytest.mark.parametrize("n", [1, 37, 16383, 16384, 20000])      # 4 lanes per prompt below 16384 prompts, 1 lane above
+def test_hash_chains_match_the_host_store(bb, n, hash_ix):
+    """Every prompt's chain against a numpy XXH64 of the same messages, which in turn matches the host store's
+    xxhash64 on the first prompts.  Large batches keep most texts short; a few hundred prompts still run to 3 blocks."""
+    np.seterr(over="ignore")
     rng = np.random.default_rng(bb * 7 + n)
-    ix = dev_store(10, 4)
-    lens = rng.integers(0, 3 * bb + 40 if n < 1000 else 2 * bb + 8, n)
+    top = 3 * bb + 40
+    long_ = rng.random(n) < (1.0 if n < 1000 else min(1.0, 600.0 / top))
+    lens = np.where(long_, rng.integers(0, top, n), rng.integers(0, min(top, 2 * bb + 9), n) % max(1, min(top, 80)))
     prompts = [rand_text(rng, int(m)) for m in lens]
     text, off = pack_text(prompts)
-    keys, koff = ix.text_hash_keys(text, off, bb)
-    for i, p in enumerate(prompts if n < 1000 else prompts[::97]):
-        j = i if n < 1000 else i * 97
-        assert list(keys[koff[j]:koff[j + 1]]) == host_chain(p, bb), (bb, j, len(p))
+    keys, koff = hash_ix.text_hash_keys(text, off, bb)
+    want, wkoff = chains(text, off, bb)
+    assert np.array_equal(koff, wkoff)
+    bad = np.flatnonzero(keys != want)
+    assert not len(bad), (bb, n, "first wrong key of prompt", int(np.searchsorted(koff, bad[0], side="right") - 1))
+    for i in range(min(n, 40)):
+        assert list(want[wkoff[i]:wkoff[i + 1]]) == host_chain(prompts[i], bb), (bb, i, len(prompts[i]))
 
 
 # ---- call streams against the host store -----------------------------------------------------------------------------
