@@ -13,6 +13,7 @@
 #include <mutex>
 #include <shared_mutex>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -93,6 +94,88 @@ bool is_device_accessible_host(const void* p) {
     return a.type == cudaMemoryTypeHost;     // pinned: cudaMemcpyAsync from it is truly async
 }
 
+// Every scratch buffer a call lays out is carved into sections by a Carver, twice: over a null base to size the buffer,
+// then over the buffer itself (carve()), so each section's size is written once.  Sections start on 256-byte
+// boundaries, as a cudaMalloc of their own would (TMA reads staged inputs in place and needs 16).  An empty section
+// takes no bytes: its pointer is the next section's, and a caller never dereferences it.
+struct Carver {
+    static constexpr size_t kAlign = 256;
+    uintptr_t base = 0; size_t at = 0;
+    template <class T> T* take(size_t count) {
+        static_assert(kAlign % alignof(T) == 0, "a section is aligned for its elements");
+        T* p = reinterpret_cast<T*>(base + at);
+        at += (count * sizeof(T) + kAlign - 1) & ~(kAlign - 1);
+        return p;
+    }
+};
+
+// Sizes buf for the sections `layout` takes (growing it as need() does; what it held is dropped) and carves them from it.
+template <class Buf, class Layout> cudaError_t carve(Buf& buf, Layout&& layout) {
+    Carver size;
+    layout(size);
+    if (cudaError_t e = buf.need(size.at)) return e;
+    Carver c{reinterpret_cast<uintptr_t>(buf.p)};
+    layout(c);
+    return cudaSuccess;
+}
+
+// Moves bytes between the device and a caller's host buffer: one copy when the buffer is pinned, else through two pinned
+// chunks that alternate (the copy engine fills or empties one while the host works on the other).
+struct Stager {
+    static constexpr size_t kChunk = 16u << 20;
+    PinBuf buf[2];
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    cudaError_t init() {
+        for (auto& e : ev) if (cudaError_t r = cudaEventCreateWithFlags(&e, cudaEventDisableTiming)) return r;
+        return cudaSuccess;
+    }
+    void release() {
+        buf[0].release(); buf[1].release();
+        for (auto& e : ev) { if (e) cudaEventDestroy(e); e = nullptr; }
+    }
+    // device -> host; every byte is in dst when it returns
+    int d2h(void* dst, const void* src, size_t n, cudaStream_t st) {
+        if (n == 0) return 0;
+        if (is_device_accessible_host(dst)) {
+            CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            return 0;
+        }
+        CK(buf[0].need(kChunk));
+        CK(buf[1].need(kChunk));
+        const size_t nc = (n + kChunk - 1) / kChunk;
+        for (size_t k = 0; k <= nc; ++k) {
+            if (k < nc) {
+                const size_t off = k * kChunk, len = std::min(kChunk, n - off);
+                CK(cudaMemcpyAsync(buf[k & 1].p, static_cast<const char*>(src) + off, len, cudaMemcpyDeviceToHost, st));
+                CK(cudaEventRecord(ev[k & 1], st));
+            }
+            if (k > 0) {
+                const size_t j = k - 1, off = j * kChunk, len = std::min(kChunk, n - off);
+                CK(cudaEventSynchronize(ev[j & 1]));
+                memcpy(static_cast<char*>(dst) + off, buf[j & 1].p, len);
+            }
+        }
+        return 0;
+    }
+    // host -> device, queued on st
+    int h2d(void* dst, const void* src, size_t n, cudaStream_t st) {
+        if (n == 0) return 0;
+        if (is_device_accessible_host(src)) { CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, st)); return 0; }
+        CK(buf[0].need(kChunk));
+        CK(buf[1].need(kChunk));
+        const size_t nc = (n + kChunk - 1) / kChunk;
+        for (size_t k = 0; k < nc; ++k) {
+            const size_t off = k * kChunk, len = std::min(kChunk, n - off);
+            CK(cudaEventSynchronize(ev[k & 1]));          // the copy out of this chunk two steps (or one call) ago is done
+            memcpy(buf[k & 1].p, static_cast<const char*>(src) + off, len);
+            CK(cudaMemcpyAsync(static_cast<char*>(dst) + off, buf[k & 1].p, len, cudaMemcpyHostToDevice, st));
+            CK(cudaEventRecord(ev[k & 1], st));
+        }
+        return 0;
+    }
+};
+
 }  // namespace
 
 // Concurrent host-buffer Score() callers (one goroutine / OS thread per RPC, server.go:70-96) are coalesced: whoever finds
@@ -112,9 +195,7 @@ struct SubmitQueue {
     bool enabled = true;
     int64_t max_prompts = 65536, max_tokens = 64ll << 20;
     std::atomic<uint64_t> coalesced{0}, batches{0};
-    // combined host-side batch (pinned), owned by the current leader
-    void* h_in = nullptr; size_t h_in_cap = 0;
-    void* h_out = nullptr; size_t h_out_cap = 0;
+    PinBuf h_in, h_out;                            // the combined batch and its rows, owned by the current leader
 };
 
 struct kvidx {
@@ -145,11 +226,10 @@ struct kvidx {
     DevBuf d_misc, d_ev, d_hash, d_evtok, d_qoff, d_wkeys, d_wpred, d_wready, d_wmap;
     DevBuf d_sweep;                 // CLOCK sweep scratch: bitmap image, per-tile counts, control block
     PinBuf h_misc;
-    // snapshot / restore (guarded by mu_w): two pinned chunks between the device and a caller's buffer, which may be
-    // pageable; the device scratch (records, sort buffers) is released when the call returns
+    // snapshot / restore (guarded by mu_w): the stager between the device and a caller's buffer, which may be pageable;
+    // the device scratch (records, sort buffers) is released when the call returns
     DevBuf d_snap;
-    PinBuf h_snap[2];
-    cudaEvent_t ev_snap[2] = {nullptr, nullptr};
+    Stager snap;
     // collective pod removal (kvidx_shard_remove_pods, guarded by mu_w): phase 0 ran on this handle with these masks and
     // neither phase 1 nor any write call has run since, so the removal bitmaps describe exactly that removal
     bool rm_armed = false;
@@ -356,12 +436,8 @@ int clock_sweep(kvidx* x) {
     if (!x->tv.req_ref) return 0;
     const uint64_t slots = x->tv.req_mask + 1;        // both tables have the same slot count
     const uint64_t words = slots / 32, tiles = (slots + kSweepTile - 1) / kSweepTile;
-    const size_t tile_off = (words * 4 + 255) & ~(size_t)255, ctl_off = tile_off + ((tiles * 16 + 255) & ~(size_t)255);
-    CK(x->d_sweep.need(ctl_off + sizeof(SweepCtl)));
-    uint8_t* d = x->d_sweep.as<uint8_t>();
-    uint32_t* snap = reinterpret_cast<uint32_t*>(d);
-    unsigned long long* tile_cnt = reinterpret_cast<unsigned long long*>(d + tile_off);
-    SweepCtl* ctl = reinterpret_cast<SweepCtl*>(d + ctl_off);
+    uint32_t* snap; unsigned long long* tile_cnt; SweepCtl* ctl;
+    CK(carve(x->d_sweep, [&](Carver& c) { snap = c.take<uint32_t>(words); tile_cnt = c.take<unsigned long long>(tiles * 2); ctl = c.take<SweepCtl>(1); }));
     cudaStream_t st = wstream(x);
     const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)x->sm_count * 8);
     const unsigned wgrid = (unsigned)std::min<uint64_t>((words + 255) / 256, (uint64_t)x->sm_count * 8);
@@ -390,21 +466,9 @@ int cap_keys(kvidx* x) {
 int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks);
 
 // ---- Round-pipeline batch plans ------------------------------------------------------------------------------------
-// Both round pipelines take a batch's scratch from one device arena, kvidx::d_rounds.  A plan lays out its sections with a
-// Carver twice: over a null base to size the arena, then over the arena itself, so each section's size is written once.
-// Sections start on 256-byte boundaries, as a cudaMalloc of their own would, and parts start on kPartSlots boundaries:
-// the kernels' vector accesses of a part's slice stay aligned (kernel C reads fate 8 slots at a time; kernels H and P clear
-// nfol and need_snap by words, map and grp by 4 words).
-struct Carver {
-    static constexpr size_t kAlign = 256;
-    uintptr_t base = 0; size_t at = 0;
-    template <class T> T* take(size_t count) {
-        static_assert(kAlign % alignof(T) == 0, "a section is aligned for its elements");
-        T* p = reinterpret_cast<T*>(base + at);
-        at += (count * sizeof(T) + kAlign - 1) & ~(kAlign - 1);
-        return p;
-    }
-};
+// Both round pipelines take a batch's scratch from one device arena, kvidx::d_rounds, carved by the plan.  Parts start on
+// kPartSlots boundaries: the kernels' vector accesses of a part's slice stay aligned (kernel C reads fate 8 slots at a
+// time; kernels H and P clear nfol and need_snap by words, map and grp by 4 words).
 
 // A batch of n prompts in np parts: part q holds slots off[q] .. off[q] + size[q] of the sorted batch.  Every part but the
 // last ones holds ceil(n / np) prompts rounded up to kPartSlots; the last ones hold fewer, or none.
@@ -506,11 +570,7 @@ template <class Plan> int carve_rounds(kvidx* x, const ScoreArgs& a, cudaStream_
     if (x->sort_prefix)
         CK(cub::DeviceRadixSort::SortPairs(nullptr, p.su.sort_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const uint32_t*)nullptr,
                                            (uint32_t*)nullptr, (int)a.n_prompts, 32, 64, st));
-    Carver size;
-    p.carve(size);
-    CK(x->d_rounds.need(size.at));
-    Carver c{reinterpret_cast<uintptr_t>(x->d_rounds.p)};
-    p.carve(c);
+    CK(carve(x->d_rounds, [&](Carver& c) { p.carve(c); }));
     return 0;
 }
 
@@ -689,12 +749,43 @@ int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int
 // elements tok_off[i] .. tok_off[i+1] of p, with the offsets and everything else about the call in a ScoreArgs.
 // A conversation turn (kvidx_score_turn*) is keys followed by tokens: `t` holds the tokens' CSR and where the new keys go
 // (t.keys unused: the held keys are at p).
+//
+// A host-buffer call moves as CSR sections (Csr): its inputs (tokens, keys, or a turn's keys then its tokens) and, for a
+// turn that wants them, the new keys it returns.  A section moved elsewhere is a View: its elements from the first
+// moved prompt's on, that prompt's offsets on, and the first offset (the base the kernels subtract).
+struct Csr {
+    const void* p; const int64_t* off; size_t esz;      // prompt i owns elements off[i] .. off[i+1] of p, esz bytes each
+    size_t bytes(int64_t i0, int64_t i1) const { return (size_t)(off[i1] - off[i0]) * esz; }
+    uint8_t* at(int64_t i) const { return p ? static_cast<uint8_t*>(const_cast<void*>(p)) + (size_t)off[i] * esz : nullptr; }
+    // are the elements of prompts 0 .. n pinned host memory (or none at all)?
+    bool pinned(int64_t n) const { return off[n] == off[0] || is_device_accessible_host(p); }
+};
+struct View { const void* p; const int64_t* off; int64_t base; };
+
 struct ScoreIn {
     const void* p; bool keys;
     TurnArgs t = {};
     bool turn() const { return t.tok_off != nullptr; }
-    size_t elem() const { return keys ? 8 : 4; }
-    const uint8_t* at(int64_t i) const { return static_cast<const uint8_t*>(p) + (size_t)i * elem(); }
+    // the sections of the host call h: s[0 .. inputs) the inputs, then s[inputs] the new keys when wanted; -> their count
+    int sections(const ScoreArgs& h, Csr s[3], int* inputs) const {
+        int k = 0;
+        s[k++] = Csr{p, h.tok_off, keys ? 8u : 4u};
+        if (turn()) s[k++] = Csr{t.tok, t.tok_off, 4};
+        *inputs = k;
+        if (t.new_keys) s[k++] = Csr{t.new_keys, t.new_off, 8};
+        return k;
+    }
+    // this call with its sections at v (as sections() lists them); a's offsets are set
+    ScoreIn moved(const View* v, ScoreArgs& a) const {
+        ScoreIn r{v[0].p, keys, t};
+        a.tok = nullptr; a.tok_off = v[0].off; a.tok_base = v[0].base;
+        if (turn()) { r.t.tok = static_cast<const uint32_t*>(v[1].p); r.t.tok_off = v[1].off; r.t.tok_base = v[1].base; }
+        if (t.new_keys) {
+            const View& nk = v[turn() ? 2 : 1];
+            r.t.new_keys = static_cast<uint64_t*>(const_cast<void*>(nk.p)); r.t.new_off = nk.off; r.t.new_base = nk.base;
+        }
+        return r;
+    }
 };
 
 // Exact-LRU handles take the thread-per-prompt kernel: Lookup must touch every present key of a prompt (no early exit).
@@ -718,6 +809,9 @@ bool score_warp_per_prompt(const kvidx* x, bool keys, int64_t n) {
 // place)?  At every block size the kernel is built for, on default and CLOCK handles; elsewhere it is composed of the hash,
 // a concatenation and Score() from keys.
 bool score_turn_fused(const kvidx* x) { return x->score_kernel != 1 && !x->tv.req_stamp && coop_block_size(x->tv.block_size); }
+
+// Does the kernel of a call of n prompts read its inputs in place (score_host_zerocopy)?
+bool reads_in_place(const kvidx* x, const ScoreIn& in, int64_t n) { return in.turn() ? score_turn_fused(x) : score_warp_per_prompt(x, in.keys, n); }
 
 template <class E>
 int launch_score_v1(kvidx* x, const ScoreArgs& a, const E* src, cudaStream_t st) {
@@ -803,15 +897,11 @@ int launch_turn(kvidx* x, const ScoreIn& in, const ScoreArgs& a, cudaStream_t st
     CK(cudaStreamSynchronize(st));
     const uint32_t B = x->tv.block_size;
     const int64_t cap = (e[1] - e[0]) + (e[3] - e[2]) / B;             // >= the concatenated key count
-    auto al = [](size_t b) { return (b + 63) & ~(size_t)63; };
-    const size_t o_dst = al((size_t)(n + 1) * 8), o_par = o_dst + al((size_t)n * 8), o_pv = o_par + al((size_t)n * 8), o_cat = o_pv + al((size_t)n);
-    CK(x->d_turn.need(o_cat + (size_t)std::max<int64_t>(cap, 1) * 8));
-    uint8_t* d = x->d_turn.as<uint8_t>();
-    int64_t* cat_off = reinterpret_cast<int64_t*>(d);
-    int64_t* new_dst = reinterpret_cast<int64_t*>(d + o_dst);
-    uint64_t* parent = reinterpret_cast<uint64_t*>(d + o_par);
-    uint8_t* pv = d + o_pv;
-    uint64_t* cat = reinterpret_cast<uint64_t*>(d + o_cat);
+    int64_t *cat_off, *new_dst; uint64_t *parent, *cat; uint8_t* pv;
+    CK(carve(x->d_turn, [&](Carver& c) {
+        cat_off = c.take<int64_t>(n + 1); new_dst = c.take<int64_t>(n); parent = c.take<uint64_t>(n); pv = c.take<uint8_t>(n);
+        cat = c.take<uint64_t>(std::max<int64_t>(cap, 1));
+    }));
     turn_offsets_kernel<<<1, kTurnScanThreads, 0, st>>>(ta.keys, a.tok_off, a.tok_base, ta.tok_off, n, B, cat_off, new_dst, parent, pv);
     const int T = 128;
     hash_keys_kernel_v1<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, ta.tok, ta.tok_off, ta.tok_base, n, parent, pv, new_dst, 0, cat);
@@ -842,14 +932,21 @@ int check_csr(const int64_t* off, int64_t n, const char* what = "tok_off") {
 struct RowLayout {
     uint32_t P; bool sparse;
     size_t row() const { return sparse ? (size_t)kMaxEnt * (sizeof(double) + sizeof(uint16_t)) + 2 : (size_t)P * sizeof(double) + 1; }
+    // f(array, bytes) for each array of c rows, in buffer order (array: the ScoreArgs member that points at it)
+    template <class F> void each(int64_t c, F f) const {
+        if (sparse) {
+            f(&ScoreArgs::sp_scores, (size_t)c * kMaxEnt * sizeof(double));
+            f(&ScoreArgs::sp_pods, (size_t)c * kMaxEnt * sizeof(uint16_t));
+            f(&ScoreArgs::sp_cnt, (size_t)c);
+        } else {
+            f(&ScoreArgs::dense, (size_t)c * P * sizeof(double));
+        }
+        f(&ScoreArgs::has_keys, (size_t)c);
+    }
     // point the outputs of `a` into a buffer of n rows
     void carve(void* buf, int64_t n, ScoreArgs& a) const {
         uint8_t* b = static_cast<uint8_t*>(buf);
-        if (!sparse) { a.dense = reinterpret_cast<double*>(b); a.has_keys = b + (size_t)n * P * sizeof(double); return; }
-        a.sp_scores = reinterpret_cast<double*>(b);
-        a.sp_pods = reinterpret_cast<uint16_t*>(b + (size_t)n * kMaxEnt * sizeof(double));
-        a.sp_cnt = reinterpret_cast<uint8_t*>(a.sp_pods + (size_t)n * kMaxEnt);
-        a.has_keys = a.sp_cnt + n;
+        each(n, [&](auto m, size_t bytes) { a.*m = reinterpret_cast<std::remove_reference_t<decltype(a.*m)>>(b); b += bytes; });
     }
     // the outputs of `a` from row i on
     ScoreArgs at(ScoreArgs a, int64_t i) const {
@@ -858,22 +955,16 @@ struct RowLayout {
         if (a.has_keys) a.has_keys += i;
         return a;
     }
-    // copy c rows from the outputs of src to those of dst: memcpy, or with st device to host on *st.  has_keys only when
-    // dst has it.
+    // copy c rows from the outputs of src to those of dst: memcpy, or with st device to host on *st.  Only the arrays dst
+    // has (has_keys is optional).
     int copy(const ScoreArgs& dst, const ScoreArgs& src, int64_t c, const cudaStream_t* st = nullptr) const {
-        auto cp = [st](void* d, const void* s, size_t bytes) {
-            if (st) return cudaMemcpyAsync(d, s, bytes, cudaMemcpyDeviceToHost, *st);
-            memcpy(d, s, bytes);
-            return cudaSuccess;
-        };
-        if (sparse) {
-            CK(cp(dst.sp_scores, src.sp_scores, (size_t)c * kMaxEnt * sizeof(double)));
-            CK(cp(dst.sp_pods, src.sp_pods, (size_t)c * kMaxEnt * sizeof(uint16_t)));
-            CK(cp(dst.sp_cnt, src.sp_cnt, (size_t)c));
-        } else {
-            CK(cp(dst.dense, src.dense, (size_t)c * P * sizeof(double)));
-        }
-        if (dst.has_keys) CK(cp(dst.has_keys, src.has_keys, (size_t)c));
+        cudaError_t e = cudaSuccess;
+        each(c, [&](auto m, size_t bytes) {
+            if (!(dst.*m) || e != cudaSuccess) return;
+            if (st) e = cudaMemcpyAsync(dst.*m, src.*m, bytes, cudaMemcpyDeviceToHost, *st);
+            else memcpy(dst.*m, src.*m, bytes);
+        });
+        CK(e);
         return 0;
     }
     // are all of the outputs of `a` pinned host memory?
@@ -884,52 +975,29 @@ struct RowLayout {
     }
 };
 
-// The input sections of a host-buffer call over c prompts in one pinned buffer, each 64-byte aligned: the offsets (c + 1),
-// the model ids and the filter rows (when the call has them), then the elements (when they are staged).
-// A conversation turn adds a second section after them: the tokens' offsets, the new keys' offsets (when the keys are
-// wanted), then the tokens (when they are staged).
-struct StageLayout {
-    size_t model, filter, elem, bytes;            // section starts (the offsets start the buffer) and the total
-    size_t off2 = 0, noff = 0, elem2 = 0;         // a turn's second section
-    static size_t al(size_t b) { return (b + 63) & ~(size_t)63; }
-    StageLayout(int64_t c, bool has_model, bool has_filter, uint32_t fw, size_t elem_bytes) {
-        model = al((size_t)(c + 1) * 8);
-        filter = model + (has_model ? al((size_t)c * 4) : 0);
-        elem = filter + (has_filter ? al((size_t)c * fw * 8) : 0);
-        bytes = elem + elem_bytes;
+// Stage prompts i0 .. i0+c of the host call h (sections s[0 .. ns), the inputs first) in one pinned buffer: each
+// section's offsets, the model ids and filter rows when h has them, then the elements of each input that is not pinned.
+// -> a: the chunk's call (the staged offsets, model ids and filter rows; h's outputs), v: each section's view (the
+// elements of a pinned input and of the output stay in the caller's buffers).
+int stage_inputs(PinBuf& buf, const ScoreArgs& h, const Csr* s, int ns, int nin, const bool* pinned, int64_t i0, int64_t c, uint32_t FW,
+                 ScoreArgs& a, View* v) {
+    int64_t* off[3]; uint32_t* model; uint64_t* filter; uint8_t* el[2];
+    CK(carve(buf, [&](Carver& cv) {
+        for (int k = 0; k < ns; ++k) off[k] = cv.take<int64_t>(c + 1);
+        model = cv.take<uint32_t>(h.model ? c : 0);
+        filter = cv.take<uint64_t>(h.filter ? c * FW : 0);
+        for (int k = 0; k < nin; ++k) el[k] = cv.take<uint8_t>(pinned[k] ? 0 : s[k].bytes(i0, i0 + c));
+    }));
+    a = h; a.n_prompts = c;
+    if (h.model) { memcpy(model, h.model + i0, (size_t)c * 4); a.model = model; }
+    if (h.filter) { memcpy(filter, h.filter + i0 * FW, (size_t)c * FW * 8); a.filter = filter; }
+    for (int k = 0; k < ns; ++k) {
+        memcpy(off[k], s[k].off + i0, (size_t)(c + 1) * 8);
+        v[k] = View{s[k].at(i0), off[k], s[k].off[i0]};
+        if (k < nin && !pinned[k]) { memcpy(el[k], v[k].p, s[k].bytes(i0, i0 + c)); v[k].p = el[k]; }
     }
-    StageLayout& turn(int64_t c, bool want_keys, size_t tok_bytes) {
-        off2 = al(bytes);
-        noff = off2 + al((size_t)(c + 1) * 8);
-        elem2 = noff + (want_keys ? al((size_t)(c + 1) * 8) : 0);
-        bytes = elem2 + tok_bytes;
-        return *this;
-    }
-    // copy the token and new-key offsets of prompts i0 .. i0+c of the host turn `t` into buf; the packed turn's tok and
-    // new_keys point at the chunk's first token and first new key in the caller's buffers (move them when staged)
-    TurnArgs pack_turn(uint8_t* buf, const TurnArgs& t, int64_t i0, int64_t c) const {
-        TurnArgs r = t;
-        memcpy(buf + off2, t.tok_off + i0, (size_t)(c + 1) * 8);
-        r.tok_off = reinterpret_cast<int64_t*>(buf + off2); r.tok_base = t.tok_off[i0];
-        if (t.tok) r.tok = t.tok + r.tok_base;
-        if (t.new_keys) {
-            memcpy(buf + noff, t.new_off + i0, (size_t)(c + 1) * 8);
-            r.new_off = reinterpret_cast<int64_t*>(buf + noff); r.new_base = t.new_off[i0];
-            r.new_keys = t.new_keys + r.new_base;
-        }
-        return r;
-    }
-    // copy the offsets, model ids and filter rows of prompts i0 .. i0+c of the host call `h` into buf: the packed call, with
-    // the outputs of h
-    ScoreArgs pack(uint8_t* buf, const ScoreArgs& h, int64_t i0, int64_t c, uint32_t fw) const {
-        ScoreArgs a = h;
-        a.tok = nullptr; a.tok_off = reinterpret_cast<int64_t*>(buf); a.tok_base = h.tok_off[i0]; a.n_prompts = c;
-        memcpy(buf, h.tok_off + i0, (size_t)(c + 1) * 8);
-        if (h.model) { memcpy(buf + model, h.model + i0, (size_t)c * 4); a.model = reinterpret_cast<const uint32_t*>(buf + model); }
-        if (h.filter) { memcpy(buf + filter, h.filter + i0 * fw, (size_t)c * fw * 8); a.filter = reinterpret_cast<const uint64_t*>(buf + filter); }
-        return a;
-    }
-};
+    return 0;
+}
 
 // Host-buffer scoring of the call `h` (host pointers; h.tok unused, the elements are at in.p).  Chunks of prompts flow
 // through two slots and three streams so that the H2D copy of chunk c+1, the kernel of chunk c and the D2H of chunk c-1
@@ -961,87 +1029,69 @@ int score_host(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     return rc;
 }
 
-// A handful of prompts (the size of one RPC, or of what the submission queue gathers at low load) that take a warp-per-prompt
-// kernel: no copy engine, no second stream.  The cooperative kernel reads the tokens straight from PINNED HOST memory -- its
-// TMA bulk copies fetch each 2 KB chunk over PCIe one chunk ahead of the chain -- and writes the result rows straight back
-// into pinned host memory; the call is one launch and one stream synchronisation.  (cudaMallocHost memory is
-// device-addressable under UVA.)  Request keys are read the same way by the key kernel, one coalesced 256-byte read per 32
-// keys.
+// A handful of prompts (the size of one RPC, or of what the submission queue gathers at low load) whose kernel reads its
+// inputs in place: no copy engine, no second stream.  The cooperative kernel reads the tokens straight from PINNED HOST
+// memory -- its TMA bulk copies fetch each 2 KB chunk over PCIe one chunk ahead of the chain -- and writes the result rows
+// straight back into pinned host memory; the call is one launch and one stream synchronisation.  (cudaMallocHost memory
+// is device-addressable under UVA.)  Request keys are read the same way by the key kernel, one coalesced 256-byte read per
+// 32 keys.
 int score_host_zerocopy(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
-    const int64_t n = h.n_prompts, tb = h.tok_off[0], nt = h.tok_off[n] - tb;
+    const int64_t n = h.n_prompts;
     const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
-    const bool in_pinned = nt == 0 || is_device_accessible_host(in.p);
-    StageLayout sl(n, h.model != nullptr, h.filter != nullptr, x->tv.filter_words, in_pinned ? 0 : (size_t)nt * in.elem());
-    // a turn: its tokens read in place when pinned, its new keys written in place when pinned, else both staged
-    const TurnArgs& t = in.t;
-    const int64_t nt2 = in.turn() ? t.tok_off[n] - t.tok_off[0] : 0, nnk = t.new_keys ? t.new_off[n] - t.new_off[0] : 0;
-    const bool tok_pinned = nt2 == 0 || is_device_accessible_host(t.tok);
-    const bool nk_pinned = nnk == 0 || is_device_accessible_host(t.new_keys + t.new_off[0]);
-    if (in.turn()) sl.turn(n, t.new_keys != nullptr, tok_pinned ? 0 : (size_t)nt2 * 4);
-    CK(x->h_stage[0].need(sl.bytes + 64));
-    uint8_t* hs = x->h_stage[0].as<uint8_t>();
-    ScoreArgs a = sl.pack(hs, h, 0, n, x->tv.filter_words);
-    const uint8_t* src = in.p ? in.at(tb) : nullptr;                    // element of absolute index tb
-    if (!in_pinned) { memcpy(hs + sl.elem, src, (size_t)nt * in.elem()); src = hs + sl.elem; }
-    ScoreIn z{src, in.keys};
-    if (in.turn()) {
-        z.t = sl.pack_turn(hs, t, 0, n);
-        if (!tok_pinned) { memcpy(hs + sl.elem2, z.t.tok, (size_t)nt2 * 4); z.t.tok = reinterpret_cast<const uint32_t*>(hs + sl.elem2); }
-    }
+    Csr s[3]; int nin;
+    const int ns = in.sections(h, s, &nin);
+    bool pinned[3];
+    for (int k = 0; k < ns; ++k) pinned[k] = s[k].pinned(n);
+    ScoreArgs a; View v[3];
+    if (int rc = stage_inputs(x->h_stage[0], h, s, ns, nin, pinned, 0, n, x->tv.filter_words, a, v)) return rc;
     // results: straight into the caller's buffers when those are pinned, else through the pinned staging (new keys after
     // the rows)
-    const bool out_direct = rows.pinned(h);
-    const size_t nk_at = StageLayout::al((size_t)n * rows.row());
-    if (!out_direct || !nk_pinned) CK(x->h_out[0].need(nk_at + (size_t)nnk * 8 + 64));
-    if (!out_direct) rows.carve(x->h_out[0].p, n, a);
-    if (!nk_pinned) z.t.new_keys = reinterpret_cast<uint64_t*>(x->h_out[0].as<uint8_t>() + nk_at);
+    const bool out_direct = rows.pinned(h), nk_direct = ns == nin || pinned[nin];
+    if (!out_direct || !nk_direct) {
+        uint8_t* r; uint64_t* nk;
+        CK(carve(x->h_out[0], [&](Carver& c) { r = c.take<uint8_t>(n * rows.row()); nk = c.take<uint64_t>(ns > nin ? s[nin].bytes(0, n) / 8 : 0); }));
+        if (!out_direct) rows.carve(r, n, a);
+        if (!nk_direct) v[nin].p = nk;
+    }
+    const ScoreIn z = in.moved(v, a);
     CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
     if (int rc = launch_score(x, z, a, x->stream)) return rc;
     CK(cudaStreamSynchronize(x->stream));
-    if (!nk_pinned) memcpy(t.new_keys + t.new_off[0], z.t.new_keys, (size_t)nnk * 8);
+    if (!nk_direct) memcpy(s[nin].at(0), v[nin].p, s[nin].bytes(0, n));
     return out_direct ? 0 : rows.copy(h, a, n);
 }
 
 int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     int rc = 0;
     const int64_t n = h.n_prompts;
-    const int64_t* tok_off = h.tok_off;
-    const size_t esz = in.elem();
-    // a turn's second section: its tokens (T: their offsets) and new keys (NK: their offsets, when wanted)
-    const TurnArgs& t = in.t;
-    const int64_t* T = t.tok_off;
-    const int64_t* NK = t.new_keys ? t.new_off : nullptr;
-    // the zero-copy and chunk budgets are bytes of input: 4 Mi tokens / 32 Mi tokens (KVIDX_HOST_CHUNK_TOKENS), or as
-    // many bytes of keys (of keys and tokens, for a turn)
-    const int64_t zc_max = (int64_t)((16ll << 20) / esz);
-    if (in.turn()) {
-        if (n <= x->zerocopy_max && (tok_off[n] - tok_off[0]) * 8 + (T[n] - T[0]) * 4 <= (16ll << 20) && score_turn_fused(x)) return score_host_zerocopy(x, in, h);
-    } else if (n <= x->zerocopy_max && tok_off[n] - tok_off[0] <= zc_max && score_warp_per_prompt(x, in.keys, n)) {
-        return score_host_zerocopy(x, in, h);
-    }
+    Csr s[3]; int nin;
+    const int ns = in.sections(h, s, &nin);
+    const Csr* nk = ns > nin ? &s[nin] : nullptr;      // a turn's new keys, when wanted
+    // the zero-copy and chunk budgets are bytes of input: 16 MiB and host_chunk_tokens x 4 (32 Mi tokens, or as many bytes
+    // of keys, or of a turn's keys and tokens)
+    auto in_bytes = [&](int64_t i0, int64_t i1) { size_t b = 0; for (int k = 0; k < nin; ++k) b += s[k].bytes(i0, i1); return b; };
+    if (n <= x->zerocopy_max && in_bytes(0, n) <= (16u << 20) && reads_in_place(x, in, n)) return score_host_zerocopy(x, in, h);
     const uint32_t FW = x->tv.filter_words;
     const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
-    // chunk = up to 32 Mi tokens (128 MiB): the H2D copy of a chunk must outlast its kernel for the
-    // pipeline to be PCIe bound, and smaller chunks leave the fixed cost of a launch exposed.
-    const int64_t kMaxTokChunk = (int64_t)(x->host_chunk_tokens * 4 / (int64_t)esz);
+    // chunk = up to 128 MiB of input: the H2D copy of a chunk must outlast its kernel for the pipeline to be PCIe bound, and
+    // smaller chunks leave the fixed cost of a launch exposed.
+    const size_t kMaxChunkBytes = (size_t)x->host_chunk_tokens * 4;
     const int64_t kMaxRowsChunk = std::max<int64_t>(1, (128ll << 20) / (int64_t)rows.row());
-    const bool tok_pinned = in.p && is_device_accessible_host(in.p);
-    const bool tok2_pinned = t.tok && is_device_accessible_host(t.tok);
-    const bool nk_pinned = NK && is_device_accessible_host(t.new_keys);
+    bool pinned[3];
+    for (int k = 0; k < ns; ++k) pinned[k] = s[k].pinned(n);
     // dense rows are written straight into the caller's buffers when those are pinned; sparse rows are always staged
     const bool out_pinned = !rows.sparse && rows.pinned(h);
     cudaStream_t s_k = x->stream, s_in = x->copy_stream, s_out = x->d2h_stream;
-    struct Pending { bool live = false; int64_t i0 = 0, cnt = 0; } pend[2];
-    auto drain = [&](int s) -> int {
-        if (!pend[s].live) return 0;
-        CK(cudaEventSynchronize(x->ev_done[s]));
-        pend[s].live = false;
-        const int64_t i0 = pend[s].i0, c = pend[s].cnt;
-        if (NK && !nk_pinned && NK[i0 + c] > NK[i0])   // the new keys, staged after the rows
-            memcpy(t.new_keys + NK[i0], x->h_out[s].as<uint8_t>() + StageLayout::al((size_t)c * rows.row()), (size_t)(NK[i0 + c] - NK[i0]) * 8);
+    struct Pending { bool live = false; int64_t i0 = 0, cnt = 0; const uint64_t* nk = nullptr; } pend[2];   // nk: staged new keys
+    auto drain = [&](int sl) -> int {
+        if (!pend[sl].live) return 0;
+        CK(cudaEventSynchronize(x->ev_done[sl]));
+        pend[sl].live = false;
+        const int64_t i0 = pend[sl].i0, c = pend[sl].cnt;
+        if (pend[sl].nk) memcpy(nk->at(i0), pend[sl].nk, nk->bytes(i0, i0 + c));
         if (out_pinned) return 0;                 // results were written straight into the caller's buffers
         ScoreArgs staged{};
-        rows.carve(x->h_out[s].p, c, staged);
+        rows.carve(x->h_out[sl].p, c, staged);
         return rows.copy(rows.at(h, i0), staged, c);
     };
     // the first chunk must see everything already queued on the handle's stream, and asynchronous write batches issued before
@@ -1052,74 +1102,45 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     int slot = 0;
     while (i0 < n) {
         int64_t i1 = i0;
-        if (T) {                                  // a turn: keys and tokens share the byte budget
-            while (i1 < n && (i1 - i0) < kMaxRowsChunk && (tok_off[i1 + 1] - tok_off[i0]) * 8 + (T[i1 + 1] - T[i0]) * 4 <= x->host_chunk_tokens * 4) ++i1;
-        } else {
-            while (i1 < n && (i1 - i0) < kMaxRowsChunk && (tok_off[i1 + 1] - tok_off[i0]) <= kMaxTokChunk) ++i1;
-        }
+        while (i1 < n && (i1 - i0) < kMaxRowsChunk && in_bytes(i0, i1 + 1) <= kMaxChunkBytes) ++i1;
         if (i1 == i0) i1 = i0 + 1;                // a single prompt larger than the chunk budget
-        const int64_t c = i1 - i0, tb = tok_off[i0], nt = tok_off[i1] - tb;
-        const int64_t nt2 = T ? T[i1] - T[i0] : 0, nnk = NK ? NK[i1] - NK[i0] : 0;
+        const int64_t c = i1 - i0, nnk = nk ? nk->off[i1] - nk->off[i0] : 0;
         rc = drain(slot);                         // slot's previous results are home; its device buffers are free
         if (rc) return rc;
-        const size_t tok2_at = StageLayout::al((size_t)std::max<int64_t>(nt, 1) * esz);   // a turn's tokens after the keys
-        CK(x->d_tok[slot].need(T ? tok2_at + (size_t)nt2 * 4 + 64 : (size_t)std::max<int64_t>(nt, 1) * esz + 64));
-        CK(x->d_off[slot].need((size_t)(c + 1) * 8 * (T ? 3 : 1)));
-        StageLayout sl(c, h.model != nullptr, h.filter != nullptr, FW, tok_pinned ? 0 : (size_t)nt * esz);
-        if (T) sl.turn(c, NK != nullptr, tok2_pinned ? 0 : (size_t)nt2 * 4);
-        CK(x->h_stage[slot].need(sl.bytes + 64));
-        uint8_t* hs = x->h_stage[slot].as<uint8_t>();
-        const ScoreArgs hc = sl.pack(hs, h, i0, c, FW);
-        ScoreArgs d = hc;                         // the chunk on the device
-        d.tok_off = x->d_off[slot].as<int64_t>();
-        CK(cudaMemcpyAsync(x->d_off[slot].p, hc.tok_off, (size_t)(c + 1) * 8, cudaMemcpyHostToDevice, s_in));
-        if (hc.model) {
+        ScoreArgs d; View v[3];                   // the chunk staged, then on the device
+        if ((rc = stage_inputs(x->h_stage[slot], h, s, ns, nin, pinned, i0, c, FW, d, v))) return rc;
+        int64_t* doff[3]; uint8_t* del[2];
+        CK(carve(x->d_off[slot], [&](Carver& cv) { for (int k = 0; k < ns; ++k) doff[k] = cv.take<int64_t>(c + 1); }));
+        CK(carve(x->d_tok[slot], [&](Carver& cv) { for (int k = 0; k < nin; ++k) del[k] = cv.take<uint8_t>(s[k].bytes(i0, i1)); }));
+        for (int k = 0; k < ns; ++k) {
+            CK(cudaMemcpyAsync(doff[k], v[k].off, (size_t)(c + 1) * 8, cudaMemcpyHostToDevice, s_in));
+            v[k].off = doff[k];
+            if (k >= nin) continue;
+            if (s[k].bytes(i0, i1) > 0) CK(cudaMemcpyAsync(del[k], v[k].p, s[k].bytes(i0, i1), cudaMemcpyHostToDevice, s_in));
+            v[k].p = del[k];
+        }
+        if (d.model) {
             CK(x->d_model[slot].need((size_t)c * 4));
-            CK(cudaMemcpyAsync(x->d_model[slot].p, hc.model, (size_t)c * 4, cudaMemcpyHostToDevice, s_in));
+            CK(cudaMemcpyAsync(x->d_model[slot].p, d.model, (size_t)c * 4, cudaMemcpyHostToDevice, s_in));
             d.model = x->d_model[slot].as<uint32_t>();
         }
-        if (hc.filter) {
+        if (d.filter) {
             CK(x->d_filter[slot].need((size_t)c * FW * 8));
-            CK(cudaMemcpyAsync(x->d_filter[slot].p, hc.filter, (size_t)c * FW * 8, cudaMemcpyHostToDevice, s_in));
+            CK(cudaMemcpyAsync(x->d_filter[slot].p, d.filter, (size_t)c * FW * 8, cudaMemcpyHostToDevice, s_in));
             d.filter = x->d_filter[slot].as<uint64_t>();
         }
-        if (nt > 0) {
-            const uint8_t* src = in.at(tb);
-            if (!tok_pinned) { memcpy(hs + sl.elem, src, (size_t)nt * esz); src = hs + sl.elem; }
-            CK(cudaMemcpyAsync(x->d_tok[slot].p, src, (size_t)nt * esz, cudaMemcpyHostToDevice, s_in));
-        }
-        // output sizes: the rows, then (a turn that wants them) the new keys
-        const size_t nk_at = StageLayout::al((size_t)c * rows.row());
-        const size_t out_bytes = nnk > 0 ? nk_at + (size_t)nnk * 8 + 64 : (size_t)c * rows.row() + 64;
-        TurnArgs dt = {};                         // the chunk's turn on the device
-        if (T) {
-            const TurnArgs ht = sl.pack_turn(hs, t, i0, c);
-            int64_t* doff = x->d_off[slot].as<int64_t>();
-            dt = ht;
-            dt.tok_off = doff + (c + 1);
-            CK(cudaMemcpyAsync(doff + (c + 1), ht.tok_off, (size_t)(c + 1) * 8, cudaMemcpyHostToDevice, s_in));
-            if (NK) {
-                dt.new_off = doff + 2 * (c + 1);
-                CK(cudaMemcpyAsync(doff + 2 * (c + 1), ht.new_off, (size_t)(c + 1) * 8, cudaMemcpyHostToDevice, s_in));
-            }
-            dt.tok = reinterpret_cast<const uint32_t*>(x->d_tok[slot].as<uint8_t>() + tok2_at);
-            if (nt2 > 0) {
-                const uint32_t* src = ht.tok;
-                if (!tok2_pinned) { memcpy(hs + sl.elem2, src, (size_t)nt2 * 4); src = reinterpret_cast<const uint32_t*>(hs + sl.elem2); }
-                CK(cudaMemcpyAsync(const_cast<uint32_t*>(dt.tok), src, (size_t)nt2 * 4, cudaMemcpyHostToDevice, s_in));
-            }
-        }
         CK(cudaEventRecord(x->ev_h2d[slot], s_in));
-        // kernel
-        CK(x->d_out[slot].need(out_bytes));
-        if (!out_pinned || (nnk > 0 && !nk_pinned)) CK(x->h_out[slot].need(out_bytes));
-        if (NK) dt.new_keys = reinterpret_cast<uint64_t*>(x->d_out[slot].as<uint8_t>() + nk_at);
-        rows.carve(x->d_out[slot].p, c, d);
+        // outputs: the rows, then (a turn that wants them) the new keys, on the device and in the pinned staging alike
+        uint8_t *drow, *hrow = nullptr; uint64_t *dnk, *hnk = nullptr;
+        CK(carve(x->d_out[slot], [&](Carver& cv) { drow = cv.take<uint8_t>(c * rows.row()); dnk = cv.take<uint64_t>(nnk); }));
+        if (!out_pinned || (nnk > 0 && !pinned[nin]))
+            CK(carve(x->h_out[slot], [&](Carver& cv) { hrow = cv.take<uint8_t>(c * rows.row()); hnk = cv.take<uint64_t>(nnk); }));
+        if (nk) v[nin].p = dnk;
+        rows.carve(drow, c, d);
         CK(cudaStreamWaitEvent(s_k, x->ev_h2d[slot], 0));
         int64_t maxb = 0;                         // the round pipelines' block count (tokens)
-        if (!in.keys) for (int64_t q = i0; q < i1; ++q) maxb = std::max<int64_t>(maxb, (tok_off[q + 1] - tok_off[q]) / x->tv.block_size);
-        ScoreIn din{x->d_tok[slot].p, in.keys};
-        din.t = dt;
+        if (!in.keys) for (int64_t q = i0; q < i1; ++q) maxb = std::max<int64_t>(maxb, (h.tok_off[q + 1] - h.tok_off[q]) / x->tv.block_size);
+        const ScoreIn din = in.moved(v, d);
         rc = launch_score(x, din, d, s_k, maxb);
         if (rc) return rc;
         CK(cudaEventRecord(x->ev_k[slot], s_k));
@@ -1130,28 +1151,17 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
         if (out_pinned) {
             if ((rc = rows.copy(rows.at(h, i0), d, c, &s_out))) return rc;
         } else {
-            CK(cudaMemcpyAsync(x->h_out[slot].p, x->d_out[slot].p, (size_t)c * rows.row(), cudaMemcpyDeviceToHost, s_out));
+            CK(cudaMemcpyAsync(hrow, drow, (size_t)c * rows.row(), cudaMemcpyDeviceToHost, s_out));
         }
-        if (nnk > 0) CK(cudaMemcpyAsync(nk_pinned ? static_cast<void*>(t.new_keys + NK[i0]) : static_cast<void*>(x->h_out[slot].as<uint8_t>() + nk_at),
-                                        dt.new_keys, (size_t)nnk * 8, cudaMemcpyDeviceToHost, s_out));
+        if (nnk > 0) CK(cudaMemcpyAsync(pinned[nin] ? static_cast<void*>(nk->at(i0)) : hnk, dnk, (size_t)nnk * 8, cudaMemcpyDeviceToHost, s_out));
         CK(cudaEventRecord(x->ev_done[slot], s_out));
         pend[slot].live = true; pend[slot].i0 = i0; pend[slot].cnt = c;
+        pend[slot].nk = nnk > 0 && !pinned[nin] ? hnk : nullptr;
         slot ^= 1;
         i0 = i1;
     }
     rc = drain(slot); if (rc) return rc;
     rc = drain(slot ^ 1); if (rc) return rc;
-    return 0;
-}
-
-
-int pin_need(void** p, size_t* cap, size_t n) {
-    if (n <= *cap) return 0;
-    if (*p) cudaFreeHost(*p);
-    *p = nullptr; *cap = 0;
-    const size_t want = n + n / 4 + 4096;
-    CK(cudaMallocHost(p, want));
-    *cap = want;
     return 0;
 }
 
@@ -1167,14 +1177,14 @@ int run_combined(kvidx* x, SubmitQueue* q, const std::vector<SubmitReq*>& batch)
         any_model |= r->a.model != nullptr || r->a.model0 != a0.model0; any_filter |= r->a.filter != nullptr;
     }
     const RowLayout rows{x->tv.max_pods, a0.sp_cnt != nullptr};
-    const StageLayout sl(n, any_model, any_filter, FW, (size_t)nt * 4);
-    int rc = pin_need(&q->h_in, &q->h_in_cap, sl.bytes + 64); if (rc) return rc;
-    rc = pin_need(&q->h_out, &q->h_out_cap, (size_t)n * rows.row() + 64); if (rc) return rc;
-    uint8_t* hi = static_cast<uint8_t*>(q->h_in);
-    int64_t* off = reinterpret_cast<int64_t*>(hi);
-    uint32_t* model = any_model ? reinterpret_cast<uint32_t*>(hi + sl.model) : nullptr;
-    uint64_t* filter = any_filter ? reinterpret_cast<uint64_t*>(hi + sl.filter) : nullptr;
-    uint32_t* tok = reinterpret_cast<uint32_t*>(hi + sl.elem);
+    int64_t* off; uint32_t* model; uint64_t* filter; uint32_t* tok;
+    CK(carve(q->h_in, [&](Carver& c) {
+        off = c.take<int64_t>(n + 1); model = c.take<uint32_t>(any_model ? n : 0); filter = c.take<uint64_t>(any_filter ? n * FW : 0);
+        tok = c.take<uint32_t>(nt);
+    }));
+    CK(q->h_out.need((size_t)n * rows.row()));
+    if (!any_model) model = nullptr;
+    if (!any_filter) filter = nullptr;
     int64_t at = 0, tat = 0;
     off[0] = 0;
     for (const SubmitReq* r : batch) {
@@ -1186,8 +1196,9 @@ int run_combined(kvidx* x, SubmitQueue* q, const std::vector<SubmitReq*>& batch)
         at += rn; tat += rt;
     }
     ScoreArgs all{nullptr, off, 0, n, model, a0.model0, filter, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    rows.carve(q->h_out, n, all);
-    if ((rc = score_host(x, ScoreIn{tok, false}, all))) return rc;
+    rows.carve(q->h_out.p, n, all);
+    int rc = score_host(x, ScoreIn{tok, false}, all);
+    if (rc) return rc;
     at = 0;
     for (const SubmitReq* r : batch) {
         rows.copy(r->a, rows.at(all, at), r->a.n_prompts);
@@ -1266,8 +1277,7 @@ SubmitQueue* new_submit_queue() {
 }
 void delete_submit_queue(SubmitQueue* q) {
     if (!q) return;
-    if (q->h_in) cudaFreeHost(q->h_in);
-    if (q->h_out) cudaFreeHost(q->h_out);
+    q->h_in.release(); q->h_out.release();
     delete q;
 }
 uint64_t submit_queue_coalesced(SubmitQueue* q) { return q->coalesced.load(); }
@@ -1358,7 +1368,7 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     }
     for (int q = 0; q < kMaxParts; ++q) { CK(cudaEventCreateWithFlags(&x->ev_g[q], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&x->ev_r[q], cudaEventDisableTiming)); }
     CK(cudaEventCreateWithFlags(&x->ev_write, cudaEventDisableTiming));
-    for (auto& e : x->ev_snap) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    CK(x->snap.init());
     x->stream = x->own_stream;
     for (int i = 0; i < 2; ++i) {
         CK(cudaEventCreateWithFlags(&x->ev_h2d[i], cudaEventDisableTiming));
@@ -1484,8 +1494,7 @@ void kvidx_destroy(kvidx_t* x) {
     x->d_rounds.release();
     x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_inv.release(); x->h_inv.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
-    x->d_snap.release(); x->h_snap[0].release(); x->h_snap[1].release();
-    for (auto& e : x->ev_snap) if (e) cudaEventDestroy(e);
+    x->d_snap.release(); x->snap.release();
     if (x->tv.req) cudaFree(x->tv.req);
     if (x->tv.eng) cudaFree(x->tv.eng);
     if (x->tv.req_stamp) cudaFree(x->tv.req_stamp);
@@ -1552,22 +1561,16 @@ int kvidx_hash_keys(kvidx_t* x, const uint32_t* tok, const int64_t* tok_off, int
     const int64_t tb = tok_off[0], nt = tok_off[n] - tb;
     CK(x->d_tok[0].need((size_t)nt * 4 + 64));
     CK(x->d_off[0].need((size_t)(n + 1) * 8));
-    CK(x->d_aux[0].need((size_t)(n + 1) * 8 + (size_t)n * 9));
+    int64_t* d_koff; uint64_t* d_parent; uint8_t* d_pv;
+    CK(carve(x->d_aux[0], [&](Carver& c) { d_koff = c.take<int64_t>(n + 1); d_parent = c.take<uint64_t>(n); d_pv = c.take<uint8_t>(n); }));
     CK(x->d_out[0].need((size_t)nk * 8));
     CK(cudaMemcpyAsync(x->d_tok[0].p, tok + tb, (size_t)nt * 4, cudaMemcpyHostToDevice, x->stream));
     CK(cudaMemcpyAsync(x->d_off[0].p, tok_off, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, x->stream));
-    uint8_t* aux = x->d_aux[0].as<uint8_t>();
-    int64_t* d_koff = reinterpret_cast<int64_t*>(aux);
-    uint64_t* d_parent = nullptr; uint8_t* d_pv = nullptr;
     CK(cudaMemcpyAsync(d_koff, key_off_out, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, x->stream));
-    if (parent) {
-        d_parent = reinterpret_cast<uint64_t*>(aux + (size_t)(n + 1) * 8);
-        CK(cudaMemcpyAsync(d_parent, parent, (size_t)n * 8, cudaMemcpyHostToDevice, x->stream));
-        if (parent_valid) {
-            d_pv = aux + (size_t)(n + 1) * 8 + (size_t)n * 8;
-            CK(cudaMemcpyAsync(d_pv, parent_valid, (size_t)n, cudaMemcpyHostToDevice, x->stream));
-        }
-    }
+    if (parent) CK(cudaMemcpyAsync(d_parent, parent, (size_t)n * 8, cudaMemcpyHostToDevice, x->stream));
+    if (parent && parent_valid) CK(cudaMemcpyAsync(d_pv, parent_valid, (size_t)n, cudaMemcpyHostToDevice, x->stream));
+    if (!parent) d_parent = nullptr;
+    if (!parent || !parent_valid) d_pv = nullptr;
     rc = launch_hash_keys(x, x->d_tok[0].as<uint32_t>(), x->d_off[0].as<int64_t>(), tb, n, d_parent, d_pv, d_koff, x->d_out[0].as<uint64_t>(), x->stream);
     if (rc) return rc;
     CK(cudaMemcpyAsync(keys_out, x->d_out[0].p, (size_t)nk * 8, cudaMemcpyDeviceToHost, x->stream));
@@ -1594,22 +1597,15 @@ int kvidx_lookup(kvidx_t* x, uint32_t model, const uint64_t* keys, int64_t n, co
     CK(cudaSetDevice(x->device));
     if (int rc0 = check_shards(x)) return rc0;
     const uint32_t FW = x->tv.filter_words;
-    CK(x->d_aux[0].need((size_t)n * 8 + (size_t)FW * 8 + 16));
-    CK(x->d_out[0].need((size_t)n * kMaxEnt * 2 + (size_t)n + 16));
-    uint8_t* aux = x->d_aux[0].as<uint8_t>();
-    uint64_t* d_keys = reinterpret_cast<uint64_t*>(aux);
-    uint64_t* d_f = nullptr;
-    int* d_cut = reinterpret_cast<int*>(aux + (size_t)n * 8 + (size_t)FW * 8);
+    uint64_t *d_keys, *d_f; int* d_cut; uint16_t* d_pt; uint8_t* d_cnt;
+    CK(carve(x->d_aux[0], [&](Carver& c) { d_keys = c.take<uint64_t>(n); d_f = c.take<uint64_t>(FW); d_cut = c.take<int>(1); }));
+    CK(carve(x->d_out[0], [&](Carver& c) { d_pt = c.take<uint16_t>(n * kMaxEnt); d_cnt = c.take<uint8_t>(n); }));
     CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
     CK(cudaMemcpyAsync(d_keys, keys, (size_t)n * 8, cudaMemcpyHostToDevice, x->stream));
-    if (filter) {
-        d_f = reinterpret_cast<uint64_t*>(aux + (size_t)n * 8);
-        CK(cudaMemcpyAsync(d_f, filter, (size_t)FW * 8, cudaMemcpyHostToDevice, x->stream));
-    }
+    if (filter) CK(cudaMemcpyAsync(d_f, filter, (size_t)FW * 8, cudaMemcpyHostToDevice, x->stream));
+    else d_f = nullptr;
     const int big = 0x7fffffff;
     CK(cudaMemcpyAsync(d_cut, &big, sizeof(int), cudaMemcpyHostToDevice, x->stream));
-    uint16_t* d_pt = x->d_out[0].as<uint16_t>();
-    uint8_t* d_cnt = x->d_out[0].as<uint8_t>() + (size_t)n * kMaxEnt * 2;
     const int T = 128;
     lookup_kernel_v1<<<(unsigned)((n + T - 1) / T), T, 0, x->stream>>>(x->tv, model, d_keys, n, d_f, d_pt, d_cnt, d_cut,
                                                                       reserve_stamps(x, (unsigned long long)n));
@@ -1802,7 +1798,8 @@ int kvidx_add(kvidx_t* x, uint32_t model, const uint64_t* engine, const uint64_t
     if (rc) return rc;
     std::shared_lock<std::shared_mutex> tl(x->tables);
     cudaStream_t st = wstream(x);
-    CK(x->d_misc.need((size_t)n * 17 + (size_t)m * 2 + 32));
+    uint64_t *d_engine, *d_request; uint16_t* d_pts; uint8_t* d_skip;
+    CK(carve(x->d_misc, [&](Carver& c) { d_engine = c.take<uint64_t>(n); d_request = c.take<uint64_t>(n); d_pts = c.take<uint16_t>(m); d_skip = c.take<uint8_t>(n); }));
     CK(x->h_misc.need((size_t)n + 16));
     // pairs are added in order (in_memory.go:159): an engine key that appears again later in the call keeps the later mapping
     uint8_t* skip = x->h_misc.as<uint8_t>();
@@ -1812,16 +1809,12 @@ int kvidx_add(kvidx_t* x, uint32_t model, const uint64_t* engine, const uint64_t
         last.reserve((size_t)n * 2);
         for (int64_t i = 0; i < n; ++i) { skip[i] = 0; auto it = last.find(engine[i]); if (it != last.end()) { skip[it->second] = 1; any_dup = true; it->second = i; } else last.emplace(engine[i], i); }
     }
-    uint8_t* d = x->d_misc.as<uint8_t>();
-    uint8_t* d_skip = d + (size_t)n * 16 + (((size_t)m * 2 + 15) & ~(size_t)15);
-    CK(cudaMemcpyAsync(d, engine, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + (size_t)n * 8, request, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d + (size_t)n * 16, pts, (size_t)m * 2, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_engine, engine, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_request, request, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_pts, pts, (size_t)m * 2, cudaMemcpyHostToDevice, st));
     if (any_dup) CK(cudaMemcpyAsync(d_skip, skip, (size_t)n, cudaMemcpyHostToDevice, st));
     const int T = 128;
-    add_kernel<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, model, reinterpret_cast<uint64_t*>(d),
-                                                         reinterpret_cast<uint64_t*>(d + (size_t)n * 8), n,
-                                                         reinterpret_cast<uint16_t*>(d + (size_t)n * 16), m, any_dup ? d_skip : nullptr,
+    add_kernel<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, model, d_engine, d_request, n, d_pts, m, any_dup ? d_skip : nullptr,
                                                          reserve_stamps(x, 2ull * (unsigned long long)n + 2));
     x->launches += 1;
     CK(cudaGetLastError());
@@ -1899,17 +1892,16 @@ int launch_apply_events(kvidx* x, const kvidx_event_t* d_ev_sorted, const int64_
         const uint64_t map_slots = pow2ceil((uint64_t)std::max<int64_t>(2 * n_events, 64));
         CK(x->d_wkeys.need((size_t)n_hashes * 8));
         CK(x->d_wpred.need((size_t)n_events * 8));
-        // one zeroed block: work counter (16 B) | ready[n] | next[n] | best[n] (8-byte aligned)
-        const size_t n4 = ((size_t)n_events + 3) & ~(size_t)3;
-        const size_t zbytes = 16 + n4 * 4 + n4 * 4 + (size_t)n_events * 8;
-        CK(x->d_wready.need(zbytes));
+        // one zeroed block, cleared by one memset over its sections: work counter | ready[n] | next[n] | best[n]
+        unsigned long long *d_next, *d_best; unsigned int *d_ready, *d_chain;
+        size_t zbytes = 0;
+        CK(carve(x->d_wready, [&](Carver& c) {
+            d_next = c.take<unsigned long long>(2); d_ready = c.take<unsigned int>(n_events); d_chain = c.take<unsigned int>(n_events);
+            d_best = c.take<unsigned long long>(n_events);
+            zbytes = c.at;
+        }));
         CK(x->d_wmap.need((size_t)map_slots * sizeof(WantEnt)));
-        uint8_t* zb = x->d_wready.as<uint8_t>();
-        unsigned long long* d_next = reinterpret_cast<unsigned long long*>(zb);
-        unsigned int* d_ready = reinterpret_cast<unsigned int*>(zb + 16);
-        unsigned int* d_chain = reinterpret_cast<unsigned int*>(zb + 16 + n4 * 4);
-        unsigned long long* d_best = reinterpret_cast<unsigned long long*>(zb + 16 + n4 * 8);
-        CK(cudaMemsetAsync(zb, 0, zbytes, st));
+        CK(cudaMemsetAsync(d_next, 0, zbytes, st));
         CK(cudaMemsetAsync(x->d_wmap.p, 0, (size_t)map_slots * sizeof(WantEnt), st));
         const int T = 256;
         want_parents_kernel<<<(unsigned)((n_events + T - 1) / T), T, 0, st>>>(d_ev_sorted, n_events, x->tv.block_size, x->d_wmap.as<WantEnt>(), (uint32_t)(map_slots - 1), d_chain);
@@ -2037,28 +2029,28 @@ int run_removal(kvidx* x, const uint64_t* pod_mask, uint32_t tier_mask, bool pas
     const uint64_t rs = x->tv.req_mask + 1;
     const uint32_t FW = x->tv.filter_words;
     const bool sharded = x->tv.shard_bits != 0;
-    const size_t mask_off = 32, slot_off = mask_off + (size_t)FW * 8, total = slot_off + (sharded ? 0 : remove_bitmap_bytes(rs));
-    CK(x->d_misc.need(total));                        // a no-op in phase 1: phase 0 sized it and no write call came between
+    // the layout depends on the geometry and the mask width only: d_misc is not resized in phase 1 (phase 0 sized it and no
+    // write call came between), so the bitmaps are where phase 0 left them
+    unsigned long long* out; uint64_t* mask; uint32_t* bits;
+    CK(carve(x->d_misc, [&](Carver& c) {
+        out = c.take<unsigned long long>(4); mask = c.take<uint64_t>(FW); bits = c.take<uint32_t>(sharded ? 0 : remove_bitmap_bytes(rs) / 4);
+    }));
     CK(x->h_misc.need(32));
-    uint8_t* d = x->d_misc.as<uint8_t>();
-    auto bits_of = [&](uint32_t r) {
-        return sharded ? reinterpret_cast<uint32_t*>(x->tv.req_peer[r] + rs) : reinterpret_cast<uint32_t*>(d + slot_off);
-    };
+    auto bits_of = [&](uint32_t r) { return sharded ? reinterpret_cast<uint32_t*>(x->tv.req_peer[r] + rs) : bits; };
     uint32_t* mine = bits_of(x->tv.shard_rank);
-    RemoveArgs ra{reinterpret_cast<const uint64_t*>(d + mask_off), tier_mask & 0xffffu, mine, mine + rs / 32,
-                  reinterpret_cast<unsigned long long*>(d), {}, {}};
+    RemoveArgs ra{mask, tier_mask & 0xffffu, mine, mine + rs / 32, out, {}, {}};
     for (uint32_t r = 0; r < (1u << x->tv.shard_bits); ++r) { ra.owner_slot[r] = bits_of(r); ra.owner_home[r] = bits_of(r) + rs / 32; }
-    CK(cudaMemsetAsync(d, 0, 32, st));
+    CK(cudaMemsetAsync(out, 0, 32, st));
     if (pass1) {
         CK(cudaMemsetAsync(mine, 0, remove_bitmap_bytes(rs), st));
-        CK(cudaMemcpyAsync(d + mask_off, pod_mask, (size_t)FW * 8, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(mask, pod_mask, (size_t)FW * 8, cudaMemcpyHostToDevice, st));
     }
     const unsigned ctas = (unsigned)std::min<uint64_t>(rs / kRemoveThreads, (uint64_t)x->sm_count * 8);
     if (pass1) remove_req_kernel<<<ctas, kRemoveThreads, 0, st>>>(x->tv, ra);
     if (pass2) remove_eng_kernel<<<ctas, kRemoveThreads, 0, st>>>(x->tv, ra);
     x->launches += (pass1 ? 1 : 0) + (pass2 ? 1 : 0);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(x->h_misc.p, d, 24, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(x->h_misc.p, out, 24, cudaMemcpyDeviceToHost, st));
     int rc = refresh_counters(x);                      // synchronises the write stream: the removal has taken effect
     if (rc) return rc;
     if (removed_out) memcpy(removed_out, x->h_misc.p, 24);
@@ -2112,7 +2104,6 @@ namespace {
 // ---- snapshot / restore (format v1, include/kvidx.h; kernels_snapshot.cuh) ----------------------------------------------
 constexpr uint64_t kSnapHeaderBytes = 64;
 constexpr uint32_t kSnapVersion = 1, kSnapFlagRecency = 1;
-constexpr size_t kSnapChunk = 16u << 20;          // bytes per pinned staging chunk
 const char kSnapMagic[8] = {'K', 'V', 'I', 'D', 'X', 'S', 'N', 'P'};
 
 struct SnapHeader {                               // the 64 header bytes (little-endian hosts: x86-64, aarch64)
@@ -2126,69 +2117,31 @@ static_assert(sizeof(SnapHeader) == kSnapHeaderBytes, "snapshot header is 64 byt
 
 void release_snap(kvidx* x) { x->d_snap.release(); }
 
-// device -> caller's buffer: directly if it is pinned, else through the two pinned chunks (the copy engine fills one while
-// the host empties the other)
-int stage_d2h(PinBuf* hb, cudaEvent_t* ev, void* dst, const void* src, size_t n, cudaStream_t st) {
-    if (n == 0) return 0;
-    if (is_device_accessible_host(dst)) {             // a pinned caller buffer: one copy, no staging
-        CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        return 0;
-    }
-    CK(hb[0].need(kSnapChunk));
-    CK(hb[1].need(kSnapChunk));
-    const size_t nc = (n + kSnapChunk - 1) / kSnapChunk;
-    for (size_t k = 0; k <= nc; ++k) {
-        if (k < nc) {
-            const size_t off = k * kSnapChunk, len = std::min(kSnapChunk, n - off);
-            CK(cudaMemcpyAsync(hb[k & 1].p, static_cast<const char*>(src) + off, len, cudaMemcpyDeviceToHost, st));
-            CK(cudaEventRecord(ev[k & 1], st));
-        }
-        if (k > 0) {
-            const size_t j = k - 1, off = j * kSnapChunk, len = std::min(kSnapChunk, n - off);
-            CK(cudaEventSynchronize(ev[j & 1]));
-            memcpy(static_cast<char*>(dst) + off, hb[j & 1].p, len);
-        }
-    }
-    return 0;
-}
-// caller's buffer -> device, the same way round
-int stage_h2d(PinBuf* hb, cudaEvent_t* ev, void* dst, const void* src, size_t n, cudaStream_t st) {
-    if (n == 0) return 0;
-    if (is_device_accessible_host(src)) { CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyHostToDevice, st)); return 0; }
-    CK(hb[0].need(kSnapChunk));
-    CK(hb[1].need(kSnapChunk));
-    const size_t nc = (n + kSnapChunk - 1) / kSnapChunk;
-    for (size_t k = 0; k < nc; ++k) {
-        const size_t off = k * kSnapChunk, len = std::min(kSnapChunk, n - off);
-        CK(cudaEventSynchronize(ev[k & 1]));          // the copy out of this chunk two steps (or one call) ago is done
-        memcpy(hb[k & 1].p, static_cast<const char*>(src) + off, len);
-        CK(cudaMemcpyAsync(static_cast<char*>(dst) + off, hb[k & 1].p, len, cudaMemcpyHostToDevice, st));
-        CK(cudaEventRecord(ev[k & 1], st));
-    }
-    return 0;
-}
-
 unsigned snap_ctas(kvidx* x, uint64_t n) {
     return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((n + kSnapThreads - 1) / kSnapThreads, (uint64_t)x->sm_count * 8));
 }
 
-// sort buffers of N records: keys (2 x 8 B), slot indices (2 x 4 B), models (2 x 2 B); the cub scratch follows
-size_t snap_sort_bytes(uint64_t N) { return ((size_t)N * 28 + 255) & ~(size_t)255; }
+// The sort buffers of up to N records (two of each: keys, slot indices, models) and the cub scratch
+struct SnapSort {
+    uint64_t* k[2]; uint32_t* i[2]; uint16_t* m[2]; void* tmp; size_t tmp_bytes;
+    void carve(Carver& c, uint64_t N) {
+        for (auto& p : k) p = c.take<uint64_t>(N);
+        for (auto& p : i) p = c.take<uint32_t>(N);
+        for (auto& p : m) p = c.take<uint16_t>(N);
+        tmp = c.take<uint8_t>(tmp_bytes);
+    }
+};
 
-// One table's FULL slots, sorted by (model, hash): slot indices in *sorted (inside `sc`).  `sc` holds snap_sort_bytes()
-// plus the cub scratch; `misc` is zeroed by the caller.  Slot indices are 32-bit: a table of 2^32 slots would be 128 GB.
+// One table's FULL slots, sorted by (model, hash): slot indices in *sorted (inside `so`).  `misc` is zeroed by the caller.
+// Slot indices are 32-bit: a table of 2^32 slots would be 128 GB.
 template <int kMeta>
-int snap_sort_table(kvidx* x, const void* tab, uint64_t slots, uint64_t expect, uint8_t* sc, size_t sort_tmp, SnapMisc* d_misc,
+int snap_sort_table(kvidx* x, const void* tab, uint64_t slots, uint64_t expect, const SnapSort& so, SnapMisc* d_misc,
                     const uint32_t** sorted, const char* what, cudaStream_t st) {
-    const uint64_t N = std::max<uint64_t>(expect, 1);
-    uint64_t* k0 = reinterpret_cast<uint64_t*>(sc);
-    uint64_t* k1 = k0 + N;
-    uint32_t* i0 = reinterpret_cast<uint32_t*>(k1 + N);
-    uint32_t* i1 = i0 + N;
-    uint16_t* m0 = reinterpret_cast<uint16_t*>(i1 + N);
-    uint16_t* m1 = m0 + N;
-    void* tmp = sc + snap_sort_bytes(N);
+    uint64_t *k0 = so.k[0], *k1 = so.k[1];
+    uint32_t *i0 = so.i[0], *i1 = so.i[1];
+    uint16_t *m0 = so.m[0], *m1 = so.m[1];
+    void* tmp = so.tmp;
+    const size_t sort_tmp = so.tmp_bytes;
     const unsigned ctas = (unsigned)std::min<uint64_t>(slots / kSnapThreads, (uint64_t)x->sm_count * 8);
     snap_compact_kernel<kMeta><<<ctas, kSnapThreads, 0, st>>>(static_cast<const uint4*>(tab), slots, expect, k0, i0, d_misc);
     x->launches += 1;
@@ -2220,26 +2173,24 @@ int snap_sort_table(kvidx* x, const void* tab, uint64_t slots, uint64_t expect, 
 int snapshot_impl(kvidx* x, void* buf, uint64_t R, uint64_t E, bool rec) {
     cudaStream_t st = wstream(x);
     const uint64_t N = std::max<uint64_t>(std::max(R, E), 1);
-    size_t sort_tmp = 0, t2 = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)N, 0, 64, st));
+    SnapSort so{};
+    size_t t2 = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, so.tmp_bytes, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)N, 0, 64, st));
     CK(cub::DeviceRadixSort::SortPairs(nullptr, t2, (uint16_t*)nullptr, (uint16_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)N, 0, 16, st));
-    sort_tmp = std::max(sort_tmp, t2);
-    // device scratch: misc (2 x SnapMisc) | image body | sort buffers + cub scratch
+    so.tmp_bytes = std::max(so.tmp_bytes, t2);
+    // device scratch: misc (2 x SnapMisc) | image body (its byte layout, moved in one staged copy) | sort buffers
     const size_t body = (size_t)(32 * R + 24 * E + (rec ? 8 * (R + E) : 0));
-    const size_t body_off = 256, sc_off = body_off + ((body + 255) & ~(size_t)255);
-    CK(x->d_snap.need(sc_off + snap_sort_bytes(N) + sort_tmp));
+    SnapMisc* d_req; uint8_t* out;
+    CK(carve(x->d_snap, [&](Carver& c) { d_req = c.take<SnapMisc>(2); out = c.take<uint8_t>(body); so.carve(c, N); }));
     CK(x->h_misc.need(64));
-    uint8_t* d = x->d_snap.as<uint8_t>();
-    SnapMisc* d_req = reinterpret_cast<SnapMisc*>(d);
     SnapMisc* d_eng = d_req + 1;
-    uint8_t* out = d + body_off;
-    CK(cudaMemsetAsync(d, 0, 2 * sizeof(SnapMisc), st));
+    CK(cudaMemsetAsync(d_req, 0, 2 * sizeof(SnapMisc), st));
     uint4* req_rec = reinterpret_cast<uint4*>(out);
     unsigned long long* eng_rec = reinterpret_cast<unsigned long long*>(out + 32 * R);
     unsigned long long* req_st = rec ? reinterpret_cast<unsigned long long*>(out + 32 * R + 24 * E) : nullptr;
     unsigned long long* eng_st = rec ? req_st + R : nullptr;
     const uint32_t* idx = nullptr;
-    int rc = snap_sort_table<3>(x, x->tv.req, x->tv.req_mask + 1, R, d + sc_off, sort_tmp, d_req, &idx, "request", st);
+    int rc = snap_sort_table<3>(x, x->tv.req, x->tv.req_mask + 1, R, so, d_req, &idx, "request", st);
     if (rc) return rc;
     const uint32_t model_span_req = x->h_misc.as<SnapMisc>()->model_span;
     if (R) {
@@ -2247,7 +2198,7 @@ int snapshot_impl(kvidx* x, void* buf, uint64_t R, uint64_t E, bool rec) {
         x->launches += 1;
         CK(cudaGetLastError());
     }
-    rc = snap_sort_table<0>(x, x->tv.eng, x->tv.eng_mask + 1, E, d + sc_off, sort_tmp, d_eng, &idx, "engine", st);
+    rc = snap_sort_table<0>(x, x->tv.eng, x->tv.eng_mask + 1, E, so, d_eng, &idx, "engine", st);
     if (rc) return rc;
     const uint32_t model_span_eng = x->h_misc.as<SnapMisc>()->model_span;
     if (E) {
@@ -2265,7 +2216,7 @@ int snapshot_impl(kvidx* x, void* buf, uint64_t R, uint64_t E, bool rec) {
     hd.pod_span = x->h_misc.as<SnapMisc>()->pod_span;
     hd.model_span = std::max(model_span_req, model_span_eng);
     memcpy(buf, &hd, sizeof hd);
-    return stage_d2h(x->h_snap, x->ev_snap, static_cast<char*>(buf) + kSnapHeaderBytes, out, body, st);
+    return x->snap.d2h(static_cast<char*>(buf) + kSnapHeaderBytes, out, body, st);
 }
 
 int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t restored_out[2]) {
@@ -2273,22 +2224,24 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
     const uint64_t R = hd.n_request, E = hd.n_engine;
     const bool rec = hd.flags & kSnapFlagRecency;
     const size_t nbody = (size_t)(32 * R + 24 * E + (rec ? 8 * (R + E) : 0));
-    const size_t body_off = 256, st_off = body_off + ((nbody + 255) & ~(size_t)255);
     // recency images: each section's stamps sorted (8 B per record) + the cub scratch
     size_t sort_tmp = 0;
     if (rec) CK(cub::DeviceRadixSort::SortKeys(nullptr, sort_tmp, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                                (int)std::max<uint64_t>(std::max(R, E), 1), 0, 64, st));
-    const size_t tmp_off = st_off + (rec ? ((size_t)(R + E) * 8 + 255) & ~(size_t)255 : 0);
-    CK(x->d_snap.need(tmp_off + sort_tmp));
+    // device scratch: the checks and, sharded, the records per owner (16 x 8 B) in one zeroed block | image body | sorted
+    // stamps | cub scratch
+    uint8_t *dchk, *dbody, *tmp; unsigned long long* sorted;
+    CK(carve(x->d_snap, [&](Carver& c) {
+        dchk = c.take<uint8_t>(2 * sizeof(SnapCheck) + 16 * 8); dbody = c.take<uint8_t>(nbody);
+        sorted = c.take<unsigned long long>(rec ? R + E : 0); tmp = c.take<uint8_t>(sort_tmp);
+    }));
     CK(x->h_misc.need(2 * sizeof(SnapCheck) + 16 + 16 * 8));
-    uint8_t* d = x->d_snap.as<uint8_t>();
-    SnapCheck* d_chk = reinterpret_cast<SnapCheck*>(d);
-    unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(d_chk + 2);     // sharded: records per owner (16 x 8 B)
-    CK(cudaMemsetAsync(d, 0, 2 * sizeof(SnapCheck) + 16 * 8, st));
+    SnapCheck* d_chk = reinterpret_cast<SnapCheck*>(dchk);
+    unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(d_chk + 2);
+    CK(cudaMemsetAsync(dchk, 0, 2 * sizeof(SnapCheck) + 16 * 8, st));
     CK(cudaMemsetAsync(&d_chk[0].first_bad, 0xff, 8, st));
     CK(cudaMemsetAsync(&d_chk[1].first_bad, 0xff, 8, st));
-    uint8_t* dbody = d + body_off;
-    int rc = stage_h2d(x->h_snap, x->ev_snap, dbody, body, nbody, st);
+    int rc = x->snap.h2d(dbody, body, nbody, st);
     if (rc) return rc;
     const uint4* req_rec = reinterpret_cast<const uint4*>(dbody);
     const unsigned long long* eng_rec = reinterpret_cast<const unsigned long long*>(dbody + 32 * R);
@@ -2312,13 +2265,12 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
     unsigned long long* h_hist = h_from + 2;
     h_from[0] = h_from[1] = 0;
     if (rec) {
-        unsigned long long* sorted = reinterpret_cast<unsigned long long*>(d + st_off);
         const unsigned long long* sect[2] = {req_st, eng_st};
         const uint64_t cnt[2] = {R, E};
         for (int tb = 0; tb < 2; ++tb) {
             if (!cnt[tb]) continue;
             size_t tb_bytes = sort_tmp;
-            CK(cub::DeviceRadixSort::SortKeys(d + tmp_off, tb_bytes, sect[tb], sorted, (int)cnt[tb], 0, 64, st));
+            CK(cub::DeviceRadixSort::SortKeys(tmp, tb_bytes, sect[tb], sorted, (int)cnt[tb], 0, 64, st));
             snap_check_ties_kernel<<<snap_ctas(x, cnt[tb]), kSnapThreads, 0, st>>>(sorted, cnt[tb], d_chk + tb);
             x->launches += 5;
             if (keep && cnt[tb] > x->tv.capacity)
@@ -2702,8 +2654,7 @@ struct TextStore {
     int64_t cap_blocks = 0; uint32_t B = 0;
     cudaStream_t stream = nullptr;            // kvidx_text_store_add / _find (Score() from text runs on the handle's stream)
     cudaEvent_t ev_last = nullptr;            // the end of the last store call, on whichever stream it ran: the next one waits
-    cudaEvent_t ev_stage[2] = {nullptr, nullptr};
-    PinBuf h_stage[2];                        // pinned chunks for pageable host buffers
+    Stager stage;                             // for pageable host buffers
     PinBuf h_misc;
     TextTable t{};
     void* tab = nullptr;                      // the table's arrays, one allocation
@@ -2722,8 +2673,7 @@ void delete_text_store(TextStore* s) {
     if (s->tab) cudaFree(s->tab);
     if (s->arena) cudaFree(s->arena);
     s->d_in.release(); s->d_blk.release(); s->d_scr.release(); s->d_tok.release(); s->d_cub.release(); s->d_out.release();
-    s->h_stage[0].release(); s->h_stage[1].release(); s->h_misc.release();
-    for (auto& e : s->ev_stage) if (e) cudaEventDestroy(e);
+    s->stage.release(); s->h_misc.release();
     if (s->ev_last) cudaEventDestroy(s->ev_last);
     if (s->stream) cudaStreamDestroy(s->stream);
     delete s;
@@ -2831,12 +2781,6 @@ int text_arena_room(kvidx* x, TextStore* s, int64_t incoming, cudaStream_t st) {
     return 0;
 }
 
-// scratch carved from one DevBuf, 256-byte aligned sections
-struct TextCarve {
-    uint8_t* base; size_t at = 0;
-    template <class T> T* take(int64_t n) { T* p = reinterpret_cast<T*>(base + at); at += ((size_t)std::max<int64_t>(n, 1) * sizeof(T) + 255) & ~(size_t)255; return p; }
-};
-
 // The device inputs of a store call: text (prompt i at text + text_off[i] - text_base) and its offsets.
 struct TextIn { const uint8_t* text; const int64_t* off; int64_t base; int64_t n; };
 
@@ -2852,12 +2796,10 @@ struct FindScratch { int64_t nblk = 0; uint32_t* hit = nullptr; int64_t* nhit = 
 int text_find_pass1(kvidx* x, TextStore* s, const TextIn& in, double min_ratio, FindScratch& f, cudaStream_t st) {
     const int64_t n = in.n;
     if (int rc = text_blocks(x, s, in.off, nullptr, n, &f.nblk, st)) return rc;
-    TextCarve c{nullptr};
-    c.take<uint32_t>(f.nblk); c.take<int64_t>(n); c.take<int64_t>(n + 1); c.take<int64_t>(n + 1); c.take<double>(n); c.take<uint8_t>(n);
-    TK(s->d_scr.need(c.at), "find scratch");
-    c = TextCarve{s->d_scr.as<uint8_t>()};
-    f.hit = c.take<uint32_t>(f.nblk); f.nhit = c.take<int64_t>(n); f.tok_off = c.take<int64_t>(n + 1); f.score_off = c.take<int64_t>(n + 1);
-    f.ratio = c.take<double>(n); f.tokenize = c.take<uint8_t>(n);
+    TK(carve(s->d_scr, [&](Carver& c) {
+        f.hit = c.take<uint32_t>(std::max<int64_t>(f.nblk, 1)); f.nhit = c.take<int64_t>(n); f.tok_off = c.take<int64_t>(n + 1);
+        f.score_off = c.take<int64_t>(n + 1); f.ratio = c.take<double>(n); f.tokenize = c.take<uint8_t>(n);
+    }), "find scratch");
     CK(cudaMemsetAsync(f.tok_off, 0, 8, st));
     CK(cudaMemsetAsync(f.score_off, 0, 8, st));
     const bool score = min_ratio >= 0;
@@ -2897,15 +2839,11 @@ int text_add(kvidx* x, TextStore* s, const TextIn& in, const uint32_t* tok, cons
     // room for every key of the call at load <= 1/2 before the cut
     const uint64_t want = pow2ceil((uint64_t)std::max<int64_t>(2 * (s->resident + nblk), 1024));
     if (want > s->t.mask + 1) { if (int rc = text_rebuild(x, s, want, 0, st)) return rc; }
-    TextCarve c{nullptr};
-    c.take<uint64_t>(nblk); c.take<int64_t>(nblk); c.take<int64_t>(nblk + 1); c.take<uint32_t>(nblk); c.take<unsigned long long>(1);
-    TK(s->d_out.need(c.at), "add scratch");
-    c = TextCarve{s->d_out.as<uint8_t>()};
-    uint64_t* key = c.take<uint64_t>(nblk);
-    int64_t* src = c.take<int64_t>(nblk);
-    int64_t* pos = c.take<int64_t>(nblk + 1);
-    uint32_t* slot_of = c.take<uint32_t>(nblk);
-    unsigned long long* inserted = c.take<unsigned long long>(1);
+    uint64_t* key; int64_t *src, *pos; uint32_t* slot_of; unsigned long long* inserted;
+    TK(carve(s->d_out, [&](Carver& c) {
+        key = c.take<uint64_t>(nblk); src = c.take<int64_t>(nblk); pos = c.take<int64_t>(nblk + 1); slot_of = c.take<uint32_t>(nblk);
+        inserted = c.take<unsigned long long>(1);
+    }), "add scratch");
     const int64_t* bo = s->d_blk.as<int64_t>();
     text_launch_lanes(x, n, [&](auto L, unsigned grid) {
         text_hash_kernel<L.value><<<grid, kTextThreads, 0, st>>>(in.text, in.off, in.base, n, s->B, bo, key);
@@ -2936,10 +2874,9 @@ int text_add(kvidx* x, TextStore* s, const TextIn& in, const uint32_t* tok, cons
     const int64_t R = s->resident;
     size_t tb = 0;
     CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)R, 0, 64, st));
-    TK(s->d_scr.need(((size_t)R * 16 + 511) & ~(size_t)255), "eviction scratch");
+    unsigned long long *st0, *st1;
+    TK(carve(s->d_scr, [&](Carver& c) { st0 = c.take<unsigned long long>(R); st1 = c.take<unsigned long long>(R); }), "eviction scratch");
     TK(s->d_cub.need(tb), "eviction sort scratch");
-    unsigned long long* st0 = s->d_scr.as<unsigned long long>();
-    unsigned long long* st1 = st0 + R;
     CK(cudaMemsetAsync(inserted, 0, 8, st));
     text_stamps_kernel<<<text_grid(x, (int64_t)s->t.mask + 1), kTextThreads, 0, st>>>(s->t, st0, inserted, nullptr);
     CK(cub::DeviceRadixSort::SortKeys(s->d_cub.p, tb, st0, st1, (int)R, 0, 64, st));
@@ -2964,17 +2901,16 @@ int text_check(kvidx* x, int64_t n, const void* text, const int64_t* text_off) {
     return 0;
 }
 
-// Upload a host call's text and offsets to d_in: text at 0, offsets after it.  -> the device view.
-int text_upload(kvidx* x, TextStore* s, const uint8_t* text, const int64_t* text_off, int64_t n, size_t extra, TextIn* out, size_t* extra_at,
-                cudaStream_t st) {
+// Upload a host call's text and offsets to d_in, carved with the caller's own sections after them (more(Carver&)).
+// -> the device view.
+template <class More>
+int text_upload(TextStore* s, const uint8_t* text, const int64_t* text_off, int64_t n, TextIn* out, cudaStream_t st, More&& more) {
     const int64_t tb = text_off[0], nb = text_off[n] - tb;
-    const size_t off_at = ((size_t)nb + 255) & ~(size_t)255;
-    *extra_at = off_at + (((size_t)(n + 1) * 8 + 255) & ~(size_t)255);
-    TK(s->d_in.need(*extra_at + extra + 64), "input buffer");
-    uint8_t* d = s->d_in.as<uint8_t>();
-    if (int rc = stage_h2d(s->h_stage, s->ev_stage, d, text + tb, (size_t)nb, st)) return rc;
-    if (int rc = stage_h2d(s->h_stage, s->ev_stage, d + off_at, text_off, (size_t)(n + 1) * 8, st)) return rc;
-    *out = TextIn{d, reinterpret_cast<const int64_t*>(d + off_at), tb, n};
+    uint8_t* d_text; int64_t* d_off;
+    TK(carve(s->d_in, [&](Carver& c) { d_text = c.take<uint8_t>(nb); d_off = c.take<int64_t>(n + 1); more(c); }), "input buffer");
+    if (int rc = s->stage.h2d(d_text, text + tb, (size_t)nb, st)) return rc;
+    if (int rc = s->stage.h2d(d_off, text_off, (size_t)(n + 1) * 8, st)) return rc;
+    *out = TextIn{d_text, d_off, tb, n};
     return 0;
 }
 
@@ -3017,29 +2953,21 @@ int score_text_host(kvidx* x, const uint8_t* text, const int64_t* text_off, int6
     TextStore* s = c.s;
     const uint32_t FW = x->tv.filter_words;
     const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
-    const size_t model_b = model ? (size_t)n * 4 : 0, filter_b = filter ? (size_t)n * FW * 8 : 0;
-    const size_t out_b = (size_t)n * rows.row() + (size_t)n * 9;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    TextIn in; size_t at = 0;
-    int rc = text_upload(x, s, text, text_off, n, al(model_b) + al(filter_b) + al(out_b) + 512, &in, &at, c.st);
-    if (rc) return c.end(rc);
-    uint8_t* d = s->d_in.as<uint8_t>() + at;
+    // on the device after the text: the model ids and filter rows (when the call has them), the rows, ratios and flags
     ScoreArgs a{nullptr, nullptr, 0, n, nullptr, model0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    if (model) { a.model = reinterpret_cast<const uint32_t*>(d); rc = stage_h2d(s->h_stage, s->ev_stage, d, model, model_b, c.st); }
-    if (!rc && filter) { a.filter = reinterpret_cast<const uint64_t*>(d + al(model_b)); rc = stage_h2d(s->h_stage, s->ev_stage, d + al(model_b), filter, filter_b, c.st); }
+    uint32_t* d_model; uint64_t* d_filter; double* d_ratio; uint8_t* d_tokz;
+    TextIn in{};
+    int rc = text_upload(s, text, text_off, n, &in, c.st, [&](Carver& cv) {
+        d_model = cv.take<uint32_t>(model ? n : 0); d_filter = cv.take<uint64_t>(filter ? n * FW : 0);
+        rows.carve(cv.take<uint8_t>(n * rows.row()), n, a);
+        d_ratio = cv.take<double>(n); d_tokz = cv.take<uint8_t>(n);
+    });
+    if (!rc && model) { a.model = d_model; rc = s->stage.h2d(d_model, model, (size_t)n * 4, c.st); }
+    if (!rc && filter) { a.filter = d_filter; rc = s->stage.h2d(d_filter, filter, (size_t)n * FW * 8, c.st); }
     if (rc) return c.end(rc);
-    uint8_t* o = d + al(model_b) + al(filter_b);
-    rows.carve(o, n, a);
-    double* d_ratio = reinterpret_cast<double*>(o + al((size_t)n * rows.row()));
-    uint8_t* d_tokz = reinterpret_cast<uint8_t*>(d_ratio + n);
     rc = score_text_run(x, s, in, min_ratio, a, d_tokz, d_ratio, c.st);
-    auto back = [&](void* dst, const void* src, size_t b) { return dst && !rc ? (rc = stage_d2h(s->h_stage, s->ev_stage, dst, src, b, c.st)) : rc; };
-    if (rows.sparse) {
-        back(h.sp_scores, a.sp_scores, (size_t)n * kMaxEnt * 8); back(h.sp_pods, a.sp_pods, (size_t)n * kMaxEnt * 2); back(h.sp_cnt, a.sp_cnt, (size_t)n);
-    } else {
-        back(h.dense, a.dense, (size_t)n * rows.P * 8);
-    }
-    back(h.has_keys, a.has_keys, (size_t)n);
+    auto back = [&](void* dst, const void* src, size_t b) { return dst && !rc ? (rc = s->stage.d2h(dst, src, b, c.st)) : rc; };
+    rows.each(n, [&](auto m, size_t b) { back(h.*m, a.*m, b); });
     back(tokenize_out, d_tokz, (size_t)n);
     back(ratio_out, d_ratio, (size_t)n * 8);
     if (!rc) { CK(cudaStreamSynchronize(c.st)); }
@@ -3073,7 +3001,7 @@ int kvidx_text_store_init(kvidx_t* x, int64_t cache_blocks, int32_t block_bytes)
     s->cap_blocks = cache_blocks; s->B = (uint32_t)block_bytes;
     auto bail = [&](int rc) { delete_text_store(s); return rc; };
     if (cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&s->ev_last, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&s->ev_stage[0], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&s->ev_stage[1], cudaEventDisableTiming) != cudaSuccess)
+        s->stage.init() != cudaSuccess)
         return bail(fail(KVIDX_ECUDA, "prefix store: stream / event creation failed"));
     if (int rc = text_table_alloc(s, 1024, &s->t, &s->tab, s->stream)) return bail(rc);
     s->arena_cap = 1 << 16;
@@ -3105,18 +3033,15 @@ int kvidx_text_store_add(kvidx_t* x, const uint8_t* text, const int64_t* text_of
     c.st = c.s->stream;
     if (int rc = c.begin(x)) return rc;
     TextStore* s = c.s;
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t toff_b = al((size_t)(n + 1) * 8), tok_b = al((size_t)nt * 4);
-    TextIn in; size_t at = 0;
-    int rc = text_upload(x, s, text, text_off, n, toff_b + tok_b + (size_t)nt * 16, &in, &at, c.st);
-    if (rc) return c.end(rc);
-    uint8_t* d = s->d_in.as<uint8_t>() + at;
-    int64_t* d_toff = reinterpret_cast<int64_t*>(d);
-    uint32_t* d_tok = reinterpret_cast<uint32_t*>(d + toff_b);
-    uint64_t* d_span = reinterpret_cast<uint64_t*>(d + toff_b + tok_b);
-    rc = stage_h2d(s->h_stage, s->ev_stage, d_toff, tok_off, (size_t)(n + 1) * 8, c.st);
-    if (!rc && nt > 0) rc = stage_h2d(s->h_stage, s->ev_stage, d_tok, tok + tb, (size_t)nt * 4, c.st);
-    if (!rc && nt > 0) rc = stage_h2d(s->h_stage, s->ev_stage, d_span, tok_span + 2 * tb, (size_t)nt * 16, c.st);
+    // the tokens and their spans after the text (empty when nt is 0: then no prompt has a block, and text_add reads neither)
+    int64_t* d_toff; uint32_t* d_tok; uint64_t* d_span;
+    TextIn in{};
+    int rc = text_upload(s, text, text_off, n, &in, c.st, [&](Carver& cv) {
+        d_toff = cv.take<int64_t>(n + 1); d_tok = cv.take<uint32_t>(nt); d_span = cv.take<uint64_t>(nt * 2);
+    });
+    if (!rc) rc = s->stage.h2d(d_toff, tok_off, (size_t)(n + 1) * 8, c.st);
+    if (!rc && nt > 0) rc = s->stage.h2d(d_tok, tok + tb, (size_t)nt * 4, c.st);
+    if (!rc && nt > 0) rc = s->stage.h2d(d_span, tok_span + 2 * tb, (size_t)nt * 16, c.st);
     if (!rc) rc = text_add(x, s, in, d_tok, d_span, d_toff, tb, c.st);
     if (!rc) { CK(cudaStreamSynchronize(c.st)); }
     return c.end(rc);
@@ -3131,18 +3056,18 @@ int kvidx_text_store_find(kvidx_t* x, const uint8_t* text, const int64_t* text_o
     c.st = c.s->stream;
     if (int rc = c.begin(x)) return rc;
     TextStore* s = c.s;
-    TextIn in; size_t at = 0;
-    int rc = text_upload(x, s, text, text_off, n, 0, &in, &at, c.st);
+    TextIn in{};
+    int rc = text_upload(s, text, text_off, n, &in, c.st, [](Carver&) {});
     FindScratch f;
     if (!rc) rc = text_find_pass1(x, s, in, -1.0, f, c.st);
-    if (!rc) rc = stage_d2h(s->h_stage, s->ev_stage, tok_off_out, f.tok_off, (size_t)(n + 1) * 8, c.st);
-    if (!rc && ratio_out) rc = stage_d2h(s->h_stage, s->ev_stage, ratio_out, f.ratio, (size_t)n * 8, c.st);
+    if (!rc) rc = s->stage.d2h(tok_off_out, f.tok_off, (size_t)(n + 1) * 8, c.st);
+    if (!rc && ratio_out) rc = s->stage.d2h(ratio_out, f.ratio, (size_t)n * 8, c.st);
     if (rc) return c.end(rc);
     if (f.totals[0] > 0 && (!tok_out || tok_cap < f.totals[0]))       // nothing refreshed: the find has not happened
         return c.end(fail(KVIDX_ENOSPC, "tok_out holds %lld tokens, the find returns %lld", (long long)(tok_out ? tok_cap : 0), (long long)f.totals[0]));
     TK(s->d_tok.need((size_t)std::max<int64_t>(f.totals[0], 1) * 4 + 64), "token buffer");
     rc = text_find_pass2(x, s, n, f, f.tok_off, nullptr, s->d_tok.as<uint32_t>(), c.st);
-    if (!rc && f.totals[0] > 0) rc = stage_d2h(s->h_stage, s->ev_stage, tok_out, s->d_tok.p, (size_t)f.totals[0] * 4, c.st);
+    if (!rc && f.totals[0] > 0) rc = s->stage.d2h(tok_out, s->d_tok.p, (size_t)f.totals[0] * 4, c.st);
     if (!rc) { CK(cudaStreamSynchronize(c.st)); }
     return c.end(rc);
 }
@@ -3164,11 +3089,10 @@ int kvidx_text_hash_keys(kvidx_t* x, const uint8_t* text, const int64_t* text_of
     c.st = c.s->stream;
     if (int rc = c.begin(x)) return rc;
     TextStore* s = c.s;
-    TextIn in; size_t at = 0;
-    int rc = text_upload(x, s, text, text_off, n, (size_t)(n + 1) * 8 + (size_t)nk * 8 + 256, &in, &at, c.st);
+    int64_t* d_koff; uint64_t* d_keys;
+    TextIn in{};
+    int rc = text_upload(s, text, text_off, n, &in, c.st, [&](Carver& cv) { d_koff = cv.take<int64_t>(n + 1); d_keys = cv.take<uint64_t>(nk); });
     if (rc) return c.end(rc);
-    int64_t* d_koff = reinterpret_cast<int64_t*>(s->d_in.as<uint8_t>() + at);
-    uint64_t* d_keys = reinterpret_cast<uint64_t*>(d_koff + ((n + 1 + 31) & ~(int64_t)31));
     CK(cudaMemcpyAsync(d_koff, key_off_out, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, c.st));
     const uint32_t B = (uint32_t)block_bytes;
     text_launch_lanes(x, n, [&](auto L, unsigned grid) {
@@ -3176,7 +3100,7 @@ int kvidx_text_hash_keys(kvidx_t* x, const uint8_t* text, const int64_t* text_of
     });
     x->launches += 1;
     rc = cudaGetLastError() == cudaSuccess ? 0 : fail(KVIDX_ECUDA, "text hash launch failed");
-    if (!rc) rc = stage_d2h(s->h_stage, s->ev_stage, keys_out, d_keys, (size_t)nk * 8, c.st);
+    if (!rc) rc = s->stage.d2h(keys_out, d_keys, (size_t)nk * 8, c.st);
     if (!rc) { CK(cudaStreamSynchronize(c.st)); }
     return c.end(rc);
 }

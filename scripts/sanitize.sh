@@ -24,3 +24,4 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_text_store.py -x -q -m gpu -k "hash_chains or (call_streams and (7 or 1000)) or arena or enospc or slices or errors or (score_text and default and (-1] or -32] or -2048]))"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_text_store.py -x -q -m gpu -k "hash_chains and 37"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_text_store_scale.py -x -q -m gpu -k "grows_the_arena or (index_block_sizes and 32-2048) or queued_behind or clock_bits"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_pinned_staging.py -x -q -m gpu
