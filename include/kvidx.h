@@ -160,6 +160,32 @@ int kvidx_hash_keys(kvidx_t* idx, const uint32_t* tok, const int64_t* tok_off, i
 int kvidx_lookup(kvidx_t* idx, uint32_t model, const uint64_t* keys, int64_t n,
                  const uint64_t* filter, kvidx_podtier_t* podtier_out, uint8_t* cnt_out);
 
+/* The hit count of a full-depth Lookup for a batch of prompts: what the instrumented index adds to
+ * kvcache_index_max_pod_hit_count_total and kvcache_index_lookup_hits_total (instrumented_index.go:71-92) for the Lookup
+ * GetPodScores makes (indexer.go:150).  K_i are prompt i's request keys: for the tokens form TokensToKVBlockKeys(nil,
+ * tokens_i), the keys kvidx_score_batch uses; for the keys form the given list (keys/key_off as for kvidx_score_keys).  With
+ * F_i the prompt's filter row (NULL filter, or an all-zero row: all pods, as in Score()), hits_out[i] =
+ * recordHitMetrics(Lookup(K_i, F_i)): for each pod the number of its entries in the result map, then the largest of those
+ * counts (a pod with entries on two tiers of one key counts 2).  The map decides repeats: without a filter a key repeated in
+ * K_i counts once (in_memory.go:126-128), with a filter once per occurrence (:130-135).  No key -> 0.  Lookup has no early
+ * exit, so every key of every prompt is probed; its present-but-empty cut (:119-122) cannot trigger, since a present key
+ * always holds an entry.
+ * It IS a Lookup, and touches as kvidx_lookup does: exact-LRU handles stamp every present key in prompt-then-key order, with
+ * the stamp layout of Score() (a repeated key ranks as of its last occurrence); CLOCK handles set the reference bit of every
+ * present key.  A read call, ordered after kvidx_apply_events_dev batches issued before it; default, CLOCK, exact-LRU and
+ * sharded handles (peers probed from the kernel, as Score() does).  n_prompts < 0, an offset array NULL or not monotone, an
+ * element array NULL with a non-zero count, hits_out NULL -> KVIDX_EINVAL; n_prompts == 0 -> 0, nothing written;
+ * key_off[0] / tok_off[0] may be non-zero.  model, model0 and filter mean what they mean for kvidx_score_batch.
+ * The host forms are synchronous; pinned buffers are copied in place, pageable ones through pinned chunks.  The tokens
+ * forms hash the keys into scratch first.  kvidx_lookup_hits_keys_dev is one asynchronous launch on the handle's stream (on
+ * an exact-LRU handle it reads the first and last offsets back to reserve its stamps, as Score() does);
+ * kvidx_lookup_hits_dev reads the batch's first and last token offsets back to size its key scratch, and is asynchronous
+ * after that. */
+int kvidx_lookup_hits(kvidx_t* idx, const uint32_t* tok, const int64_t* tok_off, int64_t n_prompts,
+                      const uint32_t* model, uint32_t model0, const uint64_t* filter, uint32_t* hits_out);
+int kvidx_lookup_hits_keys(kvidx_t* idx, const uint64_t* keys, const int64_t* key_off, int64_t n_prompts,
+                           const uint32_t* model, uint32_t model0, const uint64_t* filter, uint32_t* hits_out);
+
 /* Indexer.GetPodScores steps 2-4 fused (indexer.go:141-163) for a batch of prompts.
  * Callers that arrive while another call's batch is on the device are queued and served together by one launch
  * (each gets exactly the rows of its own prompts; KVIDX_SUBMIT_QUEUE=0 turns the coalescing off).
@@ -412,6 +438,11 @@ int kvidx_score_turn_sparse_dev(kvidx_t* idx, const uint64_t* d_keys, const int6
                                 const int64_t* d_tok_off, int64_t n_prompts, const uint32_t* d_model, uint32_t model0,
                                 const uint64_t* d_filter, uint16_t* d_pods_out, double* d_scores_out, uint8_t* d_cnt_out,
                                 uint8_t* d_has_keys_out, const int64_t* d_new_key_off, uint64_t* d_new_keys_out);
+/* kvidx_lookup_hits[_keys] over device-resident inputs and outputs (see there for when they wait on the stream). */
+int kvidx_lookup_hits_dev(kvidx_t* idx, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n_prompts,
+                          const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, uint32_t* d_hits_out);
+int kvidx_lookup_hits_keys_dev(kvidx_t* idx, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n_prompts,
+                               const uint32_t* d_model, uint32_t model0, const uint64_t* d_filter, uint32_t* d_hits_out);
 int kvidx_hash_keys_dev(kvidx_t* idx, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n_prompts,
                         const uint64_t* d_parent, const uint8_t* d_parent_valid,
                         const int64_t* d_key_off, uint64_t* d_keys_out);

@@ -118,10 +118,13 @@ int64_t kvhost_decode_event_batch(kvhost_t* h, const char* pod, const char* mode
  * Add counts len(requestKeys) admissions and Evict len(entries) evictions whatever the call returned; every Lookup counts
  * one request and one latency observation; a successful Lookup adds max over pods of that pod's entries in the result to
  * both max_pod_hit_count and lookup_hits.  The event pool goes through the same Add / Evict (one Evict per removed hash,
- * pool.go:317-330).  With enable_metrics, kvhost_get_pod_scores issues the reference's full-depth Lookup
- * (kvidx_hash_keys + kvidx_lookup on the device) next to the fused score call, because the hit count needs every key of
- * the prompt, not only the consecutive prefix the scorer walks; kvhost_get_pod_scores_keys issues the same Lookup over the
- * keys it was given.  All zero when enable_metrics is 0. */
+ * pool.go:317-330).  The hit count is taken over the result MAP: without a pod filter a key repeated in one Lookup counts
+ * once, with one every occurrence counts (in_memory.go:126-135).  With enable_metrics, the GetPodScores entry points issue the
+ * reference's full-depth Lookup next to the score call as kvidx_lookup_hits (the hit count needs every key of the prompt,
+ * not only the consecutive prefix the scorer walks): one call (n = 1) for kvhost_get_pod_scores, _keys and _turn, and ONE
+ * call over all scored prompts of a kvhost_get_pod_scores_batch / _text batch, each of which then records one request, one
+ * latency observation of (call duration / scored prompts) and its own hit count.  kvhost_index_lookup counts from
+ * kvidx_lookup's result.  All zero when enable_metrics is 0. */
 #define KVHOST_LATENCY_BUCKETS 11          /* prometheus.DefBuckets: .005 .01 .025 .05 .1 .25 .5 1 2.5 5 10 (+Inf = count) */
 typedef struct kvhost_metrics {
     uint64_t admissions_total, evictions_total, lookup_requests_total, max_pod_hit_count_total, lookup_hits_total;

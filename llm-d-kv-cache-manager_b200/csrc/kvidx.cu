@@ -32,6 +32,7 @@
 #include "kernels_turn.cuh"
 #include "kernels_route.cuh"
 #include "kernels_text.cuh"
+#include "kernels_hits.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -222,6 +223,7 @@ struct kvidx {
     PinBuf h_stage[2], h_out[2];
     DevBuf d_turn;                  // a conversation turn on the composed path: the concatenated key CSR and its setup
     DevBuf d_inv; PinBuf h_inv;     // kvidx_pod_inventory: the 64-bit histograms on the device and their pinned copy
+    Stager rstage;                  // kvidx_lookup_hits*: a caller's host buffers to and from the device
     // write-side scratch (guarded by mu_w)
     DevBuf d_misc, d_ev, d_hash, d_evtok, d_qoff, d_wkeys, d_wpred, d_wready, d_wmap;
     DevBuf d_sweep;                 // CLOCK sweep scratch: bitmap image, per-tile counts, control block
@@ -1369,6 +1371,7 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     for (int q = 0; q < kMaxParts; ++q) { CK(cudaEventCreateWithFlags(&x->ev_g[q], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&x->ev_r[q], cudaEventDisableTiming)); }
     CK(cudaEventCreateWithFlags(&x->ev_write, cudaEventDisableTiming));
     CK(x->snap.init());
+    CK(x->rstage.init());
     x->stream = x->own_stream;
     for (int i = 0; i < 2; ++i) {
         CK(cudaEventCreateWithFlags(&x->ev_h2d[i], cudaEventDisableTiming));
@@ -1494,7 +1497,7 @@ void kvidx_destroy(kvidx_t* x) {
     x->d_rounds.release();
     x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_inv.release(); x->h_inv.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
-    x->d_snap.release(); x->snap.release();
+    x->d_snap.release(); x->snap.release(); x->rstage.release();
     if (x->tv.req) cudaFree(x->tv.req);
     if (x->tv.eng) cudaFree(x->tv.eng);
     if (x->tv.req_stamp) cudaFree(x->tv.req_stamp);
@@ -1732,6 +1735,143 @@ int kvidx_score_turn_sparse_dev(kvidx_t* x, const uint64_t* d_keys, const int64_
         return fail(KVIDX_EINVAL, "bad arguments");
     return score_dev(x, turn_dev(d_keys, d_tok, d_tok_off, d_new_key_off, d_new_keys_out),
                      ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr});
+}
+
+// ---- Lookup hit counts: recordHitMetrics(Lookup(K_i, F_i)) per prompt (kernels_hits.cuh) ----
+
+namespace {
+int launch_lookup_hits(kvidx* x, const uint64_t* d_keys, const int64_t* d_key_off, int64_t key_base, int64_t n, const uint32_t* d_model,
+                       uint32_t model0, const uint64_t* d_filter, uint32_t* d_hits, unsigned long long stamp_base, cudaStream_t st) {
+    const int64_t ctas = std::min<int64_t>(n, (int64_t)x->sm_count * kHitsCtasPerSm);
+    lookup_hits_kernel<<<(unsigned)ctas, kHitsThreads, hits_dyn_smem(x->tv.max_pods), st>>>(x->tv, d_keys, d_key_off, key_base, n, d_model,
+                                                                                           model0, d_filter, d_hits, stamp_base);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// the first and last of n + 1 device offsets, read back on st
+int read_ends(const int64_t* d_off, int64_t n, int64_t e[2], cudaStream_t st) {
+    CK(cudaMemcpyAsync(&e[0], d_off, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(&e[1], d_off + n, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// The host forms: el / off the prompts' tokens (keys false) or request keys, staged to the device with the read side's
+// stager (pinned buffers copied in place, pageable ones through its pinned chunks) into one carved buffer; tokens are
+// hashed into the keys' CSR there, and the count runs on the keys.  Synchronous.
+int lookup_hits_host_locked(kvidx* x, const void* el, bool keys, const int64_t* off, int64_t n, const uint32_t* model, uint32_t model0,
+                            const uint64_t* filter, uint32_t* hits_out) {
+    const uint32_t B = x->tv.block_size, FW = x->tv.filter_words;
+    const size_t esz = keys ? 8 : 4;
+    const int64_t e0 = off[0], ne = off[n] - e0;
+    std::vector<int64_t> koff;                        // tokens: the keys' offsets, from 0
+    if (!keys) {
+        koff.resize(n + 1);
+        koff[0] = 0;
+        for (int64_t i = 0; i < n; ++i) koff[i + 1] = koff[i] + (off[i + 1] - off[i]) / B;
+    }
+    const int64_t nk = keys ? ne : koff[n];
+    uint8_t* d_el; int64_t *d_off, *d_koff; uint32_t *d_model, *d_hits; uint64_t *d_filter, *d_keys;
+    CK(carve(x->d_aux[0], [&](Carver& c) {
+        d_el = c.take<uint8_t>((size_t)ne * esz); d_off = c.take<int64_t>(n + 1); d_model = c.take<uint32_t>(model ? n : 0);
+        d_filter = c.take<uint64_t>(filter ? (size_t)n * FW : 0); d_hits = c.take<uint32_t>(n);
+        d_koff = c.take<int64_t>(keys ? 0 : n + 1); d_keys = c.take<uint64_t>(keys ? 0 : nk);
+    }));
+    cudaStream_t st = x->stream;
+    CK(cudaStreamWaitEvent(st, x->ev_write, 0));
+    Stager& sg = x->rstage;
+    int rc = sg.h2d(d_el, static_cast<const uint8_t*>(el) + (size_t)e0 * esz, (size_t)ne * esz, st);
+    if (!rc) rc = sg.h2d(d_off, off, (size_t)(n + 1) * 8, st);
+    if (!rc && model) rc = sg.h2d(d_model, model, (size_t)n * 4, st);
+    if (!rc && filter) rc = sg.h2d(d_filter, filter, (size_t)n * FW * 8, st);
+    if (!rc && !keys) rc = sg.h2d(d_koff, koff.data(), (size_t)(n + 1) * 8, st);
+    if (rc) return rc;
+    if (!keys && nk > 0) {
+        rc = launch_hash_keys(x, reinterpret_cast<const uint32_t*>(d_el), d_off, e0, n, nullptr, nullptr, d_koff, d_keys, st);
+        if (rc) return rc;
+    }
+    const unsigned long long sb = x->tv.req_stamp ? reserve_stamps(x, (unsigned long long)nk) : 0;
+    rc = keys ? launch_lookup_hits(x, reinterpret_cast<const uint64_t*>(d_el), d_off, e0, n, model ? d_model : nullptr, model0,
+                                   filter ? d_filter : nullptr, d_hits, sb, st)
+              : launch_lookup_hits(x, d_keys, d_koff, 0, n, model ? d_model : nullptr, model0, filter ? d_filter : nullptr, d_hits, sb, st);
+    if (rc) return rc;
+    return sg.d2h(hits_out, d_hits, (size_t)n * 4, st);
+}
+
+int lookup_hits_host(kvidx* x, const void* el, bool keys, const int64_t* off, int64_t n, const uint32_t* model, uint32_t model0,
+                     const uint64_t* filter, uint32_t* hits_out) {
+    if (!x || n < 0 || !off || !hits_out) return fail(KVIDX_EINVAL, "bad arguments");
+    if (n == 0) return 0;
+    if (int rc = check_csr(off, n, keys ? "key_off" : "tok_off")) return rc;
+    if (off[n] > off[0] && !el) return fail(KVIDX_EINVAL, keys ? "NULL keys" : "NULL tokens");
+    ReadGuard g(x);
+    CK(cudaSetDevice(x->device));
+    if (int rc = check_shards(x)) return rc;
+    const int rc = lookup_hits_host_locked(x, el, keys, off, n, model, model0, filter, hits_out);
+    if (rc) {                                         // copies may still read the caller's buffers: drain before returning
+        const std::string keep = g_err;
+        cudaStreamSynchronize(x->stream);
+        cudaGetLastError();
+        g_err = keep;
+    }
+    return rc;
+}
+}  // namespace
+
+int kvidx_lookup_hits(kvidx_t* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
+                      const uint64_t* filter, uint32_t* hits_out) {
+    return lookup_hits_host(x, tok, false, tok_off, n, model, model0, filter, hits_out);
+}
+
+int kvidx_lookup_hits_keys(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, int64_t n, const uint32_t* model, uint32_t model0,
+                           const uint64_t* filter, uint32_t* hits_out) {
+    return lookup_hits_host(x, keys, true, key_off, n, model, model0, filter, hits_out);
+}
+
+int kvidx_lookup_hits_keys_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n, const uint32_t* d_model,
+                               uint32_t model0, const uint64_t* d_filter, uint32_t* d_hits_out) {
+    if (!x || n < 0 || !d_key_off || !d_hits_out) return fail(KVIDX_EINVAL, "bad arguments");
+    if (n == 0) return 0;
+    ReadGuard g(x);
+    CK(cudaSetDevice(x->device));
+    if (int rc = check_shards(x)) return rc;
+    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
+    unsigned long long sb = 0;
+    if (x->tv.req_stamp) {                            // exact-LRU: a stamp per key, counted from the offsets (as Score() does)
+        int64_t e[2];
+        if (int rc = read_ends(d_key_off, n, e, x->stream)) return rc;
+        sb = reserve_stamps(x, (unsigned long long)(e[1] - e[0]));
+    }
+    return launch_lookup_hits(x, d_keys, d_key_off, 0, n, d_model, model0, d_filter, d_hits_out, sb, x->stream);
+}
+
+int kvidx_lookup_hits_dev(kvidx_t* x, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n, const uint32_t* d_model, uint32_t model0,
+                          const uint64_t* d_filter, uint32_t* d_hits_out) {
+    if (!x || n < 0 || !d_tok_off || !d_hits_out) return fail(KVIDX_EINVAL, "bad arguments");
+    if (n == 0) return 0;
+    if (n >= (1ll << 31) - 1) return fail(KVIDX_EINVAL, "n_prompts %lld too large for one call", (long long)n);
+    ReadGuard g(x);
+    CK(cudaSetDevice(x->device));
+    if (int rc = check_shards(x)) return rc;
+    cudaStream_t st = x->stream;
+    CK(cudaStreamWaitEvent(st, x->ev_write, 0));
+    int64_t e[2];                                     // the batch's token span sizes the key scratch: >= the keys it holds
+    if (int rc = read_ends(d_tok_off, n, e, st)) return rc;
+    const int64_t cap = (e[1] - e[0]) / x->tv.block_size;
+    size_t scan_bytes = 0;                            // the keys' offsets: block counts, summed in place
+    CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (int64_t*)nullptr, (int64_t*)nullptr, (int)n, st));
+    int64_t* koff; uint64_t* keys; uint8_t* scan;
+    CK(carve(x->d_aux[0], [&](Carver& c) {
+        koff = c.take<int64_t>(n + 1); keys = c.take<uint64_t>(std::max<int64_t>(cap, 1)); scan = c.take<uint8_t>(scan_bytes);
+    }));
+    block_counts_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_tok_off, n, x->tv.block_size, koff);
+    CK(cub::DeviceScan::InclusiveSum(scan, scan_bytes, koff + 1, koff + 1, (int)n, st));
+    x->launches += 2;
+    if (int rc = launch_hash_keys(x, d_tok, d_tok_off, 0, n, nullptr, nullptr, koff, keys, st)) return rc;
+    const unsigned long long sb = x->tv.req_stamp ? reserve_stamps(x, (unsigned long long)cap) : 0;
+    return launch_lookup_hits(x, keys, koff, 0, n, d_model, model0, d_filter, d_hits_out, sb, st);
 }
 
 // ---- routed (all-to-all) form of the sharded Score(): the device steps around the exchange (kernels_route.cuh) ----

@@ -359,20 +359,35 @@ int kvhost_model_id(kvhost_t* h, const char* s) { std::lock_guard<std::mutex> g(
 
 static int need_dev(kvhost* h) { return h && h->ix ? 0 : hfail(KVIDX_ECUDA, "host-only instance: no device index (there is no CPU fallback)"); }
 
-// One Lookup as the instrumented index sees it (instrumented_index.go:47-69): request + latency always, hits on success.
-static void observe_lookup(kvhost* h, double seconds, bool ok, const kvidx_podtier_t* pt, const uint8_t* cnt, size_t n) {
-    if (!h->cfg.enable_metrics) return;
-    uint64_t mx = 0;
-    if (ok) {                                           // recordHitMetrics: entries per pod over the whole result
-        std::vector<uint32_t> per(KVIDX_MAX_PODS, 0);
-        for (size_t i = 0; i < n; ++i)
-            for (int j = 0; j < cnt[i]; ++j) { const uint32_t c = ++per[KVIDX_PT_POD(pt[i * KVIDX_MAX_PODS_PER_KEY + j])]; if (c > mx) mx = c; }
-    }
-    std::lock_guard<std::mutex> g(h->mu);
+// One Lookup as the instrumented index sees it (instrumented_index.go:47-69): request + latency always, its hit count
+// (0 for a failed Lookup) added to both hit counters.  Caller holds h->mu.
+static void record_lookup_locked(kvhost* h, double seconds, uint64_t hits) {
     h->met.lookup_requests_total += 1;
     h->met.lookup_latency_count += 1; h->met.lookup_latency_sum += seconds;
     for (int b = 0; b < KVHOST_LATENCY_BUCKETS; ++b) if (seconds <= kLatencyBuckets[b]) h->met.lookup_latency_bucket[b] += 1;
-    h->met.max_pod_hit_count_total += mx; h->met.lookup_hits_total += mx;
+    h->met.max_pod_hit_count_total += hits; h->met.lookup_hits_total += hits;
+}
+static void observe_hits(kvhost* h, double seconds, uint64_t hits) {
+    if (!h->cfg.enable_metrics) return;
+    std::lock_guard<std::mutex> g(h->mu);
+    record_lookup_locked(h, seconds, hits);
+}
+
+// A Lookup whose result came back key by key.  recordHitMetrics counts entries per pod over the result MAP: without a filter
+// (keys given) a repeated key is one map entry and counts once (in_memory.go:126-128); with one every occurrence appended
+// its entries (:130-135).
+static void observe_lookup(kvhost* h, double seconds, bool ok, const kvidx_podtier_t* pt, const uint8_t* cnt, size_t n, const uint64_t* keys) {
+    if (!h->cfg.enable_metrics) return;
+    uint64_t mx = 0;
+    if (ok) {
+        std::vector<uint32_t> per(KVIDX_MAX_PODS, 0);
+        std::unordered_set<uint64_t> seen;
+        for (size_t i = 0; i < n; ++i) {
+            if (keys && cnt[i] && !seen.insert(keys[i]).second) continue;
+            for (int j = 0; j < cnt[i]; ++j) { const uint32_t c = ++per[KVIDX_PT_POD(pt[i * KVIDX_MAX_PODS_PER_KEY + j])]; if (c > mx) mx = c; }
+        }
+    }
+    observe_hits(h, seconds, mx);
 }
 
 static bool build_filter(kvhost* h, const char* const* pods, size_t n_pods, std::vector<uint64_t>& mask) {
@@ -387,18 +402,15 @@ static bool build_filter(kvhost* h, const char* const* pods, size_t n_pods, std:
 }
 
 // With enable_metrics: the instrumented Lookup of indexer.go:150 over every key of one prompt, given as its tokens
-// (keys == nullptr, n = token count) or its request keys (n = key count).
+// (keys == nullptr, n = token count) or its request keys (n = key count): one kvidx_lookup_hits call.
 static void observe_prompt(kvhost* h, const uint32_t* tokens, const uint64_t* keys, size_t n, uint32_t mid, const uint64_t* fm) {
     if (!h->cfg.enable_metrics) return;
     const int64_t off[2] = {0, (int64_t)n};
-    const size_t nk = keys ? n : n / (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
-    std::vector<uint64_t> hashed; int64_t koff[2] = {0, 0};
-    std::vector<kvidx_podtier_t> pt(nk * KVIDX_MAX_PODS_PER_KEY); std::vector<uint8_t> kc(nk);
-    int r2 = 0;
-    if (!keys) { hashed.resize(nk); r2 = kvidx_hash_keys(h->ix, tokens, off, 1, nullptr, nullptr, hashed.data(), koff); keys = hashed.data(); }
+    uint32_t hits = 0;
     const auto t0 = std::chrono::steady_clock::now();
-    if (!r2) r2 = kvidx_lookup(h->ix, mid, keys, (int64_t)nk, fm, pt.data(), kc.data());
-    observe_lookup(h, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), r2 == 0, pt.data(), kc.data(), nk);
+    const int r2 = keys ? kvidx_lookup_hits_keys(h->ix, keys, off, 1, nullptr, mid, fm, &hits)
+                        : kvidx_lookup_hits(h->ix, tokens, off, 1, nullptr, mid, fm, &hits);
+    observe_hits(h, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), r2 == 0 ? hits : 0);
 }
 
 // GetPodScores from step 3 on for one prompt given as its tokens (keys == nullptr, n = token count) or as its request
@@ -415,7 +427,7 @@ static int pod_scores(kvhost* h, const uint32_t* tokens, const uint64_t* keys, s
         bool any = false; for (uint64_t w : mask) any |= w != 0;
         if (!any) {
             const bool has_keys = keys ? n > 0 : n >= (h->cfg.index.block_size ? h->cfg.index.block_size : 16);
-            if (has_keys) observe_lookup(h, 0.0, true, nullptr, nullptr, 0);      // the Lookup still happens; it just finds no listed pod
+            if (has_keys) observe_hits(h, 0.0, 0);      // the Lookup still happens; it just finds no listed pod
             return has_keys ? 0 : -1000;
         }
     }
@@ -471,10 +483,37 @@ static int batch_scores(kvhost* h, const uint8_t* text, const int64_t* text_off,
             to = foff.data();
         }
         const uint32_t* tb = text ? found.data() : tok;
-        for (size_t i = 0; i < n; ++i) {
+        // The hit counts of every scored prompt in ONE kvidx_lookup_hits call.  A prompt that was not scored but has a full
+        // block (text left to the tokenizer) must not be looked up -- its keys would be touched -- so such a batch passes
+        // its scored prompts' tokens, compacted; every other prompt has no key and may stay in the call.
+        const uint32_t B = h->cfg.index.block_size ? h->cfg.index.block_size : 16;
+        size_t m = 0; bool compact = false;
+        for (size_t i = 0; i < n; ++i) { m += has[i] != 0; compact |= !has[i] && to[i + 1] - to[i] >= (int64_t)B; }
+        std::vector<uint32_t> hits, ctok;
+        std::vector<int64_t> coff;
+        int r2 = 0;
+        double secs = 0.0;
+        if (!none && m > 0) {
+            const uint32_t* ct = tb; const int64_t* co = to; size_t cn = n;
+            if (compact) {
+                coff.assign(1, 0);
+                for (size_t i = 0; i < n; ++i) {
+                    if (!has[i]) continue;
+                    ctok.insert(ctok.end(), tb + to[i], tb + to[i + 1]);
+                    coff.push_back((int64_t)ctok.size());
+                }
+                ct = ctok.data(); co = coff.data(); cn = m;
+            }
+            hits.resize(cn);
+            const auto t0 = std::chrono::steady_clock::now();
+            r2 = kvidx_lookup_hits(h->ix, ct, co, (int64_t)cn, nullptr, (uint32_t)mid, fm, hits.data());
+            secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() / (double)m;
+        }
+        std::lock_guard<std::mutex> g(h->mu);
+        for (size_t i = 0, j = 0; i < n; ++i) {
             if (!has[i]) continue;
-            if (none) observe_lookup(h, 0.0, true, nullptr, nullptr, 0);
-            else observe_prompt(h, tb + (to[i] - to[0]), nullptr, (size_t)(to[i + 1] - to[i]), (uint32_t)mid, fm);
+            record_lookup_locked(h, secs, none || r2 ? 0 : hits[compact ? j : i]);
+            ++j;
         }
     }
     std::lock_guard<std::mutex> g(h->mu);
@@ -541,7 +580,7 @@ int kvhost_get_pod_scores_turn(kvhost_t* h, const uint64_t* keys, size_t n_keys,
                 if (kvidx_hash_keys(h->ix, tp, toff, 1, &parent, &pv, nk, noff)) { g_herr = kvidx_last_error(h->ix); return KVIDX_EINVAL; }
             }
             give_keys();
-            if (has_keys) observe_lookup(h, 0.0, true, nullptr, nullptr, 0);
+            if (has_keys) observe_hits(h, 0.0, 0);
             return has_keys ? 0 : -1000;
         }
     }
@@ -551,13 +590,7 @@ int kvhost_get_pod_scores_turn(kvhost_t* h, const uint64_t* keys, size_t n_keys,
     if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
     give_keys();
     if (!has) return -1000;                         // (nil, nil): no key at all
-    if (h->cfg.enable_metrics) {                    // the instrumented Lookup of indexer.go:150: every key of K
-        const size_t n = n_keys + nn;
-        std::vector<kvidx_podtier_t> pt(n * KVIDX_MAX_PODS_PER_KEY); std::vector<uint8_t> kc(n);
-        const auto t0 = std::chrono::steady_clock::now();
-        const int r2 = kvidx_lookup(h->ix, (uint32_t)mid, all.data(), (int64_t)n, fm, pt.data(), kc.data());
-        observe_lookup(h, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), r2 == 0, pt.data(), kc.data(), n);
-    }
+    observe_prompt(h, nullptr, all.data(), n_keys + nn, (uint32_t)mid, fm);     // the instrumented Lookup of indexer.go:150: every key of K
     std::lock_guard<std::mutex> g(h->mu);
     for (int i = 0; i < cnt; ++i) { pod_out[i] = h->pods.name(ids[i]); score_out[i] = sc[i]; }
     return cnt;
@@ -612,14 +645,14 @@ int kvhost_index_lookup(kvhost_t* h, const char* model, const uint64_t* keys, si
     if (int rc = need_dev(h)) return rc;
     const auto t0 = std::chrono::steady_clock::now();
     auto secs = [&] { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); };
-    if (n == 0) { observe_lookup(h, secs(), false, nullptr, nullptr, 0); return hfail(KVIDX_EINVAL, "no requestKeys provided for lookup"); }
+    if (n == 0) { observe_hits(h, secs(), 0); return hfail(KVIDX_EINVAL, "no requestKeys provided for lookup"); }
     std::shared_lock<std::shared_mutex> rl(h->read_mu);
     std::vector<uint64_t> mask; bool filtered; int mid;
     { std::lock_guard<std::mutex> g(h->mu); filtered = build_filter(h, pods, n_pods, mask); mid = h->models.id(model, 65536); }
     std::vector<kvidx_podtier_t> pt(n * KVIDX_MAX_PODS_PER_KEY);
-    if (filtered) { bool any = false; for (uint64_t w : mask) any |= w != 0; if (!any) { memset(cnt_out, 0, n); observe_lookup(h, secs(), true, pt.data(), cnt_out, n); return 0; } }
+    if (filtered) { bool any = false; for (uint64_t w : mask) any |= w != 0; if (!any) { memset(cnt_out, 0, n); observe_hits(h, secs(), 0); return 0; } }
     const int rc = kvidx_lookup(h->ix, (uint32_t)mid, keys, (int64_t)n, filtered ? mask.data() : nullptr, pt.data(), cnt_out);
-    observe_lookup(h, secs(), rc == 0, pt.data(), cnt_out, n);
+    observe_lookup(h, secs(), rc == 0, pt.data(), cnt_out, n, filtered ? nullptr : keys);
     if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
     std::lock_guard<std::mutex> g(h->mu);
     for (size_t i = 0; i < n; ++i)

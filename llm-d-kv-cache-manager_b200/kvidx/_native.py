@@ -65,7 +65,11 @@ SYMBOLS = {
     "kvidx_lookup": (C.c_int, [C.c_void_p, C.c_uint32, _u64p, C.c_int64, _u64p, _u16p, _u8p]),
     "kvidx_score_batch": (C.c_int, [C.c_void_p, _u32p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _f64p, _u8p]),
     "kvidx_score_batch_sparse": (C.c_int, [C.c_void_p, _u32p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _u16p, _f64p, _u8p, _u8p]),
-    "kvidx_score_keys": (C.c_int, [C.c_void_p, _u64p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _f64p, _u8p]),
+    "kvidx_lookup_hits": (C.c_int, [C.c_void_p, _u32p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _u32p]),
+    "kvidx_lookup_hits_keys": (C.c_int, [C.c_void_p, _u64p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _u32p]),
+    "kvidx_lookup_hits_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "kvidx_lookup_hits_keys_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "kvidx_score_keys": (C.c_int,[C.c_void_p, _u64p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _f64p, _u8p]),
     "kvidx_score_keys_sparse": (C.c_int, [C.c_void_p, _u64p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, _u16p, _f64p, _u8p, _u8p]),
     "kvidx_score_keys_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kvidx_score_keys_sparse_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -392,6 +396,42 @@ class Index:
     def score_keys_sparse_dev(self, d_keys, d_key_off, n, d_pods, d_scores, d_cnt, d_model=0, model0=0, d_filter=0, d_has_keys=0):
         self._ck(self.L.kvidx_score_keys_sparse_dev(self.h, d_keys or None, d_key_off, n, d_model or None, model0, d_filter or None,
                                                     d_pods, d_scores, d_cnt, d_has_keys or None))
+
+    # -- Lookup hit counts: recordHitMetrics(Lookup(K_i, F_i)) per prompt, the full-depth count the instrumented index adds --
+    def lookup_hits(self, tok, tok_off, model=None, model0=0, filter_mask=None):
+        """Hit count of every prompt given as tokens (uint32 (n,)); `tok` may be a numpy array or a _Raw pinned pointer."""
+        tok = np.ascontiguousarray(tok, np.uint32) if not isinstance(tok, _Raw) else tok
+        tok_off = np.ascontiguousarray(tok_off, np.int64)
+        n = len(tok_off) - 1
+        hits = np.zeros(max(n, 0), np.uint32)
+        model = None if model is None else np.ascontiguousarray(model, np.uint32)
+        filter_mask = None if filter_mask is None else np.ascontiguousarray(filter_mask, np.uint64)
+        tp = C.cast(tok.ptr, _u32p) if isinstance(tok, _Raw) else _p(tok, _u32p)
+        self._ck(self.L.kvidx_lookup_hits(self.h, tp, _p(tok_off, _i64p), n, _p(model, _u32p), model0,
+                                          _p(filter_mask, _u64p), _p(hits, _u32p)))
+        return hits
+
+    def lookup_hits_keys(self, keys, key_off, model=None, model0=0, filter_mask=None):
+        """Hit count of every prompt given as request keys; `keys` may be a numpy array or a _Raw pinned pointer."""
+        keys = np.ascontiguousarray(keys, np.uint64) if not isinstance(keys, _Raw) else keys
+        key_off = np.ascontiguousarray(key_off, np.int64)
+        n = len(key_off) - 1
+        hits = np.zeros(max(n, 0), np.uint32)
+        model = None if model is None else np.ascontiguousarray(model, np.uint32)
+        filter_mask = None if filter_mask is None else np.ascontiguousarray(filter_mask, np.uint64)
+        kp = C.cast(keys.ptr, _u64p) if isinstance(keys, _Raw) else _p(keys, _u64p)
+        self._ck(self.L.kvidx_lookup_hits_keys(self.h, kp, _p(key_off, _i64p), n, _p(model, _u32p), model0,
+                                               _p(filter_mask, _u64p), _p(hits, _u32p)))
+        return hits
+
+    def lookup_hits_dev(self, d_tok, d_tok_off, n, d_hits, d_model=0, model0=0, d_filter=0):
+        """All pointers are device addresses (ints); d_hits: n uint32.  Reads the first and last offsets back, then asynchronous."""
+        self._ck(self.L.kvidx_lookup_hits_dev(self.h, d_tok or None, d_tok_off, n, d_model or None, model0, d_filter or None, d_hits))
+
+    def lookup_hits_keys_dev(self, d_keys, d_key_off, n, d_hits, d_model=0, model0=0, d_filter=0):
+        """All pointers are device addresses (ints); d_hits: n uint32.  Asynchronous on the handle's stream."""
+        self._ck(self.L.kvidx_lookup_hits_keys_dev(self.h, d_keys or None, d_key_off, n, d_model or None, model0, d_filter or None,
+                                                   d_hits))
 
     # -- Score() for a conversation turn: prompt i is keys[key_off[i] .. key_off[i+1]) then tok[tok_off[i] .. tok_off[i+1]) --
     def _turn_args(self, keys, key_off, tok, tok_off, model, filter_mask, want_keys):

@@ -25,3 +25,5 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_text_store.py -x -q -m gpu -k "hash_chains and 37"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_text_store_scale.py -x -q -m gpu -k "grows_the_arena or (index_block_sizes and 32-2048) or queued_behind or clock_bits"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_pinned_staging.py -x -q -m gpu
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_lookup_hits.py -x -q -m gpu -k "(against_the_oracle and (257 or 4096)) or long_prompt or (tokens_form and 4) or (at_scale and (1] or 33])) or errors"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_lookup_hits.py -x -q -m gpu -k "(against_the_oracle and 257 and random) or (long_prompt and False)"
