@@ -273,6 +273,24 @@ int kvidx_score_turn_sparse(kvidx_t* idx, const uint64_t* keys, const int64_t* k
  * kvidx_text_store_find: FindLongestContainedTokens of every prompt.  tok_off_out[n_prompts + 1] (from 0) is always
  *   filled; tok_out NULL or tok_cap below the total -> KVIDX_ENOSPC, and the find refreshes nothing.  ratio_out may be NULL.
  * kvidx_text_store_len: keys resident.
+ * kvidx_text_store_snapshot / _restore (no reference counterpart): the store as an image, for a warm start after a
+ *   restart, an upgrade or a move to another GPU.  Image v1, little-endian, size 64 + 16 R + 4 T:
+ *     header (64 bytes): char[8] "KVIDXTXT", u32 version = 1, u32 flags = 0, u32 block_bytes, u32 0, u64 R (records),
+ *       u64 T (tokens), 24 zero bytes;
+ *     R records of 16 bytes, least recent first (golang-lru Keys() order): u64 key, u32 n_tok, u32 0;
+ *     T u32 token ids: record 0's n_tok tokens, then record 1's, ...
+ *   The image depends only on the resident keys, their recency order and their tokens (not on table size, arena layout,
+ *   stamps or cache_blocks), and equals kvhost_prefix_store_snapshot's after the same calls.  Records with n_tok 0 (a
+ *   block in which no token ends) are legal.
+ *   snapshot: runs after every earlier store call and every kvidx_score_text*_dev queued on the handle's stream, whose
+ *   refreshes it includes; refreshes nothing itself.  buf == NULL or cap below the size -> KVIDX_ENOSPC with *size_out
+ *   set and nothing written.  A pageable buffer is filled through pinned staging chunks, a pinned one directly.
+ *   restore: into an initialised store holding no key (else KVIDX_EINVAL); equals adding the records one by one, oldest
+ *   first: the store keeps its own cache_blocks, so a larger image leaves its newest cache_blocks records.  block_bytes
+ *   other than the store's, a bad magic, version or flags, non-zero reserved bytes or record padding, a length that does
+ *   not match the header, record token counts that do not add up to T, or a key appearing twice -> KVIDX_EINVAL.  Every
+ *   record is checked before any is inserted: a refused image leaves the store as it was.  *blocks_out (may be NULL):
+ *   keys resident afterwards.
  * kvidx_text_hash_keys: the block keys of every prompt at block_bytes (prompt-major, key_off_out[n_prompts + 1] from 0), as
  *   the store computes them; needs an initialised store (its stream and staging), whose contents it does not touch.
  * kvidx_score_text[_sparse]: processTask + GetPodScores steps 2-4.  One find over the batch (refreshing as above); prompt i
@@ -289,6 +307,8 @@ int kvidx_text_store_add(kvidx_t* idx, const uint8_t* text, const int64_t* text_
 int kvidx_text_store_find(kvidx_t* idx, const uint8_t* text, const int64_t* text_off, int64_t n_prompts,
                           uint32_t* tok_out, int64_t tok_cap, int64_t* tok_off_out, double* ratio_out);
 int kvidx_text_store_len(kvidx_t* idx, int64_t* blocks_out);
+int kvidx_text_store_snapshot(kvidx_t* idx, void* buf, uint64_t cap, uint64_t* size_out);
+int kvidx_text_store_restore(kvidx_t* idx, const void* buf, uint64_t len, int64_t* blocks_out);
 int kvidx_text_hash_keys(kvidx_t* idx, const uint8_t* text, const int64_t* text_off, int64_t n_prompts, int32_t block_bytes,
                          uint64_t* keys_out, int64_t* key_off_out);
 int kvidx_score_text(kvidx_t* idx, const uint8_t* text, const int64_t* text_off, int64_t n_prompts,

@@ -156,6 +156,14 @@ int  kvhost_prefix_store_add(kvhost_prefix_store_t* s, const char* prompt, size_
 int64_t kvhost_prefix_store_find(kvhost_prefix_store_t* s, const char* prompt, size_t prompt_len, uint32_t* tokens_out, size_t cap,
                                  double* overlap_ratio_out);
 int64_t kvhost_prefix_store_len(kvhost_prefix_store_t* s);           /* blocks resident */
+/* Snapshot / restore of the store (no counterpart; the image of kvidx_text_store_snapshot, format in kvidx.h): snapshot
+ * writes the resident blocks least recent first and refreshes nothing; buf == NULL or cap below the size -> KVIDX_ENOSPC
+ * with *size_out set and nothing written.  restore needs an empty store of the image's block_bytes and equals adding the
+ * records one by one, oldest first (the store keeps its cache_size: the newest cache_size records stay); a malformed image,
+ * a non-empty store or another block_bytes -> KVIDX_EINVAL with the store unchanged.  The device store's image after the
+ * same calls is byte-equal. */
+int kvhost_prefix_store_snapshot(kvhost_prefix_store_t* s, void* buf, uint64_t cap, uint64_t* size_out);
+int kvhost_prefix_store_restore(kvhost_prefix_store_t* s, const void* buf, uint64_t len);
 uint64_t kvhost_xxhash64(const void* data, size_t len, uint64_t seed);
 
 /* Remove a pod that has gone away (no counterpart in the reference, where a dead pod's blocks only age out of the LRU):

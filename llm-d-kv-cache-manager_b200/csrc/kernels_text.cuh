@@ -263,14 +263,61 @@ __global__ void text_add_commit_kernel(const TextTable t, int64_t nblk, unsigned
     }
 }
 
-// The stamps of the full slots, in any order (*n counts them), for the eviction cut; and the live token count.
-__global__ void text_stamps_kernel(const TextTable t, unsigned long long* __restrict__ out, unsigned long long* __restrict__ n,
-                                   unsigned long long* __restrict__ live_tokens) {
+// The stamps of the full slots, in any order (*n counts them), for the eviction cut; with slot_out (a snapshot) each
+// stamp's slot beside it; and the live token count.
+__global__ void text_stamps_kernel(const TextTable t, unsigned long long* __restrict__ out, uint32_t* __restrict__ slot_out,
+                                   unsigned long long* __restrict__ n, unsigned long long* __restrict__ live_tokens) {
     for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s <= t.mask; s += (uint64_t)gridDim.x * blockDim.x) {
         if (t.state[s] != kTextFull) continue;
-        if (out) out[atomicAdd(n, 1ull)] = t.stamp[s];
+        if (out) {
+            const unsigned long long i = atomicAdd(n, 1ull);
+            out[i] = t.stamp[s];
+            if (slot_out) slot_out[i] = (uint32_t)s;
+        }
         if (live_tokens) atomicAdd(live_tokens, (unsigned long long)t.len[s]);
     }
+}
+
+// ---- snapshot and restore: the image of kvidx_text_store_snapshot (include/kvidx.h) --------------------------------------
+// Snapshot: cnt[i + 1] = the token count of the i-th slot in recency order (slot[], sorted by stamp), to be scanned.
+__global__ void text_snap_len_kernel(const TextTable t, const uint32_t* __restrict__ slot, int64_t R, int64_t* __restrict__ cnt) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x)
+        cnt[i + 1] = t.len[slot[i]];
+}
+
+// ... then a warp per record writes it (u64 key, u32 n_tok, u32 0) to rec + 16 i and copies its tokens to tok + tok_off[i].
+__global__ void __launch_bounds__(kTextThreads) text_snapshot_kernel(const TextTable t, const uint32_t* __restrict__ arena,
+                                                                     const uint32_t* __restrict__ slot, const int64_t* __restrict__ tok_off,
+                                                                     int64_t R, uint4* __restrict__ rec, uint32_t* __restrict__ tok) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * blockDim.x / 32;
+    for (int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32; i < R; i += warps) {
+        const uint32_t s = slot[i];
+        const int64_t o = t.off[s], c = t.len[s], d = tok_off[i];
+        if (lane == 0) {
+            const uint64_t k = t.key[s];
+            rec[i] = make_uint4((uint32_t)k, (uint32_t)(k >> 32), (uint32_t)c, 0u);
+        }
+        for (int64_t j = lane; j < c; j += 32) tok[d + j] = arena[o + j];
+    }
+}
+
+// Restore, check one: every record's key to key[i] and its token count to cnt[i + 1] (to be scanned); non-zero padding
+// sets *bad.
+__global__ void text_restore_records_kernel(const uint4* __restrict__ rec, int64_t R, uint64_t* __restrict__ key, int64_t* __restrict__ cnt,
+                                            unsigned long long* __restrict__ bad) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint4 r = rec[i];
+        key[i] = (uint64_t)r.x | ((uint64_t)r.y << 32);
+        cnt[i + 1] = r.z;
+        if (r.w != 0) atomicOr(bad, 1ull);
+    }
+}
+
+// Restore, check two: a key equal to its neighbour in the sorted copy appears twice in the image.
+__global__ void text_restore_dups_kernel(const uint64_t* __restrict__ sorted, int64_t R, unsigned long long* __restrict__ bad) {
+    for (int64_t i = 1 + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < R; i += (int64_t)gridDim.x * blockDim.x)
+        if (sorted[i] == sorted[i - 1]) atomicOr(bad, 2ull);
 }
 
 // Rebuild: the full slots of `from` with stamp >= keep_from go into the empty table `to` (keys are distinct: no races on

@@ -2969,6 +2969,51 @@ int text_find_pass2(kvidx* x, TextStore* s, int64_t n, const FindScratch& f, con
     return 0;
 }
 
+// Steps two to four of an add, over keys already computed, then the cut down to cap_blocks keys: key k gets the
+// tokens tok[src[k] .. src[k] + pos[k + 1] - pos[k]), touched in order k at fresh stamps, the last touch of a key winning.
+// pos is scanned from pos0 (its first value, read back by the caller) and holds ntok = pos[nblk] - pos0 tokens in all.
+// slot_of (nblk) and inserted (one counter) are the caller's scratch.  kvidx_text_store_add and _restore both insert here.
+int text_insert(kvidx* x, TextStore* s, const uint64_t* key, int64_t nblk, const uint32_t* tok, const int64_t* src, const int64_t* pos,
+                int64_t pos0, int64_t ntok, uint32_t* slot_of, unsigned long long* inserted, cudaStream_t st) {
+    // room for every key of the call at load <= 1/2 before the cut
+    const uint64_t want = pow2ceil((uint64_t)std::max<int64_t>(2 * (s->resident + nblk), 1024));
+    if (want > s->t.mask + 1) { if (int rc = text_rebuild(x, s, want, 0, st)) return rc; }
+    if (int rc = text_arena_room(x, s, ntok, st)) return rc;
+    const int64_t arena_base = s->arena_used - pos0;
+    const unsigned long long base = s->clock + 1;
+    s->clock += (unsigned long long)nblk + 1;
+    CK(cudaMemsetAsync(inserted, 0, 8, st));
+    if (ntok > 0) text_add_copy_kernel<<<text_grid(x, nblk * 32), kTextThreads, 0, st>>>(tok, src, pos, nblk, arena_base, s->arena);
+    text_add_touch_kernel<<<text_grid(x, nblk), kTextThreads, 0, st>>>(s->t, key, nblk, base, slot_of, inserted);
+    text_add_commit_kernel<<<text_grid(x, nblk), kTextThreads, 0, st>>>(s->t, nblk, base, slot_of, pos, arena_base);
+    x->launches += 3;
+    CK(cudaGetLastError());
+    s->arena_used += ntok;
+    CK(cudaMemcpyAsync(s->h_misc.p, inserted, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    s->resident += (int64_t)*s->h_misc.as<unsigned long long>();
+    if (s->resident <= s->cap_blocks) return 0;
+    // the cut: keep the cap_blocks most recently touched keys (stamps are distinct: one sort finds the threshold)
+    const int64_t R = s->resident;
+    size_t tb = 0;
+    CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)R, 0, 64, st));
+    unsigned long long *st0, *st1;
+    TK(carve(s->d_scr, [&](Carver& c) { st0 = c.take<unsigned long long>(R); st1 = c.take<unsigned long long>(R); }), "eviction scratch");
+    TK(s->d_cub.need(tb), "eviction sort scratch");
+    CK(cudaMemsetAsync(inserted, 0, 8, st));
+    text_stamps_kernel<<<text_grid(x, (int64_t)s->t.mask + 1), kTextThreads, 0, st>>>(s->t, st0, nullptr, inserted, nullptr);
+    CK(cub::DeviceRadixSort::SortKeys(s->d_cub.p, tb, st0, st1, (int)R, 0, 64, st));
+    x->launches += 5;
+    const int64_t* tp = reinterpret_cast<const int64_t*>(st1 + (R - s->cap_blocks));
+    int64_t thr = 0;
+    if (int rc = text_read(s, &tp, 1, &thr, st)) return rc;
+    // the kept keys go into a table sized for them (load <= 1/2), not for this call: one large add does not leave a large table
+    const uint64_t keep_slots = pow2ceil((uint64_t)std::max<int64_t>(2 * s->cap_blocks, 1024));
+    if (int rc = text_rebuild(x, s, std::min<uint64_t>(keep_slots, s->t.mask + 1), (unsigned long long)thr, st)) return rc;
+    s->resident = s->cap_blocks;
+    return 0;
+}
+
 // AddTokenization for every prompt of the call, in array order; then the cut down to cap_blocks keys.
 int text_add(kvidx* x, TextStore* s, const TextIn& in, const uint32_t* tok, const uint64_t* span, const int64_t* tok_off, int64_t tok_base,
              cudaStream_t st) {
@@ -2976,9 +3021,6 @@ int text_add(kvidx* x, TextStore* s, const TextIn& in, const uint32_t* tok, cons
     int64_t nblk = 0;
     if (int rc = text_blocks(x, s, in.off, tok_off, n, &nblk, st)) return rc;
     if (nblk == 0) return 0;
-    // room for every key of the call at load <= 1/2 before the cut
-    const uint64_t want = pow2ceil((uint64_t)std::max<int64_t>(2 * (s->resident + nblk), 1024));
-    if (want > s->t.mask + 1) { if (int rc = text_rebuild(x, s, want, 0, st)) return rc; }
     uint64_t* key; int64_t *src, *pos; uint32_t* slot_of; unsigned long long* inserted;
     TK(carve(s->d_out, [&](Carver& c) {
         key = c.take<uint64_t>(nblk); src = c.take<int64_t>(nblk); pos = c.take<int64_t>(nblk + 1); slot_of = c.take<uint32_t>(nblk);
@@ -2996,39 +3038,118 @@ int text_add(kvidx* x, TextStore* s, const TextIn& in, const uint32_t* tok, cons
     int64_t ntok = 0;
     const int64_t* pp = pos + nblk;
     if (int rc = text_read(s, &pp, 1, &ntok, st)) return rc;
-    if (int rc = text_arena_room(x, s, ntok, st)) return rc;
-    const unsigned long long base = s->clock + 1;
-    s->clock += (unsigned long long)nblk + 1;
-    CK(cudaMemsetAsync(inserted, 0, 8, st));
-    if (ntok > 0) text_add_copy_kernel<<<text_grid(x, nblk * 32), kTextThreads, 0, st>>>(tok, src, pos, nblk, s->arena_used, s->arena);
-    text_add_touch_kernel<<<text_grid(x, nblk), kTextThreads, 0, st>>>(s->t, key, nblk, base, slot_of, inserted);
-    text_add_commit_kernel<<<text_grid(x, nblk), kTextThreads, 0, st>>>(s->t, nblk, base, slot_of, pos, s->arena_used);
+    return text_insert(x, s, key, nblk, tok, src, pos, 0, ntok, slot_of, inserted, st);
+}
+
+// The store's image (kvidx_text_store_snapshot, format in include/kvidx.h): the full slots sorted by stamp, least recent
+// first, each record's tokens behind the records in the same order.  Reads the store and refreshes nothing.
+int text_snapshot(kvidx* x, TextStore* s, void* buf, uint64_t cap, uint64_t* size_out, cudaStream_t st) {
+    const int64_t R = s->resident;
+    if (R >= (1ll << 31)) return fail(KVIDX_EINVAL, "prefix store: %lld keys in one snapshot", (long long)R);
+    size_t tb = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tb, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (uint32_t*)nullptr,
+                                       (uint32_t*)nullptr, (int)R, 0, 64, st));
+    unsigned long long *st0, *st1, *cnt; uint32_t *sl0, *sl1; int64_t* toff;
+    TK(carve(s->d_scr, [&](Carver& c) {
+        st0 = c.take<unsigned long long>(R); st1 = c.take<unsigned long long>(R); sl0 = c.take<uint32_t>(R); sl1 = c.take<uint32_t>(R);
+        toff = c.take<int64_t>(R + 1); cnt = c.take<unsigned long long>(2);
+    }), "snapshot scratch");
+    // 1. the full slots as (stamp, slot) pairs, and the live token count, which sizes the image
+    CK(cudaMemsetAsync(cnt, 0, 16, st));
+    text_stamps_kernel<<<text_grid(x, (int64_t)s->t.mask + 1), kTextThreads, 0, st>>>(s->t, st0, sl0, cnt, cnt + 1);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    int64_t got[2];
+    const int64_t* p[2] = {reinterpret_cast<const int64_t*>(cnt), reinterpret_cast<const int64_t*>(cnt + 1)};
+    if (int rc = text_read(s, p, 2, got, st)) return rc;
+    if (got[0] != R) return fail(KVIDX_ECUDA, "prefix store: %lld full slots, %lld keys resident", (long long)got[0], (long long)R);
+    const uint64_t T = (uint64_t)got[1], body = 16 * (uint64_t)R + 4 * T;
+    *size_out = 64 + body;
+    if (!buf || cap < 64 + body)
+        return fail(KVIDX_ENOSPC, "the prefix store image is %llu bytes, the buffer holds %llu", (unsigned long long)(64 + body),
+                    (unsigned long long)(buf ? cap : 0));
+    uint8_t* img = nullptr;
+    if (R > 0) {
+        TK(carve(s->d_out, [&](Carver& c) { img = c.take<uint8_t>(body); }), "snapshot image");
+        TK(s->d_cub.need(tb), "snapshot sort scratch");
+        // 2. recency order; 3. token offsets in that order; 4. the records and their tokens
+        CK(cub::DeviceRadixSort::SortPairs(s->d_cub.p, tb, st0, st1, sl0, sl1, (int)R, 0, 64, st));
+        CK(cudaMemsetAsync(toff, 0, 8, st));
+        text_snap_len_kernel<<<text_grid(x, R), kTextThreads, 0, st>>>(s->t, sl1, R, toff);
+        x->launches += 2;
+        CK(cudaGetLastError());
+        if (int rc = text_scan(x, s, toff, R, st)) return rc;
+        text_snapshot_kernel<<<text_grid(x, R * 32), kTextThreads, 0, st>>>(s->t, s->arena, sl1, toff, R, reinterpret_cast<uint4*>(img),
+                                                                          reinterpret_cast<uint32_t*>(img + 16 * R));
+        x->launches += 1;
+        CK(cudaGetLastError());
+    }
+    // 5. to the caller: the body through the stager, then the header
+    if (int rc = s->stage.d2h(static_cast<uint8_t*>(buf) + 64, img, body, st)) return rc;
+    uint8_t h[64] = {};
+    const uint32_t ver = 1, bb = s->B;
+    const uint64_t nr = (uint64_t)R;
+    memcpy(h, "KVIDXTXT", 8); memcpy(h + 8, &ver, 4); memcpy(h + 16, &bb, 4); memcpy(h + 24, &nr, 8); memcpy(h + 32, &T, 8);
+    memcpy(buf, h, 64);
+    return 0;
+}
+
+// The header of a prefix store image, checked against a store of block_bytes B -> its record and token counts.
+int text_image_head(const void* buf, uint64_t len, uint32_t B, uint64_t* R, uint64_t* T) {
+    if (!buf || len < 64) return fail(KVIDX_EINVAL, "prefix store image: %llu bytes, shorter than its header", (unsigned long long)len);
+    const uint8_t* p = static_cast<const uint8_t*>(buf);
+    uint32_t ver, flags, bb, z;
+    memcpy(&ver, p + 8, 4); memcpy(&flags, p + 12, 4); memcpy(&bb, p + 16, 4); memcpy(&z, p + 20, 4); memcpy(R, p + 24, 8); memcpy(T, p + 32, 8);
+    if (memcmp(p, "KVIDXTXT", 8)) return fail(KVIDX_EINVAL, "prefix store image: bad magic");
+    if (ver != 1 || flags != 0) return fail(KVIDX_EINVAL, "prefix store image: version %u flags %u (1 and 0 expected)", ver, flags);
+    bool zero = z == 0;
+    for (int i = 40; i < 64; ++i) zero = zero && p[i] == 0;
+    if (!zero) return fail(KVIDX_EINVAL, "prefix store image: non-zero reserved header bytes");
+    if (bb != B) return fail(KVIDX_EINVAL, "prefix store image: block_bytes %u, the store's is %u", bb, B);
+    const uint64_t room = len - 64;
+    if (*R > room / 16 || *T > room / 4 || 16 * *R + 4 * *T != room)
+        return fail(KVIDX_EINVAL, "prefix store image: %llu bytes do not hold %llu records and %llu tokens", (unsigned long long)len,
+                    (unsigned long long)*R, (unsigned long long)*T);
+    return 0;
+}
+
+// Load the R records and T tokens of a checked image (img: the host bytes) into the empty store: check every record on
+// the device, then insert the newest cap_blocks of them in record order through text_insert.
+int text_restore(kvidx* x, TextStore* s, const uint8_t* img, uint64_t R64, uint64_t T, cudaStream_t st) {
+    if (R64 == 0) return T ? fail(KVIDX_EINVAL, "prefix store image: no record holds its %llu tokens", (unsigned long long)T) : 0;
+    if (R64 >= (1ull << 31)) return fail(KVIDX_EINVAL, "prefix store image: %llu records in one restore", (unsigned long long)R64);
+    const int64_t R = (int64_t)R64;
+    const uint64_t body = 16 * R64 + 4 * T;
+    uint8_t* d_body; uint64_t *key, *sorted; int64_t* off; uint32_t* slot_of; unsigned long long* flags;
+    TK(carve(s->d_in, [&](Carver& c) { d_body = c.take<uint8_t>(body); sorted = c.take<uint64_t>(R); }), "restore input");
+    TK(carve(s->d_out, [&](Carver& c) {
+        key = c.take<uint64_t>(R); off = c.take<int64_t>(R + 1); slot_of = c.take<uint32_t>(R); flags = c.take<unsigned long long>(2);
+    }), "restore scratch");
+    if (int rc = s->stage.h2d(d_body, img + 64, body, st)) return rc;
+    // the records' keys and token counts, padding (flag 1) and duplicate keys (flag 2), the token offsets and their total
+    CK(cudaMemsetAsync(off, 0, 8, st));
+    CK(cudaMemsetAsync(flags, 0, 16, st));
+    text_restore_records_kernel<<<text_grid(x, R), kTextThreads, 0, st>>>(reinterpret_cast<const uint4*>(d_body), R, key, off, flags);
+    size_t tb = 0;
+    unsigned long long* k0 = reinterpret_cast<unsigned long long*>(key);
+    unsigned long long* k1 = reinterpret_cast<unsigned long long*>(sorted);
+    CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, k0, k1, (int)R, 0, 64, st));
+    TK(s->d_cub.need(tb), "restore sort scratch");
+    CK(cub::DeviceRadixSort::SortKeys(s->d_cub.p, tb, k0, k1, (int)R, 0, 64, st));
+    text_restore_dups_kernel<<<text_grid(x, R), kTextThreads, 0, st>>>(sorted, R, flags);
     x->launches += 3;
     CK(cudaGetLastError());
-    s->arena_used += ntok;
-    CK(cudaMemcpyAsync(s->h_misc.p, inserted, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    s->resident += (int64_t)*s->h_misc.as<unsigned long long>();
-    if (s->resident <= s->cap_blocks) return 0;
-    // the cut: keep the cap_blocks most recently touched keys (stamps are distinct: one sort finds the threshold)
-    const int64_t R = s->resident;
-    size_t tb = 0;
-    CK(cub::DeviceRadixSort::SortKeys(nullptr, tb, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)R, 0, 64, st));
-    unsigned long long *st0, *st1;
-    TK(carve(s->d_scr, [&](Carver& c) { st0 = c.take<unsigned long long>(R); st1 = c.take<unsigned long long>(R); }), "eviction scratch");
-    TK(s->d_cub.need(tb), "eviction sort scratch");
-    CK(cudaMemsetAsync(inserted, 0, 8, st));
-    text_stamps_kernel<<<text_grid(x, (int64_t)s->t.mask + 1), kTextThreads, 0, st>>>(s->t, st0, inserted, nullptr);
-    CK(cub::DeviceRadixSort::SortKeys(s->d_cub.p, tb, st0, st1, (int)R, 0, 64, st));
-    x->launches += 5;
-    const int64_t* tp = reinterpret_cast<const int64_t*>(st1 + (R - s->cap_blocks));
-    int64_t thr = 0;
-    if (int rc = text_read(s, &tp, 1, &thr, st)) return rc;
-    // the kept keys go into a table sized for them (load <= 1/2), not for this call: one large add does not leave a large table
-    const uint64_t keep_slots = pow2ceil((uint64_t)std::max<int64_t>(2 * s->cap_blocks, 1024));
-    if (int rc = text_rebuild(x, s, std::min<uint64_t>(keep_slots, s->t.mask + 1), (unsigned long long)thr, st)) return rc;
-    s->resident = s->cap_blocks;
-    return 0;
+    if (int rc = text_scan(x, s, off, R, st)) return rc;
+    const int64_t first = std::max<int64_t>(R - s->cap_blocks, 0);         // a larger image keeps its newest cap_blocks records
+    int64_t got[3];
+    const int64_t* p[3] = {off + R, off + first, reinterpret_cast<const int64_t*>(flags)};
+    if (int rc = text_read(s, p, 3, got, st)) return rc;
+    if (got[2] & 1) return fail(KVIDX_EINVAL, "prefix store image: non-zero record padding");
+    if (got[2] & 2) return fail(KVIDX_EINVAL, "prefix store image: a key appears twice");
+    if ((uint64_t)got[0] != T) return fail(KVIDX_EINVAL, "prefix store image: records hold %lld tokens, the header says %llu", (long long)got[0],
+                                           (unsigned long long)T);
+    return text_insert(x, s, key + first, R - first, reinterpret_cast<const uint32_t*>(d_body + 16 * R), off + first, off + first, got[1],
+                       got[0] - got[1], slot_of, flags + 1, st);
 }
 
 int text_check(kvidx* x, int64_t n, const void* text, const int64_t* text_off) {
@@ -3159,6 +3280,29 @@ int kvidx_text_store_len(kvidx_t* x, int64_t* blocks_out) {
     if (!x->text) return fail(KVIDX_EINVAL, "prefix store not initialised (kvidx_text_store_init)");
     *blocks_out = x->text->resident;
     return 0;
+}
+
+int kvidx_text_store_snapshot(kvidx_t* x, void* buf, uint64_t cap, uint64_t* size_out) {
+    if (!x || !size_out) return fail(KVIDX_EINVAL, "bad arguments");
+    TextCall c(x, nullptr);
+    if (!c.s) return fail(KVIDX_EINVAL, "prefix store not initialised (kvidx_text_store_init)");
+    c.st = c.s->stream;
+    if (int rc = c.begin(x)) return rc;              // after the last store call, a Score() from text on the handle's stream too
+    return c.end(text_snapshot(x, c.s, buf, cap, size_out, c.st));
+}
+
+int kvidx_text_store_restore(kvidx_t* x, const void* buf, uint64_t len, int64_t* blocks_out) {
+    if (!x) return fail(KVIDX_EINVAL, "NULL handle");
+    TextCall c(x, nullptr);
+    if (!c.s) return fail(KVIDX_EINVAL, "prefix store not initialised (kvidx_text_store_init)");
+    c.st = c.s->stream;
+    uint64_t R = 0, T = 0;
+    if (int rc = text_image_head(buf, len, c.s->B, &R, &T)) return rc;
+    if (c.s->resident != 0) return fail(KVIDX_EINVAL, "prefix store restore needs an empty store (%lld keys resident)", (long long)c.s->resident);
+    if (int rc = c.begin(x)) return rc;
+    int rc = text_restore(x, c.s, static_cast<const uint8_t*>(buf), R, T, c.st);
+    if (!rc && blocks_out) *blocks_out = c.s->resident;
+    return c.end(rc);
 }
 
 int kvidx_text_store_add(kvidx_t* x, const uint8_t* text, const int64_t* text_off, int64_t n, const uint32_t* tok, const uint64_t* tok_span,

@@ -1122,4 +1122,73 @@ int64_t kvhost_prefix_store_find(kvhost_prefix_store_t* s, const char* prompt, s
     return n;
 }
 
+int kvhost_prefix_store_snapshot(kvhost_prefix_store_t* s, void* buf, uint64_t cap, uint64_t* size_out) {
+    if (!s || !size_out) return hfail(KVIDX_EINVAL, "bad arguments");
+    std::lock_guard<std::mutex> g(s->mu);
+    const uint64_t R = s->order.size();
+    uint64_t T = 0;
+    for (const auto& e : s->order) T += e.second.size();
+    *size_out = 64 + 16 * R + 4 * T;
+    if (!buf || cap < *size_out) return hfail(KVIDX_ENOSPC, "the prefix store image does not fit the buffer");
+    uint8_t* p = static_cast<uint8_t*>(buf);
+    memset(p, 0, 64);
+    const uint32_t ver = 1, bb = (uint32_t)s->block_size;
+    memcpy(p, "KVIDXTXT", 8); memcpy(p + 8, &ver, 4); memcpy(p + 16, &bb, 4); memcpy(p + 24, &R, 8); memcpy(p + 32, &T, 8);
+    uint8_t* rec = p + 64;
+    uint8_t* tok = rec + 16 * R;
+    for (auto it = s->order.rbegin(); it != s->order.rend(); ++it) {        // least recent first
+        const uint32_t nt = (uint32_t)it->second.size(), zero = 0;
+        memcpy(rec, &it->first, 8); memcpy(rec + 8, &nt, 4); memcpy(rec + 12, &zero, 4);
+        rec += 16;
+        if (nt) memcpy(tok, it->second.data(), (size_t)nt * 4);
+        tok += (size_t)nt * 4;
+    }
+    return 0;
+}
+
+int kvhost_prefix_store_restore(kvhost_prefix_store_t* s, const void* buf, uint64_t len) {
+    if (!s || (!buf && len)) return hfail(KVIDX_EINVAL, "bad arguments");
+    std::lock_guard<std::mutex> g(s->mu);
+    if (!s->map.empty()) return hfail(KVIDX_EINVAL, "prefix store restore needs an empty store");
+    if (len < 64) return hfail(KVIDX_EINVAL, "prefix store image: shorter than its header");
+    const uint8_t* p = static_cast<const uint8_t*>(buf);
+    uint32_t ver, flags, bb, z; uint64_t R, T;
+    memcpy(&ver, p + 8, 4); memcpy(&flags, p + 12, 4); memcpy(&bb, p + 16, 4); memcpy(&z, p + 20, 4); memcpy(&R, p + 24, 8); memcpy(&T, p + 32, 8);
+    if (memcmp(p, "KVIDXTXT", 8)) return hfail(KVIDX_EINVAL, "prefix store image: bad magic");
+    if (ver != 1 || flags != 0) return hfail(KVIDX_EINVAL, "prefix store image: bad version or flags");
+    bool zero = z == 0;
+    for (int i = 40; i < 64; ++i) zero = zero && p[i] == 0;
+    if (!zero) return hfail(KVIDX_EINVAL, "prefix store image: non-zero reserved header bytes");
+    if (bb != (uint32_t)s->block_size) return hfail(KVIDX_EINVAL, "prefix store image: block_bytes differs from the store's");
+    const uint64_t room = len - 64;
+    if (R > room / 16 || T > room / 4 || 16 * R + 4 * T != room) return hfail(KVIDX_EINVAL, "prefix store image: length does not match the header");
+    // every record checked before any is inserted
+    const uint8_t* rec = p + 64;
+    std::unordered_set<uint64_t> seen;
+    uint64_t sum = 0;
+    for (uint64_t i = 0; i < R; ++i) {
+        uint64_t k; uint32_t nt, pad;
+        memcpy(&k, rec + 16 * i, 8); memcpy(&nt, rec + 16 * i + 8, 4); memcpy(&pad, rec + 16 * i + 12, 4);
+        if (pad) return hfail(KVIDX_EINVAL, "prefix store image: non-zero record padding");
+        if (!seen.insert(k).second) return hfail(KVIDX_EINVAL, "prefix store image: a key appears twice");
+        sum += nt;
+    }
+    if (sum != T) return hfail(KVIDX_EINVAL, "prefix store image: the records' token counts do not add up to the header's");
+    // the replay of the records as adds, oldest first, leaves the newest cache_size of them
+    const uint8_t* tok = rec + 16 * R;
+    const uint64_t first = R > (uint64_t)s->cache_size ? R - (uint64_t)s->cache_size : 0;
+    for (uint64_t i = 0; i < R; ++i) {
+        uint64_t k; uint32_t nt;
+        memcpy(&k, rec + 16 * i, 8); memcpy(&nt, rec + 16 * i + 8, 4);
+        if (i >= first) {
+            std::vector<uint32_t> blk(nt);
+            if (nt) memcpy(blk.data(), tok, (size_t)nt * 4);
+            s->order.emplace_front(k, std::move(blk));
+            s->map[k] = s->order.begin();
+        }
+        tok += (size_t)nt * 4;
+    }
+    return 0;
+}
+
 }  // extern "C"

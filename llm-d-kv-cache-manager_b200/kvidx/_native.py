@@ -110,6 +110,8 @@ SYMBOLS = {
     "kvidx_text_store_add": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, _u64p, _i64p]),
     "kvidx_text_store_find": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, C.c_int64, _i64p, _f64p]),
     "kvidx_text_store_len": (C.c_int, [C.c_void_p, _i64p]),
+    "kvidx_text_store_snapshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "kvidx_text_store_restore": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, _i64p]),
     "kvidx_text_hash_keys": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, C.c_int32, _u64p, _i64p]),
     "kvidx_score_text": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, C.c_double, _f64p, _u8p, _u8p, _f64p]),
     "kvidx_score_text_sparse": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, C.c_uint32, _u64p, C.c_double, _u16p, _f64p, _u8p, _u8p,
@@ -538,6 +540,24 @@ class Index:
     def text_store_len(self) -> int:
         out = C.c_int64(0)
         self._ck(self.L.kvidx_text_store_len(self.h, C.byref(out)))
+        return out.value
+
+    def text_store_snapshot(self) -> bytes:
+        """kvidx_text_store_snapshot: the store's image (format v1 in include/kvidx.h), least recent block first."""
+        size = C.c_uint64(0)
+        rc = self.L.kvidx_text_store_snapshot(self.h, None, 0, C.byref(size))
+        while rc == ENOSPC:                   # sized by a first call; a store call in between can grow it: size again
+            cap = size.value
+            buf = bytearray(cap)
+            rc = self.L.kvidx_text_store_snapshot(self.h, (C.c_char * cap).from_buffer(buf), cap, C.byref(size))
+        self._ck(rc)
+        return bytes(memoryview(buf)[:size.value])
+
+    def text_store_restore(self, image) -> int:
+        """kvidx_text_store_restore: load an image into this handle's empty store.  -> blocks resident afterwards."""
+        image = image if isinstance(image, bytes) else bytes(image)
+        out = C.c_int64(0)
+        self._ck(self.L.kvidx_text_store_restore(self.h, image, len(image), C.byref(out)))
         return out.value
 
     def text_hash_keys(self, text, text_off, block_bytes):

@@ -46,6 +46,8 @@ SYMBOLS = {
     "kvhost_prefix_store_add": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]),
     "kvhost_prefix_store_find": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_double)]),
     "kvhost_prefix_store_len": (C.c_int64, [C.c_void_p]),
+    "kvhost_prefix_store_snapshot": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, _u64p]),
+    "kvhost_prefix_store_restore": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64]),
     "kvhost_xxhash64": (C.c_uint64, [C.c_char_p, C.c_size_t, C.c_uint64]),
     "kvhost_get_metrics": (C.c_int, [C.c_void_p, C.POINTER(HostMetrics)]),
     "kvhost_metrics_text": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_size_t]),
@@ -366,3 +368,22 @@ class PrefixStore:
         out = np.zeros(max(int(n), 1), np.uint32)
         n = self.L.kvhost_prefix_store_find(self.h, prompt, len(prompt), out.ctypes.data_as(C.c_void_p), len(out), C.byref(ratio))
         return out[: int(n)].tolist(), ratio.value
+
+    def snapshot(self) -> bytes:
+        """kvhost_prefix_store_snapshot: the store's image (format v1 of kvidx_text_store_snapshot), least recent first."""
+        size = C.c_uint64(0)
+        rc = self.L.kvhost_prefix_store_snapshot(self.h, None, 0, C.byref(size))
+        while rc == _native.ENOSPC:
+            cap = size.value
+            buf = bytearray(cap)
+            rc = self.L.kvhost_prefix_store_snapshot(self.h, (C.c_char * cap).from_buffer(buf), cap, C.byref(size))
+        if rc:
+            raise _native.KvidxError(rc, self.L.kvhost_last_error().decode())
+        return bytes(memoryview(buf)[:size.value])
+
+    def restore(self, image):
+        """kvhost_prefix_store_restore: load an image into this empty store (it keeps its own cache_size)."""
+        image = image if isinstance(image, bytes) else bytes(image)
+        rc = self.L.kvhost_prefix_store_restore(self.h, image, len(image))
+        if rc:
+            raise _native.KvidxError(rc, self.L.kvhost_last_error().decode())

@@ -130,6 +130,15 @@ class Indexer:
                 self._dev = ix
             return self._dev
 
+    def text_store_snapshot(self) -> bytes:
+        """The device prefix store's image (kvidx_text_store_snapshot): save it with the index's to warm-start both."""
+        return self._device_store().text_store_snapshot()
+
+    def text_store_restore(self, image) -> int:
+        """Load a text_store_snapshot image into the device prefix store (created with text_cache_blocks /
+        text_block_bytes if this indexer has not used it yet; it must hold no block).  -> blocks resident."""
+        return self._device_store().text_store_restore(image)
+
     def get_pod_scores_batch(self, prompts: Sequence[str], model_name: str,
                              pod_identifiers: Sequence[str] = ()) -> List[Optional[Dict[str, float]]]:
         """GetPodScores for every prompt of a batch, on the device prefix store.  -> per prompt a dict pod -> score, or None
