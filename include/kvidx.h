@@ -363,6 +363,59 @@ int kvidx_apply_events(kvidx_t* idx, const kvidx_event_t* ev, int64_t n_events,
                        const uint64_t* hashes, int64_t n_hashes,
                        const uint32_t* tokens, int64_t n_tokens, int64_t* n_dropped_out);
 
+/* ---- KVEvents wire payloads decoded on the device (no reference counterpart) ------------------------------------------
+ * Pool.processEvent's msgpack decoding (kvevents/pool.go:177-244, events.go:38-96) of a drained batch of raw vLLM KVEvents
+ * messages, run on the GPU: the payloads go in as they came off the wire and come out as the kvidx_event_t batch the write
+ * path takes.  The rules are the host mirror's decoder (kvhost_decode_event_batch), and the records are byte-equal to its
+ * records stably sorted by pod: EventBatch = [ts, events[], dp_rank?, extra...] (an envelope error drops the message);
+ * unknown tags skipped; hashes = uint64- / int64-coded integers and non-empty bins (the last 8 bytes of a longer bin,
+ * big-endian); a parent of another type skips the event; tokens truncated to u32; Medium lower-cased (ASCII), none or nil
+ * = "gpu"; nesting deeper than 64 drops the message.
+ *   bytes / msg_off: CSR of the payloads, message i is bytes[msg_off[i] .. msg_off[i+1]) (msg_off[0] may be non-zero);
+ *   msg_pod[i] / msg_model[i]: the interned pod (< max_pods) and model (<= 65535) of message i (one pod per message);
+ *   tier table: name t is tier_bytes[tier_off[t] .. tier_off[t+1]), lower-case, compared by length and bytes (no length
+ *     cap); 1 <= n_tiers <= 16; gpu_tier: the id of a Medium-less event, or -1 when "gpu" has no id yet;
+ *   flags: KVIDX_PAYLOAD_SKIP_UNKNOWN_TIER -- an event whose Medium is not in the table is skipped (what the host decoder
+ *     does once the 16 tier ids are taken).  Without it such a batch applies nothing and the call returns KVIDX_ENOENT
+ *     with the offending messages flagged: the caller interns their names (kvhost_decode_event_batch over them, in
+ *     order) and calls again.  KVIDX_PAYLOAD_STOP_AT_CLEARED -- a batch holding an AllBlocksCleared event applies nothing
+ *     and returns KVIDX_ENOENT with its messages flagged; without it the marker decodes to nothing (pool.go:332-333);
+ *   msg_flags_out (may be NULL): n_msgs bytes, KVIDX_PAYLOAD_MSG_* per message; written whenever the decode ran;
+ *   counts_out (may be NULL): {messages decoded, events, hashes, tokens, queues (pods with events), admitted blocks
+ *     (sum of n_tokens / block_size over BlockStored events with hashes: kvcache_index_admissions_total), removed hashes
+ *     (kvcache_index_evictions_total), AllBlocksCleared markers}; written whenever the decode ran.
+ * Errors: n_msgs < 0, NULL or non-monotone offsets, a NULL array with a non-zero count, an empty tier table, gpu_tier >=
+ * n_tiers, unknown flags -> KVIDX_EINVAL; a pod id >= max_pods or a model id > 65535 -> KVIDX_ERANGE; n_msgs == 0 -> 0.
+ *
+ * kvidx_decode_event_payloads_dev: decode only, device buffers in and out, in exactly the form kvidx_apply_events_dev
+ *   takes: events stably sorted by pod (queue q owns d_ev_out[d_queue_off_out[q] .. d_queue_off_out[q+1])), hashes and
+ *   tokens in message order.  Capacities are element counts (queue_cap counts offsets: queues + 1); an output below its
+ *   total -> KVIDX_ENOSPC with counts_out filled and no output written.  The tier table and counts_out are host memory.
+ *   The inputs must be complete when the call is made.  It runs on the handle's write stream, reads its totals back once
+ *   (its only wait), and is asynchronous after that: a later kvidx_apply_events_dev and every later read call on the
+ *   handle are ordered after it, kvidx_synchronize waits for it.
+ * kvidx_apply_event_payloads: host buffers (pinned ones copied in place, pageable ones through pinned chunks): decode and
+ *   apply in one synchronous write call, as kvidx_apply_events applies the decoded batch (*n_dropped_out the same).  It
+ *   makes room for the decoded batch's BlockStored hashes and holds the write side for the whole call.  A device-resident
+ *   caller composes kvidx_decode_event_payloads_dev and kvidx_apply_events_dev.
+ * Both work on default, CLOCK, exact-LRU and sharded handles; the ingest rule is kvidx_apply_events': one rank per pod. */
+#define KVIDX_PAYLOAD_SKIP_UNKNOWN_TIER 1u
+#define KVIDX_PAYLOAD_STOP_AT_CLEARED   2u
+#define KVIDX_PAYLOAD_MSG_DECODED       1u   /* the envelope decoded (else the whole message was dropped)        */
+#define KVIDX_PAYLOAD_MSG_UNKNOWN_TIER  2u   /* an event names a Medium the tier table lacks                      */
+#define KVIDX_PAYLOAD_MSG_CLEARED       4u   /* an AllBlocksCleared event                                          */
+#define KVIDX_PAYLOAD_COUNTS            8
+int kvidx_decode_event_payloads_dev(kvidx_t* idx, const uint8_t* d_bytes, const int64_t* d_msg_off, int64_t n_msgs,
+                                    const uint32_t* d_msg_pod, const uint32_t* d_msg_model, const uint8_t* tier_bytes,
+                                    const int64_t* tier_off, uint32_t n_tiers, int32_t gpu_tier, uint32_t flags,
+                                    kvidx_event_t* d_ev_out, int64_t ev_cap, int64_t* d_queue_off_out, int64_t queue_cap,
+                                    uint64_t* d_hashes_out, int64_t hash_cap, uint32_t* d_tokens_out, int64_t tok_cap,
+                                    uint8_t* d_msg_flags_out, int64_t counts_out[KVIDX_PAYLOAD_COUNTS]);
+int kvidx_apply_event_payloads(kvidx_t* idx, const uint8_t* bytes, const int64_t* msg_off, int64_t n_msgs, const uint32_t* msg_pod,
+                               const uint32_t* msg_model, const uint8_t* tier_bytes, const int64_t* tier_off, uint32_t n_tiers,
+                               int32_t gpu_tier, uint32_t flags, uint8_t* msg_flags_out, int64_t counts_out[KVIDX_PAYLOAD_COUNTS],
+                               int64_t* n_dropped_out);
+
 /* Drop every entry whose pod is in pod_mask (ceil(max_pods/64) words) and whose tier bit is set in tier_mask
  * (bit t = tier t; 0xFFFF = all tiers); request keys left without entries are removed together with the engine
  * mappings that point at them.  No reference counterpart: it removes the blocks of a pod that has gone away without

@@ -97,7 +97,10 @@ int kvhost_index_lookup(kvhost_t* h, const char* model, const uint64_t* keys, si
  * kvidx_apply_events call.  Returns the number of events applied (or a negative code).
  * With clear_on_all_blocks_cleared, the drained batch is cut at the AllBlocksCleared markers: segment k holds each pod's
  * events between its (k-1)-th and k-th marker and is one kvidx_apply_events call, followed by one kvidx_remove_pods for
- * the pods that cleared at that boundary.  Per-pod order is kept; the order between pods stays unspecified. */
+ * the pods that cleared at that boundary.  Per-pod order is kept; the order between pods stays unspecified.
+ * A drain of 1 MiB of payloads or more is decoded on the GPU instead (kvidx_apply_event_payloads, one call), with the same
+ * records, tier ids, metrics and result; a Medium new to the mirror is interned on the host first, in drain order, and a
+ * drain holding an AllBlocksCleared marker under clear_on_all_blocks_cleared takes the host path. */
 int kvhost_pool_add_task(kvhost_t* h, const char* pod, const char* model, const void* payload, size_t len);
 int kvhost_pool_queue_index(kvhost_t* h, const char* pod);
 int64_t kvhost_pool_process(kvhost_t* h, int64_t* n_dropped_out);

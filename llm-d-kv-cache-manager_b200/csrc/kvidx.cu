@@ -33,6 +33,7 @@
 #include "kernels_route.cuh"
 #include "kernels_text.cuh"
 #include "kernels_hits.cuh"
+#include "kernels_decode.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -227,6 +228,7 @@ struct kvidx {
     // write-side scratch (guarded by mu_w)
     DevBuf d_misc, d_ev, d_hash, d_evtok, d_qoff, d_wkeys, d_wpred, d_wready, d_wmap;
     DevBuf d_sweep;                 // CLOCK sweep scratch: bitmap image, per-tile counts, control block
+    DevBuf d_dec, d_decin;          // KVEvents payload decode: its scratch, and the staged payloads of a host-buffer call
     PinBuf h_misc;
     // snapshot / restore (guarded by mu_w): the stager between the device and a caller's buffer, which may be pageable;
     // the device scratch (records, sort buffers) is released when the call returns
@@ -1497,7 +1499,7 @@ void kvidx_destroy(kvidx_t* x) {
     x->d_rounds.release();
     x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_inv.release(); x->h_inv.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
     x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
-    x->d_snap.release(); x->snap.release(); x->rstage.release();
+    x->d_snap.release(); x->snap.release(); x->rstage.release(); x->d_dec.release(); x->d_decin.release();
     if (x->tv.req) cudaFree(x->tv.req);
     if (x->tv.eng) cudaFree(x->tv.eng);
     if (x->tv.req_stamp) cudaFree(x->tv.req_stamp);
@@ -2138,6 +2140,201 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
     const unsigned long long dropped_before = x->h_cnt->dropped_events, nospc_before = x->h_cnt->nospc;
     rc = launch_apply_events(x, x->d_ev.as<kvidx_event_t>(), x->d_qoff.as<int64_t>(), nq, n, x->d_hash.as<uint64_t>(), n_hashes,
                              x->d_evtok.as<uint32_t>(), st, max_ev_hashes);
+    if (rc) return rc;
+    rc = refresh_counters(x);
+    if (rc) return rc;
+    if (n_dropped_out) *n_dropped_out = (int64_t)(x->h_cnt->dropped_events - dropped_before);
+    if (x->h_cnt->nospc != nospc_before) return fail(KVIDX_ENOSPC, "%llu inserts refused: the owning shard is full", x->h_cnt->nospc - nospc_before);
+    return cap_keys(x);
+}
+
+}  // extern "C"
+
+namespace {
+// ---- KVEvents payloads decoded on the device (kernels_decode.cuh) ---------------------------------------------------------
+// A decode in two halves around the one read-back of its totals: decode_count runs the count pass, sorts the messages by pod
+// and scans the counts into positions; decode_write runs the write pass into outputs sized from the totals.  Both on the
+// write stream, under mu_w (the scratch, x->d_dec, is write-side).
+struct DecodePlan {
+    DecIn in{};
+    int64_t *ev_cnt, *hash_cnt, *tok_cnt, *ev_base, *hash_base, *tok_base, *qoff;
+    uint8_t* flags; uint32_t* sorted_val;
+    DecTotals* d_tot; DecTotals tot{};
+};
+
+int check_tier_table(const uint8_t* tier_bytes, const int64_t* tier_off, uint32_t n_tiers, int32_t gpu_tier) {
+    if (n_tiers == 0 || n_tiers > KVIDX_MAX_TIERS || !tier_off) return fail(KVIDX_EINVAL, "the tier table holds 1 to %u names", KVIDX_MAX_TIERS);
+    for (uint32_t t = 0; t < n_tiers; ++t) if (tier_off[t + 1] < tier_off[t]) return fail(KVIDX_EINVAL, "tier offsets not monotone");
+    if (tier_off[n_tiers] > tier_off[0] && !tier_bytes) return fail(KVIDX_EINVAL, "NULL tier names");
+    if (gpu_tier >= (int32_t)n_tiers) return fail(KVIDX_EINVAL, "gpu_tier %d is not in the table", gpu_tier);
+    return 0;
+}
+
+int check_payload_flags(uint32_t flags) {
+    if (flags & ~(KVIDX_PAYLOAD_SKIP_UNKNOWN_TIER | KVIDX_PAYLOAD_STOP_AT_CLEARED)) return fail(KVIDX_EINVAL, "unknown flags 0x%x", flags);
+    return 0;
+}
+
+int decode_count(kvidx* x, DecodePlan& pl, const uint8_t* tier_bytes, const int64_t* tier_off, uint32_t n_tiers, int32_t gpu_tier,
+                 cudaStream_t st) {
+    const int64_t n = pl.in.n_msgs;
+    const uint32_t P = x->tv.max_pods;
+    const uint64_t tb = (uint64_t)(tier_off[n_tiers] - tier_off[0]);
+    size_t sort_bytes = 0, scan_bytes = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
+                                       (uint32_t*)nullptr, (int)n, 0, KVIDX_POD_BITS, st));
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (int64_t*)nullptr, (int64_t*)nullptr, (int)n, st));
+    uint8_t* d_tier; unsigned long long* pod_ev; uint32_t *key, *key2, *val; void* tmp;
+    CK(carve(x->d_dec, [&](Carver& c) {
+        d_tier = c.take<uint8_t>(tb); pod_ev = c.take<unsigned long long>(P); pl.d_tot = c.take<DecTotals>(1); pl.qoff = c.take<int64_t>(P + 1);
+        pl.ev_cnt = c.take<int64_t>(n); pl.hash_cnt = c.take<int64_t>(n); pl.tok_cnt = c.take<int64_t>(n);
+        pl.ev_base = c.take<int64_t>(n); pl.hash_base = c.take<int64_t>(n); pl.tok_base = c.take<int64_t>(n);
+        pl.flags = c.take<uint8_t>(n); key = c.take<uint32_t>(n); key2 = c.take<uint32_t>(n); val = c.take<uint32_t>(n);
+        pl.sorted_val = c.take<uint32_t>(n); tmp = c.take<uint8_t>(std::max(sort_bytes, scan_bytes));
+    }));
+    TierTable& tt = pl.in.tt;
+    tt.bytes = d_tier; tt.n = n_tiers; tt.gpu = gpu_tier;
+    for (uint32_t t = 0; t <= n_tiers; ++t) tt.off[t] = (uint64_t)(tier_off[t] - tier_off[0]);
+    if (int rc = x->snap.h2d(d_tier, tier_bytes + tier_off[0], tb, st)) return rc;
+    CK(cudaMemsetAsync(pod_ev, 0, (size_t)P * 8, st));
+    CK(cudaMemsetAsync(pl.d_tot, 0, sizeof(DecTotals), st));
+    const unsigned g = (unsigned)((n + kDecThreads - 1) / kDecThreads);
+    decode_count_kernel<<<g, kDecThreads, 0, st>>>(pl.in, pl.ev_cnt, pl.hash_cnt, pl.tok_cnt, pl.flags, key, val, pod_ev, pl.d_tot);
+    decode_queues_kernel<<<1, kQueueThreads, 0, st>>>(pod_ev, P, pl.qoff, &pl.d_tot->queues);
+    size_t b = sort_bytes;
+    CK(cub::DeviceRadixSort::SortPairs(tmp, b, key, key2, val, pl.sorted_val, (int)n, 0, KVIDX_POD_BITS, st));
+    decode_gather_kernel<<<g, kDecThreads, 0, st>>>(pl.sorted_val, pl.ev_cnt, n, pl.ev_base);
+    b = scan_bytes;
+    CK(cub::DeviceScan::ExclusiveSum(tmp, b, pl.ev_base, pl.ev_base, (int)n, st));    // events: pod order
+    b = scan_bytes;
+    CK(cub::DeviceScan::ExclusiveSum(tmp, b, pl.hash_cnt, pl.hash_base, (int)n, st)); // hashes and tokens: message order
+    b = scan_bytes;
+    CK(cub::DeviceScan::ExclusiveSum(tmp, b, pl.tok_cnt, pl.tok_base, (int)n, st));
+    x->launches += 3;
+    CK(cudaGetLastError());
+    CK(x->h_misc.need(sizeof(DecTotals)));
+    CK(cudaMemcpyAsync(x->h_misc.p, pl.d_tot, sizeof(DecTotals), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    pl.tot = *x->h_misc.as<DecTotals>();
+    return 0;
+}
+
+// counts_out of the ABI, and whether the batch can be applied as it is
+int decode_verdict(kvidx* x, const DecTotals& t, uint32_t flags, int64_t* counts_out) {
+    if (counts_out) {
+        const unsigned long long c[KVIDX_PAYLOAD_COUNTS] = {t.messages, t.events, t.hashes, t.tokens, t.queues, t.admitted, t.removed_hashes, t.markers};
+        for (int i = 0; i < KVIDX_PAYLOAD_COUNTS; ++i) counts_out[i] = (int64_t)c[i];
+    }
+    if (t.bad_off) return fail(KVIDX_EINVAL, "message offsets not monotone");
+    if (t.bad_pod) return fail(KVIDX_ERANGE, "a message's pod id is >= max_pods %u", x->tv.max_pods);
+    if (t.bad_model) return fail(KVIDX_ERANGE, "a message's model id is > 65535");
+    if (t.unknown_tier && !(flags & KVIDX_PAYLOAD_SKIP_UNKNOWN_TIER))
+        return fail(KVIDX_ENOENT, "a Medium names a tier the table lacks (messages flagged KVIDX_PAYLOAD_MSG_UNKNOWN_TIER)");
+    if (t.markers && (flags & KVIDX_PAYLOAD_STOP_AT_CLEARED))
+        return fail(KVIDX_ENOENT, "%llu AllBlocksCleared markers (messages flagged KVIDX_PAYLOAD_MSG_CLEARED)", t.markers);
+    return 0;
+}
+
+int decode_write(kvidx* x, const DecodePlan& pl, kvidx_event_t* ev, int64_t* qoff, uint64_t* hashes, uint32_t* toks, cudaStream_t st) {
+    const unsigned g = (unsigned)((pl.in.n_msgs + kDecThreads - 1) / kDecThreads);
+    decode_write_kernel<<<g, kDecThreads, 0, st>>>(pl.in, pl.sorted_val, pl.ev_base, pl.hash_base, pl.hash_cnt, pl.tok_base, pl.tok_cnt,
+                                                   pl.flags, ev, hashes, toks);
+    x->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(qoff, pl.qoff, (size_t)(pl.tot.queues + 1) * 8, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int kvidx_decode_event_payloads_dev(kvidx_t* x, const uint8_t* d_bytes, const int64_t* d_msg_off, int64_t n_msgs,
+                                    const uint32_t* d_msg_pod, const uint32_t* d_msg_model, const uint8_t* tier_bytes,
+                                    const int64_t* tier_off, uint32_t n_tiers, int32_t gpu_tier, uint32_t flags,
+                                    kvidx_event_t* d_ev_out, int64_t ev_cap, int64_t* d_queue_off_out, int64_t queue_cap,
+                                    uint64_t* d_hashes_out, int64_t hash_cap, uint32_t* d_tokens_out, int64_t tok_cap,
+                                    uint8_t* d_msg_flags_out, int64_t counts_out[KVIDX_PAYLOAD_COUNTS]) {
+    if (counts_out) for (int i = 0; i < KVIDX_PAYLOAD_COUNTS; ++i) counts_out[i] = 0;
+    if (!x || n_msgs < 0 || n_msgs > INT32_MAX) return fail(KVIDX_EINVAL, "bad arguments");
+    if (int rc = check_payload_flags(flags)) return rc;
+    if (int rc = check_tier_table(tier_bytes, tier_off, n_tiers, gpu_tier)) return rc;
+    if (n_msgs == 0) return 0;
+    if (!d_bytes || !d_msg_off || !d_msg_pod || !d_msg_model) return fail(KVIDX_EINVAL, "NULL message arrays");
+    std::lock_guard<std::mutex> g(x->mu_w);
+    CK(cudaSetDevice(x->device));
+    cudaStream_t st = wstream(x);
+    DecodePlan pl;
+    pl.in.bytes = d_bytes; pl.in.msg_off = d_msg_off; pl.in.msg_pod = d_msg_pod; pl.in.msg_model = d_msg_model;
+    pl.in.n_msgs = n_msgs; pl.in.max_pods = x->tv.max_pods; pl.in.block_size = x->tv.block_size;
+    if (int rc = decode_count(x, pl, tier_bytes, tier_off, n_tiers, gpu_tier, st)) return rc;
+    const int rc = decode_verdict(x, pl.tot, flags, counts_out);
+    if (d_msg_flags_out) CK(cudaMemcpyAsync(d_msg_flags_out, pl.flags, (size_t)n_msgs, cudaMemcpyDeviceToDevice, st));
+    if (rc) return rc;
+    const DecTotals& t = pl.tot;
+    if ((int64_t)t.events > ev_cap || (int64_t)t.queues + 1 > queue_cap || (int64_t)t.hashes > hash_cap || (int64_t)t.tokens > tok_cap)
+        return fail(KVIDX_ENOSPC, "outputs too small: %llu events, %llu queue offsets, %llu hashes, %llu tokens", t.events, t.queues + 1,
+                    t.hashes, t.tokens);
+    if ((t.events && !d_ev_out) || !d_queue_off_out || (t.hashes && !d_hashes_out) || (t.tokens && !d_tokens_out))
+        return fail(KVIDX_EINVAL, "NULL output arrays");
+    if (int rc2 = decode_write(x, pl, d_ev_out, d_queue_off_out, d_hashes_out, d_tokens_out, st)) return rc2;
+    CK(cudaEventRecord(x->ev_write, st));              // reads issued after this call are ordered after it
+    return 0;
+}
+
+int kvidx_apply_event_payloads(kvidx_t* x, const uint8_t* bytes, const int64_t* msg_off, int64_t n_msgs, const uint32_t* msg_pod,
+                               const uint32_t* msg_model, const uint8_t* tier_bytes, const int64_t* tier_off, uint32_t n_tiers,
+                               int32_t gpu_tier, uint32_t flags, uint8_t* msg_flags_out, int64_t counts_out[KVIDX_PAYLOAD_COUNTS],
+                               int64_t* n_dropped_out) {
+    if (counts_out) for (int i = 0; i < KVIDX_PAYLOAD_COUNTS; ++i) counts_out[i] = 0;
+    if (n_dropped_out) *n_dropped_out = 0;
+    if (!x || n_msgs < 0 || n_msgs > INT32_MAX) return fail(KVIDX_EINVAL, "bad arguments");
+    if (int rc = check_payload_flags(flags)) return rc;
+    if (int rc = check_tier_table(tier_bytes, tier_off, n_tiers, gpu_tier)) return rc;
+    if (n_msgs == 0) return 0;
+    if (!msg_off || !msg_pod || !msg_model) return fail(KVIDX_EINVAL, "NULL message arrays");
+    for (int64_t i = 0; i < n_msgs; ++i) {
+        if (msg_off[i + 1] < msg_off[i]) return fail(KVIDX_EINVAL, "message offsets not monotone at %lld", (long long)i);
+        if (msg_pod[i] >= x->tv.max_pods) return fail(KVIDX_ERANGE, "message %lld: pod id %u >= max_pods %u", (long long)i, msg_pod[i], x->tv.max_pods);
+        if (msg_model[i] > 0xffffu) return fail(KVIDX_ERANGE, "message %lld: model id %u > 65535", (long long)i, msg_model[i]);
+    }
+    const uint64_t nb = (uint64_t)(msg_off[n_msgs] - msg_off[0]);
+    if (nb && !bytes) return fail(KVIDX_EINVAL, "NULL payload bytes");
+    std::lock_guard<std::mutex> g(x->mu_w);
+    CK(cudaSetDevice(x->device));
+    if (int rc0 = check_shards(x)) return rc0;
+    cudaStream_t st = wstream(x);
+    // the payloads on the device: bytes, offsets from 0, pods, models
+    DecodePlan pl;
+    uint8_t* d_bytes; int64_t* d_off; uint32_t *d_pod, *d_model;
+    CK(carve(x->d_decin, [&](Carver& c) {
+        d_bytes = c.take<uint8_t>(nb); d_off = c.take<int64_t>(n_msgs + 1); d_pod = c.take<uint32_t>(n_msgs); d_model = c.take<uint32_t>(n_msgs);
+    }));
+    std::vector<int64_t> off(msg_off, msg_off + n_msgs + 1);
+    for (auto& o : off) o -= msg_off[0];
+    if (int rc = x->snap.h2d(d_bytes, bytes + msg_off[0], nb, st)) return rc;
+    if (int rc = x->snap.h2d(d_off, off.data(), off.size() * 8, st)) return rc;
+    if (int rc = x->snap.h2d(d_pod, msg_pod, (size_t)n_msgs * 4, st)) return rc;
+    if (int rc = x->snap.h2d(d_model, msg_model, (size_t)n_msgs * 4, st)) return rc;
+    pl.in.bytes = d_bytes; pl.in.msg_off = d_off; pl.in.msg_pod = d_pod; pl.in.msg_model = d_model;
+    pl.in.n_msgs = n_msgs; pl.in.max_pods = x->tv.max_pods; pl.in.block_size = x->tv.block_size;
+    if (int rc = decode_count(x, pl, tier_bytes, tier_off, n_tiers, gpu_tier, st)) return rc;
+    int rc = decode_verdict(x, pl.tot, flags, counts_out);
+    if (msg_flags_out) if (int rc2 = x->snap.d2h(msg_flags_out, pl.flags, (size_t)n_msgs, st)) return rc2;
+    if (rc) return rc;
+    const DecTotals& t = pl.tot;
+    if (t.events == 0) return 0;                       // as kvidx_apply_events with no event
+    x->rm_armed = false;
+    if ((rc = ensure_room(x, t.stored_hashes))) return rc;
+    std::shared_lock<std::shared_mutex> tl(x->tables);
+    CK(x->d_ev.need((size_t)t.events * sizeof(kvidx_event_t)));
+    CK(x->d_qoff.need((size_t)(t.queues + 1) * 8));
+    CK(x->d_hash.need((size_t)std::max<uint64_t>(t.hashes, 1) * 8));
+    CK(x->d_evtok.need((size_t)std::max<uint64_t>(t.tokens, 1) * 4 + 16));
+    if ((rc = decode_write(x, pl, x->d_ev.as<kvidx_event_t>(), x->d_qoff.as<int64_t>(), x->d_hash.as<uint64_t>(), x->d_evtok.as<uint32_t>(), st)))
+        return rc;
+    const unsigned long long dropped_before = x->h_cnt->dropped_events, nospc_before = x->h_cnt->nospc;
+    rc = launch_apply_events(x, x->d_ev.as<kvidx_event_t>(), x->d_qoff.as<int64_t>(), (int64_t)t.queues, (int64_t)t.events,
+                             x->d_hash.as<uint64_t>(), (int64_t)t.hashes, x->d_evtok.as<uint32_t>(), st, (int64_t)t.max_ev_hashes);
     if (rc) return rc;
     rc = refresh_counters(x);
     if (rc) return rc;

@@ -719,33 +719,106 @@ static int64_t process_segments(kvhost* h, const std::vector<kvidx_event_t>& evs
     return applied;
 }
 
-int64_t kvhost_pool_process(kvhost_t* h, int64_t* n_dropped_out) {
-    if (int rc = need_dev(h)) return rc;
-    std::shared_lock<std::shared_mutex> wl(h->write_mu);
-    std::vector<kvidx_event_t> evs; std::vector<uint64_t> hashes; std::vector<uint32_t> toks;
-    {
-        std::lock_guard<std::mutex> g(h->mu);
-        for (auto& q : h->queues) {                      // each queue is FIFO; one pod always maps to one queue
-            for (auto& m : q) decode_batch(h, m.pod, m.model, (const uint8_t*)m.payload.data(), m.payload.size(), evs, hashes, toks);
-            q.clear();
-        }
+// Drains of at least this many payload bytes are decoded on the device (kvidx_apply_event_payloads), smaller ones by
+// decode_batch on the host.  scripts/bench_event_payloads.py (BASELINE config #5 events, 4 per message, 10 M-block index;
+// NVIDIA H100 80GB HBM3 at 700 W, DESIGN section 6): the host path was faster at 52 KB (21 K vs 14 K events/s), the
+// device path at 0.83 MB (130 K vs 96 K) and beyond; the device call has a floor of about 1.5 ms.
+static constexpr size_t kDeviceDecodeMinBytes = size_t(1) << 20;
+
+static void count_metrics(kvhost* h, const std::vector<kvidx_event_t>& evs) {
+    const uint32_t bs = h->cfg.index.block_size ? h->cfg.index.block_size : 16;
+    uint64_t adm = 0, evi = 0;
+    for (const auto& e : evs) {
+        if (e.op == KVIDX_EV_BLOCK_STORED) { if (e.n_hashes > 0) adm += e.n_tokens / bs; }      // Add(len(requestKeys)) only if there are engine keys
+        else if (e.op == KVIDX_EV_BLOCK_REMOVED) evi += e.n_hashes;                             // one Evict with one entry per hash
     }
-    if (n_dropped_out) *n_dropped_out = 0;
-    if (h->cfg.enable_metrics) {                       // digestEvents calls the instrumented Add / Evict (pool.go:299-330)
-        const uint32_t bs = h->cfg.index.block_size ? h->cfg.index.block_size : 16;
-        uint64_t adm = 0, evi = 0;
-        for (const auto& e : evs) {
-            if (e.op == KVIDX_EV_BLOCK_STORED) { if (e.n_hashes > 0) adm += e.n_tokens / bs; }      // Add(len(requestKeys)) only if there are engine keys
-            else if (e.op == KVIDX_EV_BLOCK_REMOVED) evi += e.n_hashes;                             // one Evict with one entry per hash
-        }
-        std::lock_guard<std::mutex> g(h->mu);
-        h->met.admissions_total += adm; h->met.evictions_total += evi;
-    }
+    std::lock_guard<std::mutex> g(h->mu);
+    h->met.admissions_total += adm; h->met.evictions_total += evi;
+}
+
+// The host path's apply: the drained messages decoded (and interned) by decode_batch, then one kvidx_apply_events (or the
+// segments of a drain with AllBlocksCleared markers).
+static int64_t apply_decoded(kvhost* h, const std::vector<kvidx_event_t>& evs, const std::vector<uint64_t>& hashes,
+                             const std::vector<uint32_t>& toks, int64_t* n_dropped_out) {
+    if (h->cfg.enable_metrics) count_metrics(h, evs);  // digestEvents calls the instrumented Add / Evict (pool.go:299-330)
     if (evs.empty()) return 0;
     if (h->cfg.clear_on_all_blocks_cleared) return process_segments(h, evs, hashes, toks, n_dropped_out);
     const int rc = kvidx_apply_events(h->ix, evs.data(), (int64_t)evs.size(), hashes.data(), (int64_t)hashes.size(), toks.data(), (int64_t)toks.size(), n_dropped_out);
     if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
     return (int64_t)evs.size();
+}
+
+// The device path: the payloads packed in drain order and decoded by kvidx_apply_event_payloads against a copy of the tier
+// table.  A message naming a tier the copy lacks is decoded on the host, under mu and in drain order, only to intern its
+// names exactly as the host path would; the call is then repeated with the unknown tiers skipped (they are the names that
+// found no room in the 16 ids).  A drain with AllBlocksCleared under clear_on_all_blocks_cleared goes to the host path.
+static int64_t process_on_device(kvhost* h, std::vector<Msg>& msgs, int64_t* n_dropped_out) {
+    const size_t n = msgs.size();
+    std::vector<uint8_t> bytes; std::vector<int64_t> off(n + 1, 0); std::vector<uint32_t> pod(n), model(n);
+    for (size_t i = 0; i < n; ++i) off[i + 1] = off[i] + (int64_t)msgs[i].payload.size();
+    bytes.resize((size_t)off[n]);
+    for (size_t i = 0; i < n; ++i) {
+        memcpy(bytes.data() + off[i], msgs[i].payload.data(), msgs[i].payload.size());
+        pod[i] = msgs[i].pod; model[i] = msgs[i].model;
+    }
+    std::vector<uint8_t> mflags(n);
+    uint32_t flags = h->cfg.clear_on_all_blocks_cleared ? KVIDX_PAYLOAD_STOP_AT_CLEARED : 0u;
+    int64_t counts[KVIDX_PAYLOAD_COUNTS];
+    for (;;) {
+        std::string tb; std::vector<int64_t> toff(1, 0); int gpu;
+        {
+            std::lock_guard<std::mutex> g(h->mu);
+            for (const std::string* s : h->tiers.names) { tb += *s; toff.push_back((int64_t)tb.size()); }
+            gpu = h->tiers.find("gpu");
+        }
+        const int rc = kvidx_apply_event_payloads(h->ix, bytes.data(), off.data(), (int64_t)n, pod.data(), model.data(), (const uint8_t*)tb.data(),
+                                                  toff.data(), (uint32_t)(toff.size() - 1), gpu, flags, mflags.data(), counts, n_dropped_out);
+        if (rc == KVIDX_ENOENT && (flags & KVIDX_PAYLOAD_STOP_AT_CLEARED) && counts[7] > 0) {
+            std::vector<kvidx_event_t> evs; std::vector<uint64_t> hs; std::vector<uint32_t> ts;
+            {
+                std::lock_guard<std::mutex> g(h->mu);
+                for (auto& m : msgs) decode_batch(h, m.pod, m.model, (const uint8_t*)m.payload.data(), m.payload.size(), evs, hs, ts);
+            }
+            return apply_decoded(h, evs, hs, ts, n_dropped_out);
+        }
+        if (rc == KVIDX_ENOENT && !(flags & KVIDX_PAYLOAD_SKIP_UNKNOWN_TIER)) {
+            std::vector<kvidx_event_t> evs; std::vector<uint64_t> hs; std::vector<uint32_t> ts;
+            std::lock_guard<std::mutex> g(h->mu);
+            for (size_t i = 0; i < n; ++i)
+                if (mflags[i] & KVIDX_PAYLOAD_MSG_UNKNOWN_TIER) decode_batch(h, pod[i], model[i], bytes.data() + off[i], (size_t)(off[i + 1] - off[i]), evs, hs, ts);
+            flags |= KVIDX_PAYLOAD_SKIP_UNKNOWN_TIER;
+            continue;
+        }
+        if (h->cfg.enable_metrics) {
+            std::lock_guard<std::mutex> g(h->mu);
+            h->met.admissions_total += (uint64_t)counts[5]; h->met.evictions_total += (uint64_t)counts[6];
+        }
+        if (rc) { g_herr = kvidx_last_error(h->ix); return rc; }
+        return counts[1];
+    }
+}
+
+int64_t kvhost_pool_process(kvhost_t* h, int64_t* n_dropped_out) {
+    if (int rc = need_dev(h)) return rc;
+    std::shared_lock<std::shared_mutex> wl(h->write_mu);
+    std::vector<kvidx_event_t> evs; std::vector<uint64_t> hashes; std::vector<uint32_t> toks;
+    std::vector<Msg> msgs;                               // a drain for the device path
+    {
+        std::lock_guard<std::mutex> g(h->mu);
+        size_t bytes = 0;
+        for (const auto& q : h->queues) for (const auto& m : q) bytes += m.payload.size();
+        const bool device = bytes >= kDeviceDecodeMinBytes && !h->tiers.names.empty();
+        for (auto& q : h->queues) {                      // each queue is FIFO; one pod always maps to one queue
+            for (auto& m : q) {
+                if (device) msgs.push_back(std::move(m));
+                else decode_batch(h, m.pod, m.model, (const uint8_t*)m.payload.data(), m.payload.size(), evs, hashes, toks);
+            }
+            q.clear();
+        }
+    }
+    if (n_dropped_out) *n_dropped_out = 0;
+    if (!msgs.empty()) return process_on_device(h, msgs, n_dropped_out);
+    return apply_decoded(h, evs, hashes, toks, n_dropped_out);
 }
 
 // Removes the pod's messages still waiting in its queue.  Caller holds mu.

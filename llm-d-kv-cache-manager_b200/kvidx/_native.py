@@ -19,6 +19,9 @@ MAX_TIERS = 16
 SCORE_ABSENT = -1.0
 OK, ENOENT, ECUDA, ENOMEM, EINVAL, ENOSPC, ERANGE = 0, -2, -5, -12, -22, -28, -34
 EV_BLOCK_STORED, EV_BLOCK_REMOVED = 0, 1
+PAYLOAD_SKIP_UNKNOWN_TIER, PAYLOAD_STOP_AT_CLEARED = 1, 2
+PAYLOAD_MSG_DECODED, PAYLOAD_MSG_UNKNOWN_TIER, PAYLOAD_MSG_CLEARED = 1, 2, 4
+PAYLOAD_COUNTS = ("messages", "events", "hashes", "tokens", "queues", "admitted", "removed", "markers")
 EVICT_NONE, EVICT_CLOCK = 0, 1
 ANY_MODEL, INVENTORY_ENGINE = 0xFFFFFFFF, 1
 _EVICT_POLICIES = {"none": EVICT_NONE, "clock": EVICT_CLOCK}
@@ -90,6 +93,11 @@ SYMBOLS = {
     "kvidx_score_batch_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kvidx_hash_keys_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kvidx_apply_events_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "kvidx_decode_event_payloads_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, _u8p, _i64p,
+                                                  C.c_uint32, C.c_int32, C.c_uint32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                                  C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, _i64p]),
+    "kvidx_apply_event_payloads": (C.c_int, [C.c_void_p, _u8p, _i64p, C.c_int64, _u32p, _u32p, _u8p, _i64p, C.c_uint32, C.c_int32,
+                                             C.c_uint32, _u8p, _i64p, _i64p]),
     "kvidx_score_batch_sparse_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "kvidx_shard_compact": (C.c_int, [C.c_void_p]),
     "kvidx_key_owners_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int64, C.c_void_p]),
@@ -632,6 +640,33 @@ class Index:
         rc = self.L.kvidx_apply_events(self.h, events.ctypes.data_as(C.c_void_p), len(events), _p(hashes, _u64p), len(hashes),
                                        _p(tokens, _u32p), len(tokens), C.byref(nd))
         return rc, nd.value
+
+    # -- KVEvents wire payloads decoded on the device: message i is a raw msgpack EventBatch of pod pods[i], model models[i] --
+    def decode_event_payloads_dev(self, d_bytes, d_msg_off, n_msgs, d_pods, d_models, tier_names, gpu_tier, d_ev, ev_cap, d_queue_off,
+                                  queue_cap, d_hashes, hash_cap, d_tokens, tok_cap, flags=0, d_msg_flags=0):
+        """kvidx_decode_event_payloads_dev -> (rc, counts dict).  tier_names: the table, by tier id (lower-case)."""
+        tb, toff = pack_text(tier_names)
+        counts = np.zeros(len(PAYLOAD_COUNTS), np.int64)
+        rc = self.L.kvidx_decode_event_payloads_dev(self.h, d_bytes, d_msg_off, n_msgs, d_pods, d_models, _p(tb, _u8p), _p(toff, _i64p),
+                                                    len(tier_names), gpu_tier, flags, d_ev or None, ev_cap, d_queue_off or None,
+                                                    queue_cap, d_hashes or None, hash_cap, d_tokens or None, tok_cap,
+                                                    d_msg_flags or None, _p(counts, _i64p))
+        return rc, dict(zip(PAYLOAD_COUNTS, (int(c) for c in counts)))
+
+    def apply_event_payloads(self, payloads, pods, models, tier_names, gpu_tier, flags=0):
+        """kvidx_apply_event_payloads over a list of raw messages (bytes) -> (rc, n_dropped, counts dict, per-message flags)."""
+        data, off = pack_text(payloads)
+        pods = np.ascontiguousarray(pods, np.uint32)
+        models = np.ascontiguousarray(models, np.uint32)
+        assert len(pods) == len(models) == len(payloads)
+        tb, toff = pack_text(tier_names)
+        counts = np.zeros(len(PAYLOAD_COUNTS), np.int64)
+        mflags = np.zeros(len(payloads), np.uint8)
+        nd = C.c_int64(0)
+        rc = self.L.kvidx_apply_event_payloads(self.h, _p(data, _u8p), _p(off, _i64p), len(payloads), _p(pods, _u32p), _p(models, _u32p),
+                                               _p(tb, _u8p), _p(toff, _i64p), len(tier_names), gpu_tier, flags, _p(mflags, _u8p),
+                                               _p(counts, _i64p), C.byref(nd))
+        return rc, nd.value, dict(zip(PAYLOAD_COUNTS, (int(c) for c in counts))), mflags
 
     def removal_masks(self, pod_ids, tier_ids=None):
         """(pod mask words, tier mask) of a removal: tier_ids None = all tiers."""
