@@ -10,6 +10,7 @@
 #include <atomic>
 #include <condition_variable>
 #include <deque>
+#include <memory>
 #include <mutex>
 #include <shared_mutex>
 #include <string>
@@ -58,9 +59,25 @@ int fail(int code, const char* fmt, ...) {
 
 uint64_t pow2ceil(uint64_t v) { uint64_t p = 1; while (p < v) p <<= 1; return p; }
 
-// growable device / pinned-host scratch
+// A stream or event the handle created, destroyed with its owner.  It converts to the raw handle.
+template <class T, cudaError_t (*Destroy)(T)> struct Owned {
+    T h = nullptr;
+    Owned() = default;
+    Owned(const Owned&) = delete;
+    Owned& operator=(const Owned&) = delete;
+    ~Owned() { if (h) Destroy(h); }
+    operator T() const { return h; }
+};
+using OwnStream = Owned<cudaStream_t, cudaStreamDestroy>;
+using OwnEvent = Owned<cudaEvent_t, cudaEventDestroy>;
+
+// growable device / pinned-host scratch, freed with its owner
 struct DevBuf {
     void* p = nullptr; size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
     cudaError_t need(size_t n) {
         if (n <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -76,6 +93,10 @@ struct DevBuf {
 };
 struct PinBuf {
     void* p = nullptr; size_t cap = 0;
+    PinBuf() = default;
+    PinBuf(const PinBuf&) = delete;
+    PinBuf& operator=(const PinBuf&) = delete;
+    ~PinBuf() { if (p) cudaFreeHost(p); }
     cudaError_t need(size_t n) {
         if (n <= cap) return cudaSuccess;
         if (p) cudaFreeHost(p);
@@ -86,7 +107,6 @@ struct PinBuf {
         if (e == cudaSuccess) cap = want;
         return e;
     }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
     template <class T> T* as() { return static_cast<T*>(p); }
 };
 
@@ -126,14 +146,10 @@ template <class Buf, class Layout> cudaError_t carve(Buf& buf, Layout&& layout) 
 struct Stager {
     static constexpr size_t kChunk = 16u << 20;
     PinBuf buf[2];
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    OwnEvent ev[2];
     cudaError_t init() {
-        for (auto& e : ev) if (cudaError_t r = cudaEventCreateWithFlags(&e, cudaEventDisableTiming)) return r;
+        for (auto& e : ev) if (cudaError_t r = cudaEventCreateWithFlags(&e.h, cudaEventDisableTiming)) return r;
         return cudaSuccess;
-    }
-    void release() {
-        buf[0].release(); buf[1].release();
-        for (auto& e : ev) { if (e) cudaEventDestroy(e); e = nullptr; }
     }
     // device -> host; every byte is in dst when it returns
     int d2h(void* dst, const void* src, size_t n, cudaStream_t st) {
@@ -200,6 +216,25 @@ struct SubmitQueue {
     PinBuf h_in, h_out;                            // the combined batch and its rows, owned by the current leader
 };
 
+// the device prefix store (kvidx_text_store_*); the table and the arena are freed with it
+struct TextStore {
+    int64_t cap_blocks = 0; uint32_t B = 0;
+    OwnStream stream;                         // kvidx_text_store_add / _find (Score() from text runs on the handle's stream)
+    OwnEvent ev_last;                         // the end of the last store call, on whichever stream it ran: the next one waits
+    Stager stage;                             // for pageable host buffers
+    PinBuf h_misc;
+    TextTable t{};
+    void* tab = nullptr;                      // the table's arrays, one allocation
+    uint32_t* arena = nullptr; int64_t arena_cap = 0, arena_used = 0;
+    int64_t resident = 0;
+    unsigned long long clock = 0;             // recency stamps handed out so far
+    DevBuf d_in, d_blk, d_scr, d_tok, d_cub, d_out;
+    TextStore() = default;
+    TextStore(const TextStore&) = delete;
+    TextStore& operator=(const TextStore&) = delete;
+    ~TextStore() { if (tab) cudaFree(tab); if (arena) cudaFree(arena); }
+};
+
 struct kvidx {
     kvidx_config_t cfg{};
     TableView tv{};
@@ -207,9 +242,11 @@ struct kvidx {
     int sm_count = 132;
     // Read path (Score / Lookup / hash) and write path (Add / Evict / events) run on their own streams and behind their own
     // mutexes: a Score() call and an event batch overlap on the device (table.cuh: readers never wait for writers).
-    cudaStream_t own_stream = nullptr, stream = nullptr, copy_stream = nullptr, d2h_stream = nullptr, own_wstream = nullptr;
-    cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_k[2] = {nullptr, nullptr};
-    cudaEvent_t ev_write = nullptr;   // last asynchronous (device-resident) write batch: later reads are ordered after it
+    // The streams and events below are the handle's own; `stream` is the read side's, which may be the caller's.
+    OwnStream own_stream, copy_stream, d2h_stream, own_wstream;
+    cudaStream_t stream = nullptr;
+    OwnEvent ev_h2d[2], ev_done[2], ev_k[2];
+    OwnEvent ev_write;                // last asynchronous (device-resident) write batch: later reads are ordered after it
     Counters* d_cnt = nullptr;
     Counters* h_cnt = nullptr;     // pinned mirror (write side)
     Counters* d_cnt_all = nullptr; // sharded: every owner's counters, gathered before a write batch
@@ -246,7 +283,7 @@ struct kvidx {
                                    // 4 = always the warp-per-prompt cooperative kernel
     int64_t coop_max = 2048;       // batches up to this many prompts use the warp-per-prompt cooperative kernel
     int64_t zerocopy_max = 32;     // host-buffer calls up to this many prompts skip the copy engine (tokens read from pinned host memory)
-    struct SubmitQueue* queue = nullptr;   // coalesces concurrent host-buffer Score() callers (submit.cuh)
+    std::unique_ptr<SubmitQueue> queue;    // coalesces concurrent host-buffer Score() callers (submit.cuh)
     // Batch-size thresholds, from a sweep of the forced paths on an H100 SXM (10 M-block index, bench.py's query mix): the
     // warp-per-prompt rounds beat the cooperative kernel from 4096 prompts (tie at 2048) and the fused kernel at every size
     // from 2048 up; the class pipeline beats them from 131 072 prompts.
@@ -260,14 +297,14 @@ struct kvidx {
     int rounds_dedup = 2;          // round pipeline: 0 every prompt on its own, 1 prefix classes, 2 + partial followers
     int sort_prefix = 1;           // sort the batch by first-block fingerprint before the rounds
     int64_t rounds_overlap_min = 65536;   // batches from this size run as several parts (per-prompt rounds: two halves)
-    cudaStream_t aux_stream[kMaxParts - 1] = {}; cudaEvent_t ev_fork = nullptr, ev_join[kMaxParts - 1] = {};
+    OwnStream aux_stream[kMaxParts - 1]; OwnEvent ev_fork, ev_join[kMaxParts - 1];
     int64_t rounds_warp_max = 131072;      // per-prompt rounds: kernel P warp per prompt up to this many prompts
                                    // (faster than the lane-per-prompt kernel P at every size swept up to 131 072)
     // multi-part class pipeline: a part's kernel G on a low-priority stream, its short kernels (G2, H, P, R) on a high-priority one
-    cudaStream_t hp_stream[kMaxParts] = {}, lp_stream[kMaxParts] = {}; cudaEvent_t ev_g[kMaxParts] = {}, ev_r[kMaxParts] = {};
+    OwnStream hp_stream[kMaxParts], lp_stream[kMaxParts]; OwnEvent ev_g[kMaxParts], ev_r[kMaxParts];
     // the device prefix store (kvidx_text_store_*): its own lock, independent of the read and write sides
     std::mutex mu_text;
-    struct TextStore* text = nullptr;
+    std::unique_ptr<TextStore> text;
 };
 
 namespace {
@@ -287,18 +324,6 @@ size_t remove_bitmap_bytes(uint64_t slots) { return slots / 8 + slots / 16; }
 // The stream write kernels go to.  Exact-LRU mode keeps reads and writes on ONE stream (reads write recency stamps, so the
 // two sides are not independent there); otherwise the write path has its own.
 cudaStream_t wstream(kvidx* x) { return x->tv.req_stamp ? x->stream : x->own_wstream; }
-
-// Locks of a call.  Read-side calls take mu_r (+ mu_w in exact-LRU mode, where everything is serialised as in round 1),
-// write-side calls mu_w; both hold `tables` shared while they launch.  Only rebuild() takes `tables` exclusively.
-struct ReadGuard {
-    std::unique_lock<std::mutex> w, r;
-    std::shared_lock<std::shared_mutex> t;
-    explicit ReadGuard(kvidx* x) {
-        if (x->tv.req_stamp) w = std::unique_lock<std::mutex>(x->mu_w);
-        r = std::unique_lock<std::mutex>(x->mu_r);
-        t = std::shared_lock<std::shared_mutex>(x->tables);
-    }
-};
 
 int refresh_counters(kvidx* x) {
     CK(cudaMemcpyAsync(x->h_cnt, x->d_cnt, sizeof(Counters), cudaMemcpyDeviceToHost, wstream(x)));
@@ -466,6 +491,80 @@ int cap_keys(kvidx* x) {
     int rc = clock_sweep(x);
     return rc ? rc : refresh_counters(x);
 }
+
+// ---- Call scopes ------------------------------------------------------------------------------------------------------
+// Locks of a call.  Read-side calls take mu_r (+ mu_w in exact-LRU mode, where everything is serialised as in round 1),
+// write-side calls mu_w; both hold `tables` shared while they launch.  Only rebuild() (through ensure_room) and the calls
+// that swap or map tables take `tables` exclusively.
+enum : unsigned {
+    kShards = 1,          // begin: every peer shard must be mapped (check_shards)
+    kAfterWrites = 2,     // begin (read): order the call's stream after the last asynchronous write batch (ev_write)
+    kDisarm = 4,          // begin (write): a pending collective pod removal is void (kvidx_shard_remove_pods)
+};
+
+struct ReadCall {
+    kvidx* x;
+    std::unique_lock<std::mutex> w, r;
+    std::shared_lock<std::shared_mutex> t;
+    explicit ReadCall(kvidx* x) : x(x) {
+        if (x->tv.req_stamp) w = std::unique_lock<std::mutex>(x->mu_w);
+        r = std::unique_lock<std::mutex>(x->mu_r);
+        t = std::shared_lock<std::shared_mutex>(x->tables);
+    }
+    int begin(unsigned flags) { return begin(flags, x->stream); }
+    int begin(unsigned flags, cudaStream_t st) {
+        CK(cudaSetDevice(x->device));
+        if (flags & kShards) { if (int rc = check_shards(x)) return rc; }
+        if (flags & kAfterWrites) CK(cudaStreamWaitEvent(st, x->ev_write, 0));
+        return 0;
+    }
+    // after an error: copies may still read the caller's buffers and the handle's scratch, so the streams the call used are
+    // drained before the caller gets its buffers back, and the sticky error is cleared (the call's error text is kept)
+    static int end(int rc, std::initializer_list<cudaStream_t> streams) {
+        if (!rc) return 0;
+        const std::string keep = g_err;
+        for (cudaStream_t s : streams) cudaStreamSynchronize(s);
+        cudaGetLastError();
+        g_err = keep;
+        return rc;
+    }
+};
+
+// The counters a synchronous write call compares after its launch
+struct WriteTally { unsigned long long dropped, nospc; };
+
+// A write call holds mu_w throughout, and takes `tables` shared (share) or exclusively (exclusive) for its launches.
+// ensure_room may rebuild the tables, taking `tables` exclusively itself, so it runs only inside share_with_room: before
+// the call holds them.
+struct WriteCall {
+    kvidx* x;
+    std::unique_lock<std::mutex> w;
+    std::shared_lock<std::shared_mutex> t;
+    std::unique_lock<std::shared_mutex> tx;
+    explicit WriteCall(kvidx* x) : x(x), w(x->mu_w) {}
+    int begin(unsigned flags) {
+        if (flags & kDisarm) x->rm_armed = false;
+        CK(cudaSetDevice(x->device));
+        if (flags & kShards) { if (int rc = check_shards(x)) return rc; }
+        return 0;
+    }
+    void share() { t = std::shared_lock<std::shared_mutex>(x->tables); }
+    int share_with_room(uint64_t incoming) {
+        if (int rc = ensure_room(x, incoming)) return rc;
+        share();
+        return 0;
+    }
+    void exclusive() { tx = std::unique_lock<std::shared_mutex>(x->tables); }
+    WriteTally tally() const { return WriteTally{x->h_cnt->dropped_events, x->h_cnt->nospc}; }
+    // The end of a synchronous write batch: the counters read back, the events it dropped, the inserts a full shard refused,
+    // then the key cap.
+    int settle(const WriteTally& before, int64_t* n_dropped_out) {
+        if (int rc = refresh_counters(x)) return rc;
+        if (n_dropped_out) *n_dropped_out = (int64_t)(x->h_cnt->dropped_events - before.dropped);
+        if (x->h_cnt->nospc != before.nospc) return fail(KVIDX_ENOSPC, "%llu inserts refused: the owning shard is full", x->h_cnt->nospc - before.nospc);
+        return cap_keys(x);
+    }
+};
 
 int launch_score_rounds_plain(kvidx* x, const ScoreArgs& a, cudaStream_t st, int64_t max_blocks);
 
@@ -792,6 +891,21 @@ struct ScoreIn {
     }
 };
 
+// A Score() call of n prompts (offsets off) with dense result rows (scores: n x max_pods) or sparse ones (pods, scores:
+// n x kMaxEnt, cnt: n); the prompts' elements are set where the call is launched.
+ScoreArgs dense_args(const int64_t* off, int64_t n, const uint32_t* model, uint32_t model0, const uint64_t* filter, double* scores,
+                     uint8_t* has_keys) {
+    ScoreArgs a{};
+    a.tok_off = off; a.n_prompts = n; a.model = model; a.model0 = model0; a.filter = filter; a.dense = scores; a.has_keys = has_keys;
+    return a;
+}
+ScoreArgs sparse_args(const int64_t* off, int64_t n, const uint32_t* model, uint32_t model0, const uint64_t* filter, uint16_t* pods,
+                      double* scores, uint8_t* cnt, uint8_t* has_keys) {
+    ScoreArgs a = dense_args(off, n, model, model0, filter, nullptr, has_keys);
+    a.sp_pods = pods; a.sp_scores = scores; a.sp_cnt = cnt;
+    return a;
+}
+
 // Exact-LRU handles take the thread-per-prompt kernel: Lookup must touch every present key of a prompt (no early exit).
 // So does KVIDX_SCORE_KERNEL=v1 as the cross-check, and so do token prompts of a block size the other token kernels' staging
 // is not written for: every size but 16, 32, 64 and 128.  At 32, 64 and 128 only the warp-per-prompt kernel
@@ -920,9 +1034,8 @@ int launch_turn(kvidx* x, const ScoreIn& in, const ScoreArgs& a, cudaStream_t st
 
 // The device-resident entry points: Score() on the handle's stream, after the asynchronous write batches issued before.
 int score_dev(kvidx* x, const ScoreIn& in, const ScoreArgs& a) {
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
+    ReadCall c(x);
+    if (int rc = c.begin(kAfterWrites)) return rc;
     return launch_score(x, in, a, x->stream);
 }
 
@@ -1019,18 +1132,9 @@ int score_host(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
     int rc = check_csr(h.tok_off, n, in.keys ? "key_off" : "tok_off");
     if (rc) return rc;
     if (h.tok_off[n] > h.tok_off[0] && !in.p) return fail(KVIDX_EINVAL, in.keys ? "NULL keys" : "NULL tokens");
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    rc = score_host_locked(x, in, h);
-    if (rc) {
-        // an error in the middle of the pipeline: copies may still be reading the caller's buffers and this handle's staging
-        // slots -- drain the three streams before the caller gets its buffers back (the error text is kept)
-        const std::string keep = g_err;
-        cudaStreamSynchronize(x->copy_stream); cudaStreamSynchronize(x->stream); cudaStreamSynchronize(x->d2h_stream);
-        cudaGetLastError();
-        g_err = keep;
-    }
-    return rc;
+    ReadCall c(x);
+    if ((rc = c.begin(kAfterWrites))) return rc;
+    return c.end(score_host_locked(x, in, h), {x->copy_stream, x->stream, x->d2h_stream});
 }
 
 // A handful of prompts (the size of one RPC, or of what the submission queue gathers at low load) whose kernel reads its
@@ -1058,7 +1162,6 @@ int score_host_zerocopy(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
         if (!nk_direct) v[nin].p = nk;
     }
     const ScoreIn z = in.moved(v, a);
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
     if (int rc = launch_score(x, z, a, x->stream)) return rc;
     CK(cudaStreamSynchronize(x->stream));
     if (!nk_direct) memcpy(s[nin].at(0), v[nin].p, s[nin].bytes(0, n));
@@ -1098,8 +1201,8 @@ int score_host_locked(kvidx* x, const ScoreIn& in, const ScoreArgs& h) {
         rows.carve(x->h_out[sl].p, c, staged);
         return rows.copy(rows.at(h, i0), staged, c);
     };
-    // the first chunk must see everything already queued on the handle's stream, and asynchronous write batches issued before
-    CK(cudaStreamWaitEvent(s_k, x->ev_write, 0));
+    // the first chunk must see everything already queued on the handle's stream (asynchronous write batches issued before
+    // included: score_host ordered it after them)
     CK(cudaEventRecord(x->ev_k[0], s_k));
     CK(cudaStreamWaitEvent(s_in, x->ev_k[0], 0));
     int64_t i0 = 0;
@@ -1199,7 +1302,7 @@ int run_combined(kvidx* x, SubmitQueue* q, const std::vector<SubmitReq*>& batch)
         if (filter) { if (r->a.filter) memcpy(filter + (size_t)at * FW, r->a.filter, (size_t)rn * FW * 8); else memset(filter + (size_t)at * FW, 0, (size_t)rn * FW * 8); }
         at += rn; tat += rt;
     }
-    ScoreArgs all{nullptr, off, 0, n, model, a0.model0, filter, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    ScoreArgs all = dense_args(off, n, model, a0.model0, filter, nullptr, nullptr);
     rows.carve(q->h_out.p, n, all);
     int rc = score_host(x, ScoreIn{tok, false}, all);
     if (rc) return rc;
@@ -1212,7 +1315,7 @@ int run_combined(kvidx* x, SubmitQueue* q, const std::vector<SubmitReq*>& batch)
 }
 
 int submit_score(kvidx* x, const uint32_t* tok, const ScoreArgs& a) {
-    SubmitQueue* q = x->queue;
+    SubmitQueue* q = x->queue.get();
     const int64_t n = a.n_prompts;
     // big batches and malformed calls go straight through (score_host validates); so does everything when the queue is off
     if (!q || !q->enabled || n <= 0 || !a.tok_off || n > q->max_prompts / 4) return score_host(x, ScoreIn{tok, false}, a);
@@ -1274,15 +1377,10 @@ int submit_score(kvidx* x, const uint32_t* tok, const ScoreArgs& a) {
     }
 }
 
-SubmitQueue* new_submit_queue() {
-    SubmitQueue* q = new SubmitQueue();
+std::unique_ptr<SubmitQueue> new_submit_queue() {
+    auto q = std::make_unique<SubmitQueue>();
     if (const char* k = getenv("KVIDX_SUBMIT_QUEUE")) q->enabled = atoi(k) != 0;
     return q;
-}
-void delete_submit_queue(SubmitQueue* q) {
-    if (!q) return;
-    q->h_in.release(); q->h_out.release();
-    delete q;
 }
 uint64_t submit_queue_coalesced(SubmitQueue* q) { return q->coalesced.load(); }
 
@@ -1295,8 +1393,6 @@ int launch_hash_keys(kvidx* x, const uint32_t* d_tok, const int64_t* d_off, int6
     CK(cudaGetLastError());
     return 0;
 }
-
-void delete_text_store(TextStore* s);
 
 }  // namespace
 
@@ -1353,32 +1449,32 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     CK(cudaGetDeviceProperties(&prop, c.device));
     x->sm_count = prop.multiProcessorCount;
     if (prop.major != 9 || prop.minor != 0) return fail(KVIDX_ECUDA, "device sm_%d%d is not Hopper; libkvidx is built for sm_90a only", prop.major, prop.minor);
-    CK(cudaStreamCreateWithFlags(&x->own_stream, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&x->own_wstream, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&x->copy_stream, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&x->d2h_stream, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&x->own_stream.h, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&x->own_wstream.h, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&x->copy_stream.h, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&x->d2h_stream.h, cudaStreamNonBlocking));
     for (int q = 0; q < kMaxParts - 1; ++q) {
-        CK(cudaStreamCreateWithFlags(&x->aux_stream[q], cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&x->ev_join[q], cudaEventDisableTiming));
+        CK(cudaStreamCreateWithFlags(&x->aux_stream[q].h, cudaStreamNonBlocking));
+        CK(cudaEventCreateWithFlags(&x->ev_join[q].h, cudaEventDisableTiming));
     }
-    CK(cudaEventCreateWithFlags(&x->ev_fork, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&x->ev_fork.h, cudaEventDisableTiming));
     {
         int lo = 0, hi = 0;
         CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
         for (int q = 0; q < kMaxParts; ++q) {
-            CK(cudaStreamCreateWithPriority(&x->hp_stream[q], cudaStreamNonBlocking, hi));
-            CK(cudaStreamCreateWithPriority(&x->lp_stream[q], cudaStreamNonBlocking, lo));
+            CK(cudaStreamCreateWithPriority(&x->hp_stream[q].h, cudaStreamNonBlocking, hi));
+            CK(cudaStreamCreateWithPriority(&x->lp_stream[q].h, cudaStreamNonBlocking, lo));
         }
     }
-    for (int q = 0; q < kMaxParts; ++q) { CK(cudaEventCreateWithFlags(&x->ev_g[q], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&x->ev_r[q], cudaEventDisableTiming)); }
-    CK(cudaEventCreateWithFlags(&x->ev_write, cudaEventDisableTiming));
+    for (int q = 0; q < kMaxParts; ++q) { CK(cudaEventCreateWithFlags(&x->ev_g[q].h, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&x->ev_r[q].h, cudaEventDisableTiming)); }
+    CK(cudaEventCreateWithFlags(&x->ev_write.h, cudaEventDisableTiming));
     CK(x->snap.init());
     CK(x->rstage.init());
     x->stream = x->own_stream;
     for (int i = 0; i < 2; ++i) {
-        CK(cudaEventCreateWithFlags(&x->ev_h2d[i], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&x->ev_done[i], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&x->ev_k[i], cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&x->ev_h2d[i].h, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&x->ev_done[i].h, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&x->ev_k[i].h, cudaEventDisableTiming));
     }
     uint32_t shard_bits = 0;
     if (c.shard_count > 1) {
@@ -1483,47 +1579,23 @@ int kvidx_create(const kvidx_config_t* cfg_in, kvidx_t** out) {
     return 0;
 }
 
+// The tables and counters are freed here; every other buffer, stream and event of the handle (and its prefix store) goes
+// with its member, once the device is idle.
 void kvidx_destroy(kvidx_t* x) {
     if (!x) return;
     cudaSetDevice(x->device);
     cudaDeviceSynchronize();
-    delete_text_store(x->text);
-    if (x->queue) { delete_submit_queue(x->queue); x->queue = nullptr; }
-    for (int i = 0; i < 2; ++i) {
-        x->d_tok[i].release(); x->d_off[i].release(); x->d_model[i].release(); x->d_filter[i].release();
-        x->d_out[i].release(); x->d_aux[i].release(); x->h_stage[i].release(); x->h_out[i].release();
-        if (x->ev_h2d[i]) cudaEventDestroy(x->ev_h2d[i]);
-        if (x->ev_done[i]) cudaEventDestroy(x->ev_done[i]);
-        if (x->ev_k[i]) cudaEventDestroy(x->ev_k[i]);
-    }
-    x->d_rounds.release();
-    x->d_misc.release(); x->d_rmisc.release(); x->d_turn.release(); x->d_inv.release(); x->h_inv.release(); x->d_ev.release(); x->d_hash.release(); x->d_evtok.release(); x->d_qoff.release(); x->h_misc.release();
-    x->d_wkeys.release(); x->d_wpred.release(); x->d_wready.release(); x->d_wmap.release();
-    x->d_snap.release(); x->snap.release(); x->rstage.release(); x->d_dec.release(); x->d_decin.release();
     if (x->tv.req) cudaFree(x->tv.req);
     if (x->tv.eng) cudaFree(x->tv.eng);
     if (x->tv.req_stamp) cudaFree(x->tv.req_stamp);
     if (x->tv.req_ref) cudaFree(x->tv.req_ref);
     if (x->tv.eng_ref) cudaFree(x->tv.eng_ref);
-    x->d_sweep.release();
     if (x->d_cnt) cudaFree(x->d_cnt);
     if (x->h_cnt) cudaFreeHost(x->h_cnt);
     if (x->d_cnt_all) cudaFree(x->d_cnt_all);
     if (x->h_cnt_all) cudaFreeHost(x->h_cnt_all);
-    if (x->own_stream) cudaStreamDestroy(x->own_stream);
-    if (x->own_wstream) cudaStreamDestroy(x->own_wstream);
-    if (x->copy_stream) cudaStreamDestroy(x->copy_stream);
-    if (x->d2h_stream) cudaStreamDestroy(x->d2h_stream);
-    for (int q = 0; q < kMaxParts - 1; ++q) {
-        if (x->aux_stream[q]) cudaStreamDestroy(x->aux_stream[q]);
-        if (x->ev_join[q]) cudaEventDestroy(x->ev_join[q]);
-    }
-    if (x->ev_fork) cudaEventDestroy(x->ev_fork);
-    for (int q = 0; q < kMaxParts; ++q) { if (x->hp_stream[q]) cudaStreamDestroy(x->hp_stream[q]); if (x->lp_stream[q]) cudaStreamDestroy(x->lp_stream[q]); }
-    for (int q = 0; q < kMaxParts; ++q) { if (x->ev_g[q]) cudaEventDestroy(x->ev_g[q]); if (x->ev_r[q]) cudaEventDestroy(x->ev_r[q]); }
-    if (x->ev_write) cudaEventDestroy(x->ev_write);
-    cudaGetLastError();
     delete x;
+    cudaGetLastError();
 }
 
 int kvidx_set_tier_weight(kvidx_t* x, uint32_t tier, double w) {
@@ -1536,7 +1608,7 @@ int kvidx_set_tier_weight(kvidx_t* x, uint32_t tier, double w) {
 
 int kvidx_set_stream(kvidx_t* x, void* s) {
     if (!x) return fail(KVIDX_EINVAL, "NULL handle");
-    ReadGuard g(x);
+    ReadCall c(x);
     x->stream = s ? static_cast<cudaStream_t>(s) : x->own_stream;
     return 0;
 }
@@ -1561,8 +1633,8 @@ int kvidx_hash_keys(kvidx_t* x, const uint32_t* tok, const int64_t* tok_off, int
     key_off_out[n] = nk;
     if (n == 0 || nk == 0) return 0;
     if (!keys_out || !tok) return fail(KVIDX_EINVAL, "NULL buffer");
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
+    ReadCall c(x);
+    if ((rc = c.begin(0))) return rc;
     const int64_t tb = tok_off[0], nt = tok_off[n] - tb;
     CK(x->d_tok[0].need((size_t)nt * 4 + 64));
     CK(x->d_off[0].need((size_t)(n + 1) * 8));
@@ -1587,8 +1659,8 @@ int kvidx_hash_keys_dev(kvidx_t* x, const uint32_t* d_tok, const int64_t* d_tok_
                         const uint8_t* d_parent_valid, const int64_t* d_key_off, uint64_t* d_keys_out) {
     if (!x || n < 0) return fail(KVIDX_EINVAL, "bad arguments");
     if (n == 0) return 0;
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
+    ReadCall c(x);
+    if (int rc = c.begin(0)) return rc;
     return launch_hash_keys(x, d_tok, d_tok_off, 0, n, d_parent, d_parent_valid, d_key_off, d_keys_out, x->stream);
 }
 
@@ -1598,14 +1670,12 @@ int kvidx_lookup(kvidx_t* x, uint32_t model, const uint64_t* keys, int64_t n, co
     if (n <= 0 || !keys) return fail(KVIDX_EINVAL, "no requestKeys provided for lookup");   // in_memory.go:108-110
     if (!podtier_out || !cnt_out) return fail(KVIDX_EINVAL, "NULL output");
     if (model > 0xffffu) return fail(KVIDX_ERANGE, "model id %u > 65535", model);
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
+    ReadCall c(x);
+    if (int rc = c.begin(kShards | kAfterWrites)) return rc;
     const uint32_t FW = x->tv.filter_words;
     uint64_t *d_keys, *d_f; int* d_cut; uint16_t* d_pt; uint8_t* d_cnt;
     CK(carve(x->d_aux[0], [&](Carver& c) { d_keys = c.take<uint64_t>(n); d_f = c.take<uint64_t>(FW); d_cut = c.take<int>(1); }));
     CK(carve(x->d_out[0], [&](Carver& c) { d_pt = c.take<uint16_t>(n * kMaxEnt); d_cnt = c.take<uint8_t>(n); }));
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
     CK(cudaMemcpyAsync(d_keys, keys, (size_t)n * 8, cudaMemcpyHostToDevice, x->stream));
     if (filter) CK(cudaMemcpyAsync(d_f, filter, (size_t)FW * 8, cudaMemcpyHostToDevice, x->stream));
     else d_f = nullptr;
@@ -1628,26 +1698,26 @@ int kvidx_lookup(kvidx_t* x, uint32_t model, const uint64_t* keys, int64_t n, co
 int kvidx_score_batch(kvidx_t* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
                       const uint64_t* filter, double* scores_out, uint8_t* has_keys_out) {
     if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return submit_score(x, tok, ScoreArgs{nullptr, tok_off, 0, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out, nullptr});
+    return submit_score(x, tok, dense_args(tok_off, n, model, model0, filter, scores_out, has_keys_out));
 }
 
 int kvidx_score_batch_sparse(kvidx_t* x, const uint32_t* tok, const int64_t* tok_off, int64_t n, const uint32_t* model, uint32_t model0,
                              const uint64_t* filter, uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out) {
     if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return submit_score(x, tok, ScoreArgs{nullptr, tok_off, 0, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out, nullptr});
+    return submit_score(x, tok, sparse_args(tok_off, n, model, model0, filter, pods_out, scores_out, cnt_out, has_keys_out));
 }
 
 int kvidx_score_batch_dev(kvidx_t* x, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n, const uint32_t* d_model,
                           uint32_t model0, const uint64_t* d_filter, double* d_scores_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_dev(x, ScoreIn{d_tok, false}, ScoreArgs{nullptr, d_tok_off, 0, n, d_model, model0, d_filter, d_scores_out, nullptr, nullptr, nullptr, d_has_keys_out, nullptr});
+    return score_dev(x, ScoreIn{d_tok, false}, dense_args(d_tok_off, n, d_model, model0, d_filter, d_scores_out, d_has_keys_out));
 }
 
 int kvidx_score_batch_sparse_dev(kvidx_t* x, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n, const uint32_t* d_model,
                                  uint32_t model0, const uint64_t* d_filter, uint16_t* d_pods_out, double* d_scores_out,
                                  uint8_t* d_cnt_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0 || !d_pods_out || !d_scores_out || !d_cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_dev(x, ScoreIn{d_tok, false}, ScoreArgs{nullptr, d_tok_off, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr});
+    return score_dev(x, ScoreIn{d_tok, false}, sparse_args(d_tok_off, n, d_model, model0, d_filter, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out));
 }
 
 // ---- Score() from request keys (GetPodScores steps 3-4): not coalesced, every call goes straight through ----
@@ -1655,26 +1725,26 @@ int kvidx_score_batch_sparse_dev(kvidx_t* x, const uint32_t* d_tok, const int64_
 int kvidx_score_keys(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, int64_t n, const uint32_t* model, uint32_t model0,
                      const uint64_t* filter, double* scores_out, uint8_t* has_keys_out) {
     if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_host(x, ScoreIn{keys, true}, ScoreArgs{nullptr, key_off, 0, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out, nullptr});
+    return score_host(x, ScoreIn{keys, true}, dense_args(key_off, n, model, model0, filter, scores_out, has_keys_out));
 }
 
 int kvidx_score_keys_sparse(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, int64_t n, const uint32_t* model, uint32_t model0,
                             const uint64_t* filter, uint16_t* pods_out, double* scores_out, uint8_t* cnt_out, uint8_t* has_keys_out) {
     if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_host(x, ScoreIn{keys, true}, ScoreArgs{nullptr, key_off, 0, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out, nullptr});
+    return score_host(x, ScoreIn{keys, true}, sparse_args(key_off, n, model, model0, filter, pods_out, scores_out, cnt_out, has_keys_out));
 }
 
 int kvidx_score_keys_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n, const uint32_t* d_model,
                          uint32_t model0, const uint64_t* d_filter, double* d_scores_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0 || !d_key_off || !d_scores_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_dev(x, ScoreIn{d_keys, true}, ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, d_scores_out, nullptr, nullptr, nullptr, d_has_keys_out, nullptr});
+    return score_dev(x, ScoreIn{d_keys, true}, dense_args(d_key_off, n, d_model, model0, d_filter, d_scores_out, d_has_keys_out));
 }
 
 int kvidx_score_keys_sparse_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, int64_t n, const uint32_t* d_model,
                                 uint32_t model0, const uint64_t* d_filter, uint16_t* d_pods_out, double* d_scores_out,
                                 uint8_t* d_cnt_out, uint8_t* d_has_keys_out) {
     if (!x || n < 0 || !d_key_off || !d_pods_out || !d_scores_out || !d_cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_dev(x, ScoreIn{d_keys, true}, ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr});
+    return score_dev(x, ScoreIn{d_keys, true}, sparse_args(d_key_off, n, d_model, model0, d_filter, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out));
 }
 
 // ---- Score() for a conversation turn: held keys, then the new turn's tokens; not coalesced either ----
@@ -1709,7 +1779,7 @@ int kvidx_score_turn(kvidx_t* x, const uint64_t* keys, const int64_t* key_off, c
                      const uint32_t* model, uint32_t model0, const uint64_t* filter, double* scores_out, uint8_t* has_keys_out,
                      uint64_t* new_keys_out, int64_t* new_key_off_out) {
     if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_turn_host(x, keys, key_off, tok, tok_off, ScoreArgs{nullptr, key_off, 0, n, model, model0, filter, scores_out, nullptr, nullptr, nullptr, has_keys_out, nullptr},
+    return score_turn_host(x, keys, key_off, tok, tok_off, dense_args(key_off, n, model, model0, filter, scores_out, has_keys_out),
                            new_keys_out, new_key_off_out);
 }
 
@@ -1717,7 +1787,7 @@ int kvidx_score_turn_sparse(kvidx_t* x, const uint64_t* keys, const int64_t* key
                             const uint32_t* model, uint32_t model0, const uint64_t* filter, uint16_t* pods_out, double* scores_out,
                             uint8_t* cnt_out, uint8_t* has_keys_out, uint64_t* new_keys_out, int64_t* new_key_off_out) {
     if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
-    return score_turn_host(x, keys, key_off, tok, tok_off, ScoreArgs{nullptr, key_off, 0, n, model, model0, filter, nullptr, pods_out, scores_out, cnt_out, has_keys_out, nullptr},
+    return score_turn_host(x, keys, key_off, tok, tok_off, sparse_args(key_off, n, model, model0, filter, pods_out, scores_out, cnt_out, has_keys_out),
                            new_keys_out, new_key_off_out);
 }
 
@@ -1726,7 +1796,7 @@ int kvidx_score_turn_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_ke
                          const int64_t* d_new_key_off, uint64_t* d_new_keys_out) {
     if (!x || n < 0 || !d_key_off || !d_tok_off || !d_scores_out || (d_new_keys_out && !d_new_key_off)) return fail(KVIDX_EINVAL, "bad arguments");
     return score_dev(x, turn_dev(d_keys, d_tok, d_tok_off, d_new_key_off, d_new_keys_out),
-                     ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, d_scores_out, nullptr, nullptr, nullptr, d_has_keys_out, nullptr});
+                     dense_args(d_key_off, n, d_model, model0, d_filter, d_scores_out, d_has_keys_out));
 }
 
 int kvidx_score_turn_sparse_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t* d_key_off, const uint32_t* d_tok, const int64_t* d_tok_off,
@@ -1736,7 +1806,7 @@ int kvidx_score_turn_sparse_dev(kvidx_t* x, const uint64_t* d_keys, const int64_
     if (!x || n < 0 || !d_key_off || !d_tok_off || !d_pods_out || !d_scores_out || !d_cnt_out || (d_new_keys_out && !d_new_key_off))
         return fail(KVIDX_EINVAL, "bad arguments");
     return score_dev(x, turn_dev(d_keys, d_tok, d_tok_off, d_new_key_off, d_new_keys_out),
-                     ScoreArgs{nullptr, d_key_off, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr});
+                     sparse_args(d_key_off, n, d_model, model0, d_filter, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out));
 }
 
 // ---- Lookup hit counts: recordHitMetrics(Lookup(K_i, F_i)) per prompt (kernels_hits.cuh) ----
@@ -1782,7 +1852,6 @@ int lookup_hits_host_locked(kvidx* x, const void* el, bool keys, const int64_t* 
         d_koff = c.take<int64_t>(keys ? 0 : n + 1); d_keys = c.take<uint64_t>(keys ? 0 : nk);
     }));
     cudaStream_t st = x->stream;
-    CK(cudaStreamWaitEvent(st, x->ev_write, 0));
     Stager& sg = x->rstage;
     int rc = sg.h2d(d_el, static_cast<const uint8_t*>(el) + (size_t)e0 * esz, (size_t)ne * esz, st);
     if (!rc) rc = sg.h2d(d_off, off, (size_t)(n + 1) * 8, st);
@@ -1808,17 +1877,9 @@ int lookup_hits_host(kvidx* x, const void* el, bool keys, const int64_t* off, in
     if (n == 0) return 0;
     if (int rc = check_csr(off, n, keys ? "key_off" : "tok_off")) return rc;
     if (off[n] > off[0] && !el) return fail(KVIDX_EINVAL, keys ? "NULL keys" : "NULL tokens");
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    if (int rc = check_shards(x)) return rc;
-    const int rc = lookup_hits_host_locked(x, el, keys, off, n, model, model0, filter, hits_out);
-    if (rc) {                                         // copies may still read the caller's buffers: drain before returning
-        const std::string keep = g_err;
-        cudaStreamSynchronize(x->stream);
-        cudaGetLastError();
-        g_err = keep;
-    }
-    return rc;
+    ReadCall c(x);
+    if (int rc = c.begin(kShards | kAfterWrites)) return rc;
+    return c.end(lookup_hits_host_locked(x, el, keys, off, n, model, model0, filter, hits_out), {x->stream});
 }
 }  // namespace
 
@@ -1836,10 +1897,8 @@ int kvidx_lookup_hits_keys_dev(kvidx_t* x, const uint64_t* d_keys, const int64_t
                                uint32_t model0, const uint64_t* d_filter, uint32_t* d_hits_out) {
     if (!x || n < 0 || !d_key_off || !d_hits_out) return fail(KVIDX_EINVAL, "bad arguments");
     if (n == 0) return 0;
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    if (int rc = check_shards(x)) return rc;
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
+    ReadCall c(x);
+    if (int rc = c.begin(kShards | kAfterWrites)) return rc;
     unsigned long long sb = 0;
     if (x->tv.req_stamp) {                            // exact-LRU: a stamp per key, counted from the offsets (as Score() does)
         int64_t e[2];
@@ -1854,11 +1913,9 @@ int kvidx_lookup_hits_dev(kvidx_t* x, const uint32_t* d_tok, const int64_t* d_to
     if (!x || n < 0 || !d_tok_off || !d_hits_out) return fail(KVIDX_EINVAL, "bad arguments");
     if (n == 0) return 0;
     if (n >= (1ll << 31) - 1) return fail(KVIDX_EINVAL, "n_prompts %lld too large for one call", (long long)n);
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    if (int rc = check_shards(x)) return rc;
+    ReadCall c(x);
+    if (int rc = c.begin(kShards | kAfterWrites)) return rc;
     cudaStream_t st = x->stream;
-    CK(cudaStreamWaitEvent(st, x->ev_write, 0));
     int64_t e[2];                                     // the batch's token span sizes the key scratch: >= the keys it holds
     if (int rc = read_ends(d_tok_off, n, e, st)) return rc;
     const int64_t cap = (e[1] - e[0]) / x->tv.block_size;
@@ -1881,8 +1938,8 @@ int kvidx_lookup_hits_dev(kvidx_t* x, const uint32_t* d_tok, const int64_t* d_to
 int kvidx_key_owners_dev(kvidx_t* x, const uint64_t* d_keys, const uint32_t* d_model, uint32_t model0, int64_t n, uint8_t* d_owner_out) {
     if (!x || n < 0) return fail(KVIDX_EINVAL, "bad arguments");
     if (n == 0) return 0;
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
+    ReadCall c(x);
+    if (int rc = c.begin(0)) return rc;
     key_owners_kernel<<<(unsigned)((n + 255) / 256), 256, 0, x->stream>>>(x->tv, d_keys, d_model, model0, n, d_owner_out);
     x->launches += 1;
     CK(cudaGetLastError());
@@ -1892,10 +1949,8 @@ int kvidx_key_owners_dev(kvidx_t* x, const uint64_t* d_keys, const uint32_t* d_m
 int kvidx_probe_slots_dev(kvidx_t* x, const uint64_t* d_keys, const uint32_t* d_model, uint32_t model0, int64_t n, void* d_slots_out) {
     if (!x || n < 0) return fail(KVIDX_EINVAL, "bad arguments");
     if (n == 0) return 0;
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
+    ReadCall c(x);
+    if (int rc = c.begin(kShards | kAfterWrites)) return rc;
     probe_slots_kernel<<<(unsigned)((n + 255) / 256), 256, 0, x->stream>>>(x->tv, d_keys, d_model, model0, n, static_cast<uint4*>(d_slots_out));
     x->launches += 1;
     CK(cudaGetLastError());
@@ -1906,8 +1961,8 @@ int kvidx_score_slots_dev(kvidx_t* x, const void* d_slots, const int64_t* d_key_
                           double* d_scores_out, uint8_t* d_has_keys_out) {
     if (!x || n_prompts < 0 || !d_scores_out) return fail(KVIDX_EINVAL, "bad arguments");
     if (n_prompts == 0) return 0;
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
+    ReadCall c(x);
+    if (int rc = c.begin(0)) return rc;
     score_slots_kernel<<<(unsigned)((n_prompts + 127) / 128), 128, 0, x->stream>>>(x->tv, static_cast<const uint4*>(d_slots), d_key_off, n_prompts, d_filter,
                                                                                    d_scores_out, d_has_keys_out);
     x->launches += 1;
@@ -1932,13 +1987,9 @@ int kvidx_add(kvidx_t* x, uint32_t model, const uint64_t* engine, const uint64_t
     if (n <= 0 || m <= 0 || !engine || !request || !pts) return fail(KVIDX_EINVAL, "no keys or entries provided for adding to index");
     if (model > 0xffffu) return fail(KVIDX_ERANGE, "model id %u > 65535", model);
     if (int rc0 = check_podtiers(x, pts, m)) return rc0;
-    std::lock_guard<std::mutex> g(x->mu_w);
-    x->rm_armed = false;
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
-    int rc = ensure_room(x, (uint64_t)n);
-    if (rc) return rc;
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    WriteCall w(x);
+    if (int rc = w.begin(kDisarm | kShards)) return rc;
+    if (int rc = w.share_with_room((uint64_t)n)) return rc;
     cudaStream_t st = wstream(x);
     uint64_t *d_engine, *d_request; uint16_t* d_pts; uint8_t* d_skip;
     CK(carve(x->d_misc, [&](Carver& c) { d_engine = c.take<uint64_t>(n); d_request = c.take<uint64_t>(n); d_pts = c.take<uint16_t>(m); d_skip = c.take<uint8_t>(n); }));
@@ -1955,16 +2006,13 @@ int kvidx_add(kvidx_t* x, uint32_t model, const uint64_t* engine, const uint64_t
     CK(cudaMemcpyAsync(d_request, request, (size_t)n * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_pts, pts, (size_t)m * 2, cudaMemcpyHostToDevice, st));
     if (any_dup) CK(cudaMemcpyAsync(d_skip, skip, (size_t)n, cudaMemcpyHostToDevice, st));
+    const WriteTally t = w.tally();
     const int T = 128;
     add_kernel<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(x->tv, model, d_engine, d_request, n, d_pts, m, any_dup ? d_skip : nullptr,
                                                          reserve_stamps(x, 2ull * (unsigned long long)n + 2));
     x->launches += 1;
     CK(cudaGetLastError());
-    const unsigned long long nospc_before = x->h_cnt->nospc;
-    rc = refresh_counters(x);
-    if (rc) return rc;
-    if (x->h_cnt->nospc != nospc_before) return fail(KVIDX_ENOSPC, "%llu inserts refused: the owning shard is full", x->h_cnt->nospc - nospc_before);
-    return cap_keys(x);
+    return w.settle(t, nullptr);
 }
 
 int kvidx_evict(kvidx_t* x, uint32_t model, uint64_t engine, const kvidx_podtier_t* pts, int32_t m) {
@@ -1972,11 +2020,9 @@ int kvidx_evict(kvidx_t* x, uint32_t model, uint64_t engine, const kvidx_podtier
     if (m <= 0 || !pts) return fail(KVIDX_EINVAL, "no entries provided for eviction from index");
     if (model > 0xffffu) return fail(KVIDX_ERANGE, "model id %u > 65535", model);
     if (int rc0 = check_podtiers(x, pts, m)) return rc0;
-    std::lock_guard<std::mutex> g(x->mu_w);
-    x->rm_armed = false;
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    WriteCall w(x);
+    if (int rc = w.begin(kDisarm | kShards)) return rc;
+    w.share();
     cudaStream_t st = wstream(x);
     CK(x->d_misc.need((size_t)m * 2 + 16));
     CK(cudaMemcpyAsync(x->d_misc.p, pts, (size_t)m * 2, cudaMemcpyHostToDevice, st));
@@ -1989,13 +2035,11 @@ int kvidx_evict(kvidx_t* x, uint32_t model, uint64_t engine, const kvidx_podtier
 
 int kvidx_get_request_key(kvidx_t* x, uint32_t model, uint64_t engine, uint64_t* out) {
     if (!x || !out) return fail(KVIDX_EINVAL, "bad arguments");
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
+    ReadCall c(x);
+    if (int rc = c.begin(kShards | kAfterWrites)) return rc;
     CK(x->d_rmisc.need(32));
     uint64_t* d_out = x->d_rmisc.as<uint64_t>();
     int* d_found = reinterpret_cast<int*>(d_out + 1);
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
     get_request_key_kernel<<<1, 32, 0, x->stream>>>(x->tv, model, engine, d_out, d_found, x->tv.req_stamp ? reserve_stamps(x, 1) : 0);
     x->launches += 1;
     CK(cudaGetLastError());
@@ -2068,13 +2112,10 @@ int kvidx_apply_events_dev(kvidx_t* x, const kvidx_event_t* d_ev_sorted, const i
                            const uint64_t* d_hashes, int64_t n_hashes, const uint32_t* d_tokens, int64_t* d_n_dropped) {
     if (!x || n_queues < 0 || n_events < 0 || n_hashes < 0) return fail(KVIDX_EINVAL, "bad arguments");
     if (n_queues == 0 || n_events == 0) return 0;
-    std::lock_guard<std::mutex> g(x->mu_w);
-    x->rm_armed = false;
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
-    int rc = ensure_room(x, (uint64_t)n_hashes);       // every hash of the batch may be a new key
+    WriteCall w(x);
+    if (int rc = w.begin(kDisarm | kShards)) return rc;
+    int rc = w.share_with_room((uint64_t)n_hashes);    // every hash of the batch may be a new key
     if (rc) return rc;
-    std::shared_lock<std::shared_mutex> tl(x->tables);
     cudaStream_t st = wstream(x);
     rc = launch_apply_events(x, d_ev_sorted, d_queue_off, n_queues, n_events, d_hashes, n_hashes, d_tokens, st, -1);
     if (rc) return rc;
@@ -2108,13 +2149,9 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
         }
         qcount[KVIDX_PT_POD(e.podtier) + 1]++;
     }
-    std::lock_guard<std::mutex> g(x->mu_w);
-    x->rm_armed = false;
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
-    int rc = ensure_room(x, new_keys);
-    if (rc) return rc;
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    WriteCall w(x);
+    if (int rc = w.begin(kDisarm | kShards)) return rc;
+    if (int rc = w.share_with_room(new_keys)) return rc;
     cudaStream_t st = wstream(x);
     // compact non-empty queues
     std::vector<int64_t> start(KVIDX_MAX_PODS + 1, 0);
@@ -2137,15 +2174,11 @@ int kvidx_apply_events(kvidx_t* x, const kvidx_event_t* ev, int64_t n, const uin
     CK(cudaMemcpyAsync(x->d_qoff.p, qoff, (size_t)(nq + 1) * 8, cudaMemcpyHostToDevice, st));
     if (n_hashes > 0) CK(cudaMemcpyAsync(x->d_hash.p, hashes, (size_t)n_hashes * 8, cudaMemcpyHostToDevice, st));
     if (n_tokens > 0) CK(cudaMemcpyAsync(x->d_evtok.p, tokens, (size_t)n_tokens * 4, cudaMemcpyHostToDevice, st));
-    const unsigned long long dropped_before = x->h_cnt->dropped_events, nospc_before = x->h_cnt->nospc;
-    rc = launch_apply_events(x, x->d_ev.as<kvidx_event_t>(), x->d_qoff.as<int64_t>(), nq, n, x->d_hash.as<uint64_t>(), n_hashes,
-                             x->d_evtok.as<uint32_t>(), st, max_ev_hashes);
-    if (rc) return rc;
-    rc = refresh_counters(x);
-    if (rc) return rc;
-    if (n_dropped_out) *n_dropped_out = (int64_t)(x->h_cnt->dropped_events - dropped_before);
-    if (x->h_cnt->nospc != nospc_before) return fail(KVIDX_ENOSPC, "%llu inserts refused: the owning shard is full", x->h_cnt->nospc - nospc_before);
-    return cap_keys(x);
+    const WriteTally t = w.tally();
+    if (int rc = launch_apply_events(x, x->d_ev.as<kvidx_event_t>(), x->d_qoff.as<int64_t>(), nq, n, x->d_hash.as<uint64_t>(), n_hashes,
+                                     x->d_evtok.as<uint32_t>(), st, max_ev_hashes))
+        return rc;
+    return w.settle(t, n_dropped_out);
 }
 
 }  // extern "C"
@@ -2260,8 +2293,8 @@ int kvidx_decode_event_payloads_dev(kvidx_t* x, const uint8_t* d_bytes, const in
     if (int rc = check_tier_table(tier_bytes, tier_off, n_tiers, gpu_tier)) return rc;
     if (n_msgs == 0) return 0;
     if (!d_bytes || !d_msg_off || !d_msg_pod || !d_msg_model) return fail(KVIDX_EINVAL, "NULL message arrays");
-    std::lock_guard<std::mutex> g(x->mu_w);
-    CK(cudaSetDevice(x->device));
+    WriteCall w(x);
+    if (int rc = w.begin(0)) return rc;
     cudaStream_t st = wstream(x);
     DecodePlan pl;
     pl.in.bytes = d_bytes; pl.in.msg_off = d_msg_off; pl.in.msg_pod = d_msg_pod; pl.in.msg_model = d_msg_model;
@@ -2299,9 +2332,8 @@ int kvidx_apply_event_payloads(kvidx_t* x, const uint8_t* bytes, const int64_t* 
     }
     const uint64_t nb = (uint64_t)(msg_off[n_msgs] - msg_off[0]);
     if (nb && !bytes) return fail(KVIDX_EINVAL, "NULL payload bytes");
-    std::lock_guard<std::mutex> g(x->mu_w);
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
+    WriteCall w(x);
+    if (int rc = w.begin(kShards)) return rc;
     cudaStream_t st = wstream(x);
     // the payloads on the device: bytes, offsets from 0, pods, models
     DecodePlan pl;
@@ -2324,23 +2356,17 @@ int kvidx_apply_event_payloads(kvidx_t* x, const uint8_t* bytes, const int64_t* 
     const DecTotals& t = pl.tot;
     if (t.events == 0) return 0;                       // as kvidx_apply_events with no event
     x->rm_armed = false;
-    if ((rc = ensure_room(x, t.stored_hashes))) return rc;
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    if ((rc = w.share_with_room(t.stored_hashes))) return rc;
     CK(x->d_ev.need((size_t)t.events * sizeof(kvidx_event_t)));
     CK(x->d_qoff.need((size_t)(t.queues + 1) * 8));
     CK(x->d_hash.need((size_t)std::max<uint64_t>(t.hashes, 1) * 8));
     CK(x->d_evtok.need((size_t)std::max<uint64_t>(t.tokens, 1) * 4 + 16));
     if ((rc = decode_write(x, pl, x->d_ev.as<kvidx_event_t>(), x->d_qoff.as<int64_t>(), x->d_hash.as<uint64_t>(), x->d_evtok.as<uint32_t>(), st)))
         return rc;
-    const unsigned long long dropped_before = x->h_cnt->dropped_events, nospc_before = x->h_cnt->nospc;
+    const WriteTally tally = w.tally();
     rc = launch_apply_events(x, x->d_ev.as<kvidx_event_t>(), x->d_qoff.as<int64_t>(), (int64_t)t.queues, (int64_t)t.events,
                              x->d_hash.as<uint64_t>(), (int64_t)t.hashes, x->d_evtok.as<uint32_t>(), st, (int64_t)t.max_ev_hashes);
-    if (rc) return rc;
-    rc = refresh_counters(x);
-    if (rc) return rc;
-    if (n_dropped_out) *n_dropped_out = (int64_t)(x->h_cnt->dropped_events - dropped_before);
-    if (x->h_cnt->nospc != nospc_before) return fail(KVIDX_ENOSPC, "%llu inserts refused: the owning shard is full", x->h_cnt->nospc - nospc_before);
-    return cap_keys(x);
+    return rc ? rc : w.settle(tally, n_dropped_out);
 }
 
 }  // extern "C"
@@ -2404,10 +2430,9 @@ int kvidx_remove_pods(kvidx_t* x, const uint64_t* pod_mask, uint32_t tier_mask, 
     // sharded index needs the removal bitmaps of every rank, which the collective kvidx_shard_remove_pods provides
     if (x->tv.shard_bits) return fail(KVIDX_EINVAL, "kvidx_remove_pods is not supported on a sharded index (kvidx_shard_remove_pods is its collective form)");
     if (int rc = check_removal(x, pod_mask, tier_mask)) return rc;
-    std::lock_guard<std::mutex> g(x->mu_w);
-    x->rm_armed = false;
-    CK(cudaSetDevice(x->device));
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    WriteCall w(x);
+    if (int rc = w.begin(kDisarm)) return rc;
+    w.share();
     return run_removal(x, pod_mask, tier_mask, true, true, removed_out);
 }
 
@@ -2416,9 +2441,8 @@ int kvidx_shard_remove_pods(kvidx_t* x, const uint64_t* pod_mask, uint32_t tier_
     if (phase > 1) return fail(KVIDX_EINVAL, "phase %u: a removal has phases 0 and 1", phase);
     if (int rc = check_removal(x, pod_mask, tier_mask)) return rc;
     const uint32_t FW = x->tv.filter_words;
-    std::lock_guard<std::mutex> g(x->mu_w);
-    CK(cudaSetDevice(x->device));
-    if (int rc = check_shards(x)) return rc;
+    WriteCall w(x);
+    if (int rc = w.begin(kShards)) return rc;
     if (phase == 1) {
         if (!x->rm_armed)
             return fail(KVIDX_EINVAL, "phase 1 without a preceding phase 0 on this handle, or a write call came between the phases");
@@ -2426,7 +2450,7 @@ int kvidx_shard_remove_pods(kvidx_t* x, const uint64_t* pod_mask, uint32_t tier_
             return fail(KVIDX_EINVAL, "phase 1 with other pod / tier masks than phase 0");
     }
     x->rm_armed = false;
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    w.share();
     int rc = run_removal(x, pod_mask, tier_mask, phase == 0, phase == 1, removed_out);
     if (rc || phase == 1) return rc;
     x->rm_armed = true;
@@ -2747,9 +2771,9 @@ int merge_images(const void* const* parts, const std::vector<SnapHeader>& hd, ui
 }
 
 int snapshot_call(kvidx* x, void* buf, uint64_t cap, uint64_t* size_out) {
-    std::lock_guard<std::mutex> g(x->mu_w);
-    CK(cudaSetDevice(x->device));
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    WriteCall w(x);
+    if (int rc = w.begin(0)) return rc;
+    w.share();
     int rc = refresh_counters(x);                     // synchronises the write stream: earlier asynchronous batches are in
     if (rc) return rc;
     const uint64_t R = x->h_cnt->req_full, E = x->h_cnt->eng_full;
@@ -2777,10 +2801,9 @@ int restore_call(kvidx* x, const void* buf, uint64_t len, uint64_t restored_out[
     if (hd.pod_span > x->tv.max_pods) return fail(KVIDX_ERANGE, "snapshot holds pod ids up to %u, max_pods is %u", hd.pod_span - 1, x->tv.max_pods);
     if (hd.model_span > 65536) return fail(KVIDX_EINVAL, "malformed snapshot image: model_span %u", hd.model_span);
     if (x->tv.req_stamp && !rec) return fail(KVIDX_EINVAL, "an exact-LRU index needs an image with recency (taken from an exact-LRU index)");
-    std::lock_guard<std::mutex> g(x->mu_w);
-    x->rm_armed = false;
-    CK(cudaSetDevice(x->device));
-    std::shared_lock<std::shared_mutex> tl(x->tables);
+    WriteCall w(x);
+    if (int rc = w.begin(kDisarm)) return rc;
+    w.share();
     int rc = refresh_counters(x);
     if (rc) return rc;
     if (x->h_cnt->req_full || x->h_cnt->eng_full)
@@ -2861,8 +2884,8 @@ int kvidx_snapshot_merge(const void* const* parts, const uint64_t* lens, uint32_
 
 int kvidx_shard_export(kvidx_t* x, void* out) {
     if (!x || !out) return fail(KVIDX_EINVAL, "bad arguments");
-    std::lock_guard<std::mutex> g(x->mu_w);
-    CK(cudaSetDevice(x->device));
+    WriteCall w(x);
+    if (int rc = w.begin(0)) return rc;
     cudaIpcMemHandle_t h[3];
     CK(cudaIpcGetMemHandle(&h[0], x->tv.req));
     CK(cudaIpcGetMemHandle(&h[1], x->tv.eng));
@@ -2876,9 +2899,9 @@ int kvidx_shard_import(kvidx_t* x, uint32_t rank, const void* handle) {
     if (!x || !handle) return fail(KVIDX_EINVAL, "bad arguments");
     if (rank >= (1u << x->tv.shard_bits)) return fail(KVIDX_ERANGE, "rank %u outside shard_count", rank);
     if (rank == x->tv.shard_rank) return 0;
-    std::lock_guard<std::mutex> g(x->mu_w);
-    std::unique_lock<std::shared_mutex> tl(x->tables);
-    CK(cudaSetDevice(x->device));
+    WriteCall w(x);
+    w.exclusive();
+    if (int rc = w.begin(0)) return rc;
     cudaIpcMemHandle_t h[3];
     memcpy(h, handle, sizeof h);
     void* p[3] = {nullptr, nullptr, nullptr};
@@ -2894,9 +2917,9 @@ int kvidx_shard_attach(kvidx_t* x, uint32_t rank, kvidx_t* other) {
     if (rank == x->tv.shard_rank) return 0;
     if (other->tv.req_mask != x->tv.req_mask || other->tv.shard_bits != x->tv.shard_bits || other->tv.shard_rank != rank)
         return fail(KVIDX_EINVAL, "shard geometry mismatch");
-    std::lock_guard<std::mutex> g(x->mu_w);
-    std::unique_lock<std::shared_mutex> tl(x->tables);
-    CK(cudaSetDevice(x->device));
+    WriteCall w(x);
+    w.exclusive();
+    if (int rc = w.begin(0)) return rc;
     if (other->device != x->device) {
         int can = 0;
         CK(cudaDeviceCanAccessPeer(&can, x->device, other->device));
@@ -2911,10 +2934,9 @@ int kvidx_shard_attach(kvidx_t* x, uint32_t rank, kvidx_t* other) {
 
 int kvidx_shard_compact(kvidx_t* x) {
     if (!x) return fail(KVIDX_EINVAL, "NULL handle");
-    std::lock_guard<std::mutex> g(x->mu_w);
-    x->rm_armed = false;
-    std::unique_lock<std::shared_mutex> tl(x->tables);
-    CK(cudaSetDevice(x->device));
+    WriteCall w(x);
+    w.exclusive();
+    if (int rc = w.begin(kDisarm)) return rc;
     return rebuild(x, x->tv.shard_bits != 0);
 }
 
@@ -2938,15 +2960,14 @@ int kvidx_get_sweeps(kvidx_t* x, uint64_t out[2]) {
 
 int kvidx_get_stats(kvidx_t* x, kvidx_stats_t* out) {
     if (!x || !out) return fail(KVIDX_EINVAL, "bad arguments");
-    std::lock_guard<std::mutex> g(x->mu_w);
-    CK(cudaSetDevice(x->device));
-    int rc = refresh_counters(x);
-    if (rc) return rc;
+    WriteCall w(x);
+    if (int rc = w.begin(0)) return rc;
+    if (int rc = refresh_counters(x)) return rc;
     out->request_keys = x->h_cnt->req_full; out->engine_keys = x->h_cnt->eng_full;
     out->request_tombs = x->h_cnt->req_tomb; out->engine_tombs = x->h_cnt->eng_tomb;
     out->request_slots = x->tv.req_mask + 1; out->engine_slots = x->tv.eng_mask + 1;
     out->rebuilds = x->rebuilds; out->kernel_launches = x->launches.load();
-    out->rehashed_events = x->h_cnt->rehashed; out->coalesced_calls = x->queue ? submit_queue_coalesced(x->queue) : 0;
+    out->rehashed_events = x->h_cnt->rehashed; out->coalesced_calls = x->queue ? submit_queue_coalesced(x->queue.get()) : 0;
     return 0;
 }
 
@@ -2958,15 +2979,13 @@ int kvidx_pod_inventory(kvidx_t* x, uint32_t model, uint32_t flags, uint64_t* en
     if (!entries_out && !keys_out && !sole_out && !sole_engine_out && !totals_out) return fail(KVIDX_EINVAL, "every output is NULL");
     if (flags & ~KVIDX_INVENTORY_ENGINE) return fail(KVIDX_EINVAL, "unknown inventory flags 0x%x", flags);
     if (model != KVIDX_ANY_MODEL && model > 0xffffu) return fail(KVIDX_ERANGE, "model id %u > 65535", model);
-    ReadGuard g(x);
-    CK(cudaSetDevice(x->device));
-    if (int rc0 = check_shards(x)) return rc0;
+    ReadCall c(x);
+    if (int rc = c.begin(kShards | kAfterWrites)) return rc;
     const size_t P = x->tv.max_pods, n_ent = P * KVIDX_MAX_TIERS, words = n_ent + 3 * P + 4;
     CK(x->d_inv.need(words * 8));
     CK(x->h_inv.need(words * 8));
     unsigned long long* d = x->d_inv.as<unsigned long long>();
     InvArgs ia{model, d, d + n_ent, d + n_ent + P, d + n_ent + 2 * P, d + n_ent + 3 * P};
-    CK(cudaStreamWaitEvent(x->stream, x->ev_write, 0));
     CK(cudaMemsetAsync(d, 0, words * 8, x->stream));
     auto ctas = [&](uint64_t slots) { return (unsigned)std::min<uint64_t>((slots + kInvThreads - 1) / kInvThreads, (uint64_t)x->sm_count * 8); };
     inventory_req_kernel<<<ctas(x->tv.req_mask + 1), kInvThreads, inv_req_smem(x->tv.max_pods), x->stream>>>(x->tv, ia);
@@ -2987,34 +3006,9 @@ int kvidx_pod_inventory(kvidx_t* x, uint32_t model, uint32_t flags, uint64_t* en
 }  // extern "C"
 
 // ---- the device prefix store (kvidx_text_store_*, kernels_text.cuh) -----------------------------------------------------
-struct TextStore {
-    int64_t cap_blocks = 0; uint32_t B = 0;
-    cudaStream_t stream = nullptr;            // kvidx_text_store_add / _find (Score() from text runs on the handle's stream)
-    cudaEvent_t ev_last = nullptr;            // the end of the last store call, on whichever stream it ran: the next one waits
-    Stager stage;                             // for pageable host buffers
-    PinBuf h_misc;
-    TextTable t{};
-    void* tab = nullptr;                      // the table's arrays, one allocation
-    uint32_t* arena = nullptr; int64_t arena_cap = 0, arena_used = 0;
-    int64_t resident = 0;
-    unsigned long long clock = 0;             // recency stamps handed out so far
-    DevBuf d_in, d_blk, d_scr, d_tok, d_cub, d_out;
-};
-
 namespace {
 
 constexpr int64_t kTextLaneMax = 16384;       // batches below this many prompts hash with 4 lanes per prompt, larger ones with 1
-
-void delete_text_store(TextStore* s) {
-    if (!s) return;
-    if (s->tab) cudaFree(s->tab);
-    if (s->arena) cudaFree(s->arena);
-    s->d_in.release(); s->d_blk.release(); s->d_scr.release(); s->d_tok.release(); s->d_cub.release(); s->d_out.release();
-    s->stage.release(); s->h_misc.release();
-    if (s->ev_last) cudaEventDestroy(s->ev_last);
-    if (s->stream) cudaStreamDestroy(s->stream);
-    delete s;
-}
 
 int nomem(cudaError_t e, const char* what) {
     cudaGetLastError();
@@ -3376,11 +3370,11 @@ int text_upload(TextStore* s, const uint8_t* text, const int64_t* text_off, int6
 struct TextCall {
     std::unique_lock<std::mutex> lk;
     TextStore* s; cudaStream_t st;
-    TextCall(kvidx* x, cudaStream_t stream) : lk(x->mu_text), s(x->text), st(stream) {}
+    TextCall(kvidx* x, cudaStream_t stream) : lk(x->mu_text), s(x->text.get()), st(stream) {}
     int begin(kvidx* x) { CK(cudaSetDevice(x->device)); CK(cudaStreamWaitEvent(st, s->ev_last, 0)); return 0; }
     // after an error: let nothing of this call run on past the return (the caller's buffers, the store's scratch)
     int end(int rc) {
-        if (rc) { const std::string keep = g_err; cudaStreamSynchronize(st); cudaGetLastError(); g_err = keep; }
+        ReadCall::end(rc, {st});
         cudaEventRecord(s->ev_last, st);
         return rc;
     }
@@ -3396,8 +3390,8 @@ int score_text_run(kvidx* x, TextStore* s, const TextIn& in, double min_ratio, S
     if (tokenize) CK(cudaMemcpyAsync(tokenize, f.tokenize, (size_t)in.n, cudaMemcpyDeviceToDevice, st));
     if (ratio) CK(cudaMemcpyAsync(ratio, f.ratio, (size_t)in.n * 8, cudaMemcpyDeviceToDevice, st));
     a.tok_off = f.score_off; a.tok_base = 0; a.n_prompts = in.n;
-    ReadGuard g(x);
-    CK(cudaStreamWaitEvent(st, x->ev_write, 0));
+    ReadCall c(x);                                    // lock order: mu_text (the caller's TextCall), then the read side's
+    if (int rc = c.begin(kAfterWrites, st)) return rc;
     return launch_score(x, ScoreIn{s->d_tok.p, false}, a, st);
 }
 
@@ -3412,7 +3406,7 @@ int score_text_host(kvidx* x, const uint8_t* text, const int64_t* text_off, int6
     const uint32_t FW = x->tv.filter_words;
     const RowLayout rows{x->tv.max_pods, h.sp_cnt != nullptr};
     // on the device after the text: the model ids and filter rows (when the call has them), the rows, ratios and flags
-    ScoreArgs a{nullptr, nullptr, 0, n, nullptr, model0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    ScoreArgs a = dense_args(nullptr, n, nullptr, model0, nullptr, nullptr, nullptr);
     uint32_t* d_model; uint64_t* d_filter; double* d_ratio; uint8_t* d_tokz;
     TextIn in{};
     int rc = text_upload(s, text, text_off, n, &in, c.st, [&](Carver& cv) {
@@ -3455,19 +3449,18 @@ int kvidx_text_store_init(kvidx_t* x, int64_t cache_blocks, int32_t block_bytes)
     std::lock_guard<std::mutex> g(x->mu_text);
     if (x->text) return fail(KVIDX_EINVAL, "prefix store already initialised on this handle");
     CK(cudaSetDevice(x->device));
-    TextStore* s = new TextStore();
+    auto s = std::make_unique<TextStore>();         // a store that fails to initialise is freed on the way out
     s->cap_blocks = cache_blocks; s->B = (uint32_t)block_bytes;
-    auto bail = [&](int rc) { delete_text_store(s); return rc; };
-    if (cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&s->ev_last, cudaEventDisableTiming) != cudaSuccess ||
+    if (cudaStreamCreateWithFlags(&s->stream.h, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&s->ev_last.h, cudaEventDisableTiming) != cudaSuccess ||
         s->stage.init() != cudaSuccess)
-        return bail(fail(KVIDX_ECUDA, "prefix store: stream / event creation failed"));
-    if (int rc = text_table_alloc(s, 1024, &s->t, &s->tab, s->stream)) return bail(rc);
+        return fail(KVIDX_ECUDA, "prefix store: stream / event creation failed");
+    if (int rc = text_table_alloc(s.get(), 1024, &s->t, &s->tab, s->stream)) return rc;
     s->arena_cap = 1 << 16;
-    if (cudaError_t e = cudaMalloc((void**)&s->arena, (size_t)s->arena_cap * 4)) return bail(nomem(e, "token arena"));
-    if (s->h_misc.need(64) != cudaSuccess) return bail(fail(KVIDX_ENOMEM, "prefix store: pinned scratch"));
+    if (cudaError_t e = cudaMalloc((void**)&s->arena, (size_t)s->arena_cap * 4)) return nomem(e, "token arena");
+    if (s->h_misc.need(64) != cudaSuccess) return fail(KVIDX_ENOMEM, "prefix store: pinned scratch");
     if (cudaEventRecord(s->ev_last, s->stream) != cudaSuccess || cudaStreamSynchronize(s->stream) != cudaSuccess)
-        return bail(fail(KVIDX_ECUDA, "prefix store: initialisation failed"));
-    x->text = s;
+        return fail(KVIDX_ECUDA, "prefix store: initialisation failed");
+    x->text = std::move(s);
     return 0;
 }
 
@@ -3590,7 +3583,7 @@ int kvidx_score_text(kvidx_t* x, const uint8_t* text, const int64_t* text_off, i
                      const uint64_t* filter, double min_ratio, double* scores_out, uint8_t* has_keys_out, uint8_t* tokenize_out, double* ratio_out) {
     if (!x || !scores_out) return fail(KVIDX_EINVAL, "bad arguments");
     return score_text_host(x, text, text_off, n, model, model0, filter, min_ratio,
-                           ScoreArgs{nullptr, nullptr, 0, n, nullptr, model0, nullptr, scores_out, nullptr, nullptr, nullptr, has_keys_out, nullptr},
+                           dense_args(nullptr, n, nullptr, model0, nullptr, scores_out, has_keys_out),
                            tokenize_out, ratio_out);
 }
 
@@ -3599,7 +3592,7 @@ int kvidx_score_text_sparse(kvidx_t* x, const uint8_t* text, const int64_t* text
                             uint8_t* has_keys_out, uint8_t* tokenize_out, double* ratio_out) {
     if (!x || !pods_out || !scores_out || !cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
     return score_text_host(x, text, text_off, n, model, model0, filter, min_ratio,
-                           ScoreArgs{nullptr, nullptr, 0, n, nullptr, model0, nullptr, nullptr, pods_out, scores_out, cnt_out, has_keys_out, nullptr},
+                           sparse_args(nullptr, n, nullptr, model0, nullptr, pods_out, scores_out, cnt_out, has_keys_out),
                            tokenize_out, ratio_out);
 }
 
@@ -3608,7 +3601,7 @@ int kvidx_score_text_dev(kvidx_t* x, const uint8_t* d_text, const int64_t* d_tex
                          double* d_ratio_out) {
     if (!x || !d_scores_out) return fail(KVIDX_EINVAL, "bad arguments");
     return score_text_dev(x, d_text, d_text_off, n, min_ratio,
-                          ScoreArgs{nullptr, nullptr, 0, n, d_model, model0, d_filter, d_scores_out, nullptr, nullptr, nullptr, d_has_keys_out, nullptr},
+                          dense_args(nullptr, n, d_model, model0, d_filter, d_scores_out, d_has_keys_out),
                           d_tokenize_out, d_ratio_out);
 }
 
@@ -3617,7 +3610,7 @@ int kvidx_score_text_sparse_dev(kvidx_t* x, const uint8_t* d_text, const int64_t
                                 uint8_t* d_has_keys_out, uint8_t* d_tokenize_out, double* d_ratio_out) {
     if (!x || !d_pods_out || !d_scores_out || !d_cnt_out) return fail(KVIDX_EINVAL, "bad arguments");
     return score_text_dev(x, d_text, d_text_off, n, min_ratio,
-                          ScoreArgs{nullptr, nullptr, 0, n, d_model, model0, d_filter, nullptr, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out, nullptr},
+                          sparse_args(nullptr, n, d_model, model0, d_filter, d_pods_out, d_scores_out, d_cnt_out, d_has_keys_out),
                           d_tokenize_out, d_ratio_out);
 }
 
