@@ -481,8 +481,8 @@ int kvidx_restore(kvidx_t* idx, const void* buf, uint64_t len, uint64_t restored
 int kvidx_set_stream(kvidx_t* idx, void* cuda_stream);
 int kvidx_synchronize(kvidx_t* idx);
 
-/* Score() over device-resident inputs and outputs, launched on the handle's stream.  Batches below 4096 prompts
- * (KVIDX_ROUNDS_MIN) are a single asynchronous kernel; larger ones run the round pipelines, which wait on the stream ONCE at the start (the number
+/* Score() over device-resident inputs and outputs, launched on the handle's stream.  Batches up to 2048 prompts
+ * (KVIDX_COOP_MAX) are a single asynchronous kernel; larger ones run the round pipelines, which wait on the stream ONCE at the start (the number
  * of rounds is the longest prompt's block count, computed on the device) and are asynchronous after that.  Results are
  * complete when the stream reaches the point after the call (kvidx_synchronize, or an event recorded by the caller). */
 int kvidx_score_batch_dev(kvidx_t* idx, const uint32_t* d_tok, const int64_t* d_tok_off, int64_t n_prompts,

@@ -662,7 +662,7 @@ __device__ __forceinline__ void resolve_round(const TableView& t, const ScoreArg
 // Lane per partial follower.  It shares the first d blocks of the chunk with representative R (same walk state before,
 // same tokens): if R's walk ended inside those blocks, so does this one, with R's result.  Otherwise it resumes from
 // R's snapshot after block d-1 and R's key of that block, and walks the rest of its chunk by itself -- hash one block,
-// probe it, score it (the order of the fused kernel) -- which normally ends at the first block it does not share.
+// probe it, score it -- which normally ends at the first block it does not share.
 __device__ __forceinline__ uint64_t hash_block16(uint64_t parent, const uint32_t* __restrict__ tk) {
     Fnv f;
     f.begin_block(parent, 16);

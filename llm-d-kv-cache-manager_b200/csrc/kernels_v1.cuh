@@ -1,6 +1,6 @@
 // kernels_v1.cuh -- first-correct kernels: one thread per prompt / key / queue, tokens read
-// straight from global memory.  Kept as the in-library cross-check for the tuned kernels
-// (KVIDX_SCORE_KERNEL=v1) and used for the small, latency-insensitive entry points.
+// straight from global memory.  Kept as the in-library cross-check for the warp-per-prompt
+// and round-pipeline kernels (KVIDX_SCORE_KERNEL=v1) and used for the small, latency-insensitive entry points.
 #pragma once
 #include "score_common.cuh"
 

@@ -25,7 +25,6 @@
 #include "kernels_remove.cuh"
 #include "kernels_snapshot.cuh"
 #include "kernels_inventory.cuh"
-#include "kernels_score.cuh"
 #include "kernels_rounds.cuh"
 #include "kernels_rounds_plain.cuh"
 #include "kernels_coop.cuh"
@@ -279,16 +278,15 @@ struct kvidx {
     int write_phase1 = -1;          // -1: by batch size, 0: never, 1: always (phase 1 = hash_events_kernel)
     int64_t write_phase1_min = 1024; // engine hashes in a batch from which phase 1 pays
     int score_kernel = 2;          // 1 = v1 (thread per prompt, global tokens), 2 = tuned
-    int score_path = 0;            // 0 = by batch size, 1 = always the fused persistent kernel, 2 / 3 = always the plain / class round pipeline,
+    int score_path = 0;            // 0 = by batch size, 2 / 3 = always the plain / class round pipeline,
                                    // 4 = always the warp-per-prompt cooperative kernel
     int64_t coop_max = 2048;       // batches up to this many prompts use the warp-per-prompt cooperative kernel
     int64_t zerocopy_max = 32;     // host-buffer calls up to this many prompts skip the copy engine (tokens read from pinned host memory)
     std::unique_ptr<SubmitQueue> queue;    // coalesces concurrent host-buffer Score() callers (submit.cuh)
     // Batch-size thresholds, from a sweep of the forced paths on an H100 SXM (10 M-block index, bench.py's query mix): the
-    // warp-per-prompt rounds beat the cooperative kernel from 4096 prompts (tie at 2048) and the fused kernel at every size
-    // from 2048 up; the class pipeline beats them from 131 072 prompts.
-    int64_t rounds_min = 2048;     // batches at least this large (and above coop_max) use the round pipeline
-    int64_t classes_min = 131072;  // ... and at least this large, the prefix-class round pipeline
+    // warp-per-prompt rounds beat the cooperative kernel from 4096 prompts (tie at 2048); the class pipeline beats them from
+    // 131 072 prompts.
+    int64_t classes_min = 131072;  // batches at least this large (and above coop_max) use the prefix-class round pipeline
     double classes_min_sharing = 0.85;   // ... if at least this fraction of the batch follows a representative in round 0
     DevBuf d_rounds;               // the round pipelines' scratch, carved per batch (ClassPlan / PlainPlan)
     int64_t host_chunk_tokens = 32ll << 20;   // tokens per H2D chunk of the host-buffer pipeline
@@ -910,7 +908,7 @@ ScoreArgs sparse_args(const int64_t* off, int64_t n, const uint32_t* model, uint
 // So does KVIDX_SCORE_KERNEL=v1 as the cross-check, and so do token prompts of a block size the other token kernels' staging
 // is not written for: every size but 16, 32, 64 and 128.  At 32, 64 and 128 only the warp-per-prompt kernel
 // (coop_score_kernel) is built, so a token batch of n prompts takes it where it would at 16 (n <= coop_max, or
-// KVIDX_SCORE_PATH=coop) and v1 otherwise; the round pipelines and the fused kernel are 16-token only.
+// KVIDX_SCORE_PATH=coop) and v1 otherwise; the round pipelines are 16-token only.
 bool score_takes_v1(const kvidx* x, bool keys, int64_t n) {
     if (x->score_kernel == 1 || x->tv.req_stamp) return true;
     if (keys || x->tv.block_size == 16) return false;
@@ -976,15 +974,13 @@ int launch_score(kvidx* x, const ScoreIn& in, ScoreArgs a, cudaStream_t st, int6
             coop_score_kernel<bs.value><<<(unsigned)ctas, kCoopThreads, sizeof(CoopSmem<bs.value>), st>>>(x->tv, a);
         });
         x->launches += 1;
-    } else if (n < (1ll << 31) && ((x->score_path >= 2 && x->score_path <= 3) || (x->score_path == 0 && n >= x->rounds_min))) {
+    } else if (n < (1ll << 31)) {
         // path 2: plain rounds, 3: prefix classes; automatic: by batch size (the class pipeline has a fixed cost per round)
         const bool classes = x->score_path == 3 || (x->score_path == 0 && n >= x->classes_min);
         return classes ? launch_score_rounds(x, a, st, max_blocks) : launch_score_rounds_plain(x, a, st, max_blocks);
     } else {
-        uint64_t nl = 0;
-        int rc = launch_score_tuned(x->tv, x->sm_count, a, &x->d_cnt->pad, st, &nl);
-        x->launches += nl;
-        if (rc) return fail(KVIDX_ECUDA, "score launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+        // the round pipelines index prompts with 32 bits; the thread-per-prompt kernel indexes them with 64
+        if (int rc = launch_score_v1(x, a, a.tok, st)) return rc;
     }
     CK(cudaGetLastError());
     return 0;
@@ -1518,10 +1514,9 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     t.req_peer[t.shard_rank] = t.req; t.eng_peer[t.shard_rank] = t.eng; t.cnt_peer[t.shard_rank] = t.cnt;
     CK(cudaStreamSynchronize(x->stream));
     if (const char* k = getenv("KVIDX_SCORE_KERNEL")) x->score_kernel = (k[0] == 'v' ? atoi(k + 1) : atoi(k)) == 1 ? 1 : 2;
-    if (const char* k = getenv("KVIDX_SCORE_PATH")) x->score_path = !strcmp(k, "fused") ? 1 : !strcmp(k, "rounds") ? 2 : !strcmp(k, "classes") ? 3 : !strcmp(k, "coop") ? 4 : 0;
+    if (const char* k = getenv("KVIDX_SCORE_PATH")) x->score_path = !strcmp(k, "rounds") ? 2 : !strcmp(k, "classes") ? 3 : !strcmp(k, "coop") ? 4 : 0;
     if (const char* k = getenv("KVIDX_COOP_MAX")) x->coop_max = atoll(k);
     if (const char* k = getenv("KVIDX_ZEROCOPY_MAX")) x->zerocopy_max = atoll(k);
-    if (const char* k = getenv("KVIDX_ROUNDS_MIN")) x->rounds_min = atoll(k);
     if (const char* k = getenv("KVIDX_CLASSES_MIN")) x->classes_min = atoll(k);
     if (const char* k = getenv("KVIDX_CLASSES_SHARING")) x->classes_min_sharing = atof(k);
     if (const char* k = getenv("KVIDX_SORT_PREFIX")) x->sort_prefix = atoi(k) != 0;
@@ -1535,7 +1530,6 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
     if (const char* k = getenv("KVIDX_WRITE_PHASE1")) x->write_phase1 = atoi(k);
     x->queue = new_submit_queue();
     if (rounds_init() || plain::rounds_init() || coop_init() || turn_init()) return fail(KVIDX_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (score_tuned_init()) return fail(KVIDX_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaGetLastError()));
     return 0;
 }
 }  // namespace

@@ -69,7 +69,6 @@ struct ScoreArgs {
     const uint32_t* tok; const int64_t* tok_off; int64_t tok_base; int64_t n_prompts;
     const uint32_t* model; uint32_t model0; const uint64_t* filter;
     double* dense; uint16_t* sp_pods; double* sp_scores; uint8_t* sp_cnt; uint8_t* has_keys;
-    unsigned long long* next;      // global work counter (zeroed before launch)
 };
 
 __device__ __forceinline__ bool filter_has(const uint64_t* __restrict__ frow, uint32_t pod) {

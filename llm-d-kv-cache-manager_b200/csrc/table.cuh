@@ -79,13 +79,12 @@ struct Counters {
     unsigned long long dropped_events;     // BlockStored with key-count mismatch (in_memory.go:153-155)
     unsigned long long nospc;              // inserts refused because the owning shard is full
     unsigned long long clock;              // recency clock (exact-LRU mode)
-    unsigned long long pad;                // work counter of the fused score kernel
     unsigned long long rehashed;           // write path: events whose parent resolved differently from the prediction
     unsigned long long cap_evicted[2];     // request keys / engine mappings dropped by the capacity bound (CLOCK or exact LRU)
     unsigned long long hand[2];            // CLOCK mode: the sweep's hand in the request / engine table (a rebuild resets it)
     unsigned long long sweeps;             // CLOCK mode: sweeps that evicted (both tables) ...
     unsigned long long turns2;             // ... and those of them that went past a full turn of the hand
-    unsigned long long rsv[1];
+    unsigned long long rsv[2];
 };
 static_assert(sizeof(Counters) == 16 * 8, "counter block layout");
 

@@ -57,5 +57,5 @@ if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] != "all":
         run(sys.argv[1])
     else:
-        for p in ("coop", "fused", "auto"):
+        for p in ("coop", "auto"):
             subprocess.check_call([sys.executable, os.path.abspath(__file__), p] + sys.argv[2:])

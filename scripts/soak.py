@@ -13,7 +13,7 @@ import numpy as np
 
 def one(seed):
     rng = np.random.default_rng(seed)
-    cfg = [("classes", "1"), ("classes", "2"), ("classes", "8"), ("rounds", "2"), ("classes", "4"), ("coop", "1"), ("coop", "1"), ("fused", "1")][int(rng.integers(0, 8))]
+    cfg = [("classes", "1"), ("classes", "2"), ("classes", "8"), ("rounds", "2"), ("classes", "4"), ("coop", "1"), ("coop", "1")][int(rng.integers(0, 7))]
     os.environ["KVIDX_ROUNDS_WARP_MAX"] = ("0", "131072")[int(rng.integers(0, 2))]   # per-prompt rounds: lane- / warp-per-prompt walk kernel
     os.environ["KVIDX_ZEROCOPY_MAX"] = str(int(rng.choice([0, 32])))
     os.environ["KVIDX_SCORE_PATH"] = cfg[0]

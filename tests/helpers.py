@@ -172,7 +172,7 @@ def _index_pair(**kw):
 
 
 def _select_path(monkeypatch, path):
-    """v1: thread-per-prompt kernel; fused: persistent lane-worker kernel; rounds*: hash / walk rounds, every prompt on
+    """v1: thread-per-prompt kernel; rounds*: hash / walk rounds, every prompt on
     its own (one stream / two halves on two streams / without the prefix sort); classes*: the round pipeline that hashes
     and walks one representative per distinct prefix (one part / 2 / 8 / 16 parts / unsorted / sharing switched off /
     whole chunks only, no partial followers; the variants also with the batch split into parts)."""
@@ -180,8 +180,8 @@ def _select_path(monkeypatch, path):
         monkeypatch.setenv("KVIDX_SCORE_KERNEL", "v1")
         return
     if path == "auto":                       # the library chooses: here every batch is "large", so it is the class pipeline
-        monkeypatch.setenv("KVIDX_ROUNDS_MIN", "1")        # or the per-prompt rounds, by how much the batch repeats itself
-        monkeypatch.setenv("KVIDX_COOP_MAX", "0")          # (small batches would otherwise take the warp-per-prompt kernel)
+        monkeypatch.setenv("KVIDX_COOP_MAX", "0")          # or the per-prompt rounds, by how much the batch repeats itself
+                                                           # (small batches would otherwise take the warp-per-prompt kernel)
         monkeypatch.setenv("KVIDX_CLASSES_MIN", "64")
         monkeypatch.setenv("KVIDX_ROUNDS_OVERLAP_MIN", "64")
         return
@@ -207,4 +207,9 @@ def _select_path(monkeypatch, path):
 ROUND_PATHS = ["rounds", "rounds2", "rounds-nosort", "rounds2-nosort", "rounds-lane", "rounds2-lane", "classes", "classes2", "classes8",
                "classes16", "classes-nosort", "classes2-nosort", "classes8-nosort", "classes-nodedup", "classes2-nodedup",
                "classes8-nodedup", "classes-whole", "classes2-whole", "classes4-whole", "classes8-whole", "auto"]
-PATHS = ["v1", "fused", "coop"] + ROUND_PATHS
+PATHS = ["v1", "coop"] + ROUND_PATHS
+# Tests seed a path's random inputs from its position in one of these lists.  Both keep "fused", a Score() kernel since
+# retired, so that every remaining path keeps the inputs it has always been checked on: SEED_ORDER for PATHS,
+# SEED_ORDER_SIZES for the sorted names of test_gpu_remove_pods.PATH_SIZES.
+SEED_ORDER = ["v1", "fused", "coop"] + ROUND_PATHS
+SEED_ORDER_SIZES = ["auto", "classes", "coop", "default", "fused", "rounds", "v1"]

@@ -10,7 +10,7 @@ import pytest
 import kvidx
 import snapshot_oracle as so
 from clock_oracle import referenced_keys
-from helpers import EVENT_DTYPE, PATHS, _select_path, csr
+from helpers import EVENT_DTYPE, PATHS, SEED_ORDER, _select_path, csr
 from kvidx.host import HostIndexer
 from oracle import kvoracle as ko
 
@@ -187,7 +187,7 @@ def _second_chance(ix, rng, n_queries, k_less, with_filters=True):
 @pytest.mark.parametrize("path", PATHS)
 def test_second_chance_on_every_path(path, monkeypatch):
     _select_path(monkeypatch, path)
-    rng = np.random.default_rng(PATHS.index(path) + 100)
+    rng = np.random.default_rng(SEED_ORDER.index(path) + 100)
     _second_chance(clock_index(1024), rng, 300, 0)
     _second_chance(clock_index(1024), rng, 300, 17)
 
@@ -294,10 +294,10 @@ def test_restore_cuts_to_capacity():
 
 
 # ---- 3. bound under random streams ------------------------------------------------------------------------------------
-@pytest.mark.parametrize("path", ["v1", "fused", "coop", "rounds", "rounds-lane", "classes", "classes8-nodedup"])
+@pytest.mark.parametrize("path", ["v1", "coop", "rounds", "rounds-lane", "classes", "classes8-nodedup"])
 def test_random_stream_stays_bounded(path, monkeypatch):
     _select_path(monkeypatch, path)
-    rng = np.random.default_rng(PATHS.index(path) + 300)
+    rng = np.random.default_rng(SEED_ORDER.index(path) + 300)
     CAP = 1024
     ix = clock_index(CAP)
     docs = [rng.integers(0, 128256, size=BS * int(rng.integers(2, 24))).tolist() for _ in range(400)]

@@ -217,7 +217,7 @@ def _random_stream(rng, n_steps, BS, P, NT, docs, model=0):
     return np.array(ev, EVENT_DTYPE), np.array(hs, np.uint64), np.array(tk, np.uint64).astype(np.uint32)
 
 
-@pytest.mark.parametrize("seed,BS,path", [(11, 16, "fused"), (12, 16, "rounds"), (13, 4, "fused"), (14, 16, "classes"), (15, 16, "coop")])
+@pytest.mark.parametrize("seed,BS,path", [(11, 16, "v1"), (12, 16, "rounds"), (13, 4, "v1"), (14, 16, "classes"), (15, 16, "coop")])
 def test_random_event_stream_and_queries_vs_cpp_oracle(seed, BS, path, monkeypatch):
     """Differential test on a few thousand events (sequential replay => identical linearisation)."""
     _select_path(monkeypatch, path)
@@ -331,7 +331,7 @@ def test_config2_at_its_stated_size():
     assert np.array_equal(k1, k2)
 
 
-@pytest.mark.parametrize("kernel", ["fused", "coop", "rounds2", "classes", "classes8"])
+@pytest.mark.parametrize("kernel", ["coop", "rounds2", "classes", "classes8"])
 def test_synth_config3_shape_long_prompts(kernel, monkeypatch):
     """BASELINE config #3 shape at reduced N: 8192-token prompts (512 blocks = 16 rounds), 256 pods."""
     _select_path(monkeypatch, kernel)
@@ -348,9 +348,9 @@ def test_synth_config3_shape_long_prompts(kernel, monkeypatch):
     assert m.max() > 480                                   # some walks go through (nearly) all 16 rounds
 
 
-@pytest.mark.parametrize("kernel", ["fused", "coop"] + ROUND_PATHS)
-def test_tuned_kernel_ragged_misaligned_and_many_prompts(kernel, monkeypatch):
-    """Lane refill / round lists, unaligned prompt starts (per-lane staging fallback), empty and sub-block
+@pytest.mark.parametrize("kernel", ["v1", "coop"] + ROUND_PATHS)
+def test_ragged_misaligned_and_many_prompts(kernel, monkeypatch):
+    """Round lists, unaligned prompt starts (per-lane staging fallback), empty and sub-block
     prompts, pod filters, against the oracle."""
     _select_path(monkeypatch, kernel)
     rng = np.random.default_rng(31)

@@ -25,7 +25,7 @@ import pytest
 
 import kvidx
 import snapshot_oracle as so
-from helpers import EVENT_DTYPE, PATHS, SNAP_REQ_DTYPE, _select_path
+from helpers import EVENT_DTYPE, PATHS, SEED_ORDER, SNAP_REQ_DTYPE, _select_path
 from history_oracle import Checker, History, Window
 from oracle import kvoracle as ko
 from oracle.kvoracle_c import COracle
@@ -450,7 +450,8 @@ def _evidence_ok(evidence, n_handles, kinds, rebuilds=True):
             assert ev["rebuild"], "handle %d: no read overlapped a rebuild (%s)" % (h, ev)
 
 
-GROUPS = [PATHS[i::4] for i in range(4)]
+# the groups as they were cut from helpers.SEED_ORDER, so that each path keeps its group and the group's seeds
+GROUPS = [[p for p in SEED_ORDER[i::4] if p in PATHS] for i in range(4)]
 
 
 @pytest.mark.parametrize("group", range(4))
@@ -464,7 +465,8 @@ def test_every_score_path_beside_the_writer(group, monkeypatch):
     writer = Writer(work, handles, np.random.default_rng(group), ALL_KINDS)
     reads = Reads()
     rng = [np.random.default_rng(100 + h) for h in range(len(handles))]
-    readers = [_score_reader(work, ix, h, reads, rng[h], 4096, Until(writer, h, 3, KINDS, rebuild=True))
+    # a fast path makes dozens of calls before the writer's cycle has reached every kind on its handle: it reads on until then
+    readers = [_score_reader(work, ix, h, reads, rng[h], 4096, Until(writer, h, 3, KINDS, rebuild=True, cap=400))
                for h, ix in enumerate(handles)]
     _race(work, writer, readers, 40)
     hist = writer.history(work)

@@ -7,7 +7,7 @@ import msgpack
 import numpy as np
 import pytest
 
-from helpers import EVENT_DTYPE, csr
+from helpers import EVENT_DTYPE, SEED_ORDER_SIZES, csr
 import kvidx
 from kvidx.host import HostIndexer
 from oracle import kvoracle as ko
@@ -91,7 +91,7 @@ def _prompts(rng, docs, n, BS):
 
 # batch sizes on both sides of the dispatch thresholds: 2048 / 2049 prompts straddle the cooperative kernel's limit and the
 # round pipeline's start; "auto" lowers the class pipeline's start to 64 prompts (tests/test_gpu_parity.py _select_path)
-PATH_SIZES = {"v1": (1, 32), "fused": (1, 32), "coop": (1, 32), "rounds": (1, 32), "classes": (1, 32), "default": (2048, 2049),
+PATH_SIZES = {"v1": (1, 32), "coop": (1, 32), "rounds": (1, 32), "classes": (1, 32), "default": (2048, 2049),
               "auto": (63, 64)}
 
 
@@ -102,7 +102,7 @@ def test_random_stream_with_removals_vs_oracle(path, monkeypatch):
     GetRequestKey of every engine key, the key counts and Score() on the path are bit-exact against the oracle."""
     if path != "default":
         _select_path(monkeypatch, path)
-    rng = np.random.default_rng(sorted(PATH_SIZES).index(path) + 70)
+    rng = np.random.default_rng(SEED_ORDER_SIZES.index(path) + 70)
     BS, P, NT = 16, 12, 3
     ix, ox, pool = _pair(P=16)
     docs = [rng.integers(0, 128256, size=BS * int(rng.integers(1, 30))).tolist() for _ in range(24)]

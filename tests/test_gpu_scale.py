@@ -36,8 +36,8 @@ QA = Q + (1 << 16)                   # ... and its host-buffer batch after it
 MIB, GIB = 1 << 20, 1 << 30
 NEED_BYTES = 48 * GIB                # device memory the module needs (measured peak plus room)
 CHECK_ROWS = 1 << 17                 # rows of expected scores built at a time
-DISPATCH_VARS = ("KVIDX_SCORE_KERNEL", "KVIDX_SCORE_PATH", "KVIDX_COOP_MAX", "KVIDX_ZEROCOPY_MAX", "KVIDX_ROUNDS_MIN",
-                 "KVIDX_CLASSES_MIN", "KVIDX_CLASSES_SHARING", "KVIDX_SORT_PREFIX", "KVIDX_HOST_CHUNK_TOKENS", "KVIDX_ROUNDS_PARTS",
+DISPATCH_VARS = ("KVIDX_SCORE_KERNEL", "KVIDX_SCORE_PATH", "KVIDX_COOP_MAX", "KVIDX_ZEROCOPY_MAX", "KVIDX_CLASSES_MIN",
+                 "KVIDX_CLASSES_SHARING", "KVIDX_SORT_PREFIX", "KVIDX_HOST_CHUNK_TOKENS", "KVIDX_ROUNDS_PARTS",
                  "KVIDX_ROUNDS_WARP_MAX", "KVIDX_ROUNDS_DEDUP", "KVIDX_ROUNDS_OVERLAP_MIN")
 
 # (start, prompts, path) windows of batch A.  Below 131 072 prompts the size alone decides; from there the class pipeline

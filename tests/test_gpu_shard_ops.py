@@ -138,7 +138,7 @@ def _scores_ok(ix, ox, pkeys, tok_off):
 
 
 @pytest.mark.parametrize("chain", [("same-gpu", (2, 8)), ("multi-gpu", (2,))])
-@pytest.mark.parametrize("path", ["fused", "coop", "rounds", "classes"])
+@pytest.mark.parametrize("path", ["coop", "rounds", "classes"])
 def test_resharding_round_trips(path, chain, monkeypatch):
     """An unsharded image restored into 2 shards, their merged image into 8, and theirs into one unsharded handle again:
     after each restore, Lookup / GetRequestKey / key counts and Score() on the path through every rank are bit-exact

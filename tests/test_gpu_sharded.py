@@ -32,9 +32,9 @@ def _devices(layout, world):
 
 
 @pytest.mark.parametrize("layout,world", [("same-gpu", 2), ("same-gpu", 8), ("multi-gpu", 2), ("multi-gpu", 4)])
-@pytest.mark.parametrize("path", ["fused", "coop", "rounds", "classes"])
+@pytest.mark.parametrize("path", ["coop", "rounds", "classes"])
 def test_shards_one_process(path, layout, world, monkeypatch):
-    monkeypatch.setenv("KVIDX_SCORE_PATH", path)   # fused | coop | rounds | classes
+    monkeypatch.setenv("KVIDX_SCORE_PATH", path)   # coop | rounds | classes
     wl = synth.Workload(5, 1024, 1 << 14, 32)
     devs = _devices(layout, world)
     shards = [kvidx.Index(capacity=1 << 15, max_pods=32, device=devs[r], shard_rank=r, shard_count=world) for r in range(world)]

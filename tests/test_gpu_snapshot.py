@@ -9,7 +9,7 @@ import msgpack
 import numpy as np
 import pytest
 
-from helpers import EVENT_DTYPE, csr
+from helpers import EVENT_DTYPE, SEED_ORDER_SIZES, csr
 import kvidx
 from kvidx.host import HostIndexer
 from oracle import kvoracle as ko
@@ -46,7 +46,7 @@ def test_random_stream_snapshot_restore_continue_vs_oracle(path, monkeypatch):
     bit-exact against the oracle, also as the stream continues (parents resolve through restored engine mappings)."""
     if path != "default":
         _select_path(monkeypatch, path)
-    rng = np.random.default_rng(sorted(PATH_SIZES).index(path) + 170)
+    rng = np.random.default_rng(SEED_ORDER_SIZES.index(path) + 170)
     BS, P, NT = 16, 12, 3
     ix, ox, pool = _pair(P=16)
     docs = [rng.integers(0, 128256, size=BS * int(rng.integers(1, 30))).tolist() for _ in range(24)]

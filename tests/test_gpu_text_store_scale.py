@@ -18,7 +18,7 @@ import pytest
 import kvidx
 from kvidx import pack_text
 from kvidx.host import PrefixStore
-from helpers import PATHS, _index_pair, _select_path
+from helpers import PATHS, SEED_ORDER, _index_pair, _select_path
 from oracle.kvoracle_c import COracle
 from test_gpu_text_store import host_find
 
@@ -391,7 +391,7 @@ def _model_filter(rng, n):
 def test_score_text_on_every_score_path(path, monkeypatch):
     """Each Score() path (a handle each) scores 4096 prompts from text, dense and sparse, host and _dev, with prompts
     exactly at min_ratio 0.75 and prompts that pass it with no contained token."""
-    rng = np.random.default_rng(PATHS.index(path) + 500)
+    rng = np.random.default_rng(SEED_ORDER.index(path) + 500)
     with monkeypatch.context() as mp:
         _select_path(mp, path)
         ix, co = _index_pair(block_size=16, capacity=1 << 16, max_pods=P)
