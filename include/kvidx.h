@@ -118,7 +118,26 @@ typedef struct kvidx_config {
                                   each key before or after its eviction, and may or may not protect the keys it touches.
                                   KVIDX_EVICT_NONE (0, default): `capacity` only sizes the table.  Other values, CLOCK with
                                   lru_exact, or CLOCK on a sharded handle -> KVIDX_EINVAL. */
-    uint32_t reserved[4];
+    uint32_t grow_tables;      /* 1: both tables grow on demand up to C = pow2ceil(max(4 * capacity, 1024)) slots, what a fixed
+                                  handle with table_slots 0 allocates, so that `capacity` is a limit and not an up-front
+                                  allocation (golang-lru's maps grow as keys arrive, in_memory.go:33).  The tables start at
+                                  table_slots (rounded up to a power of two, at least 1024), or at min(C, 2^20) slots when
+                                  table_slots is 0.  Before a write batch (add, apply_events[_dev], apply_event_payloads) with
+                                  S slots, L = the larger of the live request keys and live engine mappings (tombstones do not
+                                  count) and I = the batch's bound on new keys: if S < C and 4 (L + I) > S, both tables are
+                                  rehashed, in one step, into min(C, the smallest power of two >= 4 (L + I)) slots, keeping
+                                  the load at most 1/4 as on a fixed handle; exact-LRU stamps and CLOCK reference bits move
+                                  with their keys, the CLOCK hands restart at slot 0.  Every other rule (compaction from
+                                  80 %, KVIDX_ENOSPC beyond 90 %) then runs on the new size, so a handle grown to C behaves
+                                  like the fixed one.  A growth takes the tables exclusively inside the write call that
+                                  needs it and drains the device: read calls wait for it and see the index wholly before or
+                                  after it, asynchronous reads already queued complete on the old tables (for
+                                  kvidx_apply_events_dev the growth is synchronous, the batch stays asynchronous).  A growth
+                                  whose allocation fails leaves the old tables in use under the fixed rules; its peak is old +
+                                  new tables (3x the old size).  It counts in kvidx_stats_t.rebuilds.  0 (default): the
+                                  tables are allocated whole at create.  Other values, table_slots > C, or a sharded handle
+                                  -> KVIDX_EINVAL. */
+    uint32_t reserved[3];
 } kvidx_config_t;
 
 #define KVIDX_EVICT_NONE  0u
@@ -432,7 +451,8 @@ int kvidx_remove_pods(kvidx_t* idx, const uint64_t* pod_mask, uint32_t tier_mask
  * The index's contents as a canonical image, and a bulk load of such an image into a fresh handle: an indexer that
  * restarts, is upgraded, moves to another GPU or is replicated keeps the blocks the fleet has already cached (vLLM
  * announces a block once, when it is first stored).  Restoring into a handle created with a larger capacity / table_slots
- * is also how an index outgrows its configuration.  Events sent while no indexer ran are not in any image: a block stored
+ * is also how an index outgrows its configuration; a handle with grow_tables grows by itself up to its capacity's table,
+ * and needs this only to go beyond it.  Events sent while no indexer ran are not in any image: a block stored
  * or removed in that window is missed until Evict, kvidx_remove_pods or a later event of the same block corrects it.
  *
  * Image format v1, all values little-endian:
@@ -464,7 +484,9 @@ int kvidx_remove_pods(kvidx_t* idx, const uint64_t* pod_mask, uint32_t tier_mask
  * 1 <= count <= pods_per_key, distinct entries with pod < max_pods, zero padding and entries past count, spans equal to
  * the header's) -> KVIDX_EINVAL, and the handle is left as it was.  Every record is validated before any is inserted.
  * table_slots / capacity may differ from the source's; more keys than the write path admits (90 % of a table's slots) ->
- * KVIDX_ENOSPC.  An exact-LRU handle needs an image with recency (else KVIDX_EINVAL) and keeps the most recent `capacity`
+ * KVIDX_ENOSPC.  A grow_tables handle first applies its growth rule with L = 0 and I = max(R, E): the 90 % check is made
+ * on the size the rule gives, and the (still empty) tables are reallocated at that size once every record has passed
+ * validation, so a refused image leaves the handle at its old size.  An exact-LRU handle needs an image with recency (else KVIDX_EINVAL) and keeps the most recent `capacity`
  * keys of each map, as after any write call (found from the sorted recency values: the cut costs one sort, not one table
  * sweep per excess key); a default handle ignores recency, but a repeated value is still malformed.  A concurrent reader sees each key absent
  * or whole.  restored_out (may be NULL): {request keys, engine keys} resident after the call.

@@ -251,6 +251,7 @@ struct kvidx {
     Counters* d_cnt_all = nullptr; // sharded: every owner's counters, gathered before a write batch
     Counters* h_cnt_all = nullptr;
     uint64_t rebuilds = 0;
+    uint64_t grow_max = 0;          // grow_tables: the slot count the tables may grow to (C); 0: fixed tables
     std::atomic<uint64_t> launches{0};
     std::atomic<unsigned long long> clock{1};   // exact-LRU mode: recency stamps handed to kernels
     std::mutex mu_r, mu_w;          // read-side / write-side scratch and stream
@@ -340,28 +341,51 @@ int alloc_tables(kvidx* x, uint64_t req_slots, uint64_t eng_slots, ReqSlot** req
     return 0;
 }
 
-// Drop tombstones: re-insert the live slots into fresh tables.  Caller holds mu_w and `tables` EXCLUSIVELY; every stream of
-// the device is drained first (asynchronous Score() calls may still be reading the old tables).
-//   unsharded: the fresh tables replace the old ones;
-//   sharded  : peers have this shard mapped (CUDA IPC), so the fresh tables are copied back into the same allocation.  The
-//              caller of kvidx_shard_compact guarantees that no rank touches the index meanwhile (a barrier either side).
-int rebuild(kvidx* x, bool in_place) {
+// The fresh arrays of a rebuild: both tables of `slots` slots, and the exact-LRU stamps and CLOCK reference bits the handle
+// keeps beside them.  Allocated all or nothing; whatever the rebuild has not handed to the handle is freed with this.
+struct FreshTables {
+    ReqSlot* req = nullptr; EngSlot* eng = nullptr;
+    unsigned long long* stamp = nullptr;
+    uint32_t *rref = nullptr, *eref = nullptr;
+    FreshTables() = default;
+    FreshTables(const FreshTables&) = delete;
+    FreshTables& operator=(const FreshTables&) = delete;
+    ~FreshTables() { cudaFree(req); cudaFree(eng); cudaFree(stamp); cudaFree(rref); cudaFree(eref); }
+    int alloc(const TableView& tv, uint64_t slots, cudaStream_t st) {
+        cudaError_t e = cudaMalloc((void**)&req, slots * sizeof(ReqSlot));
+        if (e == cudaSuccess) e = cudaMalloc((void**)&eng, slots * sizeof(EngSlot));
+        if (e == cudaSuccess && tv.req_stamp) e = cudaMalloc((void**)&stamp, slots * 8);
+        if (e == cudaSuccess && tv.req_ref) e = cudaMalloc((void**)&rref, slots / 8);
+        if (e == cudaSuccess && tv.req_ref) e = cudaMalloc((void**)&eref, slots / 8);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(KVIDX_ENOMEM, "cudaMalloc of two %llu-slot tables: %s", (unsigned long long)slots, cudaGetErrorString(e));
+        }
+        CK(cudaMemsetAsync(req, 0, slots * sizeof(ReqSlot), st));
+        CK(cudaMemsetAsync(eng, 0, slots * sizeof(EngSlot), st));
+        if (stamp) CK(cudaMemsetAsync(stamp, 0, slots * 8, st));
+        if (rref) { CK(cudaMemsetAsync(rref, 0, slots / 8, st)); CK(cudaMemsetAsync(eref, 0, slots / 8, st)); }
+        return 0;
+    }
+};
+
+// Re-insert the live slots into fresh tables of `slots` slots each, dropping the tombstones: a compaction keeps the slot
+// count, a growth (grow_tables, see ensure_room) raises it.  Exact-LRU stamps and CLOCK reference bits move with their keys.
+// Caller holds mu_w and `tables` EXCLUSIVELY; every stream of the device is drained first (asynchronous Score() calls may
+// still be reading the old tables).  A failed allocation (KVIDX_ENOMEM) leaves the handle exactly as it was.
+//   unsharded: the fresh tables replace the old ones, which are freed only once the fresh ones are complete;
+//   sharded  : peers have this shard mapped (CUDA IPC), so the fresh tables are copied back into the same allocation (same
+//              slot count only).  The caller of kvidx_shard_compact guarantees that no rank touches the index meanwhile
+//              (a barrier either side).
+int rebuild(kvidx* x, bool in_place, uint64_t slots) {
     CK(cudaDeviceSynchronize());
     cudaStream_t st = wstream(x);
     const uint64_t rs = x->tv.req_mask + 1, es = x->tv.eng_mask + 1;
-    ReqSlot* nreq; EngSlot* neng;
-    int rc = alloc_tables(x, rs, es, &nreq, &neng, st);
-    if (rc) return rc;
+    FreshTables f;
+    if (int rc = f.alloc(x->tv, slots, st)) return rc;
     const int T = 256;
-    unsigned long long* nstamp = nullptr;
-    if (x->tv.req_stamp) { CK(cudaMalloc((void**)&nstamp, rs * 8)); CK(cudaMemsetAsync(nstamp, 0, rs * 8, st)); }
-    uint32_t *nrref = nullptr, *neref = nullptr;       // CLOCK: every key's reference bit moves with it
-    if (x->tv.req_ref) {
-        CK(cudaMalloc((void**)&nrref, rs / 8)); CK(cudaMemsetAsync(nrref, 0, rs / 8, st));
-        CK(cudaMalloc((void**)&neref, es / 8)); CK(cudaMemsetAsync(neref, 0, es / 8, st));
-    }
-    rebuild_req_kernel<<<(unsigned)((rs + T - 1) / T), T, 0, st>>>(x->tv.req, rs, nreq, rs - 1, x->tv.req_stamp, nstamp, x->tv.req_ref, nrref);
-    rebuild_eng_kernel<<<(unsigned)((es + T - 1) / T), T, 0, st>>>(x->tv.eng, es, neng, es - 1, x->tv.eng_ref, neref);
+    rebuild_req_kernel<<<(unsigned)((rs + T - 1) / T), T, 0, st>>>(x->tv.req, rs, f.req, slots - 1, x->tv.req_stamp, f.stamp, x->tv.req_ref, f.rref);
+    rebuild_eng_kernel<<<(unsigned)((es + T - 1) / T), T, 0, st>>>(x->tv.eng, es, f.eng, slots - 1, x->tv.eng_ref, f.eref);
     x->launches += 2;
     CK(cudaGetLastError());
     // zero the tombstone counters on the device, and the CLOCK hands (slot positions of the old layout)
@@ -369,32 +393,56 @@ int rebuild(kvidx* x, bool in_place) {
     CK(cudaMemsetAsync(&x->d_cnt->eng_tomb, 0, sizeof(unsigned long long), st));
     CK(cudaMemsetAsync(x->d_cnt->hand, 0, sizeof x->d_cnt->hand, st));
     if (in_place) {
-        CK(cudaMemcpyAsync(x->tv.req, nreq, rs * sizeof(ReqSlot), cudaMemcpyDeviceToDevice, st));
-        CK(cudaMemcpyAsync(x->tv.eng, neng, es * sizeof(EngSlot), cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(x->tv.req, f.req, rs * sizeof(ReqSlot), cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(x->tv.eng, f.eng, es * sizeof(EngSlot), cudaMemcpyDeviceToDevice, st));
         CK(cudaStreamSynchronize(st));
-        cudaFree(nreq); cudaFree(neng);
     } else {
         CK(cudaStreamSynchronize(st));
-        cudaFree(x->tv.req); cudaFree(x->tv.eng);
-        if (x->tv.req_stamp) { cudaFree(x->tv.req_stamp); x->tv.req_stamp = nstamp; }
-        if (x->tv.req_ref) { cudaFree(x->tv.req_ref); cudaFree(x->tv.eng_ref); x->tv.req_ref = nrref; x->tv.eng_ref = neref; }
-        x->tv.req = nreq; x->tv.eng = neng;
-        x->tv.req_peer[0] = nreq; x->tv.eng_peer[0] = neng;
+        cudaFree(x->tv.req); cudaFree(x->tv.eng); cudaFree(x->tv.req_stamp); cudaFree(x->tv.req_ref); cudaFree(x->tv.eng_ref);
+        x->tv.req = f.req; x->tv.eng = f.eng; x->tv.req_stamp = f.stamp; x->tv.req_ref = f.rref; x->tv.eng_ref = f.eref;
+        f.req = nullptr; f.eng = nullptr; f.stamp = nullptr; f.rref = nullptr; f.eref = nullptr;
+        x->tv.req_mask = slots - 1; x->tv.eng_mask = slots - 1;
+        x->tv.req_peer[0] = x->tv.req; x->tv.eng_peer[0] = x->tv.eng;
     }
     ++x->rebuilds;
     return refresh_counters(x);
 }
 
+// grow_tables: the slot count the growth rule gives for `live` keys and `incoming` new ones.  It is the current count when
+// the tables are at their ceiling C (always, for fixed tables) or 4 (live + incoming) fits in them; otherwise
+// min(C, the smallest power of two >= 4 (live + incoming)), which keeps the load at most 1/4, the fixed default's.
+uint64_t grow_target(const kvidx* x, uint64_t live, uint64_t incoming) {
+    const uint64_t s = x->tv.req_mask + 1, need = live + incoming;
+    if (s >= x->grow_max) return s;
+    if (need >= x->grow_max / 4) return x->grow_max;
+    return 4 * need > s ? pow2ceil(4 * need) : s;
+}
+
 // Make room for up to `incoming` new keys in each table before a write batch.  Caller holds mu_w and NOT `tables`.
-//   unsharded: this handle's counters decide; tombstones are compacted away here when they are what fills the table;
+//   unsharded: this handle's counters decide.  A growable handle below its ceiling first grows both tables by the rule of
+//              grow_target (one rebuild, however many doublings); then tombstones are compacted away when they are what
+//              fills the table.  A growth that cannot allocate leaves the call on the old tables under these rules;
 //   sharded  : the keys may land on any owner, so every owner's counters are read (through the mapped peer memory) and
 //              each must have room for the whole batch; compaction is the collective kvidx_shard_compact.
 int ensure_room(kvidx* x, uint64_t incoming) {
-    const uint64_t rs = x->tv.req_mask + 1, es = x->tv.eng_mask + 1;
     // CLOCK: every eviction leaves a tombstone, so under churn tombstones are the steady state.  The host copy of the counters
     // is stale after an asynchronous batch (kvidx_apply_events_dev never reads them back): read them here, after the batches
-    // queued before this call, so that the tombstones are compacted before they fill the table
-    if (x->tv.req_ref) { int rc = refresh_counters(x); if (rc) return rc; }
+    // queued before this call, so that the tombstones are compacted before they fill the table.  A growable handle below its
+    // ceiling reads them for the same reason: the growth rule counts the live keys those batches added.
+    const bool growable = x->tv.req_mask + 1 < x->grow_max;
+    if (x->tv.req_ref || growable) { int rc = refresh_counters(x); if (rc) return rc; }
+    std::string grow_failed;
+    if (growable) {
+        const uint64_t want = grow_target(x, std::max(x->h_cnt->req_full, x->h_cnt->eng_full), incoming);
+        if (want > x->tv.req_mask + 1) {
+            std::unique_lock<std::shared_mutex> tl(x->tables);
+            if (int rc = rebuild(x, false, want)) {
+                if (rc != KVIDX_ENOMEM) return rc;
+                grow_failed = "; growing them to " + std::to_string(want) + " slots failed: " + g_err;
+            }
+        }
+    }
+    const uint64_t rs = x->tv.req_mask + 1, es = x->tv.eng_mask + 1;
     auto over = [&](uint64_t full, uint64_t tomb, uint64_t slots) { return (full + tomb + incoming) * 10 > slots * 8; };
     if (x->tv.shard_bits) {
         const uint32_t ns = 1u << x->tv.shard_bits;
@@ -415,13 +463,13 @@ int ensure_room(kvidx* x, uint64_t incoming) {
     if (over(c.req_full, c.req_tomb, rs) || over(c.eng_full, c.eng_tomb, es)) {
         if (c.req_tomb || c.eng_tomb) {
             std::unique_lock<std::shared_mutex> tl(x->tables);
-            int rc = rebuild(x, false);
+            int rc = rebuild(x, false, rs);
             if (rc) return rc;
         }
         const Counters& d = *x->h_cnt;
         if ((d.req_full + incoming) * 10 > rs * 9 || (d.eng_full + incoming) * 10 > es * 9)
-            return fail(KVIDX_ENOSPC, "table full: %llu request keys + %llu incoming in %llu slots",
-                        (unsigned long long)d.req_full, (unsigned long long)incoming, (unsigned long long)rs);
+            return fail(KVIDX_ENOSPC, "table full: %llu request keys + %llu incoming in %llu slots%s",
+                        (unsigned long long)d.req_full, (unsigned long long)incoming, (unsigned long long)rs, grow_failed.c_str());
     }
     return 0;
 }
@@ -492,8 +540,8 @@ int cap_keys(kvidx* x) {
 
 // ---- Call scopes ------------------------------------------------------------------------------------------------------
 // Locks of a call.  Read-side calls take mu_r (+ mu_w in exact-LRU mode, where everything is serialised as in round 1),
-// write-side calls mu_w; both hold `tables` shared while they launch.  Only rebuild() (through ensure_room) and the calls
-// that swap or map tables take `tables` exclusively.
+// write-side calls mu_w; both hold `tables` shared while they launch.  Only rebuild() (through ensure_room, or a growable
+// handle's restore) and the calls that swap or map tables take `tables` exclusively.
 enum : unsigned {
     kShards = 1,          // begin: every peer shard must be mapped (check_shards)
     kAfterWrites = 2,     // begin (read): order the call's stream after the last asynchronous write batch (ev_write)
@@ -553,6 +601,15 @@ struct WriteCall {
         return 0;
     }
     void exclusive() { tx = std::unique_lock<std::shared_mutex>(x->tables); }
+    // grow_tables: rebuild into `slots` slots part way through a call that holds `tables` shared (kvidx_restore grows the
+    // empty tables once the image has passed validation).  No other writer runs meanwhile: the call keeps mu_w.
+    int grow_shared(uint64_t slots) {
+        t.unlock();
+        int rc;
+        { std::unique_lock<std::shared_mutex> tl(x->tables); rc = rebuild(x, false, slots); }
+        t.lock();
+        return rc;
+    }
     WriteTally tally() const { return WriteTally{x->h_cnt->dropped_events, x->h_cnt->nospc}; }
     // The end of a synchronous write batch: the counters read back, the events it dropped, the inserts a full shard refused,
     // then the key cap.
@@ -1478,8 +1535,13 @@ int create_impl(const kvidx_config_t& c, kvidx* x) {
         while ((1u << shard_bits) < c.shard_count) ++shard_bits;
     }
     const uint64_t per_shard = c.shard_count > 1 ? (c.capacity + c.shard_count - 1) / c.shard_count : c.capacity;
-    uint64_t slots = c.table_slots ? pow2ceil(c.table_slots) : pow2ceil(std::max<uint64_t>(4 * per_shard, 1024));
+    const uint64_t full = pow2ceil(std::max<uint64_t>(4 * per_shard, 1024));
+    uint64_t slots = c.table_slots ? pow2ceil(c.table_slots) : full;
     if (slots < 1024) slots = 1024;
+    if (c.grow_tables) {                      // the tables start small and may grow up to what a fixed handle allocates
+        x->grow_max = full;
+        if (!c.table_slots) slots = std::min<uint64_t>(full, 1ull << 20);
+    }
     TableView& t = x->tv;
     t.req_mask = slots - 1; t.eng_mask = slots - 1;
     t.capacity = c.capacity; t.init_hash = c.init_hash; t.block_size = c.block_size; t.pods_per_key = c.pods_per_key;
@@ -1554,6 +1616,12 @@ int kvidx_create(const kvidx_config_t* cfg_in, kvidx_t** out) {
     if (c.evict_policy > KVIDX_EVICT_CLOCK) return fail(KVIDX_EINVAL, "unknown evict_policy %u", c.evict_policy);
     if (c.evict_policy == KVIDX_EVICT_CLOCK && c.lru_exact) return fail(KVIDX_EINVAL, "evict_policy CLOCK and lru_exact exclude each other");
     if (c.evict_policy == KVIDX_EVICT_CLOCK && c.shard_count > 1) return fail(KVIDX_EINVAL, "evict_policy CLOCK is not supported on a sharded index");
+    if (c.grow_tables > 1) return fail(KVIDX_EINVAL, "unknown grow_tables %u", c.grow_tables);
+    if (c.grow_tables && c.shard_count > 1) return fail(KVIDX_EINVAL, "grow_tables is not supported on a sharded index");
+    if (c.grow_tables && c.table_slots > pow2ceil(std::max<uint64_t>(4 * c.capacity, 1024)))
+        return fail(KVIDX_EINVAL, "table_slots %llu is above the %llu slots grow_tables may reach with capacity %llu",
+                    (unsigned long long)c.table_slots, (unsigned long long)pow2ceil(std::max<uint64_t>(4 * c.capacity, 1024)),
+                    (unsigned long long)c.capacity);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -2574,7 +2642,8 @@ int snapshot_impl(kvidx* x, void* buf, uint64_t R, uint64_t E, bool rec) {
     return x->snap.d2h(static_cast<char*>(buf) + kSnapHeaderBytes, out, body, st);
 }
 
-int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t restored_out[2]) {
+// slots: the size a growable handle's tables take before the insert (restore_call); the current size otherwise
+int restore_impl(kvidx* x, WriteCall& w, const uint8_t* body, const SnapHeader& hd, uint64_t slots, uint64_t restored_out[2]) {
     cudaStream_t st = wstream(x);
     const uint64_t R = hd.n_request, E = hd.n_engine;
     const bool rec = hd.flags & kSnapFlagRecency;
@@ -2662,7 +2731,20 @@ int restore_impl(kvidx* x, const uint8_t* body, const SnapHeader& hd, uint64_t r
                 return fail(KVIDX_ENOSPC, "shard %u full: it owns %llu request / %llu engine keys of the image, %llu / %llu slots", o,
                             h_hist[o], h_hist[8 + o], (unsigned long long)rs, (unsigned long long)es);
     }
-    // 2. the target's tombstones go (it holds no live key, so this is clearing both tables)
+    // 2. a growable handle's tables grow to the size the image needs: they hold no live key, so the rebuild only reallocates
+    //    them (and drops their tombstones).  If that allocation fails, the image goes into the old tables if the write
+    //    path's limit admits it there.
+    if (slots > x->tv.req_mask + 1) {
+        if ((rc = w.grow_shared(slots))) {
+            if (rc != KVIDX_ENOMEM) return rc;
+            const uint64_t rs = x->tv.req_mask + 1;
+            if (R * 10 > rs * 9 || E * 10 > rs * 9)
+                return fail(KVIDX_ENOSPC, "table full: %llu request / %llu engine keys in %llu slots; growing them to %llu slots failed: %s",
+                            (unsigned long long)R, (unsigned long long)E, (unsigned long long)rs, (unsigned long long)slots,
+                            std::string(g_err).c_str());
+        }
+    }
+    // the target's tombstones go (it holds no live key, so this is clearing both tables)
     const Counters& c = *x->h_cnt;
     if (c.req_tomb || c.eng_tomb) {
         CK(cudaMemsetAsync(x->tv.req, 0, (x->tv.req_mask + 1) * sizeof(ReqSlot), st));
@@ -2803,11 +2885,13 @@ int restore_call(kvidx* x, const void* buf, uint64_t len, uint64_t restored_out[
     if (x->h_cnt->req_full || x->h_cnt->eng_full)
         return fail(KVIDX_EINVAL, "restore needs an empty index: this one holds %llu request and %llu engine keys",
                     x->h_cnt->req_full, x->h_cnt->eng_full);
-    const uint64_t rs = x->tv.req_mask + 1, es = x->tv.eng_mask + 1;
-    if (!x->tv.shard_bits && (R * 10 > rs * 9 || E * 10 > es * 9))          // the write path's limit: at most 90 % of a table's slots live
+    // a growable handle is checked at the size its growth rule gives the image (as an empty handle: L = 0, I = max(R, E)),
+    // which restore_impl allocates once every record has passed validation
+    const uint64_t slots = x->tv.shard_bits ? x->tv.req_mask + 1 : grow_target(x, 0, std::max(R, E));
+    if (!x->tv.shard_bits && (R * 10 > slots * 9 || E * 10 > slots * 9))   // the write path's limit: at most 90 % of a table's slots live
         return fail(KVIDX_ENOSPC, "table full: %llu request / %llu engine keys in %llu / %llu slots", (unsigned long long)R,
-                    (unsigned long long)E, (unsigned long long)rs, (unsigned long long)es);
-    rc = restore_impl(x, static_cast<const uint8_t*>(buf) + kSnapHeaderBytes, hd, restored_out);
+                    (unsigned long long)E, (unsigned long long)slots, (unsigned long long)slots);
+    rc = restore_impl(x, w, static_cast<const uint8_t*>(buf) + kSnapHeaderBytes, hd, slots, restored_out);
     release_snap(x);
     return rc;
 }
@@ -2931,7 +3015,7 @@ int kvidx_shard_compact(kvidx_t* x) {
     WriteCall w(x);
     w.exclusive();
     if (int rc = w.begin(kDisarm)) return rc;
-    return rebuild(x, x->tv.shard_bits != 0);
+    return rebuild(x, x->tv.shard_bits != 0, x->tv.req_mask + 1);
 }
 
 // Counters of the device block read without the write lock, on no stream of the handle: a call never waits behind a write

@@ -33,7 +33,8 @@ class Config(C.Structure):
                 ("pods_per_key", C.c_uint32), ("init_hash", C.c_uint64), ("capacity", C.c_uint64),
                 ("table_slots", C.c_uint64), ("max_pods", C.c_uint32), ("n_tier_weights", C.c_uint32),
                 ("tier_weight", C.c_double * MAX_TIERS), ("lru_exact", C.c_uint32), ("shard_rank", C.c_uint32),
-                ("shard_count", C.c_uint32), ("evict_policy", C.c_uint32), ("reserved", C.c_uint32 * 4)]
+                ("shard_count", C.c_uint32), ("evict_policy", C.c_uint32), ("grow_tables", C.c_uint32),
+                ("reserved", C.c_uint32 * 3)]
 
 
 class Stats(C.Structure):
@@ -183,9 +184,11 @@ class Index:
 
     def __init__(self, block_size=16, init_hash=None, hash_seed="", capacity=1 << 20, pods_per_key=10,
                  tier_weights=(1.0, 0.8), max_pods=256, table_slots=0, device=0, lru_exact=0, shard_rank=0, shard_count=0,
-                 evict_policy="none"):
+                 evict_policy="none", grow_tables=False):
         """evict_policy: "none" (capacity only sizes the table) or "clock" (each map held to `capacity` keys by a CLOCK
-        sweep after every write call, include/kvidx.h); an int is passed to the C ABI as it is."""
+        sweep after every write call, include/kvidx.h); an int is passed to the C ABI as it is.
+        grow_tables: the tables start small and grow on demand up to the size a fixed handle allocates for `capacity`
+        (include/kvidx.h); an int is passed to the C ABI as it is."""
         self.L = load()
         cfg = Config()
         self.L.kvidx_config_default(C.byref(cfg))
@@ -202,6 +205,7 @@ class Index:
         cfg.lru_exact = lru_exact
         cfg.shard_rank, cfg.shard_count = shard_rank, shard_count
         cfg.evict_policy = _EVICT_POLICIES[evict_policy] if isinstance(evict_policy, str) else int(evict_policy)
+        cfg.grow_tables = int(grow_tables)
         h = C.c_void_p()
         rc = self.L.kvidx_create(C.byref(cfg), C.byref(h))
         if rc:

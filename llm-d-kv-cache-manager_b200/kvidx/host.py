@@ -104,7 +104,7 @@ class HostIndexer:
 
     def __init__(self, block_size=16, hash_seed="", capacity=1 << 20, pods_per_key=10, tiers=(("gpu", 1.0), ("cpu", 0.8)), max_pods=256,
                  concurrency=4, device=0, no_device=False, lru_exact=0, enable_metrics=False, clear_on_all_blocks_cleared=False,
-                 evict_policy="none"):
+                 evict_policy="none", grow_tables=False, table_slots=0):
         self.L = _lib()
         self.block_size, self.max_pods = block_size, max_pods
         cfg = HostConfig()
@@ -112,6 +112,7 @@ class HostIndexer:
         cfg.index.block_size, cfg.index.capacity, cfg.index.pods_per_key = block_size, capacity, pods_per_key
         cfg.index.max_pods, cfg.index.device, cfg.index.lru_exact = max_pods, device, lru_exact
         cfg.index.evict_policy = _native._EVICT_POLICIES[evict_policy] if isinstance(evict_policy, str) else int(evict_policy)
+        cfg.index.grow_tables, cfg.index.table_slots = int(grow_tables), table_slots
         cfg.concurrency, cfg.n_tiers, cfg.no_device = concurrency, len(tiers), 1 if no_device else 0
         cfg.enable_metrics = 1 if enable_metrics else 0
         cfg.clear_on_all_blocks_cleared = 1 if clear_on_all_blocks_cleared else 0
